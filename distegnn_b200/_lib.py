@@ -11,7 +11,7 @@ from typing import Optional
 import torch
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("DISTEGNN_B200_LIB") or os.path.join(_PKG, "libdistegnn_b200.so")   # env override: A/B builds
+LIB_PATH = os.path.join(_PKG, "libdistegnn_b200.so")
 
 # field ids of the per-layer parameter block — must match the enum in include/distegnn_b200.h
 P_FIELDS = [

@@ -4,7 +4,7 @@
 
   libdistegnn_b200.so          the product: every entry point of include/distegnn_b200.h (csrc/*.cu)
   libdistegnn_b200_testing.so  cross-check twins of include/distegnn_b200_testing.h (csrc/testing/*.cu); loaded only by
-                               tests/twin_backend.py and the A/B scripts, never by the package
+                               tests/twin_backend.py, never by the package
 
 The shared libraries and objects are build products (git-ignored); `build()` rebuilds them whenever a source, header or
 this file is newer.
@@ -46,9 +46,9 @@ def _deps_mtime():
     return max(os.path.getmtime(h) for h in hdrs)
 
 
-def _compile(src, verbose, objdir=None, defs=None):
-    obj = os.path.join(objdir or OBJ, src.replace(os.sep, "_")[:-3] + ".o")
-    extra = os.environ.get("DISTEGNN_NVCC_DEFS", "").split() + list(defs or [])   # e.g. "-DT16_CHUNK_UNROLL=4"
+def _compile(src, verbose):
+    obj = os.path.join(OBJ, src.replace(os.sep, "_")[:-3] + ".o")
+    extra = []
     if src.startswith("testing" + os.sep):        # the twins' declarations (default visibility) come from the testing header
         extra += ["-include", os.path.join(INC, "distegnn_b200_testing.h")]
     cmd = [NVCC, *ARCH, *CFLAGS, *extra, "-c", os.path.join(CSRC, src), "-o", obj]
@@ -72,40 +72,23 @@ def _link(lib, objs):
     return lib
 
 
-def _build_into(objdir, lib, lib_testing, verbose, defs=None):
-    os.makedirs(objdir, exist_ok=True)
-    srcs, tsrcs = sources(), testing_sources()
-    with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs) + len(tsrcs))) as ex:
-        objs = dict(zip(srcs + tsrcs, ex.map(lambda s: _compile(s, verbose, objdir, defs), srcs + tsrcs)))
-    _link(lib, [objs[s] for s in srcs])
-    _link(lib_testing, [objs[s] for s in COMMON] + [objs[s] for s in tsrcs])
-    return lib
-
-
 def build(force: bool = False, verbose: bool = False) -> str:
-    srcs = [os.path.join(CSRC, s) for s in sources() + testing_sources()]
-    newest = max([os.path.getmtime(s) for s in srcs] + [_deps_mtime(), os.path.getmtime(__file__)])
+    srcs, tsrcs = sources(), testing_sources()
+    newest = max([os.path.getmtime(os.path.join(CSRC, s)) for s in srcs + tsrcs]
+                 + [_deps_mtime(), os.path.getmtime(__file__)])
     if not force and all(os.path.exists(l) and os.path.getmtime(l) >= newest for l in (LIB, LIB_TESTING)):
         return LIB
-    return _build_into(OBJ, LIB, LIB_TESTING, verbose)
-
-
-def build_variant(tag: str, defs, verbose: bool = False) -> str:
-    """A/B build: the same sources with extra -D flags -> distegnn_b200/variants/libdistegnn_b200.<tag>.so
-    (select it at run time with DISTEGNN_B200_LIB=<path>)."""
-    vdir = os.path.join(PKG, "variants")
-    return _build_into(os.path.join(vdir, "build_" + tag), os.path.join(vdir, f"libdistegnn_b200.{tag}.so"),
-                       os.path.join(vdir, f"libdistegnn_b200_testing.{tag}.so"), verbose, defs)
+    os.makedirs(OBJ, exist_ok=True)
+    with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs) + len(tsrcs))) as ex:
+        objs = dict(zip(srcs + tsrcs, ex.map(lambda s: _compile(s, verbose), srcs + tsrcs)))
+    _link(LIB, [objs[s] for s in srcs])
+    _link(LIB_TESTING, [objs[s] for s in COMMON] + [objs[s] for s in tsrcs])
+    return LIB
 
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--force", action="store_true")
     ap.add_argument("--verbose", action="store_true")
-    ap.add_argument("--variant", metavar="TAG", help="build an A/B variant; flags via --defs")
-    ap.add_argument("--defs", default="", help="extra nvcc flags for --variant, e.g. --defs=-DDEGNN_SILU_MODE=0")
     a = ap.parse_args()
-    if a.variant:
-        print(build_variant(a.variant, a.defs.split(), a.verbose))
-    else:
-        print(build(a.force, a.verbose))
+    print(build(a.force, a.verbose))

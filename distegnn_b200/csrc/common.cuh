@@ -49,9 +49,6 @@ void ensure_dynamic_smem(const void* kernel, int bytes);
 
 // ---- device helpers -----------------------------------------------------------------------------
 __device__ __forceinline__ float silu(float x) {
-#ifdef DEGNN_DIAG_NO_SILU      // diagnostic build only (timing apportionment): NOT the model's activation
-    return x * 0.5f;
-#endif
     // x·σ(x) = x · rcp(1 + 2^{-x·log2 e}): FMUL, MUFU.EX2, FADD, MUFU.RCP, FMUL — no range fix-ups needed:
     // x → −∞ gives 2^{+big} = inf, rcp(inf) = 0, x·0 = −0;  x → +∞ gives rcp(1) = 1.  |rel err| ≲ 5e-7.
     float e, r;
@@ -66,14 +63,9 @@ __device__ __forceinline__ float4 silu4(float4 v) {
 // ---- fp32 register pairs --------------------------------------------------------------------------------------------
 // The elementwise chains around the MMAs work on register PAIRS (f32x2: two fp32 in one 64-bit value, even column in the
 // low half) so that they line up with the packed fp16 words of the A operand.  sm_90 has no packed fp32 instructions:
-// add2 / sub2 / mul2 / fma2 are two scalar round-to-nearest operations each.  DEGNN_SILU_MODE selects the SiLU flavour:
-//   0  one reciprocal per activation
-//   1  the same, through the pair helpers
-//   2  one reciprocal per FOUR activations:  1/d_i = d_j·d_k·d_l / (d_0 d_1 d_2 d_3)  (5 MUFU per 4 instead of 8; falls
-//      back to 4 RCPs when the product leaves the fp32 range, i.e. some x < about −21)
-#ifndef DEGNN_SILU_MODE
-#define DEGNN_SILU_MODE 2
-#endif
+// add2 / sub2 / mul2 / fma2 are two scalar round-to-nearest operations each.  The SiLU of the pair chains takes one
+// reciprocal per FOUR activations:  1/d_i = d_j·d_k·d_l / (d_0 d_1 d_2 d_3)  (5 MUFU per 4 instead of 8; falls back to
+// 4 RCPs when the product leaves the fp32 range, i.e. some x < about −21)
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pk2(float lo, float hi) {
     f32x2 r;
@@ -109,33 +101,16 @@ __device__ __forceinline__ f32x2 rcp2(f32x2 d) {
     upk2(d, d0, d1);
     return pk2(rcp_approx(d0), rcp_approx(d1));
 }
-__device__ __forceinline__ f32x2 silu2(f32x2 x) {
-#if DEGNN_SILU_MODE == 0 || defined(DEGNN_DIAG_NO_SILU)
-    float x0, x1;
-    upk2(x, x0, x1);
-    return pk2(silu(x0), silu(x1));
-#else
-    return mul2(x, rcp2(silu_den2(x)));
-#endif
-}
-// Four activations (two pairs) at once.  In mode 2 the caller owns the range guard: `qmax` accumulates the largest
+__device__ __forceinline__ f32x2 silu2(f32x2 x) { return mul2(x, rcp2(silu_den2(x))); }
+// Four activations (two pairs) at once.  The caller owns the range guard: `qmax` accumulates the largest
 // product d0·d1·d2·d3 seen; if silu_q_overflow(qmax) the results of that batch are invalid (1/q is not a normal
 // number: some x < about −21) and must be recomputed with SAFE = true, which is the per-element-reciprocal form.
 // A guard per quad would either be if-converted by ptxas into predicated MUFUs on the hot path or, as a real
 // branch, serialise the quads — so it is hoisted to once per stage, next to the fp16-range rescue.
 constexpr float SILU_Q_LIMIT = 8.0e37f;
-#if DEGNN_SILU_MODE == 2 && !defined(DEGNN_DIAG_NO_SILU)
-constexpr bool kSiluGuard = true;
-#else
-constexpr bool kSiluGuard = false;
-#endif
-__device__ __forceinline__ bool silu_q_overflow(float qmax) { return kSiluGuard && !(qmax < SILU_Q_LIMIT); }
+__device__ __forceinline__ bool silu_q_overflow(float qmax) { return !(qmax < SILU_Q_LIMIT); }
 template <bool SAFE>
 __device__ __forceinline__ void silu4p(f32x2& a, f32x2& b, float& qmax) {
-#if DEGNN_SILU_MODE != 2 || defined(DEGNN_DIAG_NO_SILU)
-    a = silu2(a);
-    b = silu2(b);
-#else
     if (SAFE) {
         a = silu2(a);
         b = silu2(b);
@@ -152,7 +127,6 @@ __device__ __forceinline__ void silu4p(f32x2& a, f32x2& b, float& qmax) {
                                                               // register pair directly (a packed form needs 3 MOVs)
     a = mul2(a, mul2(u, db));                                 // x · (1/d0, 1/d1)
     b = mul2(b, mul2(u, da));                                 // x · (1/d2, 1/d3)
-#endif
 }
 // The same in the "t domain": the inputs are t = −log2(e)·x (the producer folds the factor into its weights / biases), the
 // outputs s = t / (1 + 2^t) = −log2(e)·SiLU(x) — the consumer folds −ln 2 into whatever multiplies s next.  Saves the
@@ -167,7 +141,7 @@ __device__ __forceinline__ f32x2 silu_den2_t(f32x2 t) {
 template <bool SAFE>
 __device__ __forceinline__ void silu4t(f32x2& a, f32x2& b, float& qmax) {
     const f32x2 da = silu_den2_t(a), db = silu_den2_t(b);
-    if (SAFE || !kSiluGuard) {
+    if (SAFE) {
         a = mul2(a, rcp2(da));
         b = mul2(b, rcp2(db));
         return;

@@ -57,53 +57,13 @@ struct EdgeCsArgs {
     float* agg_x;
 };
 
-// A/B build knobs (python -m distegnn_b200.build --variant ... --defs=-DCS_SEGSUM_V2=0):
-//   CS_SEGSUM_V2  1: segment sum of m as one straight pass over the warp's 16 edges with a flush at run starts;
-//                    0: loop over runs with an inner loop per run
-#ifndef CS_SEGSUM_V2
-#define CS_SEGSUM_V2 1
-#endif
-#ifndef CS_REFILL_BARRIER
-#define CS_REFILL_BARRIER 0     // 1: group barrier before the staging buffer is refilled; 0: per-warp ordering only
-#endif
-#ifndef CS_S1_UNROLL
-#define CS_S1_UNROLL 2          // chunks (of 8 columns) of stage 1 unrolled together (P / Q loads of both in flight)
-#endif
-#ifndef CS_P_PREFETCH
-#define CS_P_PREFETCH 1         // L1 prefetch of the next tile's P rows after MMA 1
-#endif
-#ifndef CS_SEGSUM_FAST
-#define CS_SEGSUM_FAST 1        // 1: warps whose 16 edges all share one destination row take a test-free summation path
-#endif
-#ifndef CS_DEFER_AGGX
-#define CS_DEFER_AGGX 0         // 1: the shuffle reduction + RED.ADD of Δx·φ of tile i runs after MMA 1 of tile i+1
-#endif
-#ifndef CS_X_STAGED
-#define CS_X_STAGED 1           // 1: the next tile's coordinates x[row], x[col] are gathered by cp.async into shared memory (one
-#endif                          // copy per edge, issued after the stage-1 barrier, visible to both column halves after the
-                                // stage-2 barrier); 0: every thread loads them with LDG after the segment sum
-#ifndef CS_P_AHEAD
-#define CS_P_AHEAD 1            // 1: stage 1 requests P[row] one chunk ahead (chunk 0 at the end of the previous tile)
-#endif
-#ifndef CS_SCHED_FENCE
-#define CS_SCHED_FENCE 0        // bit mask of the stages (1, 2, 4 = stage 1, 2, 3) whose read-ahead load is pinned above the
-#endif                          // current chunk's math by a scheduling fence (__syncwarp: no instruction, but ptxas does not
-                                // move code across it)
-#ifndef CS_TDOMAIN
-#define CS_TDOMAIN 1            // 1: stages 2 and 3 run in the "t domain" (common.cuh silu4t): W2 and the biases b2 / bc carry
-#endif                          // −log2(e), w3 and the segment-sum flush carry −ln 2, and the per-pair multiply that forms the
-                                // exponent argument disappears from both stages; 0: plain SiLU on x
-constexpr bool kNeg2 = CS_TDOMAIN;      // stage-2 values are ≤ 0.41 and unbounded below in the t domain
-constexpr float kTIn = CS_TDOMAIN ? SILU_T_IN : 1.0f, kTOut = CS_TDOMAIN ? SILU_T_OUT : 1.0f;
 // One tile group per CTA: its 64 KB of tile memory and 35 KB staging buffer next to the weights leave no room for a second
 // one in 227 KB of shared memory.  The per-group indexing below follows CS_GROUPS.
 constexpr int CS_THREADS = 256, CS_GROUPS = 1, CS_GROUP = 256, CS_WARPS = 8;
-constexpr int kS1Unroll = CS_S1_UNROLL;
 // padded row pitch of the staging buffer (floats): 68 = conflict-free row-per-thread LDS.128 / STS.128
 constexpr int CS_QROW = 68;
 constexpr int CS_QBUF = TILE_M * CS_QROW;
 __host__ __device__ constexpr int cs_qoff(int r) { return r * CS_QROW; }
-static_assert(!CS_TDOMAIN || CS_SEGSUM_V2, "the t-domain flush factor is only wired into the straight-pass segment sum");
 constexpr int CS_TM_COLS = 128;                           // per tile group: A_hi 32 | A_lo 32 | D 64
 constexpr int CS_W = 64 * 64;                             // fp16 elements per weight matrix (8 KB)
 constexpr int CS_IDX = TILE_M * 4;                        // ints per index buffer: row 128 | col 128 | ea 128x2
@@ -116,7 +76,7 @@ constexpr int CS_SMEM_BYTES = tmma::tm_bytes(CS_GROUPS * CS_TM_COLS)
                               + CS_GROUPS * 2 * CS_IDX * 4    // staged indices of the next tile, double buffered
                               + CS_GROUPS * 2 * CS_WARPS * 4  // out-of-range flags per warp, one set per stage
                               + CS_GROUPS * 2 * TILE_M * 4    // row maxima of the two column halves (cold path)
-                              + (CS_X_STAGED ? CS_GROUPS * TILE_M * 8 * 4 : 0)   // x[row], x[col] of the next tile's edges
+                              + CS_GROUPS * TILE_M * 8 * 4    // x[row], x[col] of the next tile's edges
                               + 128;                          // mbarriers
 constexpr uint32_t CS_LBO = 1024;                         // fp16 K-major no-swizzle, N = 64
 using tc16::kFast;
@@ -171,7 +131,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
     uint32_t* oflag_all = reinterpret_cast<uint32_t*>(nidx_all + CS_GROUPS * 2 * CS_IDX);   // [groups][2][8]
     float* rowmax_all = reinterpret_cast<float*>(oflag_all + CS_GROUPS * 2 * CS_WARPS);      // [groups][2][128]
     float* xs_all = rowmax_all + CS_GROUPS * 2 * TILE_M;                                       // [groups][128][8]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(xs_all + (CS_X_STAGED ? CS_GROUPS * TILE_M * 8 : 0));   // [groups]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(xs_all + CS_GROUPS * TILE_M * 8);             // [groups]
 
     const int tid = threadIdx.x;
     const int grp = tid >> 8;              // tile group 0 .. CS_GROUPS-1
@@ -184,20 +144,15 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
     const int cb = 32 * hf;                // first owned column
     const int A = AT >= 0 ? AT : a.A;
     const bool normalize = a.flags & DISTEGNN_FLAG_NORMALIZE;
-    // ptxas schedules freely inside a basic block and may sink a read-ahead load below the math of the current chunk;
-    // sched_fence(stage bit) pins it (A/B knob CS_SCHED_FENCE).
-    auto sched_fence = [&](int stage_bit) {
-        if (CS_SCHED_FENCE & stage_bit) __syncwarp();
-    };
     constexpr bool need_m = !LASTL;        // the last layer only moves coordinates (DISTEGNN_FLAG_LAST): no segment sum of m
 
     // ---- one-time setup -------------------------------------------------------------------------
-    tc16::stage_weight<CS_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, kTIn);     // t2 = kTIn·(a1·W2ᵀ + b2)
-    tc16::stage_weight<CS_THREADS>(Wchi, Wclo, a.wc, 0, 64, tid);           // t3 = s2·Wcᵀ + kTIn·bc  (kTIn·kTOut = 1)
+    tc16::stage_weight<CS_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, SILU_T_IN);   // t2 = SILU_T_IN·(a1·W2ᵀ + b2)
+    tc16::stage_weight<CS_THREADS>(Wchi, Wclo, a.wc, 0, 64, tid);   // t3 = s2·Wcᵀ + SILU_T_IN·bc  (SILU_T_IN·SILU_T_OUT = 1)
     if (tid < H) {
-        b2s[tid] = a.b2[tid] * kTIn;
-        bcs[tid] = a.bc[tid] * kTIn;
-        w3s[tid] = a.w3[tid] * kTOut;
+        b2s[tid] = a.b2[tid] * SILU_T_IN;
+        bcs[tid] = a.bc[tid] * SILU_T_IN;
+        w3s[tid] = a.w3[tid] * SILU_T_OUT;
         w1rs[tid] = a.w1r[tid];
     }
     for (int i = tid; i < DISTEGNN_MAX_EDGE_ATTR * H; i += CS_THREADS) w1es[i] = i < A * H ? a.w1e[i] : 0.f;
@@ -254,7 +209,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         cp_async_commit();
     };
 
-    ulonglong2 p_first[2];        // CS_P_AHEAD: the first 8 own columns of P[row] of the tile about to be processed
+    ulonglong2 p_first[2];        // the first 8 own columns of P[row] of the tile about to be processed
     p_first[0] = p_first[1] = make_ulonglong2(0ull, 0ull);
     int row_c = -1;
     float dx = 0.f, dy = 0.f, dz = 0.f, radial = 0.f;
@@ -286,7 +241,6 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             atomicAdd(dst + 2, sz);
         }
     };
-    float dfx = 0.f, dfy = 0.f, dfz = 0.f;      // CS_DEFER_AGGX: the previous tile's Δx·φ_half of this thread's edge
 
     // ---- prologue: first tile read directly, its Q rows fetched, the second tile's indices staged ---------------
     if (tile < num_tiles) {
@@ -305,10 +259,8 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         }
         if (hf == 0 && row_c >= 0) bulk_g2s(qb + cs_qoff(r), a.Q + (size_t)col_c * H, H * 4, qbar);
         set_geometry(ldg4(a.x4 + (size_t)max(row_c, 0) * 4), ldg4(a.x4 + (size_t)col_c * 4));
-#if CS_P_AHEAD
         p_first[0] = __ldg(reinterpret_cast<const ulonglong2*>(a.P + (size_t)max(row_c, 0) * H + cb));
         p_first[1] = __ldg(reinterpret_cast<const ulonglong2*>(a.P + (size_t)max(row_c, 0) * H + cb + 4));
-#endif
     }
 
     for (int it = 0; tile < num_tiles; ++it, tile += stride) {
@@ -329,7 +281,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         const float* prow = a.P + (size_t)max(row_c, 0) * H + cb;
         float qmax = 0.f;
         const f32x2 rad2 = bc2(radial);
-        // P values of chunk j (8 columns) arrive as `pp`: on the hot path they were requested one chunk earlier (CS_P_AHEAD)
+        // P values of chunk j (8 columns) arrive as `pp`: on the hot path they were requested one chunk earlier
         auto pre_math = [&](int j, const ulonglong2 (&pp)[2], f32x2 (&v)[4], auto safe) {
 #pragma unroll
             for (int j4 = 0; j4 < 2; ++j4) {
@@ -363,7 +315,6 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         float inv_s1 = 1.0f;
         {
             __half2 mx = __floats2half2_rn(0.f, 0.f);
-#if CS_P_AHEAD
             // P[row] comes from L2 (the rows of a tile are few, but L1 keeps little between tiles): chunk 0 was requested at
             // the end of the previous tile (p_first), chunk j+1 is requested before the math of chunk j
             ulonglong2 pq[2][2];
@@ -374,23 +325,11 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 f32x2 v[4];
                 uint32_t hi[4], lo[4];
                 if (j < 3) load_p(prow, j + 1, pq[(j + 1) & 1]);
-                sched_fence(1);
                 pre_math(j, pq[j & 1], v, kFast);
                 split8<false, false>(v, 1.0f, hi, lo, mx);
                 tm_st4(tA_hi + 4 * j, hi);
                 tm_st4(tA_lo + 4 * j, lo);
             }
-#else
-#pragma unroll kS1Unroll
-            for (int j = 0; j < 4; ++j) {
-                f32x2 v[4];
-                uint32_t hi[4], lo[4];
-                pre_chunk(j, v, kFast);
-                split8<false, false>(v, 1.0f, hi, lo, mx);
-                tm_st4(tA_hi + 4 * j, hi);
-                tm_st4(tA_lo + 4 * j, lo);
-            }
-#endif
             const bool bad = __any_sync(FULL, row_overflow8<false>(mx) || silu_q_overflow(qmax));
             if (lane == 0) oflag[wk] = bad ? 1u : 0u;
         }
@@ -431,22 +370,13 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             const int prev = r > 0 ? srow[r - 1] : -2;
             const uint32_t starts = __ballot_sync(FULL, prev != row_c);
             if (lane == 0) rmask[wq] = starts;
-#if CS_X_STAGED
             if (nvalid_r) {        // coordinates of the next tile's edge: one gather per edge, consumed after stage 3
                 cp_async16(xs, a.x4 + (size_t)nrow_s[r] * 4);
                 cp_async16(xs + 4, a.x4 + (size_t)ncol_s[r] * 4);
             }
             cp_async_commit();
-#endif
         }
-#if CS_P_PREFETCH
         if (nvalid_r) prefetch_l1(a.P + (size_t)nrow_s[r] * H + cb);      // one 128-byte line per thread
-#endif
-#if CS_DEFER_AGGX
-        // the previous tile's coordinate aggregation, here because the group would otherwise idle until MMA 1 completes
-        // (its destination rows are still in the other parity slot of srow)
-        if (it > 0) reduce_aggx(dfx, dfy, dfz, srow2[((it - 1) & 1) * TILE_M + r]);
-#endif
 
         mma_done();
 
@@ -460,11 +390,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(b2s + cb + cc);
                 f32x2 m0 = fma2(pk2u(d[4 * j4 + 0], d[4 * j4 + 1]), is2, bb.x);
                 f32x2 m1 = fma2(pk2u(d[4 * j4 + 2], d[4 * j4 + 3]), is2, bb.y);
-#if CS_TDOMAIN
-                silu4t<decltype(safe)::value>(m0, m1, qmax);     // (m0, m1) = kTIn·m: the flush and Wc's consumer undo it
-#else
-                silu4p<decltype(safe)::value>(m0, m1, qmax);
-#endif
+                silu4t<decltype(safe)::value>(m0, m1, qmax);     // (m0, m1) = SILU_T_IN·m: the flush and Wc's consumer undo it
                 if (store) *reinterpret_cast<ulonglong2*>(myq + cc) = make_ulonglong2(m0, m1);
                 v[2 * j4] = m0;
                 v[2 * j4 + 1] = m1;
@@ -483,17 +409,15 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 f32x2 v[4];
                 uint32_t hi[4], lo[4];
                 m_chunk(j, v, need_m, kFast);
-                split8<false, kNeg2>(v, 1.0f, hi, lo, mx);
+                split8<false, true>(v, 1.0f, hi, lo, mx);      // t-domain values: ≤ 0.41, unbounded below
                 tm_st4(tA_hi + 4 * j, hi);
                 tm_st4(tA_lo + 4 * j, lo);
             }
-            const bool bad = __any_sync(FULL, row_overflow8<kNeg2>(mx) || silu_q_overflow(qmax));
+            const bool bad = __any_sync(FULL, row_overflow8<true>(mx) || silu_q_overflow(qmax));
             if (lane == 0) oflag[CS_WARPS + wk] = bad ? 1u : 0u;
         }
         tm_st_fence();
-#if CS_X_STAGED
         if (hf == 0) cp_async_wait_all();      // the staged coordinates: visible to both halves after the barrier
-#endif
         named_bar(bar_id, CS_GROUP);           // m tile visible in shared, A complete, D fully read
         if (group_flag(1)) {                   // cold
             float fm = 0.f, sc;
@@ -501,7 +425,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             for (int j = 0; j < 4; ++j) {
                 f32x2 v[4];
                 m_chunk(j, v, need_m, kSafe);  // also rewrites the m row in shared memory
-                fm = max8<kNeg2>(v, fm);
+                fm = max8<true>(v, fm);
             }
             rowmax[hf * TILE_M + r] = fm;
             named_bar(bar_id, CS_GROUP);
@@ -512,7 +436,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 f32x2 v[4];
                 uint32_t hi[4], lo[4];
                 m_chunk(j, v, false, kSafe);
-                split8<true, kNeg2>(v, sc, hi, lo, mx);
+                split8<true, true>(v, sc, hi, lo, mx);
                 tm_st4(tA_hi + 4 * j, hi);
                 tm_st4(tA_lo + 4 * j, lo);
             }
@@ -526,7 +450,6 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             // warp wk <-> edges 16wk .. 16wk+15 of the tile, lane <-> columns 2·lane, 2·lane+1: per edge one LDS.64
             // and one pair add; the run structure is warp-uniform, one RED.v2 per run and lane
             const float* colp = qb + cs_qoff(16 * wk) + 2 * lane;     // 16·wk is a multiple of 8: row e of the warp sits at cs_qoff(e)
-#if CS_SEGSUM_V2
             // one straight pass over the warp's 16 edges; bit e of M = edge e starts a new run of equal destination rows
             // (warp-uniform), where the running sum is flushed with one RED.v2 per lane
             const uint32_t M = (rmask[wk >> 1] >> (16 * (wk & 1))) & 0xffffu;
@@ -535,12 +458,11 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 const int rr = srw[e_last];
                 if (rr >= 0) {
                     float v0, v1;
-                    upk2(CS_TDOMAIN ? mul2(acc, bc2(kTOut)) : acc, v0, v1);
+                    upk2(mul2(acc, bc2(SILU_T_OUT)), v0, v1);
                     red_add_v2(a.agg_m + (size_t)rr * H + 2 * lane, v0, v1);
                 }
             };
             f32x2 s0 = *reinterpret_cast<const f32x2*>(colp);
-#if CS_SEGSUM_FAST
             if ((M >> 1) == 0u) {       // no run starts inside the warp's 16 edges (about half of the warps at degree 20):
                 f32x2 s1 = *reinterpret_cast<const f32x2*>(colp + cs_qoff(1));     // two plain chains, no per-edge test
 #pragma unroll
@@ -549,9 +471,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                     s1 = add2(s1, *reinterpret_cast<const f32x2*>(colp + cs_qoff(e + 1)));
                 }
                 flush(add2(s0, s1), 15);
-            } else
-#endif
-            {
+            } else {
 #pragma unroll
                 for (int e = 1; e < 16; ++e) {
                     const f32x2 v = *reinterpret_cast<const f32x2*>(colp + cs_qoff(e));
@@ -564,39 +484,12 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 }
                 flush(s0, 15);
             }
-#else
-            uint32_t M = ((rmask[wk >> 1] >> (16 * (wk & 1))) & 0xffffu) | 1u;
-            while (M) {
-                const int e0 = __ffs((int)M) - 1;
-                M &= M - 1;
-                const int e1 = M ? __ffs((int)M) - 1 : 16;
-                f32x2 s0 = 0ull, s1 = 0ull, s2 = 0ull, s3 = 0ull;
-                int e = e0;
-                for (; e + 3 < e1; e += 4) {
-                    s0 = add2(s0, *reinterpret_cast<const f32x2*>(colp + e * CS_QROW));
-                    s1 = add2(s1, *reinterpret_cast<const f32x2*>(colp + (e + 1) * CS_QROW));
-                    s2 = add2(s2, *reinterpret_cast<const f32x2*>(colp + (e + 2) * CS_QROW));
-                    s3 = add2(s3, *reinterpret_cast<const f32x2*>(colp + (e + 3) * CS_QROW));
-                }
-                for (; e < e1; ++e) s0 = add2(s0, *reinterpret_cast<const f32x2*>(colp + e * CS_QROW));
-                const int rr = srow[16 * wk + e0];
-                if (rr >= 0) {
-                    float v0, v1;
-                    upk2(add2(add2(s0, s1), add2(s2, s3)), v0, v1);
-                    red_add_v2(a.agg_m + (size_t)rr * H + 2 * lane, v0, v1);
-                }
-            }
-#endif
         }
         // The rows a warp refills (16·wk .. +15) were last read by that same warp (segment sum) — their stage-1 / stage-2
         // accesses by the owner threads lie before the previous group barrier — so no group barrier is needed here: warp-level
         // ordering of the generic accesses before the async-proxy refill is enough.
         fence_proxy_async_smem();
-#if CS_REFILL_BARRIER
-        named_bar(bar_id, CS_GROUP);
-#else
         __syncwarp();
-#endif
 
         // ---- Q rows of the next tile, addresses from the staged indices ----------------------------------------------------
         if (ntile < num_tiles) {
@@ -608,16 +501,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             if (lane < 16 && ntile * TILE_M + rr < nE)
                 bulk_g2s(qb + rr * CS_QROW, a.Q + (size_t)ncol_s[rr] * H, H * 4, qbar);
         }
-        // coordinates of the next tile's edge (consumed after stage 3)
-        int row_n = -1;
-        float4 xi_n = make_float4(0.f, 0.f, 0.f, 0.f), xj_n = xi_n;
-        if (nvalid_r) {
-            row_n = nrow_s[r];
-#if !CS_X_STAGED
-            xi_n = ldg4(a.x4 + (size_t)row_n * 4);
-            xj_n = ldg4(a.x4 + (size_t)ncol_s[r] * 4);
-#endif
-        }
+        const int row_n = nvalid_r ? nrow_s[r] : -1;      // destination row of the next tile's edge
 
         mma_done();
 
@@ -636,11 +520,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                     const ulonglong2 ww = *reinterpret_cast<const ulonglong2*>(w3s + cc);
                     f32x2 s0 = fma2(pk2u(d[4 * j4 + 0], d[4 * j4 + 1]), is2, bb.x);
                     f32x2 s1 = fma2(pk2u(d[4 * j4 + 2], d[4 * j4 + 3]), is2, bb.y);
-#if CS_TDOMAIN
                     silu4t<decltype(safe)::value>(s0, s1, qmax);
-#else
-                    silu4p<decltype(safe)::value>(s0, s1, qmax);
-#endif
                     ph01 = fma2(s0, ww.x, ph01);
                     ph23 = fma2(s1, ww.y, ph23);
                 }
@@ -653,23 +533,17 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             }
         };
         phi_pass(kFast);
-        if (kSiluGuard && __any_sync(FULL, silu_q_overflow(qmax))) phi_pass(kSafe);      // cold (warp-local: no scale)
+        if (__any_sync(FULL, silu_q_overflow(qmax))) phi_pass(kSafe);      // cold (warp-local: no scale)
         float ph0, ph1, ph2, ph3;
         upk2(ph01, ph0, ph1);
         upk2(ph23, ph2, ph3);
         const float phi = (ph0 + ph1) + (ph2 + ph3);
-#if CS_P_AHEAD
         {   // the next tile's first P chunk: in flight across the shuffle reduction, the roll and the wait for the Q rows
             const float* pn = a.P + (size_t)max(row_n, 0) * H + cb;
             p_first[0] = __ldg(reinterpret_cast<const ulonglong2*>(pn));
             p_first[1] = __ldg(reinterpret_cast<const ulonglong2*>(pn + 4));
         }
-#endif
-#if CS_DEFER_AGGX
-        dfx = dx * phi; dfy = dy * phi; dfz = dz * phi;      // reduced and added to agg_x after the next MMA 1 (or the epilogue)
-#else
         reduce_aggx(dx * phi, dy * phi, dz * phi, row_c);
-#endif
 
         // ---- roll the next tile's edge into place -------------------------------------------------------------
         row_c = row_n;
@@ -689,22 +563,13 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                     if (k < A) ea_c[k] = __ldg(a.ea + e * A + k);
             }
         }
-#if CS_X_STAGED
+        float4 xi_n = make_float4(0.f, 0.f, 0.f, 0.f), xj_n = xi_n;
         if (nvalid_r) {
             xi_n = *reinterpret_cast<const float4*>(xs);
             xj_n = *reinterpret_cast<const float4*>(xs + 4);
         }
-#endif
         set_geometry(xi_n, xj_n);
     }
-
-#if CS_DEFER_AGGX
-    {   // the last tile's deferred aggregation (it_done tiles were processed by this group)
-        const int64_t first = (int64_t)blockIdx.x * CS_GROUPS + grp;
-        const int64_t it_done = first < num_tiles ? (num_tiles - first + stride - 1) / stride : 0;
-        if (it_done > 0) reduce_aggx(dfx, dfy, dfz, srow2[((it_done - 1) & 1) * TILE_M + r]);
-    }
-#endif
 }
 
 }  // namespace degnn

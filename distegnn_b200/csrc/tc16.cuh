@@ -19,10 +19,6 @@ namespace degnn {
 namespace tc16 {
 
 constexpr float RANGE = 3.0e4f;
-#ifndef TC16_CHUNK_UNROLL
-#define TC16_CHUNK_UNROLL 1    // chunks (of 16 columns) unrolled in encode_row: code size (I-cache) vs ILP
-#endif
-constexpr int kChunkUnroll = TC16_CHUNK_UNROLL;
 // (hi, lo) fp16 pairs of the fp32 pair x: hi = rn(x), lo = rn(x − hi).  x − hi is exact in fp32 (hi is within half an fp16
 // ulp of x).
 __device__ __forceinline__ void split_pair(f32x2 x, uint32_t& hi, uint32_t& lo) {
@@ -39,30 +35,20 @@ __device__ __forceinline__ void split_pair(f32x2 x, uint32_t& hi, uint32_t& lo) 
 // stage W[n][k] (given k-major: wt[k*64+n]) as rows n_off..n_off+63 of an N_total-row B operand, fp16 hi/lo
 // NTHREADS is a template parameter so that the H·H / NTHREADS loads of a thread are all issued before the first conversion
 // (a rolled load -> convert -> store loop pays one global round trip per element and thread).
-#ifndef TC16_STAGE_BATCH
-#define TC16_STAGE_BATCH 1
-#endif
 template <int NTHREADS>
 __device__ __forceinline__ void stage_weight(__half* hi, __half* lo, const float* __restrict__ wt_kmajor, int n_off,
                                              int n_total, int tid, float scale = 1.0f) {
     static_assert((H * H) % NTHREADS == 0, "thread count must divide the matrix");
     constexpr int R = H * H / NTHREADS;
     const uint32_t lbo_h = (uint32_t)(n_total / 8) * 64u;     // halfs per K chunk of 8
-#if TC16_STAGE_BATCH
     float w[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) w[r] = __ldg(wt_kmajor + tid + r * NTHREADS);
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-#else
-    float w[1];
-#pragma unroll 1
-    for (int r = 0; r < R; ++r) {
-        w[0] = __ldg(wt_kmajor + tid + r * NTHREADS);
-#endif
         const int i = tid + r * NTHREADS;
         const int k = i >> 6, n = (i & 63) + n_off;
-        const float ws = w[TC16_STAGE_BATCH ? r : 0] * scale;
+        const float ws = w[r] * scale;
         const __half h = __float2half_rn(ws);
         const uint32_t o = (uint32_t)(k >> 3) * lbo_h + (uint32_t)(n >> 3) * 64u + (uint32_t)(n & 7) * 8u + (k & 7);
         hi[o] = h;
@@ -145,7 +131,7 @@ __device__ __forceinline__ float encode_row_s(F&& f, uint32_t ta_hi, uint32_t ta
     __half2 mx = __floats2half2_rn(0.f, 0.f);
     const bool pre_scaled = __any_sync(FULL, s_in != 1.0f);
     if (!pre_scaled) {
-#pragma unroll kChunkUnroll
+#pragma unroll 1
         for (int c = 0; c < 4; ++c) {
             float v[16];
             uint32_t hi[8], lo[8];
@@ -202,7 +188,7 @@ __device__ __forceinline__ float encode_row2_s(F&& f, uint32_t ta_hi, uint32_t t
     float qmax = 0.f;
     const bool pre_scaled = __any_sync(FULL, s_in != 1.0f);
     if (!pre_scaled) {
-#pragma unroll kChunkUnroll
+#pragma unroll 1
         for (int c = 0; c < 4; ++c) {
             f32x2 v[8];
             uint32_t hi[8], lo[8];
@@ -246,7 +232,7 @@ __device__ __forceinline__ float encode_row2_tm(F&& f, uint32_t t_src, uint32_t 
     __half2 mx = __floats2half2_rn(0.f, 0.f);
     float qmax = 0.f;
     {
-#pragma unroll kChunkUnroll
+#pragma unroll 1
         for (int c = 0; c < 4; ++c) {
             f32x2 v[8];
             uint32_t hi[8], lo[8], d[16];

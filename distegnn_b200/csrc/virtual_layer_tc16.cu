@@ -9,7 +9,7 @@
 // (tile_mma.cuh): A_hi 32 + A_lo 32 + D 64 columns (the two coordinate heads reuse D one after the other).
 //   stage 1  a1 = SiLU(Hn[node] + G[graph,c] + w_r·‖ΔX‖)  -> A              MMA 1: D = a1·W2vᵀ
 //            (the C x 64 G rows of the group's current graph are cached in shared memory: every (node, channel) row re-reads
-//             its G row, and shared memory leaves little L1; V16_G_SMEM)
+//             its G row, and shared memory leaves little L1)
 //   stage 2  mv = SiLU(D + b2v) -> shared tile + A                            MMA 2: D = mv·Wxvᵀ
 //            (then: agg_v[node] = mean_c mv, per-graph Σ_i mv accumulated in shared memory)
 //   stage 3a φ_xv = w3xv·SiLU(D + bxv)                                        MMA 3: D = mv·WXᵀ
@@ -39,24 +39,6 @@ struct VirtT16Args {
     int g_smem;     // the launch reserved V16_GROUPS * C * 68 floats behind V16_SMEM_BYTES for the G rows of the current graph
 };
 
-#ifndef V16_HN_TMA
-#define V16_HN_TMA 0            // 1: the tile's Hn block arrives by one TMA bulk copy a tile ahead; 0: LDG behind an L1 prefetch
-#endif                          // (Hn was just written by the node kernel and is L2-resident)
-#ifndef V16_HN_PREFETCH
-#define V16_HN_PREFETCH 1       // L1 prefetch of the next tile's Hn rows at the start of a tile
-#endif
-#ifndef V16_SHFL_ACCX
-#define V16_SHFL_ACCX 1         // 1: per-graph Σ ΔX·φ_X by warp butterflies + shared atomics when C is a power of two (no barrier)
-#endif
-#ifndef V16_END_BARRIER
-#define V16_END_BARRIER 0       // 1: group barrier at the end of every tile; 0: only for tiles that straddle two graphs
-#endif
-#ifndef V16_TDOMAIN
-#define V16_TDOMAIN 1           // 1: stages 2, 3a, 3b run in the "t domain" (common.cuh silu4t): W2v and the biases carry −log2(e),
-#endif                          // the head weights and every consumer of mv (means, per-graph sums) carry −ln 2
-#ifndef V16_G_SMEM
-#define V16_G_SMEM 1            // 1: the G rows of the group's current graph (C x 64 floats) are cached in shared memory
-#endif
 constexpr int V16_THREADS = 128, V16_GROUPS = 1, V16_GROUP = 128;
 constexpr int V16_TM_COLS = 128;                  // per tile group: A_hi 32 | A_lo 32 | D 64
 constexpr int V16_ROW = 68;
@@ -74,7 +56,6 @@ constexpr int V16_SMEM_BYTES = tmma::tm_bytes(V16_GROUPS * V16_TM_COLS)
                                // + (launch time, if it fits) V16_GROUPS * C * V16_ROW * 4: G rows of the current graph
                                + 128;
 constexpr uint32_t V16_LBO = 1024;
-constexpr float kVIn = V16_TDOMAIN ? SILU_T_IN : 1.0f, kVOut = V16_TDOMAIN ? SILU_T_OUT : 1.0f;
 
 __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const VirtT16Args a) {
     using namespace tmma;
@@ -110,16 +91,16 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
     const int lane = tid & 31;
 
     // ---- one-time setup ---------------------------------------------------------------------------
-    tc16::stage_weight<V16_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, kVIn);     // t2 = kVIn·(a1·W2vᵀ + b2v); mv' = kVIn·mv
+    tc16::stage_weight<V16_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, SILU_T_IN);   // t2 = SILU_T_IN·(a1·W2vᵀ + b2v); mv' = SILU_T_IN·mv
     tc16::stage_weight<V16_THREADS>(Wxvhi, Wxvlo, a.wxv, 0, 64, tid);
     tc16::stage_weight<V16_THREADS>(Wxhi, Wxlo, a.wx, 0, 64, tid);
     if (tid < H) {
         w1rs[tid] = a.w1r[tid];
-        b2s[tid] = a.b2[tid] * kVIn;
-        bxvs[tid] = a.bxv[tid] * kVIn;              // t3 = mv'·Wᵀ + kVIn·b  (kVIn·kVOut = 1: the 64x64 head weights stay as they are)
-        w3xvs[tid] = a.w3xv[tid] * kVOut;
-        bxs[tid] = a.bx[tid] * kVIn;
-        w3xs[tid] = a.w3x[tid] * kVOut;
+        b2s[tid] = a.b2[tid] * SILU_T_IN;
+        bxvs[tid] = a.bxv[tid] * SILU_T_IN;   // t3 = mv'·Wᵀ + SILU_T_IN·b  (SILU_T_IN·SILU_T_OUT = 1: the 64x64 head weights stay)
+        w3xvs[tid] = a.w3xv[tid] * SILU_T_OUT;
+        bxs[tid] = a.bx[tid] * SILU_T_IN;
+        w3xs[tid] = a.w3x[tid] * SILU_T_OUT;
     }
     for (int i = tid; i < V16_GROUPS * (V16_MAXC * H + 4 * V16_MAXC); i += V16_THREADS) accH_all[i] = 0.f;
     if (tid == 0) {
@@ -143,9 +124,8 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
     float* phis = phi_all + grp * 2 * TILE_M;
     int* sgraph = sgraph_all + grp * TILE_M;
     float* gs = gs_all + grp * a.C * V16_ROW;          // [C][68]: pitch 68 keeps the channel rows of a node on distinct banks
-    const bool g_smem = V16_G_SMEM && a.g_smem;
-    uint64_t* hbar = bars + grp;                  // Hn block landed (V16_HN_TMA)
-    uint32_t hph = 0;
+    const bool g_smem = a.g_smem;
+    uint64_t* hbar = bars + grp;                  // Hn block landed (fetch_hn)
     const uint32_t bar_id = 1 + grp;
     int cur_graph = -1;
 
@@ -154,7 +134,7 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
             float* dst = a.vsum + (size_t)g * K;
             if (need_feat)
                 for (int i = t; i < C * H; i += V16_GROUP) {
-                    atomicAdd(dst + 4 + 3 * C + i, accH[i] * kVOut);
+                    atomicAdd(dst + 4 + 3 * C + i, accH[i] * SILU_T_OUT);
                     accH[i] = 0.f;
                 }
             if (t < 3 * C) {
@@ -175,8 +155,10 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
     const int64_t tstride = (int64_t)gridDim.x * V16_GROUPS;
     // Hn rows n0 .. n0+nvalid-1 of tile `tl` -> the start of the group's mv tile at the padded pitch V16_ROW (the channel rows
     // of 4 different nodes that a warp reads together then sit on different banks): one 256-byte bulk copy per node, issued by
-    // the first `nvalid` threads of the group; thread 0 posts the byte count
-    auto fetch_hn = [&](int64_t tl) {
+    // the first `nvalid` threads of the group; thread 0 posts the byte count.
+    // Not called: stage 1 reads Hn with LDG behind an L1 prefetch.  Deleting even this unused lambda changes the kernel's
+    // SASS, so it goes together with the Hn mbarrier init above in a change that is benchmarked on its own.
+    [[maybe_unused]] auto fetch_hn = [&](int64_t tl) {
         if (tl < num_tiles) {
             const int64_t m0 = tl * TN;
             const int nv = (int)min((int64_t)TN, a.N - m0);
@@ -184,9 +166,6 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
             if (t < nv) bulk_g2s(tile_s + t * V16_ROW, a.Hn + (size_t)(m0 + t) * H, H * 4, hbar);
         }
     };
-#if V16_HN_TMA
-    fetch_hn((int64_t)blockIdx.x * V16_GROUPS + grp);
-#endif
     for (int64_t tile = (int64_t)blockIdx.x * V16_GROUPS + grp; tile < num_tiles; tile += tstride) {
         const int64_t n0 = tile * TN;
         const int nvalid = (int)min((int64_t)TN, a.N - n0);
@@ -194,9 +173,7 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
         {   // pull the next tile's small inputs (x4, graph ids) into L1 while this one computes
             const int64_t nn0 = (tile + tstride) * TN;
             const int nnv = (int)min((int64_t)TN, a.N - nn0);
-#if !V16_HN_TMA && V16_HN_PREFETCH
             for (int i = t; i < 2 * nnv; i += V16_GROUP) prefetch_l1(a.Hn + (size_t)nn0 * H + 32 * i);
-#endif
             if (nnv > 0) {
                 if (t < (nnv * 16 + 127) / 128) prefetch_l1(a.x4 + (size_t)nn0 * 4 + 32 * t);
                 if (t == 127) prefetch_l1(a.batch + nn0);
@@ -232,32 +209,17 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
             vr = sqrtf(dx * dx + dy * dy + dz * dz);
             *reinterpret_cast<float4*>(dXs + 4 * t) = make_float4(dx, dy, dz, 0.f);
         }
-#if V16_HN_TMA
-        mbar_wait(hbar, hph);                          // this tile's Hn block (requested during the previous tile)
-        hph ^= 1;
-        __syncwarp();
-        const float* hrow = tile_s + nl * V16_ROW;
-        auto ld_h = [](const float* p) { return *reinterpret_cast<const ulonglong2*>(p); };
-#else
         const float* hrow = a.Hn + node * H;
-        auto ld_h = [](const float* p) { return __ldg(reinterpret_cast<const ulonglong2*>(p)); };
-#endif
-#if V16_G_SMEM
         // rows of the cached graph read shared memory, the others (tiles that straddle graphs) global memory: generic loads
         const float* grow = (g_smem && g == cur_graph) ? (const float*)(gs + ch * V16_ROW) : a.G + ((size_t)g * C + ch) * H;
-        auto ld_g = [](const float* p) { return *reinterpret_cast<const ulonglong2*>(p); };
-#else
-        const float* grow = a.G + ((size_t)g * C + ch) * H;
-        auto ld_g = [](const float* p) { return __ldg(reinterpret_cast<const ulonglong2*>(p)); };
-#endif
         const f32x2 vr2 = bc2(vr);
         const float inv1 = tc16::encode_row2(
             [&](int c, f32x2 (&v)[8], bool, auto safe, float& qmax) {
 #pragma unroll
                 for (int j4 = 0; j4 < 4; ++j4) {
                     const int cc = 16 * c + 4 * j4;
-                    const ulonglong2 hh = ld_h(hrow + cc);
-                    const ulonglong2 gg = ld_g(grow + cc);
+                    const ulonglong2 hh = __ldg(reinterpret_cast<const ulonglong2*>(hrow + cc));
+                    const ulonglong2 gg = *reinterpret_cast<const ulonglong2*>(grow + cc);
                     const ulonglong2 wr = *reinterpret_cast<const ulonglong2*>(w1rs + cc);
                     f32x2 p0 = fma2(vr2, wr.x, add2(hh.x, gg.x)), p1 = fma2(vr2, wr.y, add2(hh.y, gg.y));
                     silu4p<decltype(safe)::value>(p0, p1, qmax);
@@ -281,11 +243,7 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
                     const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(b2s + cc);
                     f32x2 m0 = fma2(pk2u(d[4 * j4 + 0], d[4 * j4 + 1]), is2, bb.x);
                     f32x2 m1 = fma2(pk2u(d[4 * j4 + 2], d[4 * j4 + 3]), is2, bb.y);
-#if V16_TDOMAIN
                     silu4t<decltype(safe)::value>(m0, m1, qmax);
-#else
-                    silu4p<decltype(safe)::value>(m0, m1, qmax);
-#endif
                     if (first && need_feat) *reinterpret_cast<ulonglong2*>(myrow + cc) = make_ulonglong2(m0, m1);
                     v[2 * j4] = m0;
                     v[2 * j4 + 1] = m1;
@@ -299,7 +257,7 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
             // thread <-> (column pair, quarter): one LDS.64 + one pair add per two elements, two chains per sum
             const int c2 = 2 * (t & 31), q4 = t >> 5;
             auto ld2 = [](const float* p) { return *reinterpret_cast<const f32x2*>(p); };
-            const f32x2 invC2 = bc2(kVOut / (float)C);          // the tile holds mv' = kVIn·mv
+            const f32x2 invC2 = bc2(SILU_T_OUT / (float)C);     // the tile holds mv' = SILU_T_IN·mv
             for (int n = q4; n < nvalid; n += 4) {          // mean over channels per node
                 const float* base = tile_s + (n * C) * V16_ROW + c2;
                 f32x2 s0 = 0ull, s1 = 0ull;
@@ -331,8 +289,8 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
                     for (int c = 0; c < C; ++c) {
                         float v0, v1;
                         upk2(ld2(tile_s + (n * C + c) * V16_ROW + c2), v0, v1);
-                        atomicAdd(dst + c * H, v0 * kVOut);
-                        atomicAdd(dst + c * H + 1, v1 * kVOut);
+                        atomicAdd(dst + c * H, v0 * SILU_T_OUT);
+                        atomicAdd(dst + c * H + 1, v1 * SILU_T_OUT);
                     }
                 }
             }
@@ -351,16 +309,12 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
                     const ulonglong2 ww = *reinterpret_cast<const ulonglong2*>(ws + cc);
                     f32x2 s0 = fma2(pk2u(d[4 * j4 + 0], d[4 * j4 + 1]), is2, bb.x);
                     f32x2 s1 = fma2(pk2u(d[4 * j4 + 2], d[4 * j4 + 3]), is2, bb.y);
-#if V16_TDOMAIN
                     silu4t<decltype(safe)::value>(s0, s1, qmax);
-#else
-                    silu4p<decltype(safe)::value>(s0, s1, qmax);
-#endif
                     ph01 = fma2(s0, ww.x, ph01);
                     ph23 = fma2(s1, ww.y, ph23);
                 }
             };
-#pragma unroll tc16::kChunkUnroll
+#pragma unroll 1
             for (int c = 0; c < 4; ++c) {
                 uint32_t d[16];
                 tm_ld16(lane_off + tD + 16 * c, d);
@@ -374,18 +328,12 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
         auto head = [&](const float* bs, const float* ws) {
             float qmax = 0.f;
             float phi = head_pass(bs, ws, tc16::kFast, qmax);
-            if (kSiluGuard && __any_sync(FULL, silu_q_overflow(qmax))) phi = head_pass(bs, ws, tc16::kSafe, qmax);   // cold
+            if (__any_sync(FULL, silu_q_overflow(qmax))) phi = head_pass(bs, ws, tc16::kSafe, qmax);   // cold
             return phi;
         };
         phis[t] = head(bxvs, w3xvs);
-#if V16_HN_TMA
-        fence_proxy_async_smem();                      // the pools' reads of the mv tile, ordered before the async refill below
-#endif
         named_bar(bar_id, V16_GROUP);                  // D fully read (A still holds mv); nobody reads the mv tile any more
         issue(dWxhi, dWxlo);
-#if V16_HN_TMA
-        fetch_hn(tile + tstride);
-#endif
         // trans_v[node] = mean_c(−ΔX_c·φ_xv,c)
         for (int i = t; i < nvalid * 3; i += V16_GROUP) {
             const int n = i / 3, d = i - 3 * n;
@@ -397,7 +345,7 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
 
         // ---- stage 3b: φ_X = w3x·SiLU(D + bx); Σ_i ΔX_ic·φ_X,ic per graph [3][C] -----------------------------
         const float phiX = head(bxs, w3xs);
-        if (V16_SHFL_ACCX && single && pow2C) {
+        if (single && pow2C) {
             // rows of one channel sit C lanes apart: butterfly over the lane bits above log2(C), then one shared-memory atomic per
             // (component, channel) and warp — no group barrier, no serial loop on the critical path of the tile
             const float4 d4 = *reinterpret_cast<const float4*>(dXs + 4 * t);      // own ΔX, written by this thread in stage 1
@@ -430,7 +378,7 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
         }
         // dXs / phis / the mv tile are rewritten by the next tile only after ITS first group barrier, which the threads of the
         // loop above reach after their reads; sgraph is rewritten before that barrier, and read above only on the straddling path
-        if (V16_END_BARRIER || !single) named_bar(bar_id, V16_GROUP);
+        if (!single) named_bar(bar_id, V16_GROUP);
     }
     named_bar(bar_id, V16_GROUP);      // the last tile's shared-memory atomics into accX, before other threads flush them
     flush(cur_graph);
@@ -464,7 +412,7 @@ extern "C" int distegnn_virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, 
     a.agg_v = agg_v; a.trans_v = trans_v; a.vsum = vsum;
     // the G cache is taken when it fits next to the fixed layout
     const int g_bytes = V16_GROUPS * C * V16_ROW * 4;
-    a.g_smem = (V16_G_SMEM && V16_SMEM_BYTES + g_bytes <= 232448 - 1024) ? 1 : 0;
+    a.g_smem = (V16_SMEM_BYTES + g_bytes <= 232448 - 1024) ? 1 : 0;
     const int smem_bytes = V16_SMEM_BYTES + (a.g_smem ? g_bytes : 0);
     static_assert(V16_SMEM_BYTES + V16_GROUPS * V16_MAXC * V16_ROW * 4 <= 232448, "G cache of the widest C must fit");
     ensure_dynamic_smem((const void*)virtual_layer_t16_kernel, (int)V16_SMEM_BYTES + V16_GROUPS * V16_MAXC * V16_ROW * 4);

@@ -16,8 +16,7 @@ from distegnn_b200._lib import ptr
 from distegnn_b200.backend import CudaBackend
 
 _i64, _i32, _u32, _vp = C.c_int64, C.c_int, C.c_uint, C.c_void_p
-TESTING_LIB_PATH = os.environ.get("DISTEGNN_B200_TESTING_LIB") or os.path.join(
-    os.path.dirname(_lib.LIB_PATH), "libdistegnn_b200_testing.so")
+TESTING_LIB_PATH = os.path.join(os.path.dirname(_lib.LIB_PATH), "libdistegnn_b200_testing.so")
 
 TWIN_SIGNATURES = {
     "distegnn_embed_fwd_simt": [_i64, _i32, _i32, _i32, _i32, _i32] + [_vp] * 14,
