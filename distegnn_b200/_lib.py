@@ -32,9 +32,11 @@ SIGNATURES = {
     "distegnn_csr_workspace_bytes": [_i64, _i64, C.POINTER(_i64)],
     "distegnn_build_csr": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp],
     "distegnn_gather_rows": [_vp, _vp, _i64, _i32, _vp, _vp],
+    "distegnn_scatter_rows": [_vp, _vp, _i64, _i32, _vp, _vp],
     "distegnn_embed_fwd": [_i64, _i32, _i32, _i32, _i32, _i32] + [_vp] * 15,
     "distegnn_edge_layer_fwd": [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 11,
     "distegnn_edge_layer_bwd": [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 15,
+    "distegnn_edge_layer_bwd_inputs": [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 16,
     "distegnn_radius_csr_workspace_bytes": [_i64, _i64, C.POINTER(_i64)],
     "distegnn_radius_graph_csr": [_i64, _i32, _vp, _vp, C.c_float, _i32, _i32, _i64, _i64] + [_vp] * 6 + [_i64, _vp],
     "distegnn_kmeans_lloyd": [_i64, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp],
@@ -48,6 +50,8 @@ SIGNATURES = {
     "distegnn_virtual_update_bwd": [_i32, _i32, _i32, _i32, _u32] + [_vp] * 14,
     "distegnn_node_layer_bwd": [_i64, _i32, _i32, _i32, _u32] + [_vp] * 24,
     "distegnn_embed_bwd": [_i64, _i32, _i32, _i32, _i32] + [_vp] * 11,
+    "distegnn_node_layer_bwd_inputs": [_i64, _i32, _i32, _i32, _u32] + [_vp] * 26,
+    "distegnn_embed_bwd_inputs": [_i64, _i32, _i32, _i32, _i32] + [_vp] * 17,
     "distegnn_comm_handle_bytes": [],
     "distegnn_comm_init": [_i32, _i32, _i32, _i32, C.POINTER(_vp), _vp],
     "distegnn_comm_connect": [_vp, _vp],

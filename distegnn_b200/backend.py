@@ -59,11 +59,13 @@ class CudaBackend:
             raise ValueError(f"edge_index has {int(bad.item())} edge(s) with a node id outside [0, {n_nodes})")
         return rowptr, row, col, perm
 
-    def gather_rows(self, src: Tensor, perm: Tensor) -> Tensor:
+    def gather_rows(self, src: Tensor, perm: Tensor, inverse: bool = False) -> Tensor:
+        """dst[i] = src[perm[i]]; with `inverse` dst[perm[i]] = src[i] (CSR order back to the caller's edge order)."""
         dst = torch.empty_like(src)
         if src.numel():
-            check(self.lib.distegnn_gather_rows(ptr(src), ptr(perm), src.shape[0], src.shape[1], ptr(dst),
-                                                self._s(src)), "gather_rows")
+            fn = self.lib.distegnn_scatter_rows if inverse else self.lib.distegnn_gather_rows
+            check(fn(ptr(src), ptr(perm), src.shape[0], src.shape[1], ptr(dst), self._s(src)),
+                  "scatter_rows" if inverse else "gather_rows")
             self.launches += 1
         return dst
 
@@ -88,12 +90,16 @@ class CudaBackend:
         self.launches += 1 if E else 0
 
     def edge_layer_bwd(self, dims, flags, row, col, ea, x4, P, Q, lp, g_agg_m, g_agg_x, g_P, g_Q, g_x4, g_lp,
-                       n_edges_dev=None) -> None:
-        """Backward of edge_layer: accumulates into g_P, g_Q, g_x4 and the parameter-gradient block g_lp."""
+                       n_edges_dev=None, g_ea=None) -> None:
+        """Backward of edge_layer: accumulates into g_P, g_Q, g_x4 and the parameter-gradient block g_lp; with `g_ea`
+        ([E,A], CSR order) also into the gradient w.r.t. the edge attributes."""
         N, E, A, Cn, Na = dims
-        check(self.lib.distegnn_edge_layer_bwd(N, E, A, Cn, Na, flags, ptr(row), ptr(col), ptr(ea), ptr(x4), ptr(P),
-                                               ptr(Q), ptr(lp), ptr(g_agg_m), ptr(g_agg_x), ptr(g_P), ptr(g_Q),
-                                               ptr(g_x4), ptr(g_lp), ptr(n_edges_dev), self._s(x4)), "edge_layer_bwd")
+        args = (N, E, A, Cn, Na, flags, ptr(row), ptr(col), ptr(ea), ptr(x4), ptr(P), ptr(Q), ptr(lp), ptr(g_agg_m),
+                ptr(g_agg_x), ptr(g_P), ptr(g_Q), ptr(g_x4), ptr(g_lp), ptr(n_edges_dev))
+        if g_ea is None:
+            check(self.lib.distegnn_edge_layer_bwd(*args, self._s(x4)), "edge_layer_bwd")
+        else:
+            check(self.lib.distegnn_edge_layer_bwd_inputs(*args, ptr(g_ea), self._s(x4)), "edge_layer_bwd_inputs")
         self.launches += 1 if E else 0
 
     def virtual_bwd_prepare(self, A, Cn, Na, lp) -> "torch.Tensor":
@@ -156,22 +162,35 @@ class CudaBackend:
         self.launches += 1 if N else 0
 
     def node_layer_bwd(self, dims, flags, rowptr, batch32, h, vel, attr, agg_m, agg_v, lp, lp_next, g_x_out, g_vsum,
-                       g_h_out, g_P, g_Q, g_Hn, g_h, g_x, g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lp, g_lp_next) -> None:
+                       g_h_out, g_P, g_Q, g_Hn, g_h, g_x, g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lp, g_lp_next,
+                       g_vel=None, g_attr=None) -> None:
         """Backward of node_layer (csrc/node_layer_bwd.cu): writes g_h, g_x [N,3], g_agg_x, g_trans_v [N,4], g_agg_m, g_agg_v;
-        accumulates parameter gradients into g_lp (this layer) and g_lp_next (the projections of the next layer)."""
+        accumulates parameter gradients into g_lp (this layer) and g_lp_next (the projections of the next layer), and, when
+        given, the input gradients g_vel [N,3] and g_attr [N,Na]."""
         N, B, A, Cn, Na = dims
-        check(self.lib.distegnn_node_layer_bwd(N, A, Cn, Na, flags, ptr(rowptr), ptr(h), ptr(vel), ptr(attr), ptr(agg_m),
-                                               ptr(agg_v), ptr(lp), ptr(lp_next), ptr(g_x_out), ptr(g_vsum), ptr(batch32),
-                                               ptr(g_h_out), ptr(g_P), ptr(g_Q), ptr(g_Hn), ptr(g_h), ptr(g_x),
-                                               ptr(g_agg_x), ptr(g_trans_v), ptr(g_agg_m), ptr(g_agg_v), ptr(g_lp),
-                                               ptr(g_lp_next), self._s(h)), "node_layer_bwd")
+        args = (N, A, Cn, Na, flags, ptr(rowptr), ptr(h), ptr(vel), ptr(attr), ptr(agg_m), ptr(agg_v), ptr(lp),
+                ptr(lp_next), ptr(g_x_out), ptr(g_vsum), ptr(batch32), ptr(g_h_out), ptr(g_P), ptr(g_Q), ptr(g_Hn),
+                ptr(g_h), ptr(g_x), ptr(g_agg_x), ptr(g_trans_v), ptr(g_agg_m), ptr(g_agg_v), ptr(g_lp), ptr(g_lp_next))
+        if g_vel is None and g_attr is None:
+            check(self.lib.distegnn_node_layer_bwd(*args, self._s(h)), "node_layer_bwd")
+        else:
+            check(self.lib.distegnn_node_layer_bwd_inputs(*args, ptr(g_vel), ptr(g_attr), self._s(h)),
+                  "node_layer_bwd_inputs")
         self.launches += 1 if N else 0
 
-    def embed_bwd(self, dims, node_feat, h0, lp0, g_h, g_P, g_Q, g_Hn, g_emb_wt, g_emb_b, g_lp0) -> None:
-        """Backward of embed: accumulates g_emb_wt [F,64], g_emb_b [64] and layer 0's projection gradients into g_lp0."""
+    def embed_bwd(self, dims, node_feat, h0, lp0, g_h, g_P, g_Q, g_Hn, g_emb_wt, g_emb_b, g_lp0, g_feat=None, g_loc=None,
+                  emb_wt=None, batch32=None, g_x0=None, g_vsum0=None) -> None:
+        """Backward of embed: accumulates g_emb_wt [F,64], g_emb_b [64] and layer 0's projection gradients into g_lp0.  With
+        `g_feat` writes the gradient w.r.t. node_feat (needs `emb_wt`); with `g_loc` the gradient w.r.t. node_loc,
+        g_x0 + g_vsum0[batch, 0:3] (g_x0: w.r.t. layer 0's coordinates; g_vsum0: w.r.t. the initial statistics)."""
         N, B, F, A, Cn, Na = dims
-        check(self.lib.distegnn_embed_bwd(N, F, A, Cn, Na, ptr(node_feat), ptr(h0), ptr(lp0), ptr(g_h), ptr(g_P), ptr(g_Q),
-                                          ptr(g_Hn), ptr(g_emb_wt), ptr(g_emb_b), ptr(g_lp0), self._s(h0)), "embed_bwd")
+        args = (N, F, A, Cn, Na, ptr(node_feat), ptr(h0), ptr(lp0), ptr(g_h), ptr(g_P), ptr(g_Q), ptr(g_Hn), ptr(g_emb_wt),
+                ptr(g_emb_b), ptr(g_lp0))
+        if g_feat is None and g_loc is None:
+            check(self.lib.distegnn_embed_bwd(*args, self._s(h0)), "embed_bwd")
+        else:
+            check(self.lib.distegnn_embed_bwd_inputs(*args, ptr(emb_wt), ptr(batch32), ptr(g_x0), ptr(g_vsum0),
+                                                     ptr(g_feat), ptr(g_loc), self._s(h0)), "embed_bwd_inputs")
         self.launches += 1 if N else 0
 
     def virtual_update(self, dims, flags, vsum, Xv, Hv, lp, lp_next, G, init_loc_mean=None, init_hv0=None,

@@ -54,6 +54,16 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, const int32_t*
     }
 }
 
+__global__ void scatter_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ perm,
+                                    int64_t n, int width, float* __restrict__ dst) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n * width) {
+        int64_t r = i / width;
+        int c = (int)(i - r * width);
+        dst[(int64_t)perm[r] * width + c] = src[i];
+    }
+}
+
 static int key_bits(int64_t n_nodes) {
     int b = 1;
     while (b < 31 && ((int64_t)1 << b) < n_nodes) ++b;
@@ -148,6 +158,19 @@ int distegnn_gather_rows(const float* src, const int32_t* perm, int64_t n_rows, 
     int64_t n = n_rows * width;
     gather_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(src, perm, n_rows,
                                                                                       width, dst);
+    DEGNN_CHECK_LAUNCH();
+    return DISTEGNN_OK;
+}
+
+int distegnn_scatter_rows(const float* src, const int32_t* perm, int64_t n_rows, int width, float* dst,
+                          void* stream_) {
+    using namespace degnn;
+    if (n_rows == 0 || width == 0) return DISTEGNN_OK;
+    DEGNN_CHECK_ARG(src && perm && dst, "null pointer");
+    DEGNN_CHECK_ARG(width > 0 && n_rows > 0, "bad shape");
+    int64_t n = n_rows * width;
+    scatter_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(src, perm, n_rows,
+                                                                                       width, dst);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

@@ -43,6 +43,17 @@ struct NodeBwdArgs {
     float* d_xa; float* d_xb1; float* d_xb; float* d_xh;        // next layer's block: E_W1A, E_B1, E_W1B, V_W1H
 };
 
+// Gradients with respect to the model's inputs (the kInputs instantiations; the <false> ones are the weights-only kernels)
+struct InputGradArgs {
+    // node stage, ACCUMULATED over the layers: g_vel += φ_v·g_x',  g_attr += g_z·N_W1[3H:3H+Na]ᵀ (not with FLAG_LAST)
+    float* g_vel; float* g_attr;
+    const float* lb3;        // L_B3 (φ_v's bias)
+    // embedding prologue, WRITTEN: g_feat = g_h0·emb_wtᵀ,  g_loc = g_x0 + g_vsum0[batch, 0:3] (Σx of the initial x̄)
+    float* g_feat; float* g_loc;
+    const float* emb_wt; const int32_t* batch; const float* g_x0; const float* g_vsum0;
+    int K;
+};
+
 constexpr int NB_TILE = TILE_M * LDA;                            // floats per tile
 constexpr int NB_SMEM_BYTES = 5 * NB_TILE * 4 + 2 * TILE_M * 4 + 64;
 
@@ -103,7 +114,8 @@ __device__ __forceinline__ void proj_backward(float (&acc)[8][4], const NodeBwdA
     }
 }
 
-__global__ void __launch_bounds__(NTHREADS, 1) node_layer_bwd_kernel(const NodeBwdArgs a) {
+template <bool kInputs>
+__global__ void __launch_bounds__(NTHREADS, 1) node_layer_bwd_kernel(const NodeBwdArgs a, const InputGradArgs in) {
     extern __shared__ __align__(16) float nb_smem[];
     float* TA = nb_smem;                 // operand tile (h, agg_m/deg, agg_v, upstream gradients)
     float* TZ = TA + NB_TILE;            // z, later u
@@ -227,6 +239,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) node_layer_bwd_kernel(const NodeB
                     atomicAdd(a.d_n1 + (size_t)(3 * H + k) * H + tid, s);
                 }
             }
+            if constexpr (kInputs) {                              // g_attr[r][k] += Σ_n g_z[r][n]·N_W1[3H+k][n]
+                const int r = tid & (TILE_M - 1);
+                if (in.g_attr && r < nvalid) {
+                    for (int k = tid / TILE_M; k < Na; k += NTHREADS / TILE_M) {
+                        const float* w = a.n1 + (size_t)(3 * H + k) * H;
+                        float s = 0.f;
+#pragma unroll 16
+                        for (int n = 0; n < H; ++n) s = fmaf(TG[r * LDA + n], __ldg(w + n), s);
+                        in.g_attr[(size_t)(n0 + r) * Na + k] += s;
+                    }
+                }
+            }
             // ---- node MLP layer 1: [g_h | g_agg_m·deg | g_agg_v] = g_z·N_W1ᵀ, weight gradients per 64-row block --------
             gemm_tile_gt(accH, TG, a.n1, ty, tx);                 // block 0 lands in g_h
             __syncthreads();
@@ -272,6 +296,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) node_layer_bwd_kernel(const NodeB
                 *reinterpret_cast<float4*>(TT + r * LDA + 4 * tx) = make_float4(s.x * gp, s.y * gp, s.z * gp, s.w * gp);   // for g_L_W3
                 *reinterpret_cast<float4*>(TG + r * LDA + 4 * tx) =
                     make_float4(gp * w3.x * dsilu(u.x), gp * w3.y * dsilu(u.y), gp * w3.z * dsilu(u.z), gp * w3.w * dsilu(u.w));
+            }
+            if constexpr (kInputs) {                              // g_vel += φ_v·g_x'; φ_v summed over the 16 tx lanes
+                if (in.g_vel) {
+                    const float b3 = __ldg(in.lb3);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int r = ty + 16 * i;
+                        const float4 s = silu4(make_float4(acc[i][0] + b.x, acc[i][1] + b.y, acc[i][2] + b.z, acc[i][3] + b.w));
+                        float p = s.x * w3.x + s.y * w3.y + s.z * w3.z + s.w * w3.w;
+                        p += __shfl_xor_sync(FULL, p, 8);
+                        p += __shfl_xor_sync(FULL, p, 4);
+                        p += __shfl_xor_sync(FULL, p, 2);
+                        p += __shfl_xor_sync(FULL, p, 1);
+                        if (tx == 0 && r < nvalid) {
+                            const size_t node = (size_t)(n0 + r);
+                            float gx[3] = {__ldg(a.g_xn + node * 3), __ldg(a.g_xn + node * 3 + 1), __ldg(a.g_xn + node * 3 + 2)};
+                            if (a.g_vsum) {
+                                const float* gv = a.g_vsum + (size_t)__ldg(a.batch + node) * a.K;
+                                gx[0] += __ldg(gv); gx[1] += __ldg(gv + 1); gx[2] += __ldg(gv + 2);
+                            }
+                            const float phi = p + b3;
+                            for (int d = 0; d < 3; ++d) in.g_vel[node * 3 + d] += phi * gx[d];
+                        }
+                    }
+                }
             }
             __syncthreads();
             if (tid < H) {
@@ -328,7 +377,8 @@ struct EmbedBwdArgs {
     float* d_b;              // [64]
 };
 
-__global__ void __launch_bounds__(NTHREADS, 1) embed_bwd_kernel(const EmbedBwdArgs e) {
+template <bool kInputs>
+__global__ void __launch_bounds__(NTHREADS, 1) embed_bwd_kernel(const EmbedBwdArgs e, const InputGradArgs in) {
     extern __shared__ __align__(16) float nb_smem[];
     const NodeBwdArgs& a = e.nb;
     float* TA = nb_smem;
@@ -359,6 +409,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) embed_bwd_kernel(const EmbedBwdAr
         __syncthreads();
         store_acc(TG, accG, ty, tx);
         __syncthreads();
+        if constexpr (kInputs) {
+            const int r = tid & (TILE_M - 1);
+            if (in.g_feat && r < nvalid) {                        // g_feat[r][k] = Σ_n g_h0[r][n]·emb_wt[k][n]
+                for (int k = tid / TILE_M; k < e.F; k += NTHREADS / TILE_M) {
+                    const float* w = in.emb_wt + (size_t)k * H;
+                    float s = 0.f;
+#pragma unroll 16
+                    for (int n = 0; n < H; ++n) s = fmaf(TG[r * LDA + n], __ldg(w + n), s);
+                    in.g_feat[(size_t)(n0 + r) * e.F + k] = s;
+                }
+            }
+            if (in.g_loc && tid < nvalid) {                       // layer 0's x is node_loc; Σx feeds the initial x̄
+                const size_t node = (size_t)(n0 + tid);
+                const float* gv = in.g_vsum0 ? in.g_vsum0 + (size_t)__ldg(in.batch + node) * in.K : nullptr;
+                for (int d = 0; d < 3; ++d) in.g_loc[node * 3 + d] = __ldg(in.g_x0 + node * 3 + d) + (gv ? __ldg(gv + d) : 0.f);
+            }
+        }
         if (tid < H) {
             bE += colsum(TG, tid);
             for (int r = 0; r < nvalid; ++r) {
@@ -381,16 +448,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) embed_bwd_kernel(const EmbedBwdAr
     }
 }
 
-}  // namespace degnn
-
-extern "C" int distegnn_node_layer_bwd(int64_t n_nodes, int A, int C, int Na, unsigned flags, const int32_t* rowptr,
-                                       const float* h, const float* node_vel, const float* node_attr, const float* agg_m,
-                                       const float* agg_v, const float* layer_params, const float* next_layer_params,
-                                       const float* g_x_out, const float* g_vsum, const int32_t* batch32, const float* g_h_out,
-                                       const float* g_P, const float* g_Q, const float* g_Hn, float* g_h, float* g_x, float* g_agg_x, float* g_trans_v,
-                                       float* g_agg_m, float* g_agg_v, float* g_layer_params, float* g_next_layer_params,
-                                       void* stream) {
-    using namespace degnn;
+static int node_layer_bwd_launch(int64_t n_nodes, int A, int C, int Na, unsigned flags, const int32_t* rowptr,
+                                 const float* h, const float* node_vel, const float* node_attr, const float* agg_m,
+                                 const float* agg_v, const float* layer_params, const float* next_layer_params,
+                                 const float* g_x_out, const float* g_vsum, const int32_t* batch32, const float* g_h_out,
+                                 const float* g_P, const float* g_Q, const float* g_Hn, float* g_h, float* g_x, float* g_agg_x,
+                                 float* g_trans_v, float* g_agg_m, float* g_agg_v, float* g_layer_params,
+                                 float* g_next_layer_params, float* g_node_vel, float* g_node_attr, void* stream) {
     if (int rc = check_dims(A, C, Na)) return rc;
     if (n_nodes == 0) return DISTEGNN_OK;
     const bool last = flags & DISTEGNN_FLAG_LAST;
@@ -427,24 +491,38 @@ extern "C" int distegnn_node_layer_bwd(int64_t n_nodes, int A, int C, int Na, un
     a.d_xb1 = dn ? dn + L.off[DISTEGNN_P_E_B1] : nullptr;
     a.d_xb = dn ? dn + L.off[DISTEGNN_P_E_W1B] : nullptr;
     a.d_xh = dn ? dn + L.off[DISTEGNN_P_V_W1H] : nullptr;
-    ensure_dynamic_smem((const void*)node_layer_bwd_kernel, (int)NB_SMEM_BYTES);
+    InputGradArgs in;
+    memset(&in, 0, sizeof(in));
+    in.g_vel = g_node_vel;
+    in.g_attr = (Na > 0 && !last) ? g_node_attr : nullptr;       // the last layer has no node MLP: no attr term
+    in.lb3 = lp + L.off[DISTEGNN_P_L_B3];
+    const bool inputs = in.g_vel || in.g_attr;
+    const void* kernel = inputs ? (const void*)node_layer_bwd_kernel<true> : (const void*)node_layer_bwd_kernel<false>;
+    ensure_dynamic_smem(kernel, (int)NB_SMEM_BYTES);
     const int64_t tiles = (n_nodes + TILE_M - 1) / TILE_M;
     int64_t grid = sm_count();
     if (grid > tiles) grid = tiles;
-    node_layer_bwd_kernel<<<(unsigned)grid, NTHREADS, NB_SMEM_BYTES, (cudaStream_t)stream>>>(a);
+    if (inputs)
+        node_layer_bwd_kernel<true><<<(unsigned)grid, NTHREADS, NB_SMEM_BYTES, (cudaStream_t)stream>>>(a, in);
+    else
+        node_layer_bwd_kernel<false><<<(unsigned)grid, NTHREADS, NB_SMEM_BYTES, (cudaStream_t)stream>>>(a, in);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }
 
-extern "C" int distegnn_embed_bwd(int64_t n_nodes, int F, int A, int C, int Na, const float* node_feat, const float* h0,
-                                  const float* layer0_params, const float* g_h, const float* g_P, const float* g_Q,
-                                  const float* g_Hn, float* g_emb_wt, float* g_emb_b, float* g_layer0_params, void* stream) {
-    using namespace degnn;
+static int embed_bwd_launch(int64_t n_nodes, int F, int A, int C, int Na, const float* node_feat, const float* h0,
+                            const float* layer0_params, const float* g_h, const float* g_P, const float* g_Q,
+                            const float* g_Hn, float* g_emb_wt, float* g_emb_b, float* g_layer0_params, const float* emb_wt,
+                            const int32_t* batch32, const float* g_x0, const float* g_vsum0, float* g_node_feat,
+                            float* g_node_loc, void* stream) {
     if (int rc = check_dims(A, C, Na)) return rc;
     if (n_nodes == 0) return DISTEGNN_OK;
     DEGNN_CHECK_ARG(n_nodes > 0 && F >= 1 && F <= DISTEGNN_MAX_NODE_FEAT, "bad size");
     DEGNN_CHECK_ARG(node_feat && h0 && layer0_params && g_P && g_Q && g_Hn && g_emb_wt && g_emb_b && g_layer0_params,
                     "null pointer");
+    DEGNN_CHECK_ARG(!g_node_feat || emb_wt, "g_node_feat needs emb_wt");
+    DEGNN_CHECK_ARG(!g_node_loc || g_x0, "g_node_loc needs g_x0");
+    DEGNN_CHECK_ARG(!g_node_loc || !g_vsum0 || batch32, "g_vsum0 needs batch32");
     Layout L = make_layout(A, C, Na);
     EmbedBwdArgs e;
     memset(&e, 0, sizeof(e));
@@ -457,12 +535,69 @@ extern "C" int distegnn_embed_bwd(int64_t n_nodes, int F, int A, int C, int Na, 
     e.nb.d_xb = g_layer0_params + L.off[DISTEGNN_P_E_W1B];
     e.nb.d_xh = g_layer0_params + L.off[DISTEGNN_P_V_W1H];
     e.F = F; e.feat = node_feat; e.d_wt = g_emb_wt; e.d_b = g_emb_b;
+    InputGradArgs in;
+    memset(&in, 0, sizeof(in));
+    in.g_feat = g_node_feat; in.g_loc = g_node_loc; in.emb_wt = emb_wt; in.batch = batch32; in.g_x0 = g_x0;
+    in.g_vsum0 = g_vsum0; in.K = 4 + 3 * C + H * C;
+    const bool inputs = g_node_feat || g_node_loc;
     const int smem = 3 * NB_TILE * 4;
-    ensure_dynamic_smem((const void*)embed_bwd_kernel, smem);
+    const void* kernel = inputs ? (const void*)embed_bwd_kernel<true> : (const void*)embed_bwd_kernel<false>;
+    ensure_dynamic_smem(kernel, smem);
     const int64_t tiles = (n_nodes + TILE_M - 1) / TILE_M;
     int64_t grid = sm_count();
     if (grid > tiles) grid = tiles;
-    embed_bwd_kernel<<<(unsigned)grid, NTHREADS, smem, (cudaStream_t)stream>>>(e);
+    if (inputs)
+        embed_bwd_kernel<true><<<(unsigned)grid, NTHREADS, smem, (cudaStream_t)stream>>>(e, in);
+    else
+        embed_bwd_kernel<false><<<(unsigned)grid, NTHREADS, smem, (cudaStream_t)stream>>>(e, in);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
+}
+
+}  // namespace degnn
+
+extern "C" int distegnn_node_layer_bwd(int64_t n_nodes, int A, int C, int Na, unsigned flags, const int32_t* rowptr,
+                                       const float* h, const float* node_vel, const float* node_attr, const float* agg_m,
+                                       const float* agg_v, const float* layer_params, const float* next_layer_params,
+                                       const float* g_x_out, const float* g_vsum, const int32_t* batch32, const float* g_h_out,
+                                       const float* g_P, const float* g_Q, const float* g_Hn, float* g_h, float* g_x, float* g_agg_x, float* g_trans_v,
+                                       float* g_agg_m, float* g_agg_v, float* g_layer_params, float* g_next_layer_params,
+                                       void* stream) {
+    return degnn::node_layer_bwd_launch(n_nodes, A, C, Na, flags, rowptr, h, node_vel, node_attr, agg_m, agg_v,
+                                        layer_params, next_layer_params, g_x_out, g_vsum, batch32, g_h_out, g_P, g_Q, g_Hn,
+                                        g_h, g_x, g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_layer_params,
+                                        g_next_layer_params, nullptr, nullptr, stream);
+}
+
+extern "C" int distegnn_node_layer_bwd_inputs(int64_t n_nodes, int A, int C, int Na, unsigned flags, const int32_t* rowptr,
+                                              const float* h, const float* node_vel, const float* node_attr,
+                                              const float* agg_m, const float* agg_v, const float* layer_params,
+                                              const float* next_layer_params, const float* g_x_out, const float* g_vsum,
+                                              const int32_t* batch32, const float* g_h_out, const float* g_P,
+                                              const float* g_Q, const float* g_Hn, float* g_h, float* g_x, float* g_agg_x,
+                                              float* g_trans_v, float* g_agg_m, float* g_agg_v, float* g_layer_params,
+                                              float* g_next_layer_params, float* g_node_vel, float* g_node_attr,
+                                              void* stream) {
+    return degnn::node_layer_bwd_launch(n_nodes, A, C, Na, flags, rowptr, h, node_vel, node_attr, agg_m, agg_v,
+                                        layer_params, next_layer_params, g_x_out, g_vsum, batch32, g_h_out, g_P, g_Q, g_Hn,
+                                        g_h, g_x, g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_layer_params,
+                                        g_next_layer_params, g_node_vel, g_node_attr, stream);
+}
+
+extern "C" int distegnn_embed_bwd(int64_t n_nodes, int F, int A, int C, int Na, const float* node_feat, const float* h0,
+                                  const float* layer0_params, const float* g_h, const float* g_P, const float* g_Q,
+                                  const float* g_Hn, float* g_emb_wt, float* g_emb_b, float* g_layer0_params, void* stream) {
+    return degnn::embed_bwd_launch(n_nodes, F, A, C, Na, node_feat, h0, layer0_params, g_h, g_P, g_Q, g_Hn, g_emb_wt,
+                                   g_emb_b, g_layer0_params, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int distegnn_embed_bwd_inputs(int64_t n_nodes, int F, int A, int C, int Na, const float* node_feat,
+                                         const float* h0, const float* layer0_params, const float* g_h, const float* g_P,
+                                         const float* g_Q, const float* g_Hn, float* g_emb_wt, float* g_emb_b,
+                                         float* g_layer0_params, const float* emb_wt, const int32_t* batch32,
+                                         const float* g_x0, const float* g_vsum0, float* g_node_feat, float* g_node_loc,
+                                         void* stream) {
+    return degnn::embed_bwd_launch(n_nodes, F, A, C, Na, node_feat, h0, layer0_params, g_h, g_P, g_Q, g_Hn, g_emb_wt,
+                                   g_emb_b, g_layer0_params, emb_wt, batch32, g_x0, g_vsum0, g_node_feat, g_node_loc,
+                                   stream);
 }

@@ -18,6 +18,11 @@ included — replays as one CUDA graph (`model.cuda_graph = True`), for any worl
 In grad mode the same kernels run with per-layer activations kept and the outputs are attached to autograd
 (``_FastEGNNFunction``): backward = hand-written kernels for the per-edge and real<->virtual stages, torch
 recompute for the dense per-node stages, one packed all-reduce of the statistics' gradient per layer (DESIGN §9).
+By default the inputs are constants of that graph, as in the reference's training loop; with `model.input_grads = True`
+every floating input that requires grad (node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr) receives the
+gradient the reference module's autograd would give it — multi-step rollout training, edge_attr computed in torch from the
+positions, sensitivity analysis.  edge_index / data_batch / CSRGraph are not differentiable, and neither is the edge_attr
+that `radius_graph_csr` builds on the device: compute edge_attr in torch when gradients must flow through edge lengths.
 """
 from __future__ import annotations
 
@@ -213,6 +218,7 @@ class FastEGNN(nn.Module):
         self._graph_max_captures = 8
         self.process_group = None          # torch.distributed group for the virtual-node sync (None = WORLD)
         self.validate_inputs = True        # check edge ids / data_batch once per distinct tensor (one host sync each)
+        self.input_grads = False           # opt-in: back-propagate into the floating inputs too (see _FastEGNNFunction)
         self._validated_batch = None       # (tensor, version, N, B) of the last data_batch that passed
         self._workspaces: Dict[tuple, Dict[str, Tensor]] = {}
         self._keep_state = None            # tests: a list that receives the training-path forward's saved state
@@ -306,7 +312,10 @@ class FastEGNN(nn.Module):
     # ---- forward -------------------------------------------------------------------------------
     def forward(self, node_feat, node_loc, node_vel, loc_mean, edge_index, data_batch, edge_attr=None,
                 node_attr=None) -> Tuple[Tensor, Tensor]:
-        training_path = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+        inputs = (node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr)
+        want_inputs = self.input_grads and torch.is_grad_enabled() and \
+            any(t is not None and t.requires_grad for t in inputs)
+        training_path = want_inputs or (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()))
         dev = node_loc.device
         be = self._get_backend(dev)
         A, Cn, Na, F = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf, self.node_feat_nf
@@ -340,11 +349,12 @@ class FastEGNN(nn.Module):
             if training_path:
                 for name, t in (("node_feat", node_feat), ("node_loc", node_loc), ("node_vel", node_vel),
                                 ("edge_attr", edge_attr), ("node_attr", node_attr)):
-                    if t is not None and t.requires_grad:
+                    if t is not None and t.requires_grad and not self.input_grads:
                         import warnings
                         warnings.warn(f"distegnn_b200.FastEGNN: `{name}` requires grad, but the fused path treats inputs "
                                       "as constants (the reference trains weights only, utils/train.py:149-158): no "
-                                      "gradient will flow to it", RuntimeWarning, stacklevel=2)
+                                      "gradient will flow to it; set `model.input_grads = True` to back-propagate into "
+                                      "the inputs", RuntimeWarning, stacklevel=2)
                 return self._forward_autograd(be, dev, (N, E, B, K), f32, node_feat, node_loc, node_vel, loc_mean,
                                               edge_index, data_batch, edge_attr, node_attr)
             with torch.no_grad():
@@ -406,7 +416,8 @@ class FastEGNN(nn.Module):
                           edge_attr, node_attr) -> Tuple[Tensor, Tensor]:
         """Forward with a backward: same kernels as the inference path, per-layer activations kept (N-sized only:
         nothing of size [E,.] or [N,C,.] is ever stored), gradients through `_FastEGNNFunction`.  Inputs are treated
-        as constants (the reference trains weights only: utils/train.py:149-158)."""
+        as constants (the reference trains weights only: utils/train.py:149-158) unless `self.input_grads` is set: then the
+        six raw input tensors are inputs of the autograd node as well."""
         A, Cn, Na = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf
         N, E, B, K = dims
         offs, total = _lib.param_layout(A, Cn, Na)
@@ -420,7 +431,13 @@ class FastEGNN(nn.Module):
             args = dict(node_feat=f32(node_feat), node_loc=f32(node_loc), node_vel=f32(node_vel),
                         loc_mean=f32(loc_mean), attr=f32(node_attr) if Na > 0 else None,
                         data_batch=data_batch.contiguous(), rowptr=rowptr, row=row, col=col, ea=ea, nE=nE)
-        return _FastEGNNFunction.apply(self, be, dims, args, emb_wt, emb_b, hv0, *lps)
+            from .shards import CSRGraph
+            if self.input_grads and A > 0 and not isinstance(edge_index, CSRGraph):   # CSR position -> caller's edge
+                args["perm"] = self._graphs.get(be, edge_index, N, self.validate_inputs)[3]
+        if not self.input_grads:
+            return _FastEGNNFunction.apply(self, be, dims, args, emb_wt, emb_b, hv0, *lps)
+        return _FastEGNNFunction.apply(self, be, dims, args, emb_wt, emb_b, hv0, *lps,
+                                       node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr)
 
     def _run_saving(self, be, dims, a: Dict[str, Tensor], emb_wt, emb_b, hv0, layers: List[Tensor]):
         """`_run` with fresh buffers per layer; returns (out, Xv_L, saved state for the backward)."""
@@ -596,15 +613,23 @@ class _FastEGNNFunction(torch.autograd.Function):
     reverse: virtual-node update, ONE packed all-reduce of the statistics' gradient (the reference's _AllReduce.backward,
     FastEGNN.py:19-21, issues one per aggregate), per-node stage, real<->virtual stage, per-edge stage, and finally the
     initial virtual state and the embedding prologue — every one a hand-written kernel behind the C ABI (csrc/*bwd*.cu,
-    csrc/virtual_update.cu); torch only adds three gradient tensors per layer."""
+    csrc/virtual_update.cu); torch only adds three gradient tensors per layer.
+
+    With `model.input_grads` the six raw inputs (node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr) follow
+    the parameter blocks, and the same kernels also produce the gradients of those that need one (ctx.needs_input_grad):
+    edge_attr and node_vel / node_attr accumulate over the layers in the edge and node kernels, node_feat and node_loc
+    come out of the embedding backward (node_loc = layer 0's coordinate gradient + the Σx term of the initial centroid,
+    summed over the partitions by one more packed exchange), loc_mean is the channel sum of the initial Xv's gradient."""
 
     @staticmethod
-    def forward(ctx, model, be, dims, a, emb_wt, emb_b, hv0, *lps):
-        layers = [lp.detach().contiguous() for lp in lps]
+    def forward(ctx, model, be, dims, a, emb_wt, emb_b, hv0, *rest):
+        L = model.n_layers
+        layers = [lp.detach().contiguous() for lp in rest[:L]]
         out, Xv, st = model._run_saving(be, dims, a, emb_wt.detach().contiguous(), emb_b.detach().contiguous(),
                                         hv0.detach().contiguous(), layers)
         ctx.model, ctx.be, ctx.dims, ctx.a, ctx.st = model, be, dims, a, st
         ctx.params = (emb_wt.detach(), emb_b.detach(), hv0.detach(), layers)
+        ctx.inputs = [None if t is None else (t.dtype, t.shape) for t in rest[L:]]
         return out, Xv
 
     @staticmethod
@@ -619,11 +644,21 @@ class _FastEGNNFunction(torch.autograd.Function):
         zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         g_lps = [zeros(total) for _ in range(L)]
         g_emb_wt, g_emb_b, g_hv0 = torch.zeros_like(emb_wt), torch.zeros_like(emb_b), torch.zeros_like(hv0)
-        if L == 0:
-            return (None, None, None, None, g_emb_wt, g_emb_b, g_hv0)
-        attr = a["attr"]
+        n_in = len(ctx.inputs)
+        want = ctx.needs_input_grad[7 + L:7 + L + n_in] if n_in else (False,) * 6
+        w_feat, w_loc, w_vel, w_lm, w_ea, w_attr = want
         g_x = g_out.contiguous().to(torch.float32) if g_out is not None else zeros(N, 3)
         g_Xv = g_Xv_out.contiguous().to(torch.float32) if g_Xv_out is not None else zeros(B, 3, Cn)
+        if L == 0:                                           # out = node_loc, Xv = loc_mean broadcast
+            g_in = (None, g_x if w_loc else None, None, g_Xv.sum(-1) if w_lm else None, None, None)
+            return (None, None, None, None, g_emb_wt, g_emb_b, g_hv0) + _FastEGNNFunction._input_grads(ctx, g_in)
+        attr = a["attr"]
+        # input-gradient accumulators, only for the inputs that need one (the kernels then take the *_inputs entry points)
+        g_vel = zeros(N, 3) if w_vel else None
+        g_attr = zeros(N, Na) if (w_attr and Na > 0) else None
+        g_ea = zeros(E, A) if (w_ea and A > 0 and E > 0) else None          # CSR order
+        kw_node = dict(g_vel=g_vel, g_attr=g_attr) if (g_vel is not None or g_attr is not None) else {}
+        kw_edge = dict(g_ea=g_ea) if g_ea is not None else {}
         g_Hv = g_G = g_h = g_P = g_Q = g_Hn = None
         for i in reversed(range(L)):
             S = st["layers"][i]
@@ -643,7 +678,7 @@ class _FastEGNNFunction(torch.autograd.Function):
             g_agg_v = None if last else torch.empty(N, H, device=dev)
             be.node_layer_bwd((N, B, A, Cn, Na), S["flags"], a["rowptr"], st["batch32"], S["h"], a["node_vel"], attr,
                               S["agg_m"], S["agg_v"], lp, lp_next, g_x, g_vsum, g_h, g_P, g_Q, g_Hn, g_h_i, g_x_i,
-                              g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lps[i], None if last else g_lps[i + 1])
+                              g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lps[i], None if last else g_lps[i + 1], **kw_node)
             # ---- 3. real<->virtual stage (CUDA) ------------------------------------------------------------------------
             wT = be.virtual_bwd_prepare(A, Cn, Na, lp)           # operand images of the stage's weights for the tensor cores
             g_Hn_i, g_xv = torch.empty(N, H, device=dev), torch.empty(N, 4, device=dev)
@@ -653,7 +688,7 @@ class _FastEGNNFunction(torch.autograd.Function):
             # ---- 4. per-edge stage (CUDA) --------------------------------------------------------------------------------
             g_P_i, g_Q_i, g_x4e = zeros(N, H), zeros(N, H), zeros(N, 4)
             be.edge_layer_bwd((N, E, A, Cn, Na), S["flags"], a["row"], a["col"], a["ea"], S["x4"], S["P"], S["Q"], lp,
-                              g_agg_m, g_agg_x, g_P_i, g_Q_i, g_x4e, g_lps[i], a["nE"])
+                              g_agg_m, g_agg_x, g_P_i, g_Q_i, g_x4e, g_lps[i], a["nE"], **kw_edge)
             g_x = g_x_i + g_xv[:, :3] + g_x4e[:, :3]
             g_h, g_P, g_Q, g_Hn = g_h_i, g_P_i, g_Q_i, g_Hn_i
             g_Xv, g_Hv, g_G = g_Xv_acc, g_Hv_i, g_G_i
@@ -661,10 +696,41 @@ class _FastEGNNFunction(torch.autograd.Function):
         Xv0 = a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn).contiguous()
         Hv0 = hv0.unsqueeze(0).expand(B, Cn, H).contiguous()
         g_Hv0 = torch.empty(B, Cn, H, device=dev)
-        be.virtual_update_bwd((B, A, Cn, Na), _lib.FLAG_INIT, st["vsum_init"], Xv0, Hv0, None, layers[0], None, g_Hv, g_G,
-                              torch.empty(B, K, device=dev), torch.empty(B, 3, Cn, device=dev), g_Hv0, None, g_lps[0])
+        g_vsum0, g_Xv0 = torch.empty(B, K, device=dev), torch.empty(B, 3, Cn, device=dev)
+        # with loc_mean wanted, layer 0's g_Xv goes in as the upstream of X_0, so g_Xv0 is the whole gradient w.r.t. X_0
+        be.virtual_update_bwd((B, A, Cn, Na), _lib.FLAG_INIT, st["vsum_init"], Xv0, Hv0, None, layers[0],
+                              g_Xv if w_lm else None, g_Hv, g_G, g_vsum0, g_Xv0, g_Hv0, None, g_lps[0])
         g_hv0 += g_Hv0.sum(0)                                # virtual_node_feat is shared by the graphs of the batch
+        if w_loc and model.world_size > 1:                   # x̄_0 is all-reduced: its Σx gradient is summed back
+            model._sync_virtual(g_vsum0, be, st.get("comm"))
         # ---- embedding + layer-0 projections (CUDA) ----------------------------------------------------------------------------
+        g_feat = torch.empty(N, model.node_feat_nf, device=dev) if w_feat else None
+        g_loc = torch.empty(N, 3, device=dev) if w_loc else None
+        kw_emb = {} if (g_feat is None and g_loc is None) else dict(
+            g_feat=g_feat, g_loc=g_loc, emb_wt=emb_wt, batch32=st["batch32"], g_x0=g_x.contiguous() if w_loc else None,
+            g_vsum0=g_vsum0 if w_loc else None)
         be.embed_bwd((N, B, model.node_feat_nf, A, Cn, Na), a["node_feat"], st["layers"][0]["h"], layers[0], g_h, g_P, g_Q,
-                     g_Hn, g_emb_wt, g_emb_b, g_lps[0])
-        return (None, None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps)
+                     g_Hn, g_emb_wt, g_emb_b, g_lps[0], **kw_emb)
+        grads = (None, None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps)
+        if not n_in:
+            return grads
+        if g_ea is not None and "perm" in a:                 # CSR order -> the caller's edge order
+            g_ea = be.gather_rows(g_ea, a["perm"], inverse=True)
+        g_in = (g_feat, g_loc, g_vel, g_Xv0.sum(-1) if w_lm else None, g_ea if w_ea else None, g_attr if w_attr else None)
+        return grads + _FastEGNNFunction._input_grads(ctx, g_in)
+
+    @staticmethod
+    def _input_grads(ctx, g_in):
+        """Gradients of the six raw inputs in their own dtype; zeros for a wanted input that has no path to the outputs
+        (edge_attr with edge_attr_nf = 0, node_attr with node_attr_nf = 0 or a single layer)."""
+        if not ctx.inputs:
+            return ()
+        out = []
+        for want, meta, g in zip(ctx.needs_input_grad[7 + len(ctx.params[3]):], ctx.inputs, g_in):
+            if not want:
+                out.append(None)
+                continue
+            dtype, shape = meta
+            dev = ctx.params[0].device
+            out.append(torch.zeros(shape, dtype=dtype, device=dev) if g is None else g.to(dtype).reshape(shape))
+        return tuple(out)

@@ -146,6 +146,11 @@ DISTEGNN_API int distegnn_build_csr(const int64_t *edge_index, int64_t n_nodes, 
 DISTEGNN_API int distegnn_gather_rows(const float *src, const int32_t *perm, int64_t n_rows, int width, float *dst,
                          void *stream);
 
+/* The inverse of distegnn_gather_rows: dst[perm[i],:] = src[i,:] for i < n_rows (gradients w.r.t. edge_attr in CSR order
+ * back into the caller's edge order).  perm must be a permutation of [0, n_rows). */
+DISTEGNN_API int distegnn_scatter_rows(const float *src, const int32_t *perm, int64_t n_rows, int width, float *dst,
+                                       void *stream);
+
 /* ---- embedding + per-forward setup ---------------------------------------------------------------
  * FastEGNN.forward prologue (FastEGNN.py:298-302): h0 = embedding_in(node_feat); also converts
  * node_loc [N,3] → x4, data_batch int64 → batch32, computes P/Q/Hn of layer 0 from `layer0_params`,
@@ -189,6 +194,15 @@ DISTEGNN_API int distegnn_edge_layer_bwd(int64_t n_nodes, int64_t n_edges, int A
                                          const float* x4, const float* P, const float* Q, const float* layer_params,
                                          const float* g_agg_m, const float* g_agg_x, float* g_P, float* g_Q,
                                          float* g_x4, float* g_layer_params, const int32_t* n_edges_dev, void* stream);
+/* distegnn_edge_layer_bwd plus the gradient w.r.t. the edge attributes (model input edge_attr, in CSR order):
+ * g_edge_attr_sorted [E,A] is ACCUMULATED (+=), so one buffer collects every layer.  NULL (or A = 0) is exactly
+ * distegnn_edge_layer_bwd. */
+DISTEGNN_API int distegnn_edge_layer_bwd_inputs(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags,
+                                                const int32_t* row, const int32_t* col, const float* edge_attr_sorted,
+                                                const float* x4, const float* P, const float* Q, const float* layer_params,
+                                                const float* g_agg_m, const float* g_agg_x, float* g_P, float* g_Q,
+                                                float* g_x4, float* g_layer_params, const int32_t* n_edges_dev,
+                                                float* g_edge_attr_sorted, void* stream);
 
 /* Backward of distegnn_virtual_layer_fwd (SURVEY §8 f-1; in the reference: autograd through models/FastEGNN.py:154-163,
  * 180, 191-193, 207, 220-223, 252-253).  Rows are recomputed tile by tile; the six row-wise tile GEMMs run on the tensor cores (wgmma).
@@ -299,6 +313,29 @@ DISTEGNN_API int distegnn_embed_bwd(int64_t n_nodes, int F, int A, int C, int Na
                                     const float *layer0_params, const float *g_h, const float *g_P, const float *g_Q,
                                     const float *g_Hn, float *g_emb_wt, float *g_emb_b, float *g_layer0_params,
                                     void *stream);
+/* The same two backward passes plus the gradients w.r.t. the model inputs.  distegnn_node_layer_bwd_inputs ACCUMULATES
+ * (+=) g_node_vel [N,3] (φ_v·g_x') and g_node_attr [N,Na] (the attr rows of N_W1; no term with FLAG_LAST), so one buffer
+ * each collects every layer; either may be NULL.  distegnn_embed_bwd_inputs WRITES g_node_feat [N,F] = g_h0·emb_wtᵀ
+ * (emb_wt [F][64] as in distegnn_embed_fwd) and g_node_loc [N,3] = g_x0 + g_vsum0[batch32[i], 0:3], where g_x0 [N,3] is
+ * the gradient w.r.t. layer 0's coordinates and g_vsum0 [B,K] (may be NULL) the gradient of the initial statistics
+ * (Σx of the initial centroid; already summed over the partitions); either output may be NULL.  With all extra outputs
+ * NULL both are exactly their plain counterparts. */
+DISTEGNN_API int distegnn_node_layer_bwd_inputs(int64_t n_nodes, int A, int C, int Na, unsigned flags,
+                                                const int32_t *rowptr, const float *h, const float *node_vel,
+                                                const float *node_attr, const float *agg_m, const float *agg_v,
+                                                const float *layer_params, const float *next_layer_params,
+                                                const float *g_x_out, const float *g_vsum, const int32_t *batch32,
+                                                const float *g_h_out, const float *g_P, const float *g_Q,
+                                                const float *g_Hn, float *g_h, float *g_x, float *g_agg_x,
+                                                float *g_trans_v, float *g_agg_m, float *g_agg_v, float *g_layer_params,
+                                                float *g_next_layer_params, float *g_node_vel, float *g_node_attr,
+                                                void *stream);
+DISTEGNN_API int distegnn_embed_bwd_inputs(int64_t n_nodes, int F, int A, int C, int Na, const float *node_feat,
+                                           const float *h0, const float *layer0_params, const float *g_h,
+                                           const float *g_P, const float *g_Q, const float *g_Hn, float *g_emb_wt,
+                                           float *g_emb_b, float *g_layer0_params, const float *emb_wt,
+                                           const int32_t *batch32, const float *g_x0, const float *g_vsum0,
+                                           float *g_node_feat, float *g_node_loc, void *stream);
 
 /* ---- virtual-node sync: packed SUM all-reduce over NVLink peer memory ------------------------------------------------
  * Replaces weighted_average_reduce / _AllReduce (models/FastEGNN.py:10-43, 310-319; call sites :195-197, 225-227,
