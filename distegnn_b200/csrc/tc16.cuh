@@ -95,6 +95,39 @@ __device__ __forceinline__ void mma_f16x3(uint32_t d, uint32_t a_hi, uint32_t a_
     }
 }
 
+// Register-operand flavour for one 64-row block held by a warpgroup: D = A_lo·B_hiᵀ + A_hi·B_loᵀ + A_hi·B_hiᵀ, K = 64,
+// N = 64.  a_hi / a_lo are the A fragments of the four k-steps (tile_mma.cuh wgmma_f16_m64n64k16_rA: registers 4ks ..
+// 4ks+3 for k-step ks), i.e. element (row, k) sits where an m64n64 accumulator keeps (row, column k).  Asynchronous:
+// issues the 12 wgmma and commits them; mma_f16x3_rA_wait completes the group before d is read or a_hi / a_lo reused.
+template <uint32_t LBO>
+__device__ __forceinline__ void mma_f16x3_rA(float (&d)[32], const uint32_t (&a_hi)[16], const uint32_t (&a_lo)[16],
+                                             uint64_t b_hi, uint64_t b_lo) {
+    constexpr uint64_t B_KSTEP = (2 * LBO) >> 4;
+    auto mma = [&](auto acc, const uint32_t (&a)[16], int ks, uint64_t b) {
+        tmma::wgmma_f16_m64n64k16_rA<decltype(acc)::value>(d, a[4 * ks], a[4 * ks + 1], a[4 * ks + 2], a[4 * ks + 3],
+                                                            b + ks * B_KSTEP);
+    };
+    tmma::wgmma_fence();
+    mma(std::false_type{}, a_lo, 0, b_hi);
+#pragma unroll
+    for (int ks = 1; ks < 4; ++ks) mma(std::true_type{}, a_lo, ks, b_hi);
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) mma(std::true_type{}, a_hi, ks, b_lo);
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) mma(std::true_type{}, a_hi, ks, b_hi);
+    tmma::wgmma_commit();
+}
+__device__ __forceinline__ void mma_f16x3_rA_wait(float (&d)[32], uint32_t (&a_hi)[16], uint32_t (&a_lo)[16]) {
+    tmma::wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) tmma::wgmma_keep(d[i]);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        tmma::wgmma_keep(a_hi[i]);
+        tmma::wgmma_keep(a_lo[i]);
+    }
+}
+
 // 16 fp32 values (·s) -> 8 packed hi words + 8 packed lo words; `mx` tracks max |hi|
 template <bool SCALED>
 __device__ __forceinline__ void split16(const float (&v)[16], float s, uint32_t (&hi)[8], uint32_t (&lo)[8],

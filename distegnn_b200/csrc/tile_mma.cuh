@@ -103,6 +103,36 @@ __device__ __forceinline__ void wgmma_f16_m64n64k16(float (&d)[32], uint64_t a_d
         : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
+// Same with the A operand in registers.  A fragment of m64k16 (thread = lane l of warp w, g = 16w + l/4, c = 2(l%4)):
+// a[0] = row g, k = c, c+1;  a[1] = row g + 8, k = c, c+1;  a[2] = row g, k = c+8, c+9;  a[3] = row g + 8, k = c+8, c+9
+// (two fp16 per register, even k in the low half).  For k-step ks these are exactly the accumulator pairs
+// d[8ks .. 8ks+7] of an m64n64 result, so one GEMM's output feeds the next GEMM without leaving the registers.
+// The registers are read asynchronously: they must stay untouched until wgmma_wait_all (see wgmma_keep).
+// ACCUMULATE = false overwrites d (scale-d 0) and reads nothing of it.
+#define DEGNN_WGMMA_RA_D(c)                                                                                             \
+    c(d[0]), c(d[1]), c(d[2]), c(d[3]), c(d[4]), c(d[5]), c(d[6]), c(d[7]), c(d[8]), c(d[9]), c(d[10]), c(d[11]),      \
+        c(d[12]), c(d[13]), c(d[14]), c(d[15]), c(d[16]), c(d[17]), c(d[18]), c(d[19]), c(d[20]), c(d[21]), c(d[22]),  \
+        c(d[23]), c(d[24]), c(d[25]), c(d[26]), c(d[27]), c(d[28]), c(d[29]), c(d[30]), c(d[31])
+#define DEGNN_WGMMA_RA_ASM(scale_d)                                                                                     \
+    "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "                                                               \
+    "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30," \
+    "%31}, {%32,%33,%34,%35}, %36, " scale_d ", 1, 1, 0;\n"
+template <bool ACCUMULATE>
+__device__ __forceinline__ void wgmma_f16_m64n64k16_rA(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                       uint64_t b_desc) {
+    if (ACCUMULATE)
+        asm volatile(DEGNN_WGMMA_RA_ASM("1") : DEGNN_WGMMA_RA_D("+f")
+                     : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
+    else
+        asm volatile(DEGNN_WGMMA_RA_ASM("0") : DEGNN_WGMMA_RA_D("=f")
+                     : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc) : "memory");
+}
+#undef DEGNN_WGMMA_RA_D
+#undef DEGNN_WGMMA_RA_ASM
+// Keep registers that an in-flight wgmma reads or writes alive and in place up to this point: the compiler sees the
+// wgmma's register operands only at its issue, so without this it may reuse A registers or read D before the wait.
+__device__ __forceinline__ void wgmma_keep(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+__device__ __forceinline__ void wgmma_keep(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
 // fragment of the 64-row block `mb` <-> 64 tile-memory columns starting at `col` (rows 64·mb .. 64·mb + 63)
 __device__ __forceinline__ void frag_rows(int mb, uint32_t& r0, uint32_t& q) {
     const uint32_t w = (threadIdx.x >> 5) & 3u, l = threadIdx.x & 31u;
