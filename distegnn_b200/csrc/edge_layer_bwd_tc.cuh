@@ -305,8 +305,9 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
                     }
                 }
             }
-            // geometry: gΔ_raw = g_aggx[i]·φ/norm + 2·g_r·Δ_raw
-            if (valid) {
+            // geometry: gΔ_raw = g_aggx[i]·φ/norm + 2·g_r·Δ_raw.  A self loop's +gΔ and −gΔ land on the same node and its
+            // exact gradient is zero, but under FLAG_NORMALIZE gΔ carries 1/(0 + 1e-8): the pair would round the node's sum
+            if (valid && r != c) {
                 const float s = phi * invn, t2 = 2.0f * gr;
                 const float gdx = fmaf(gx.x, s, t2 * dx), gdy = fmaf(gx.y, s, t2 * dy), gdz = fmaf(gx.z, s, t2 * dz);
                 atomicAdd(a.g_x + (size_t)r * 4 + 0, gdx);

@@ -277,11 +277,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) edge_layer_bwd_kernel(const EdgeB
         }
         __syncthreads();
 
-        // ---- 7. geometry: gΔ_raw = g_aggx[i]·φ/norm + 2·g_r·Δ_raw ----------------------------------------------------
+        // ---- 7. geometry: gΔ_raw = g_aggx[i]·φ/norm + 2·g_r·Δ_raw (none for a self loop: +gΔ − gΔ on one node) ---------
         if (tid < TILE_M) {
-            const int r = srow[tid];
-            if (r >= 0) {
-                const int c = scol[tid];
+            const int r = srow[tid], c = scol[tid];
+            if (r >= 0 && r != c) {
                 const float4 d = *reinterpret_cast<const float4*>(dxs + 4 * tid);
                 const float4 gx = ldg4(a.g_aggx + (size_t)r * 4);
                 const float s = phis[tid] * invn[tid], t2 = 2.0f * grs[tid];

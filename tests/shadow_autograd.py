@@ -15,8 +15,9 @@ from .shadow_backend import _fields
 H = 64
 
 
-def edge_stage(dims, flags, row, col, ea, x3, P, Q, lp):
-    """-> (agg_m [N,64] sums, agg_x [N,3] sums)"""
+def edge_stage(dims, flags, row, col, ea, x3, P, Q, lp, z1_shift=None):
+    """-> (agg_m [N,64] sums, agg_x [N,3] sums).  z1_shift: optional [E,64] added to the first pre-activation (zeros
+    whose gradient is the per-edge g_z1)."""
     N, E, A, C, Na = dims
     f = _fields(lp, A, C, Na)
     r, c = row.long(), col.long()
@@ -27,6 +28,8 @@ def edge_stage(dims, flags, row, col, ea, x3, P, Q, lp):
     pre = P[r] + Q[c] + radial * f["E_W1R"]
     if A:
         pre = pre + ea @ f["E_W1E"]
+    if z1_shift is not None:
+        pre = pre + z1_shift
     m = F.silu(F.silu(pre) @ f["E_W2"] + f["E_B2"])
     phi = F.silu(m @ f["E_WC"] + f["E_BC"]) @ f["E_W3"]
     agg_m = torch.zeros(N, H, dtype=P.dtype, device=P.device).index_add(0, r, m)
