@@ -20,7 +20,7 @@ P_FIELDS = [
     "V_WX", "V_BX", "V_W3X", "L_W", "L_B", "L_W3", "L_B3", "N_W1", "N_B1", "N_W2", "N_B2",
     "M_W1", "M_B1", "M_W2", "M_B2",
 ]
-FLAG_NORMALIZE, FLAG_LAST, FLAG_INIT, FLAG_ZERO_VSUM, FLAG_ZERO_AGG = 1, 2, 4, 8, 16
+FLAG_NORMALIZE, FLAG_LAST, FLAG_INIT, FLAG_ZERO_VSUM, FLAG_ZERO_AGG, FLAG_INIT_CENTROID = 1, 2, 4, 8, 16, 32
 MAX_CHANNELS, MAX_EDGE_ATTR, MAX_NODE_ATTR, MAX_NODE_FEAT, HIDDEN = 16, 8, 8, 16, 64
 
 _i64, _i32, _u32, _vp = C.c_int64, C.c_int, C.c_uint, C.c_void_p
@@ -39,6 +39,9 @@ SIGNATURES = {
     "distegnn_edge_layer_bwd_inputs": [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 16,
     "distegnn_radius_csr_workspace_bytes": [_i64, _i64, C.POINTER(_i64)],
     "distegnn_radius_graph_csr": [_i64, _i32, _vp, _vp, C.c_float, _i32, _i32, _i64, _i64] + [_vp] * 6 + [_i64, _vp],
+    "distegnn_rollout_advance": [_i64, _i32, _i32, C.c_float, _i32] + [_vp] * 10,
+    "distegnn_edge_lengths_csr": [_i64, _i32] + [_vp] * 6,
+    "distegnn_rollout_centroid": [_i64, _i32] + [_vp] * 4,
     "distegnn_kmeans_lloyd": [_i64, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp],
     "distegnn_virtual_layer_bwd": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 16,
     "distegnn_virtual_bwd_prepare": [_i32, _i32, _i32, _vp, _vp, _vp],

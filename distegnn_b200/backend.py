@@ -213,6 +213,40 @@ class CudaBackend:
                                                    ptr(g_lp), ptr(g_lp_next), self._s(vsum)), "virtual_update_bwd")
         self.launches += 1 if B else 0
 
+    # ---- rollout (csrc/rollout.cu) -------------------------------------------------------------------------------------
+    def graph_buffers(self, n_nodes: int, capacity: int, edge_attr_nf: int, device):
+        from .partition import RadiusGraphBuffers
+        return RadiusGraphBuffers(n_nodes, capacity, edge_attr_nf, device)
+
+    def radius_graph_into(self, buf, pos: Tensor, r: float, batch: Optional[Tensor], n_graphs: int, loop: bool) -> None:
+        """Capacity-mode radius graph of `pos` into the preallocated `partition.RadiusGraphBuffers` (no host sync)."""
+        from .partition import radius_graph_csr
+        radius_graph_csr(pos, r, batch, loop=loop, edge_attr_nf=buf.edge_attr_nf, n_graphs=n_graphs, out=buf)
+        self.launches += 7 if pos.shape[0] else 0            # ours; the cub scans and the radix sort come on top
+
+    def edge_lengths(self, row: Tensor, col: Tensor, pos: Tensor, n_edges_dev: Optional[Tensor], ea: Tensor) -> None:
+        """edge_attr[e, :] = ‖pos[row[e]] − pos[col[e]]‖ in CSR order, in place."""
+        E, A = int(ea.shape[0]), int(ea.shape[1])
+        check(self.lib.distegnn_edge_lengths_csr(E, A, ptr(row), ptr(col), ptr(pos), ptr(n_edges_dev), ptr(ea),
+                                                 self._s(pos)), "edge_lengths_csr")
+        self.launches += 1 if E and A else 0
+
+    def rollout_advance(self, speed_col: int, tau: float, pred: Tensor, loc: Tensor, vel: Tensor, feat: Optional[Tensor],
+                        traj: Optional[Tensor], edge_count: Tensor, overflow: Optional[Tensor], n_edges: Tensor,
+                        counter: Tensor) -> None:
+        """One step's state update (see distegnn_rollout_advance); `feat` None = no speed feature."""
+        N, F = int(loc.shape[0]), (int(feat.shape[1]) if feat is not None else 0)
+        check(self.lib.distegnn_rollout_advance(N, F, speed_col if feat is not None else -1, float(tau), int(n_edges.numel()),
+                                                ptr(pred), ptr(loc), ptr(vel), ptr(feat), ptr(traj), ptr(edge_count),
+                                                ptr(overflow), ptr(n_edges), ptr(counter), self._s(loc)), "rollout_advance")
+        self.launches += 1
+
+    def rollout_centroid(self, pos: Tensor, batch: Optional[Tensor], sums: Tensor) -> None:
+        """sums float64 [B,4] += per-graph (Σx, Σy, Σz, count)."""
+        check(self.lib.distegnn_rollout_centroid(int(pos.shape[0]), int(sums.shape[0]), ptr(pos), ptr(batch), ptr(sums),
+                                                 self._s(pos)), "rollout_centroid")
+        self.launches += 1 if pos.shape[0] else 0
+
     def allreduce_packed(self, comm: "Comm", buf: Tensor) -> None:
         """In-place SUM of `buf` over the partitions through the communicator's peer-mapped segments."""
         check(self.lib.distegnn_allreduce_packed(comm.handle, ptr(buf), buf.numel(), self._s(buf)), "allreduce_packed")

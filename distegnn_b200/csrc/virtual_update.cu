@@ -56,7 +56,9 @@ __global__ void __launch_bounds__(VU_THREADS) virtual_update_kernel(const VUpdAr
     const float inv = 1.0f / fmaxf(vs[3], 1.0f);
 
     if (tid < 3 * C) {
-        float x = (init && a.init_loc_mean) ? a.init_loc_mean[(size_t)b * 3 + tid / C] : a.Xv[(size_t)b * 3 * C + tid];
+        float x;
+        if (init && (a.flags & DISTEGNN_FLAG_INIT_CENTROID)) x = vs[tid / C] * inv;   // X_0 = x̄ of these positions
+        else x = (init && a.init_loc_mean) ? a.init_loc_mean[(size_t)b * 3 + tid / C] : a.Xv[(size_t)b * 3 * C + tid];
         if (!init) x += vs[4 + tid] * inv;
         sX[tid] = x;
         a.Xv[(size_t)b * 3 * C + tid] = x;
@@ -127,6 +129,8 @@ extern "C" int distegnn_virtual_update_fwd(int n_graphs, int A, int C, int Na, u
     DEGNN_CHECK_ARG(last || (Hv && next_layer_params && G), "null pointer (non-last)");
     DEGNN_CHECK_ARG(last || init || layer_params, "null layer_params");
     DEGNN_CHECK_ARG(init || (!init_loc_mean && !init_hv0), "init_loc_mean / init_hv0 need FLAG_INIT");
+    DEGNN_CHECK_ARG(!(flags & DISTEGNN_FLAG_INIT_CENTROID) || (init && !init_loc_mean),
+                    "FLAG_INIT_CENTROID needs FLAG_INIT and no init_loc_mean");
     Layout L = make_layout(A, C, Na);
     VUpdArgs a;
     a.B = n_graphs; a.C = C; a.K = 4 + 3 * C + H * C; a.flags = flags;
@@ -345,6 +349,7 @@ extern "C" int distegnn_virtual_update_bwd(int n_graphs, int A, int C, int Na, u
     DEGNN_CHECK_ARG(n_graphs > 0 && vsum && Xv && g_vsum && g_Xv, "null pointer / bad size");
     DEGNN_CHECK_ARG(last || (Hv && g_Hv && next_layer_params && g_next_layer_params), "null pointer (non-last)");
     DEGNN_CHECK_ARG(last || init || (layer_params && g_layer_params), "null layer_params (regular layer)");
+    DEGNN_CHECK_ARG(!(flags & DISTEGNN_FLAG_INIT_CENTROID), "FLAG_INIT_CENTROID is for inference (no gradient through x̄)");
     Layout L = make_layout(A, C, Na);
     VUpdBwdArgs a;
     a.B = n_graphs; a.C = C; a.K = 4 + 3 * C + H * C; a.flags = flags;

@@ -513,10 +513,12 @@ class FastEGNN(nn.Module):
         return ws
 
     def _run(self, be, pk, dims, a: Dict[str, Tensor], ws: Dict[str, Tensor], comm=None, out: Optional[Tensor] = None,
-             Xv: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+             Xv: Optional[Tensor] = None, init_centroid: bool = False) -> Tuple[Tensor, Tensor]:
         """Enqueue one forward on the current stream: 2 + 4L kernel launches (buffers in `ws`; nothing allocates,
         nothing syncs unless a new data_batch tensor has to be validated).  Results are written to `out` / `Xv`
-        (default: the workspace's own buffers, which the next forward overwrites)."""
+        (default: the workspace's own buffers, which the next forward overwrites).  `init_centroid` (rollouts): the
+        initial virtual coordinates are the per-graph centroid of `node_loc` over all partitions, taken from the
+        statistics the first exchange already sums, instead of `loc_mean` (which is then not read)."""
         A, Cn, Na, F = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf, self.node_feat_nf
         N, E, B, K = dims
         layers: List[Tensor] = pk["layers"]
@@ -547,8 +549,9 @@ class FastEGNN(nn.Module):
         if sync:
             self._sync_virtual(vsum)
         # FastEGNN.py:299-300 (initial Hv, Xv) are folded into the INIT update
-        be.virtual_update((B, A, Cn, Na), _lib.FLAG_INIT | _lib.FLAG_ZERO_VSUM, vsum, Xv, Hv, None, layers[0], G,
-                          a["loc_mean"], pk["hv0"], comm)
+        init = _lib.FLAG_INIT | _lib.FLAG_ZERO_VSUM | (_lib.FLAG_INIT_CENTROID if init_centroid else 0)
+        be.virtual_update((B, A, Cn, Na), init, vsum, Xv, Hv, None, layers[0], G,
+                          None if init_centroid else a["loc_mean"], pk["hv0"], comm)
         for i in range(L):
             last = i == L - 1
             flags = base | (_lib.FLAG_LAST if last else 0)

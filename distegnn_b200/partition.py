@@ -28,52 +28,91 @@ Tensor = torch.Tensor
 _TABLE_CELLS = 1 << 22          # dense cell table (graphs x cells), int32: 16 MiB of workspace
 
 
+class RadiusGraphBuffers:
+    """Preallocated outputs of `radius_graph_csr` for `capacity` edges: rowptr, row, col, edge_attr, info and the build
+    workspace live at fixed addresses, so repeated builds (a rollout rebuilds the graph every step) allocate nothing and
+    can be captured in a CUDA graph.  `graph` is the CSRGraph over them (capacity-sized, count on the device)."""
+
+    def __init__(self, n_nodes: int, capacity: int, edge_attr_nf: int, device, table_cells: int = _TABLE_CELLS):
+        lib = _lib.load()
+        nbytes = C.c_int64(0)
+        check(lib.distegnn_radius_csr_workspace_bytes(n_nodes, table_cells, C.byref(nbytes)), "radius_csr_workspace_bytes")
+        self.n_nodes, self.capacity, self.edge_attr_nf, self.table_cells = int(n_nodes), int(capacity), edge_attr_nf, table_cells
+        self.ws = torch.empty(int(nbytes.value), dtype=torch.uint8, device=device)
+        self.rowptr = torch.empty(n_nodes + 1, dtype=torch.int32, device=device)
+        self.info = torch.zeros(4, dtype=torch.int32, device=device)
+        self.row = torch.empty(self.capacity, dtype=torch.int32, device=device)
+        self.col = torch.empty(self.capacity, dtype=torch.int32, device=device)
+        self.edge_attr = (torch.empty(self.capacity, edge_attr_nf, dtype=torch.float32, device=device)
+                          if edge_attr_nf > 0 else None)
+        self.graph = CSRGraph(self.rowptr, self.col, self.row)
+        self.graph.n_edges_dev, self.graph.info = self.info[0:1], self.info
+
+
+def _build_into(buf: RadiusGraphBuffers, pos: Tensor, r: float, batch: Optional[Tensor], n_graphs: int, loop: bool,
+                capacity: int) -> None:
+    """One C-ABI call; `pos` float32 contiguous, `batch` int64 contiguous or None."""
+    with torch.cuda.device(pos.device):
+        check(_lib.load().distegnn_radius_graph_csr(
+            buf.n_nodes, n_graphs, ptr(pos), ptr(batch), float(r), int(loop), buf.edge_attr_nf, capacity, buf.table_cells,
+            ptr(buf.rowptr), ptr(buf.row if capacity else None), ptr(buf.col if capacity else None),
+            ptr(buf.edge_attr if capacity else None), ptr(buf.info), ptr(buf.ws), buf.ws.numel(),
+            _lib.stream_ptr(pos.device)), "radius_graph_csr")
+
+
 def radius_graph_csr(pos: Tensor, r: float, batch: Optional[Tensor] = None, loop: bool = False, edge_attr_nf: int = 2,
-                     capacity: Optional[int] = None, n_graphs: Optional[int] = None, table_cells: int = _TABLE_CELLS
-                     ) -> Tuple[CSRGraph, Optional[Tensor]]:
+                     capacity: Optional[int] = None, n_graphs: Optional[int] = None, table_cells: int = _TABLE_CELLS,
+                     out: Optional[RadiusGraphBuffers] = None) -> Tuple[CSRGraph, Optional[Tensor]]:
     """All ordered pairs (i, j) of the same graph with ‖pos_i − pos_j‖ < r (j != i unless `loop`) as a CSRGraph grouped
     by destination i, plus edge_attr [E, edge_attr_nf] = the edge length in every column (distribute_graphs.py:43-44).
 
     capacity=None: exact allocation (one host read of the edge count).  capacity=K: no host synchronisation at all — the
     buffers hold K entries, `graph.n_edges_dev` (int32 [1] on the device) says how many are valid, the kernels read it
-    there, and `graph.overflowed()` (a sync) tells whether K was too small.  `batch` int64, sorted (PyG convention)."""
+    there, and `graph.overflowed()` (a sync) tells whether K was too small.  out=RadiusGraphBuffers: capacity mode into
+    those buffers (capacity = out.capacity); returns `(out.graph, out.edge_attr)`.  `batch` int64, sorted (PyG
+    convention)."""
     if pos.device.type != "cuda":
         raise _lib.DistEGNNError("distegnn_b200.radius_graph_csr runs only on CUDA tensors (no CPU path)")
-    lib = _lib.load()
     dev = pos.device
     N = int(pos.shape[0])
     B = 1 if batch is None else (int(n_graphs) if n_graphs is not None else int(batch[-1].item()) + 1)
     p = pos.detach().to(torch.float32).contiguous()
     b = None if batch is None else batch.to(torch.int64).contiguous()
+    if out is not None:
+        if out.n_nodes != N or out.edge_attr_nf != edge_attr_nf or out.ws.device != dev:
+            raise ValueError(f"RadiusGraphBuffers are for {out.n_nodes} nodes, edge_attr_nf={out.edge_attr_nf} on "
+                             f"{out.ws.device}; got {N}, {edge_attr_nf} on {dev}")
+        if N:
+            _build_into(out, p, r, b, B, loop, out.capacity)
+        return out.graph, out.edge_attr
     if N == 0:
         z = torch.zeros(0, dtype=torch.int32, device=dev)
         return CSRGraph(torch.zeros(1, dtype=torch.int32, device=dev), z, z.clone()), torch.zeros(0, edge_attr_nf, device=dev)
-    nbytes = C.c_int64(0)
-    check(lib.distegnn_radius_csr_workspace_bytes(N, table_cells, C.byref(nbytes)), "radius_csr_workspace_bytes")
-    ws = torch.empty(int(nbytes.value), dtype=torch.uint8, device=dev)
-    rowptr = torch.empty(N + 1, dtype=torch.int32, device=dev)
-    info = torch.empty(4, dtype=torch.int32, device=dev)
-    stream = _lib.stream_ptr(dev)
-
-    def run(cap: int):
-        row = torch.empty(cap, dtype=torch.int32, device=dev)
-        col = torch.empty(cap, dtype=torch.int32, device=dev)
-        ea = torch.empty(cap, edge_attr_nf, dtype=torch.float32, device=dev) if edge_attr_nf > 0 else None
-        with torch.cuda.device(dev):
-            check(lib.distegnn_radius_graph_csr(N, B, ptr(p), ptr(b), float(r), int(loop), edge_attr_nf, cap, table_cells,
-                                                ptr(rowptr), ptr(row), ptr(col), ptr(ea), ptr(info), ptr(ws), ws.numel(),
-                                                stream), "radius_graph_csr")
-        return row, col, ea
-
     if capacity is None:
-        run(0)                                                   # count only
-        E = int(info[0].item())
-        row, col, ea = run(E)
-        return CSRGraph(rowptr, col, row), ea
-    row, col, ea = run(int(capacity))
-    g = CSRGraph(rowptr, col, row)
-    g.n_edges_dev, g.info = info[0:1], info
-    return g, ea
+        buf = RadiusGraphBuffers(N, 0, edge_attr_nf, dev, table_cells)
+        _build_into(buf, p, r, b, B, loop, 0)                    # count only
+        E = int(buf.info[0].item())
+        buf = _resized(buf, E)
+        _build_into(buf, p, r, b, B, loop, E)
+        return CSRGraph(buf.rowptr, buf.col, buf.row), buf.edge_attr
+    buf = RadiusGraphBuffers(N, int(capacity), edge_attr_nf, dev, table_cells)
+    _build_into(buf, p, r, b, B, loop, buf.capacity)
+    return buf.graph, buf.edge_attr
+
+
+def _resized(buf: RadiusGraphBuffers, capacity: int) -> RadiusGraphBuffers:
+    """The same rowptr / info / workspace with edge buffers for `capacity` edges."""
+    new = RadiusGraphBuffers.__new__(RadiusGraphBuffers)
+    new.__dict__.update(buf.__dict__)
+    dev = buf.ws.device
+    new.capacity = int(capacity)
+    new.row = torch.empty(new.capacity, dtype=torch.int32, device=dev)
+    new.col = torch.empty(new.capacity, dtype=torch.int32, device=dev)
+    new.edge_attr = (torch.empty(new.capacity, buf.edge_attr_nf, dtype=torch.float32, device=dev)
+                     if buf.edge_attr_nf > 0 else None)
+    new.graph = CSRGraph(new.rowptr, new.col, new.row)
+    new.graph.n_edges_dev, new.graph.info = new.info[0:1], new.info
+    return new
 
 
 def kmeans_labels(pos: Tensor, n_clusters: int, random_state: int = 0, max_iter: int = 300, tol: float = 1e-4,

@@ -74,6 +74,7 @@ enum {
 #define DISTEGNN_FLAG_INIT 4u       /* virtual_update before layer 0: no X / Hv update, only x̄, m_X, G */
 #define DISTEGNN_FLAG_ZERO_VSUM 8u  /* virtual_update: leave vsum zeroed (ready for the next layer's accumulation)  */
 #define DISTEGNN_FLAG_ZERO_AGG 16u  /* node_layer: leave agg_m / agg_x zeroed (ready for the next edge stage)       */
+#define DISTEGNN_FLAG_INIT_CENTROID 32u /* virtual_update with FLAG_INIT: X_0 := the summed x̄ (inference / rollout only) */
 
 DISTEGNN_API int distegnn_abi_version(void);
 DISTEGNN_API const char *distegnn_last_error(void);
@@ -258,6 +259,26 @@ DISTEGNN_API int distegnn_radius_graph_csr(int64_t n_nodes, int n_graphs, const 
  * the squared centre shift is <= tol (then after one more assignment pass), the remaining ones are no-ops.  centers [K,3]
  * in/out (seeded by the caller, k-means++), labels int32 [N] in/out (−1 initially), sums float64 [K,4] zeroed once by the
  * caller, state int32 [4] zeroed once: [0] 0 running / 1 final pass pending / 2 converged, [1] iterations done. */
+/* ---- multi-step rollout (csrc/rollout.cu; distegnn_b200/rollout.py) ----------------------------------------------------
+ * distegnn_rollout_advance: one step's state update after the forward, in one launch, no host synchronisation:
+ *   v = (pred − loc)/tau -> vel [N,3];  ‖v‖ -> feat[:, speed_col] (feat [N,F], NULL = no speed feature);  pred -> loc;
+ *   pred -> trajectory[step] ([steps,N,3], NULL = not kept);  *edge_count -> n_edges[step] (int32 [steps]).
+ * counter int32 [8], zeroed by the caller except [2] = −1: [0] step (read by every block, advanced by one per launch, so
+ * the same launch can be replayed from a CUDA graph), [1] sticky: 1 once *overflow was nonzero (overflow may be NULL),
+ * [2] first step that overflowed, [3] largest *edge_count seen, [4] internal (block ticket; keep 0).
+ * distegnn_edge_lengths_csr: edge_attr[e, :] = ‖pos[row[e]] − pos[col[e]]‖ for e < min(*n_edges_dev, n_edges) (NULL: all),
+ * with the arithmetic of distegnn_radius_graph_csr's fill pass (fixed-graph rollouts).
+ * distegnn_rollout_centroid: sums [n_graphs,4] fp64 += (Σx, Σy, Σz, count) per graph (data_batch int64, NULL for one
+ * graph); fp64, so the count is exact and Σx keeps full precision at any graph size. */
+DISTEGNN_API int distegnn_rollout_advance(int64_t n_nodes, int F, int speed_col, float tau, int steps, const float *pred,
+                                          float *loc, float *vel, float *feat, float *trajectory,
+                                          const int32_t *edge_count, const int32_t *overflow, int32_t *n_edges,
+                                          int32_t *counter, void *stream);
+DISTEGNN_API int distegnn_edge_lengths_csr(int64_t n_edges, int edge_attr_nf, const int32_t *row, const int32_t *col,
+                                           const float *pos, const int32_t *n_edges_dev, float *edge_attr, void *stream);
+DISTEGNN_API int distegnn_rollout_centroid(int64_t n_nodes, int n_graphs, const float *pos, const int64_t *data_batch,
+                                           double *sums, void *stream);
+
 DISTEGNN_API int distegnn_kmeans_lloyd(int64_t n_nodes, int n_clusters, const float *pos, float *centers,
                                        int32_t *labels, double *sums, int32_t *state, float tol, int iters, void *stream);
 
@@ -378,6 +399,9 @@ DISTEGNN_API int distegnn_allreduce_packed(void *comm, float *buf, int64_t count
  *   x̄ = vsum[b,0:3]/n;  m_X = (Xv−x̄)ᵀ(Xv−x̄);  G_next = W1v_V·Hv + W1v_M·m_X + b1v (next layer's)
  * FLAG_INIT: skip the Xv/Hv updates (before layer 0); if init_loc_mean [B,3] / init_hv0 [C,64] are given, Xv / Hv are
  * first initialised from them (FastEGNN.py:299-300) instead of being read.  FLAG_LAST: only Xv is updated.
+ * FLAG_INIT | FLAG_INIT_CENTROID: X_0 := x̄ = vsum[b,0:3]/n, the per-graph centroid over all partitions of the positions
+ * the embedding summed (init_loc_mean must be NULL) — loc_mean of a rollout step without an exchange of its own.  The
+ * backward rejects the flag.
  * FLAG_ZERO_VSUM: vsum is left zeroed for the next layer's accumulation; otherwise it holds the summed statistics on
  * return (the training path keeps them for the backward pass).
  * layer_params: this layer's block (node_mlp_virtual); next_layer_params: the block whose virtual MLP

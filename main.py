@@ -77,6 +77,8 @@ def parse():
     p.add_argument("--virtual_channels", type=int, default=None)
     p.add_argument("--eval_steps", type=int, default=10, help="(new) forward passes to time")
     p.add_argument("--nodes", type=int, default=None, help="(new) override the synthetic node count")
+    p.add_argument("--rollout_steps", type=int, default=0, help="(new) K-step rollout from the synthetic state "
+                   "(distegnn_b200.rollout): graph rebuilt on the device every step; prints ms/step and edges/step")
     p.add_argument("--train_steps", type=int, default=0, help="(new) optimisation steps of the reference's training "
                    "step (utils/train.py:98-158) on the synthetic target")
     return p.parse_args()
@@ -180,10 +182,43 @@ def main():
               f"edges(sum over partitions)={int(cnt[1])}  forward {dt * 1e3:.3f} ms  "
               f"{1.0 / dt:.2f} graph-steps/s  {cnt[1].item() / dt / 1e6:.1f} M edges/s  "
               f"mean squared displacement {se.item() / (3 * cnt[0].item()):.4e}  virtual_loc {tuple(X.shape)}")
+    if args.rollout_steps > 0:
+        rollout_steps(args, model, inp, w, world_size, local_rank, distributed)
     if args.train_steps > 0:
         train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed)
     if distributed:
         dist.destroy_process_group()
+
+
+def rollout_steps(args, model, inp, w, world_size, local_rank, distributed):
+    """K steps of `distegnn_b200.rollout` from the partition's state (radius graph rebuilt every step, or the fully
+    connected graph kept when the dataset has no radius); ms/step from a host clock around a device synchronise, after
+    one untimed rollout that also fixes the edge capacity."""
+    from distegnn_b200 import rollout
+    from distegnn_b200.shards import CSRGraph
+    node = {k: inp[k] for k in ("node_feat", "node_loc", "node_vel", "loc_mean", "data_batch")}
+    node["node_attr"] = inp["node_attr"] if w.node_attr_nf > 0 else None
+    kw = dict(radius=w.radius) if w.radius is not None else \
+        dict(graph=CSRGraph.from_edge_index(inp["edge_index"], inp["node_loc"].shape[0])[0])
+    K = args.rollout_steps
+    # the synthetic features stand for the datasets' (|v|, ...) columns: column 0 is the speed, one frame per step
+    kw.update(speed_col=0, tau=1.0)
+    res = rollout(model, **node, steps=K, **kw)                # warm-up; sizes the capacity
+    torch.cuda.synchronize()
+    if distributed:
+        dist.barrier()
+    t0 = time.perf_counter()
+    res = rollout(model, **node, steps=K, capacity=res.capacity, **kw)
+    torch.cuda.synchronize()
+    if distributed:
+        dist.barrier()
+    dt = (time.perf_counter() - t0) / K
+    edges = res.n_edges.double().mean().reshape(1)
+    if distributed:
+        dist.all_reduce(edges)
+    if local_rank == 0:
+        print(f"[{w.name}] rollout {K} steps, world_size={world_size}: {dt * 1e3:.3f} ms/step, "
+              f"{edges.item():.0f} edges/step (sum over partitions), capacity {res.capacity}")
 
 
 def train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed):
