@@ -241,6 +241,27 @@ class CudaBackend:
                                                 ptr(overflow), ptr(n_edges), ptr(counter), self._s(loc)), "rollout_advance")
         self.launches += 1
 
+    def edge_lengths_bwd(self, row: Tensor, col: Tensor, pos: Tensor, n_edges_dev: Optional[Tensor], g_ea: Tensor,
+                         g_pos: Tensor) -> None:
+        """g_pos [N,3] += the gradient of edge_attr[e, :] = ‖pos[row[e]] − pos[col[e]]‖ given g_ea [E,A] (CSR order)."""
+        E, A = int(g_ea.shape[0]), int(g_ea.shape[1])
+        check(self.lib.distegnn_edge_lengths_bwd(E, A, ptr(row), ptr(col), ptr(pos), ptr(n_edges_dev), ptr(g_ea),
+                                                 ptr(g_pos), self._s(pos)), "edge_lengths_bwd")
+        self.launches += 1 if E and A else 0
+
+    def rollout_advance_bwd(self, speed_col: Optional[int], tau: float, x_next: Tensor, x: Tensor,
+                            g_traj: Optional[Tensor], g_x_next: Optional[Tensor], g_v_next: Optional[Tensor],
+                            g_feat_next: Optional[Tensor], g_pred: Tensor, g_x: Tensor) -> None:
+        """Backward of one rollout_advance: writes g_pred (upstream of the step's prediction) and g_x (the advance's part
+        of the gradient of x_t); reads and zeroes g_feat_next[:, speed_col]."""
+        N = int(x.shape[0])
+        F = int(g_feat_next.shape[1]) if g_feat_next is not None else 0
+        check(self.lib.distegnn_rollout_advance_bwd(N, F, speed_col if g_feat_next is not None else -1, float(tau),
+                                                    ptr(x_next), ptr(x), ptr(g_traj), ptr(g_x_next), ptr(g_v_next),
+                                                    ptr(g_feat_next), ptr(g_pred), ptr(g_x), self._s(x)),
+              "rollout_advance_bwd")
+        self.launches += 1 if N else 0
+
     def rollout_centroid(self, pos: Tensor, batch: Optional[Tensor], sums: Tensor) -> None:
         """sums float64 [B,4] += per-graph (Σx, Σy, Σz, count)."""
         check(self.lib.distegnn_rollout_centroid(int(pos.shape[0]), int(sums.shape[0]), ptr(pos), ptr(batch), ptr(sums),

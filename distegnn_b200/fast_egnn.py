@@ -22,7 +22,7 @@ By default the inputs are constants of that graph, as in the reference's trainin
 every floating input that requires grad (node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr) receives the
 gradient the reference module's autograd would give it — multi-step rollout training, edge_attr computed in torch from the
 positions, sensitivity analysis.  edge_index / data_batch / CSRGraph are not differentiable, and neither is the edge_attr
-that `radius_graph_csr` builds on the device: compute edge_attr in torch when gradients must flow through edge lengths.
+that `radius_graph_csr` builds on the device: `rollout.differentiable_rollout` back-propagates through edge lengths.
 """
 from __future__ import annotations
 
@@ -420,12 +420,7 @@ class FastEGNN(nn.Module):
         six raw input tensors are inputs of the autograd node as well."""
         A, Cn, Na = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf
         N, E, B, K = dims
-        offs, total = _lib.param_layout(A, Cn, Na)
-        lps = [pack_layer_params(getattr(self, "gcl_%d" % i), A, Cn, Na, dev, offs, total, differentiable=True)
-               for i in range(self.n_layers)]
-        emb_wt = self.embedding_in.weight.t().contiguous().to(device=dev, dtype=torch.float32)
-        emb_b = self.embedding_in.bias.to(device=dev, dtype=torch.float32)
-        hv0 = self.virtual_node_feat[0].t().contiguous().to(device=dev, dtype=torch.float32)          # [C,64]
+        emb_wt, emb_b, hv0, lps = self._differentiable_params(dev)
         with torch.no_grad():
             rowptr, row, col, ea, nE = self._csr_inputs(be, edge_index, edge_attr, N, f32)
             args = dict(node_feat=f32(node_feat), node_loc=f32(node_loc), node_vel=f32(node_vel),
@@ -439,8 +434,22 @@ class FastEGNN(nn.Module):
         return _FastEGNNFunction.apply(self, be, dims, args, emb_wt, emb_b, hv0, *lps,
                                        node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr)
 
-    def _run_saving(self, be, dims, a: Dict[str, Tensor], emb_wt, emb_b, hv0, layers: List[Tensor]):
-        """`_run` with fresh buffers per layer; returns (out, Xv_L, saved state for the backward)."""
+    def _differentiable_params(self, dev):
+        """(emb_wt, emb_b, hv0, [layer blocks]) packed from the live parameters with torch ops, so that the gradients of
+        the packed tensors flow back to the nn.Parameters through autograd."""
+        A, Cn, Na = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf
+        offs, total = _lib.param_layout(A, Cn, Na)
+        lps = [pack_layer_params(getattr(self, "gcl_%d" % i), A, Cn, Na, dev, offs, total, differentiable=True)
+               for i in range(self.n_layers)]
+        emb_wt = self.embedding_in.weight.t().contiguous().to(device=dev, dtype=torch.float32)
+        emb_b = self.embedding_in.bias.to(device=dev, dtype=torch.float32)
+        hv0 = self.virtual_node_feat[0].t().contiguous().to(device=dev, dtype=torch.float32)          # [C,64]
+        return emb_wt, emb_b, hv0, lps
+
+    def _run_saving(self, be, dims, a: Dict[str, Tensor], emb_wt, emb_b, hv0, layers: List[Tensor],
+                    init_centroid: bool = False):
+        """`_run` with fresh buffers per layer; returns (out, Xv_L, saved state for the backward).  `init_centroid` as in
+        `_run` (the differentiable rollout's steps t >= 1): X_0 is the summed x̄ of node_loc, loc_mean is not read."""
         A, Cn, Na, F = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf, self.node_feat_nf
         N, E, B, K = dims
         dev = a["node_loc"].device
@@ -448,7 +457,7 @@ class FastEGNN(nn.Module):
         zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         L = self.n_layers
         base = _lib.FLAG_NORMALIZE if self.normalize else 0
-        Xv = a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn).contiguous()
+        Xv = new(B, 3, Cn) if init_centroid else a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn).contiguous()
         Hv = hv0.unsqueeze(0).expand(B, Cn, H).contiguous()
         h, x4, batch32, P, Q, Hn = new(N, H), new(N, 4), new(N, dt=torch.int32), new(N, H), new(N, H), new(N, H)
         vsum = zeros(B, K)
@@ -463,7 +472,8 @@ class FastEGNN(nn.Module):
         if comm is None:
             self._sync_virtual(vsum)
         G = new(B, Cn, H)
-        be.virtual_update((B, A, Cn, Na), _lib.FLAG_INIT, vsum, Xv, Hv, None, layers[0], G, comm=comm)
+        init = _lib.FLAG_INIT | (_lib.FLAG_INIT_CENTROID if init_centroid else 0)
+        be.virtual_update((B, A, Cn, Na), init, vsum, Xv, Hv, None, layers[0], G, comm=comm)
         out = None
         for i in range(L):
             last = i == L - 1
@@ -637,90 +647,29 @@ class _FastEGNNFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_out, g_Xv_out):
-        model, be, a, st = ctx.model, ctx.be, ctx.a, ctx.st
+        model = ctx.model
         N, E, B, K = ctx.dims
-        A, Cn, Na = model.edge_attr_nf, model.virtual_channels, model.node_attr_nf
         emb_wt, emb_b, hv0, layers = ctx.params
         L = len(layers)
-        dev = emb_wt.device
-        offs, total = _lib.param_layout(A, Cn, Na)
-        zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        g_lps = [zeros(total) for _ in range(L)]
-        g_emb_wt, g_emb_b, g_hv0 = torch.zeros_like(emb_wt), torch.zeros_like(emb_b), torch.zeros_like(hv0)
         n_in = len(ctx.inputs)
         want = ctx.needs_input_grad[7 + L:7 + L + n_in] if n_in else (False,) * 6
-        w_feat, w_loc, w_vel, w_lm, w_ea, w_attr = want
-        g_x = g_out.contiguous().to(torch.float32) if g_out is not None else zeros(N, 3)
-        g_Xv = g_Xv_out.contiguous().to(torch.float32) if g_Xv_out is not None else zeros(B, 3, Cn)
         if L == 0:                                           # out = node_loc, Xv = loc_mean broadcast
-            g_in = (None, g_x if w_loc else None, None, g_Xv.sum(-1) if w_lm else None, None, None)
-            return (None, None, None, None, g_emb_wt, g_emb_b, g_hv0) + _FastEGNNFunction._input_grads(ctx, g_in)
-        attr = a["attr"]
-        # input-gradient accumulators, only for the inputs that need one (the kernels then take the *_inputs entry points)
-        g_vel = zeros(N, 3) if w_vel else None
-        g_attr = zeros(N, Na) if (w_attr and Na > 0) else None
-        g_ea = zeros(E, A) if (w_ea and A > 0 and E > 0) else None          # CSR order
-        kw_node = dict(g_vel=g_vel, g_attr=g_attr) if (g_vel is not None or g_attr is not None) else {}
-        kw_edge = dict(g_ea=g_ea) if g_ea is not None else {}
-        g_Hv = g_G = g_h = g_P = g_Q = g_Hn = None
-        for i in reversed(range(L)):
-            S = st["layers"][i]
-            last = i == L - 1
-            lp, lp_next = layers[i], (None if last else layers[i + 1])
-            # ---- 1. virtual-node update (CUDA): (g_Xv', g_Hv', g_G') -> g_vsum, g_Xv, g_Hv, parameter gradients -------------
-            g_vsum, g_Xv_i = torch.empty(B, K, device=dev), torch.empty(B, 3, Cn, device=dev)
-            g_Hv_i = None if last else torch.empty(B, Cn, H, device=dev)
-            be.virtual_update_bwd((B, A, Cn, Na), S["flags"] & ~_lib.FLAG_NORMALIZE, S["vsum"], S["Xv"], S["Hv"], lp, lp_next,
-                                  g_Xv, g_Hv, g_G, g_vsum, g_Xv_i, g_Hv_i, g_lps[i], None if last else g_lps[i + 1])
-            if model.world_size > 1:                     # _AllReduce.backward (FastEGNN.py:19-21), one packed call
-                model._sync_virtual(g_vsum, be, st.get("comm"))
-            # ---- 2. node stage (CUDA): (g_x', g_h', g_P', g_Q', g_Hn') -> g_h, g_x, g_agg_*, g_trans_v, parameter gradients ----
-            g_h_i, g_x_i = torch.empty(N, H, device=dev), torch.empty(N, 3, device=dev)
-            g_agg_x, g_trans_v = torch.empty(N, 4, device=dev), torch.empty(N, 4, device=dev)
-            g_agg_m = None if last else torch.empty(N, H, device=dev)
-            g_agg_v = None if last else torch.empty(N, H, device=dev)
-            be.node_layer_bwd((N, B, A, Cn, Na), S["flags"], a["rowptr"], st["batch32"], S["h"], a["node_vel"], attr,
-                              S["agg_m"], S["agg_v"], lp, lp_next, g_x, g_vsum, g_h, g_P, g_Q, g_Hn, g_h_i, g_x_i,
-                              g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lps[i], None if last else g_lps[i + 1], **kw_node)
-            # ---- 3. real<->virtual stage (CUDA) ------------------------------------------------------------------------
-            wT = be.virtual_bwd_prepare(A, Cn, Na, lp)           # operand images of the stage's weights for the tensor cores
-            g_Hn_i, g_xv = torch.empty(N, H, device=dev), torch.empty(N, 4, device=dev)
-            g_G_i, g_Xv_acc = zeros(B, Cn, H), g_Xv_i.contiguous().clone()
-            be.virtual_layer_bwd((N, B, A, Cn, Na), S["flags"], st["batch32"], S["x4"], S["Hn"], S["Xv"], S["G"], lp, wT,
-                                 g_agg_v, g_trans_v, g_vsum, g_Hn_i, g_xv, g_G_i, g_Xv_acc, g_lps[i])
-            # ---- 4. per-edge stage (CUDA) --------------------------------------------------------------------------------
-            g_P_i, g_Q_i, g_x4e = zeros(N, H), zeros(N, H), zeros(N, 4)
-            be.edge_layer_bwd((N, E, A, Cn, Na), S["flags"], a["row"], a["col"], a["ea"], S["x4"], S["P"], S["Q"], lp,
-                              g_agg_m, g_agg_x, g_P_i, g_Q_i, g_x4e, g_lps[i], a["nE"], **kw_edge)
-            g_x = g_x_i + g_xv[:, :3] + g_x4e[:, :3]
-            g_h, g_P, g_Q, g_Hn = g_h_i, g_P_i, g_Q_i, g_Hn_i
-            g_Xv, g_Hv, g_G = g_Xv_acc, g_Hv_i, g_G_i
-        # ---- initial virtual state (CUDA): G_0 = f(Hv_0 = hv0, X_0 = loc_mean, x̄_0; layer-0 parameters) ---------------------
-        Xv0 = a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn).contiguous()
-        Hv0 = hv0.unsqueeze(0).expand(B, Cn, H).contiguous()
-        g_Hv0 = torch.empty(B, Cn, H, device=dev)
-        g_vsum0, g_Xv0 = torch.empty(B, K, device=dev), torch.empty(B, 3, Cn, device=dev)
-        # with loc_mean wanted, layer 0's g_Xv goes in as the upstream of X_0, so g_Xv0 is the whole gradient w.r.t. X_0
-        be.virtual_update_bwd((B, A, Cn, Na), _lib.FLAG_INIT, st["vsum_init"], Xv0, Hv0, None, layers[0],
-                              g_Xv if w_lm else None, g_Hv, g_G, g_vsum0, g_Xv0, g_Hv0, None, g_lps[0])
-        g_hv0 += g_Hv0.sum(0)                                # virtual_node_feat is shared by the graphs of the batch
-        if w_loc and model.world_size > 1:                   # x̄_0 is all-reduced: its Σx gradient is summed back
-            model._sync_virtual(g_vsum0, be, st.get("comm"))
-        # ---- embedding + layer-0 projections (CUDA) ----------------------------------------------------------------------------
-        g_feat = torch.empty(N, model.node_feat_nf, device=dev) if w_feat else None
-        g_loc = torch.empty(N, 3, device=dev) if w_loc else None
-        kw_emb = {} if (g_feat is None and g_loc is None) else dict(
-            g_feat=g_feat, g_loc=g_loc, emb_wt=emb_wt, batch32=st["batch32"], g_x0=g_x.contiguous() if w_loc else None,
-            g_vsum0=g_vsum0 if w_loc else None)
-        be.embed_bwd((N, B, model.node_feat_nf, A, Cn, Na), a["node_feat"], st["layers"][0]["h"], layers[0], g_h, g_P, g_Q,
-                     g_Hn, g_emb_wt, g_emb_b, g_lps[0], **kw_emb)
+            dev = emb_wt.device
+            g_x = g_out.contiguous().to(torch.float32) if g_out is not None else torch.zeros(N, 3, device=dev)
+            g_Xv = g_Xv_out.contiguous().to(torch.float32) if g_Xv_out is not None else \
+                torch.zeros(B, 3, model.virtual_channels, device=dev)
+            g_in = (None, g_x if want[1] else None, None, g_Xv.sum(-1) if want[3] else None, None, None)
+            return (None, None, None, None, torch.zeros_like(emb_wt), torch.zeros_like(emb_b),
+                    torch.zeros_like(hv0)) + _FastEGNNFunction._input_grads(ctx, g_in)
+        g_emb_wt, g_emb_b, g_hv0, g_lps, g_in = _backward_saved(model, ctx.be, ctx.dims, ctx.a, ctx.st, ctx.params, g_out,
+                                                                      g_Xv_out, want)
         grads = (None, None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps)
         if not n_in:
             return grads
-        if g_ea is not None and "perm" in a:                 # CSR order -> the caller's edge order
-            g_ea = be.gather_rows(g_ea, a["perm"], inverse=True)
-        g_in = (g_feat, g_loc, g_vel, g_Xv0.sum(-1) if w_lm else None, g_ea if w_ea else None, g_attr if w_attr else None)
-        return grads + _FastEGNNFunction._input_grads(ctx, g_in)
+        g_ea = g_in[4]
+        if g_ea is not None and "perm" in ctx.a:             # CSR order -> the caller's edge order
+            g_ea = ctx.be.gather_rows(g_ea, ctx.a["perm"], inverse=True)
+        return grads + _FastEGNNFunction._input_grads(ctx, g_in[:4] + (g_ea,) + g_in[5:])
 
     @staticmethod
     def _input_grads(ctx, g_in):
@@ -737,3 +686,92 @@ class _FastEGNNFunction(torch.autograd.Function):
             dev = ctx.params[0].device
             out.append(torch.zeros(shape, dtype=dtype, device=dev) if g is None else g.to(dtype).reshape(shape))
         return tuple(out)
+
+
+def _backward_saved(model: FastEGNN, be, dims, a, st, params, g_out, g_Xv_out, want, init_centroid: bool = False):
+    """The backward kernels of one forward kept by `FastEGNN._run_saving` (L >= 1), shared by `_FastEGNNFunction` and the
+    differentiable rollout.  `want` = which of (node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr) need a
+    gradient.  Returns (g_emb_wt, g_emb_b, g_hv0, [g_layer_params], (g_feat, g_loc, g_vel, g_loc_mean, g_ea in CSR order,
+    g_attr)), None for the inputs not wanted.
+
+    `init_centroid`: the forward ran with FLAG_INIT_CENTROID (X_0 = x̄ of node_loc, from the summed initial statistics).
+    The INIT update's backward then runs as a plain FLAG_INIT one with X_0 = that x̄, which returns the gradient w.r.t. X_0
+    as if it were independent; since X_0 = Σx/n, Σ_c g_X0 / n is folded into the Σx entries of g_vsum0 before its exchange,
+    and the embedding backward spreads it onto every node's g_loc.  No loc_mean gradient then."""
+    N, E, B, K = dims
+    A, Cn, Na = model.edge_attr_nf, model.virtual_channels, model.node_attr_nf
+    emb_wt, emb_b, hv0, layers = params
+    L = len(layers)
+    dev = emb_wt.device
+    offs, total = _lib.param_layout(A, Cn, Na)
+    zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
+    g_lps = [zeros(total) for _ in range(L)]
+    g_emb_wt, g_emb_b, g_hv0 = torch.zeros_like(emb_wt), torch.zeros_like(emb_b), torch.zeros_like(hv0)
+    w_feat, w_loc, w_vel, w_lm, w_ea, w_attr = want
+    g_x = g_out.contiguous().to(torch.float32) if g_out is not None else zeros(N, 3)
+    g_Xv = g_Xv_out.contiguous().to(torch.float32) if g_Xv_out is not None else zeros(B, 3, Cn)
+    attr = a["attr"]
+    # input-gradient accumulators, only for the inputs that need one (the kernels then take the *_inputs entry points)
+    g_vel = zeros(N, 3) if w_vel else None
+    g_attr = zeros(N, Na) if (w_attr and Na > 0) else None
+    g_ea = zeros(E, A) if (w_ea and A > 0 and E > 0) else None          # CSR order
+    kw_node = dict(g_vel=g_vel, g_attr=g_attr) if (g_vel is not None or g_attr is not None) else {}
+    kw_edge = dict(g_ea=g_ea) if g_ea is not None else {}
+    g_Hv = g_G = g_h = g_P = g_Q = g_Hn = None
+    for i in reversed(range(L)):
+        S = st["layers"][i]
+        last = i == L - 1
+        lp, lp_next = layers[i], (None if last else layers[i + 1])
+        # ---- 1. virtual-node update (CUDA): (g_Xv', g_Hv', g_G') -> g_vsum, g_Xv, g_Hv, parameter gradients -------------
+        g_vsum, g_Xv_i = torch.empty(B, K, device=dev), torch.empty(B, 3, Cn, device=dev)
+        g_Hv_i = None if last else torch.empty(B, Cn, H, device=dev)
+        be.virtual_update_bwd((B, A, Cn, Na), S["flags"] & ~_lib.FLAG_NORMALIZE, S["vsum"], S["Xv"], S["Hv"], lp, lp_next,
+                              g_Xv, g_Hv, g_G, g_vsum, g_Xv_i, g_Hv_i, g_lps[i], None if last else g_lps[i + 1])
+        if model.world_size > 1:                     # _AllReduce.backward (FastEGNN.py:19-21), one packed call
+            model._sync_virtual(g_vsum, be, st.get("comm"))
+        # ---- 2. node stage (CUDA): (g_x', g_h', g_P', g_Q', g_Hn') -> g_h, g_x, g_agg_*, g_trans_v, parameter gradients ----
+        g_h_i, g_x_i = torch.empty(N, H, device=dev), torch.empty(N, 3, device=dev)
+        g_agg_x, g_trans_v = torch.empty(N, 4, device=dev), torch.empty(N, 4, device=dev)
+        g_agg_m = None if last else torch.empty(N, H, device=dev)
+        g_agg_v = None if last else torch.empty(N, H, device=dev)
+        be.node_layer_bwd((N, B, A, Cn, Na), S["flags"], a["rowptr"], st["batch32"], S["h"], a["node_vel"], attr,
+                          S["agg_m"], S["agg_v"], lp, lp_next, g_x, g_vsum, g_h, g_P, g_Q, g_Hn, g_h_i, g_x_i,
+                          g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lps[i], None if last else g_lps[i + 1], **kw_node)
+        # ---- 3. real<->virtual stage (CUDA) ------------------------------------------------------------------------
+        wT = be.virtual_bwd_prepare(A, Cn, Na, lp)           # operand images of the stage's weights for the tensor cores
+        g_Hn_i, g_xv = torch.empty(N, H, device=dev), torch.empty(N, 4, device=dev)
+        g_G_i, g_Xv_acc = zeros(B, Cn, H), g_Xv_i.contiguous().clone()
+        be.virtual_layer_bwd((N, B, A, Cn, Na), S["flags"], st["batch32"], S["x4"], S["Hn"], S["Xv"], S["G"], lp, wT,
+                             g_agg_v, g_trans_v, g_vsum, g_Hn_i, g_xv, g_G_i, g_Xv_acc, g_lps[i])
+        # ---- 4. per-edge stage (CUDA) --------------------------------------------------------------------------------
+        g_P_i, g_Q_i, g_x4e = zeros(N, H), zeros(N, H), zeros(N, 4)
+        be.edge_layer_bwd((N, E, A, Cn, Na), S["flags"], a["row"], a["col"], a["ea"], S["x4"], S["P"], S["Q"], lp,
+                          g_agg_m, g_agg_x, g_P_i, g_Q_i, g_x4e, g_lps[i], a["nE"], **kw_edge)
+        g_x = g_x_i + g_xv[:, :3] + g_x4e[:, :3]
+        g_h, g_P, g_Q, g_Hn = g_h_i, g_P_i, g_Q_i, g_Hn_i
+        g_Xv, g_Hv, g_G = g_Xv_acc, g_Hv_i, g_G_i
+    # ---- initial virtual state (CUDA): G_0 = f(Hv_0 = hv0, X_0 = loc_mean, x̄_0; layer-0 parameters) ---------------------
+    # (init_centroid: X_0 = x̄ exactly as the forward's INIT update wrote it, kept as layer 0's Xv)
+    Xv0 = st["layers"][0]["Xv"] if init_centroid else a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn).contiguous()
+    Hv0 = hv0.unsqueeze(0).expand(B, Cn, H).contiguous()
+    g_Hv0 = torch.empty(B, Cn, H, device=dev)
+    g_vsum0, g_Xv0 = torch.empty(B, K, device=dev), torch.empty(B, 3, Cn, device=dev)
+    # with loc_mean wanted, layer 0's g_Xv goes in as the upstream of X_0, so g_Xv0 is the whole gradient w.r.t. X_0
+    be.virtual_update_bwd((B, A, Cn, Na), _lib.FLAG_INIT, st["vsum_init"], Xv0, Hv0, None, layers[0],
+                          g_Xv if (w_lm or init_centroid) else None, g_Hv, g_G, g_vsum0, g_Xv0, g_Hv0, None, g_lps[0])
+    g_hv0 += g_Hv0.sum(0)                                # virtual_node_feat is shared by the graphs of the batch
+    if init_centroid and w_loc:                          # X_0 = Σx / n: fold Σ_c g_X0 / n into the Σx entries
+        g_vsum0[:, 0:3] += g_Xv0.sum(-1) / st["vsum_init"][:, 3:4].clamp(min=1.0)
+    if w_loc and model.world_size > 1:                   # x̄_0 is all-reduced: its Σx gradient is summed back
+        model._sync_virtual(g_vsum0, be, st.get("comm"))
+    # ---- embedding + layer-0 projections (CUDA) ----------------------------------------------------------------------------
+    g_feat = torch.empty(N, model.node_feat_nf, device=dev) if w_feat else None
+    g_loc = torch.empty(N, 3, device=dev) if w_loc else None
+    kw_emb = {} if (g_feat is None and g_loc is None) else dict(
+        g_feat=g_feat, g_loc=g_loc, emb_wt=emb_wt, batch32=st["batch32"], g_x0=g_x.contiguous() if w_loc else None,
+        g_vsum0=g_vsum0 if w_loc else None)
+    be.embed_bwd((N, B, model.node_feat_nf, A, Cn, Na), a["node_feat"], st["layers"][0]["h"], layers[0], g_h, g_P, g_Q,
+                 g_Hn, g_emb_wt, g_emb_b, g_lps[0], **kw_emb)
+    g_lm = g_Xv0.sum(-1) if (w_lm and not init_centroid) else None
+    return g_emb_wt, g_emb_b, g_hv0, g_lps, (g_feat, g_loc, g_vel, g_lm, g_ea if w_ea else None,
+                                             g_attr if w_attr else None)

@@ -18,6 +18,9 @@ once per chunk of `check_every` steps (an OR over the ranks: every rank takes th
 rerun from its saved start with the capacity grown to 1.25x the largest true edge count.  `check_every=0` defers the
 check to `RolloutResult.check()`: the whole rollout is then enqueued without any host synchronisation.  With
 `model.cuda_graph = True` the step is captured once (after the eager step 0) and replayed.
+
+`differentiable_rollout` (same arguments) runs the same steps and attaches `trajectory` and `virtual_locs` to autograd;
+its backward recomputes one step at a time in reverse (DESIGN §15).
 """
 from __future__ import annotations
 
@@ -34,6 +37,7 @@ from .shards import CSRGraph
 Tensor = torch.Tensor
 GROWTH = 1.25              # capacity = GROWTH x edge count (initial build and every regrowth)
 MAX_REGROWTHS = 4          # per chunk; then the rollout raises
+_bwd_timing: Optional[list] = None   # benchmarks: a list receives (step, part, CUDA event) at each part of the backward
 
 
 @dataclass
@@ -52,14 +56,19 @@ class RolloutResult:
 
     graph: Optional[CSRGraph] = None   # the last step's graph (radius mode: capacity-sized, count in graph.n_edges_dev)
     edge_attr: Optional[Tensor] = None  # its edge_attr, in CSR order
+    virtual_locs: Optional[Tensor] = None   # [steps,B,3,C] each step's virtual_loc (differentiable_rollout only)
 
     def check(self) -> None:
-        """Raise if a graph build overflowed its capacity (one host read).  Only needed with `check_every=0`."""
+        """Raise if a graph build overflowed its capacity, or if the backward of a differentiable rollout rebuilt a graph
+        that differs from the forward's (one host read).  Only needed with `check_every=0`, or after a backward."""
         s = self.status.tolist()
         if s[1]:
             raise RuntimeError(f"rollout: the radius graph first outgrew the capacity {self.capacity} at step {s[2]} (the "
                                f"largest edge count of any step was {s[3]}); the results from that step on are wrong — "
                                "pass a larger capacity or let rollout check (check_every > 0)")
+        if s[5]:
+            raise RuntimeError(f"differentiable_rollout: the backward rebuilt {s[5]} step graph(s) with another edge count "
+                               "than the forward had; the gradients are wrong")
 
 
 def _unwrap(model) -> FastEGNN:
@@ -144,6 +153,7 @@ class _Rollout:
                         and dev.type == "cuda" and m._timing is None)
         self.cuda_graph, self.graph_launches, self.replays = None, 0, 0
         self.bufs, self.capacity = None, None
+        self.keep = None                                       # differentiable_rollout: per-step state for the backward
         if graph is not None:                                  # fixed graph: only edge_attr changes
             graph.validate(dev)
             self.rowptr, self.row, self.col = graph.rowptr.contiguous(), graph.rows().contiguous(), graph.col.contiguous()
@@ -173,9 +183,22 @@ class _Rollout:
     def _gbatch(self) -> Optional[Tensor]:
         return self.batch if self.B > 1 else None
 
+    def keep_steps(self) -> None:
+        """Also keep, per step, what the backward's recompute needs besides the trajectory: the step's input velocity and
+        speed column and its virtual_loc ([steps,·] buffers written at the device step index: capturable), plus x_0."""
+        K, N, B, Cn = self.steps, self.N, self.B, self.m.virtual_channels
+        new = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.dev)
+        self.keep = dict(x0=self.loc.clone(), feat0=self.feat.clone(), vel=new(K, N, 3), Xv=new(K, B, 3, Cn),
+                         speed=new(K, N) if self.speed_col is not None else None)
+
     # ---- one step -----------------------------------------------------------------------------------------------------
     def _enqueue(self, init_centroid: bool) -> None:
         m, be = self.m, self.be
+        if self.keep is not None:
+            idx = self.counter[0:1].long()                     # this step's index, on the device
+            self.keep["vel"].index_copy_(0, idx, self.vel.unsqueeze(0))
+            if self.keep["speed"] is not None:
+                self.keep["speed"].index_copy_(0, idx, self.feat[:, self.speed_col].unsqueeze(0))
         if self.bufs is not None:
             be.radius_graph_into(self.bufs, self.loc, self.radius, self._gbatch(), self.B, self.loop)
         elif self.ea is not None:
@@ -183,6 +206,8 @@ class _Rollout:
         args = dict(node_feat=self.feat, node_loc=self.loc, node_vel=self.vel, loc_mean=self.loc_mean0, attr=self.attr,
                     data_batch=self.batch, rowptr=self.rowptr, row=self.row, col=self.col, ea=self.ea, nE=self.nE)
         m._run(be, self.pk, (self.N, self.E, self.B, self.K), args, self.ws, self.comm, init_centroid=init_centroid)
+        if self.keep is not None:
+            self.keep["Xv"].index_copy_(0, idx, self.ws["Xv"].unsqueeze(0))
         be.rollout_advance(self.speed_col, self.tau, self.ws["out"], self.loc, self.vel,
                            self.feat if self.speed_col is not None else None, self.traj, self.edge_count, self.overflow,
                            self.n_edges, self.counter)
@@ -253,36 +278,207 @@ def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_me
     with guard, torch.no_grad():
         r = _Rollout(m, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph,
                      loop, tau, speed_col, return_trajectory)
-        grown: List[int] = []
-        if radius is not None:
-            r.set_capacity(capacity if capacity is not None else r.exact_capacity())
-        cap0 = r.capacity
-        chunk = steps if check_every is None else (check_every or steps)
-        check = check_every != 0
-        t = 0
-        while t < steps:
-            n = min(chunk, steps - t)
-            saved = r.snapshot() if (check and r.bufs is not None) else None
-            for attempt in range(MAX_REGROWTHS + 1):
-                for s in range(t, t + n):
-                    r.step(s)
-                if saved is None:
-                    break
-                anywhere, mine, count = r.overflowed_anywhere()
-                if not anywhere:
-                    break
-                if attempt == MAX_REGROWTHS:
-                    raise RuntimeError(f"rollout: steps {t}..{t + n - 1} still overflow the radius graph after "
-                                       f"{MAX_REGROWTHS} regrowths (capacities {[cap0] + grown}, largest edge count "
-                                       f"on this rank {count})")
-                r.restore(saved)                               # every rank reruns the chunk
-                if mine:
-                    r.set_capacity(max(r.capacity + 1, math.ceil(GROWTH * count)))
-                    grown.append(r.capacity)
-            t += n
+        grown = _drive(r, capacity, check_every)
         loc_mean_out = r.finish()
         return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=loc_mean_out,
                              virtual_loc=r.ws["Xv"].clone(), trajectory=r.traj, n_edges=r.n_edges, capacity=r.capacity,
                              regrowths=grown, replays=r.replays, status=r.counter,
                              graph=r.bufs.graph if r.bufs is not None else CSRGraph(r.rowptr, r.col, r.row),
                              edge_attr=r.ea)
+
+
+def _drive(r: _Rollout, capacity: Optional[int], check_every: Optional[int]) -> List[int]:
+    """Run every step of `r` with the overflow policy of the module docstring; returns the capacities grown to."""
+    steps = r.steps
+    grown: List[int] = []
+    if r.radius is not None:
+        r.set_capacity(capacity if capacity is not None else r.exact_capacity())
+    cap0 = r.capacity
+    chunk = steps if check_every is None else (check_every or steps)
+    check = check_every != 0
+    t = 0
+    while t < steps:
+        n = min(chunk, steps - t)
+        saved = r.snapshot() if (check and r.bufs is not None) else None
+        for attempt in range(MAX_REGROWTHS + 1):
+            for s in range(t, t + n):
+                r.step(s)
+            if saved is None:
+                break
+            anywhere, mine, count = r.overflowed_anywhere()
+            if not anywhere:
+                break
+            if attempt == MAX_REGROWTHS:
+                raise RuntimeError(f"rollout: steps {t}..{t + n - 1} still overflow the radius graph after "
+                                   f"{MAX_REGROWTHS} regrowths (capacities {[cap0] + grown}, largest edge count "
+                                   f"on this rank {count})")
+            r.restore(saved)                                   # every rank reruns the chunk
+            if mine:
+                r.set_capacity(max(r.capacity + 1, math.ceil(GROWTH * count)))
+                grown.append(r.capacity)
+        t += n
+    return grown
+
+
+# ---- training through a rollout ---------------------------------------------------------------------------------------
+def differentiable_rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_mean: Tensor,
+                           data_batch: Tensor, node_attr: Optional[Tensor] = None, *, steps: int,
+                           radius: Optional[float] = None, graph: Optional[CSRGraph] = None, loop: bool = False,
+                           tau: float = 1.0, speed_col: Optional[int] = None, capacity: Optional[int] = None,
+                           check_every: Optional[int] = None) -> RolloutResult:
+    """`rollout()` with a backward: `trajectory` [steps,N,3] and `virtual_locs` [steps,B,3,C] are attached to autograd, so
+    a loss on any steps back-propagates into the model's parameters (summed over the steps) and into each of node_feat,
+    node_loc, node_vel, loc_mean and node_attr that requires grad.  Same arguments, checks, update rules and overflow
+    policy as `rollout()`; every other field of the result is detached and means what it means there.
+
+    The forward is `rollout()`'s step loop; per step it keeps only O(N) state (the velocity, the speed column, the virtual
+    coordinates; the positions are the trajectory).  The backward runs the steps in reverse, one at a time: it rebuilds
+    step t's graph from x_t (radius mode; the build is deterministic, so the same positions give the same graph, and a
+    differing edge count is recorded for `RolloutResult.check()`), recomputes step t's forward with its activations, and
+    runs the backward kernels, the edge-length backward and the advance backward.  Peak memory is one step's training
+    peak plus O(steps·N).  The graph is piecewise constant and gets no gradient; the edge lengths do.  loc_mean is read at
+    step 0 only (later steps use the centroid of x_t, as in `rollout()`).  `model.input_grads` is not used or changed.
+    The backward reuses the rollout's graph buffers: after it, `graph` / `edge_attr` hold step 0's graph.
+
+    With several ranks (the model may be wrapped in DistributedDataParallel: its module is used) every rank calls this
+    and then backward on its own partition.  The state gradients are exact on every rank (every cross-rank term goes
+    through the model's packed exchanges).  The parameter gradients are this rank's contribution only — DDP's reducer does
+    not see this call — so sum them over the ranks yourself, e.g. `dist.all_reduce(p.grad)` for every parameter."""
+    m = _unwrap(model)
+    _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
+              capacity, check_every)
+    dev = node_loc.device
+    be = m._get_backend(dev)
+    import contextlib
+    guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
+    with guard:
+        emb_wt, emb_b, hv0, lps = m._differentiable_params(dev)
+        out = {}
+        opts = dict(data_batch=data_batch, steps=steps, radius=radius, graph=graph, loop=loop, tau=tau,
+                    speed_col=speed_col, capacity=capacity, check_every=check_every)
+        traj, vlocs = _RolloutFunction.apply(out, m, be, opts, emb_wt, emb_b, hv0, *lps, node_feat, node_loc, node_vel,
+                                             loc_mean, node_attr)
+    r = out["r"]
+    return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=out["loc_mean"],
+                         virtual_loc=r.ws["Xv"].clone(), trajectory=traj, n_edges=r.n_edges, capacity=r.capacity,
+                         regrowths=out["grown"], replays=r.replays, status=r.counter,
+                         graph=r.bufs.graph if r.bufs is not None else CSRGraph(r.rowptr, r.col, r.row), edge_attr=r.ea,
+                         virtual_locs=vlocs)
+
+
+class _RolloutFunction(torch.autograd.Function):
+    """Autograd node of `differentiable_rollout`: inputs (packed parameters, then node_feat, node_loc, node_vel,
+    loc_mean, node_attr), outputs (trajectory, virtual_locs).  See DESIGN §15."""
+
+    @staticmethod
+    def forward(ctx, out, m, be, opts, emb_wt, emb_b, hv0, *rest):
+        L = m.n_layers
+        node_feat, node_loc, node_vel, loc_mean, node_attr = rest[L:]
+        o = opts
+        r = _Rollout(m, be, node_loc.device, node_feat, node_loc, node_vel, loc_mean, o["data_batch"], node_attr,
+                     o["steps"], o["radius"], o["graph"], o["loop"], o["tau"], o["speed_col"], True)
+        r.keep_steps()
+        out["grown"] = _drive(r, o["capacity"], o["check_every"])
+        out["loc_mean"], out["r"] = r.finish(), r
+        ctx.r = r
+        ctx.params = (emb_wt.detach().contiguous(), emb_b.detach().contiguous(), hv0.detach().contiguous(),
+                      [lp.detach().contiguous() for lp in rest[:L]])
+        ctx.inputs = [None if t is None else t.dtype for t in rest[L:]]
+        ctx.save_for_backward(r.traj)                          # an in-place change of the trajectory is caught
+        return r.traj, r.keep["Xv"]
+
+    @staticmethod
+    def backward(ctx, g_traj, g_vlocs):
+        from .fast_egnn import _backward_saved
+        r = ctx.r
+        (traj,) = ctx.saved_tensors
+        m, be, dev = r.m, r.be, r.dev
+        emb_wt, emb_b, hv0, layers = ctx.params
+        L, N, B, Cn, Na, A = len(layers), r.N, r.B, m.virtual_channels, m.node_attr_nf, r.A
+        w_feat, w_loc, w_vel, w_lm, w_attr = ctx.needs_input_grad[7 + L:7 + L + 5]
+        sc = r.speed_col
+        zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
+        g_traj = g_traj.contiguous().float() if g_traj is not None else zeros(r.steps, N, 3)
+        g_vlocs = g_vlocs.contiguous().float() if g_vlocs is not None else zeros(r.steps, B, 3, Cn)
+        g_emb_wt, g_emb_b, g_hv0 = torch.zeros_like(emb_wt), torch.zeros_like(emb_b), torch.zeros_like(hv0)
+        g_lps = [torch.zeros_like(lp) for lp in layers]
+        g_attr_sum = zeros(N, Na) if (w_attr and Na > 0) else None
+        g_x_next = g_v_next = g_f_next = g_lm = None
+        feat_t = r.keep["feat0"].clone()
+        import contextlib
+        guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
+        with guard, torch.no_grad():
+            for t in reversed(range(r.steps)):
+                mark = _marker(t)
+                mark("rebuild")
+                x_t = r.keep["x0"] if t == 0 else traj[t - 1]
+                # 1. step t's graph from x_t: rebuilt (deterministic: the forward's graph) or the kept one's lengths
+                if r.bufs is not None:
+                    be.radius_graph_into(r.bufs, x_t, r.radius, r._gbatch(), r.B, r.loop)
+                    r.counter[5:6] += (r.edge_count != r.n_edges[t:t + 1]).to(torch.int32)
+                elif r.ea is not None:
+                    be.edge_lengths(r.row, r.col, x_t, r.nE, r.ea)
+                # 2. step t's forward again, with its activations
+                if sc is not None:
+                    feat_t[:, sc] = r.keep["speed"][t]
+                a = dict(node_feat=feat_t, node_loc=x_t, node_vel=r.keep["vel"][t], loc_mean=r.loc_mean0, attr=r.attr,
+                         data_batch=r.batch, rowptr=r.rowptr, row=r.row, col=r.col, ea=r.ea, nE=r.nE)
+                dims = (N, r.E, B, r.K)
+                mark("recompute")
+                _, _, st = m._run_saving(be, dims, a, emb_wt, emb_b, hv0, layers, init_centroid=t > 0)
+                # 3. the advance: upstream of the prediction x_{t+1}, and its −g_v/tau share of g_x_t
+                mark("advance_bwd")
+                g_pred, g_x = torch.empty(N, 3, device=dev), torch.empty(N, 3, device=dev)
+                be.rollout_advance_bwd(sc, r.tau, traj[t], x_t, g_traj[t], g_x_next, g_v_next,
+                                       g_f_next if sc is not None else None, g_pred, g_x)
+                # 4. the model's backward (t >= 1: the state feeds back, so positions, velocities and the speed column
+                #    always need their gradient; at t = 0 only the inputs that require grad)
+                mark("model_bwd")
+                first = t == 0
+                want = (w_feat or (not first and sc is not None), w_loc or not first, w_vel or not first,
+                        first and w_lm, A > 0 and (w_loc or not first), w_attr)
+                ge, gb, gh, glps, g_in = _backward_saved(m, be, dims, a, st, ctx.params, g_pred, g_vlocs[t], want,
+                                                         init_centroid=not first)
+                del st, a
+                g_emb_wt += ge
+                g_emb_b += gb
+                g_hv0 += gh
+                for acc, g in zip(g_lps, glps):
+                    acc += g
+                g_feat, g_loc, g_vel, g_lm_t, g_ea, g_attr = g_in
+                if g_attr_sum is not None and g_attr is not None:
+                    g_attr_sum += g_attr
+                # 5. g_x_t = the advance's part + the model's (centroid included) + the edge lengths'
+                if g_loc is not None:
+                    g_x += g_loc
+                mark("edge_lengths_bwd")
+                if g_ea is not None:
+                    be.edge_lengths_bwd(r.row, r.col, x_t, r.nE, g_ea, g_x)
+                del g_ea
+                mark("end")
+                if g_feat is not None and g_f_next is not None:
+                    g_feat += g_f_next                         # columns other than speed_col pass straight through
+                elif g_feat is None:
+                    g_feat = g_f_next
+                g_x_next, g_v_next, g_f_next, g_lm = g_x, g_vel, g_feat, g_lm_t
+        g_in = (g_f_next if w_feat else None, g_x_next if w_loc else None, g_v_next if w_vel else None,
+                g_lm if w_lm else None, g_attr_sum if w_attr else None)
+        shapes = (N, m.node_feat_nf), (N, 3), (N, 3), (B, 3), (N, Na)
+        outs = []
+        for want, dtype, g, shape in zip((w_feat, w_loc, w_vel, w_lm, w_attr), ctx.inputs, g_in, shapes):
+            if not want:
+                outs.append(None)
+            else:
+                outs.append(torch.zeros(shape, dtype=dtype, device=dev) if g is None else g.to(dtype))
+        return (None, None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps, *outs)
+
+
+def _marker(step: int):
+    if _bwd_timing is None:
+        return lambda name: None
+
+    def mark(name: str) -> None:
+        ev = torch.cuda.Event(enable_timing=True)
+        ev.record()
+        _bwd_timing.append((step, name, ev))
+    return mark

@@ -278,6 +278,24 @@ DISTEGNN_API int distegnn_edge_lengths_csr(int64_t n_edges, int edge_attr_nf, co
                                            const float *pos, const int32_t *n_edges_dev, float *edge_attr, void *stream);
 DISTEGNN_API int distegnn_rollout_centroid(int64_t n_nodes, int n_graphs, const float *pos, const int64_t *data_batch,
                                            double *sums, void *stream);
+/* Backward of a differentiable rollout (differentiable_rollout), one step at a time in reverse.  Caller-owned buffers,
+ * nothing allocated, no host synchronisation; negative error codes like every entry point.
+ * distegnn_edge_lengths_bwd: backward of distegnn_edge_lengths_csr (and of the radius fill pass's edge_attr).  For
+ *   e < min(*n_edges_dev, n_edges) (n_edges_dev NULL: all): g = Σ_k g_edge_attr[e,k], u = Δx/‖Δx‖ with Δx = pos[row[e]] −
+ *   pos[col[e]] computed as in the forward; g_pos[row[e]] += g·u, g_pos[col[e]] −= g·u (accumulated; g_pos [N,3]).  A
+ *   zero-length edge (self loop, coincident points) contributes exactly 0.  Rows must be sorted (CSR); edges at and
+ *   beyond the count are never read.
+ * distegnn_rollout_advance_bwd: backward of distegnn_rollout_advance for one step.  Recomputes v = (x_next − x)/tau with
+ *   the forward's arithmetic, then g_v = g_v_next + g_feat_next[:, speed_col]·v/‖v‖ (0 at v = 0; g_feat_next NULL = no
+ *   speed feature, else that column is set to 0 after it is read), writes g_pred = g_traj + g_x_next + g_v/tau (the
+ *   upstream of the step's model output) and g_x = −g_v/tau.  g_traj, g_x_next, g_v_next may be NULL (zero). */
+DISTEGNN_API int distegnn_edge_lengths_bwd(int64_t n_edges, int edge_attr_nf, const int32_t *row, const int32_t *col,
+                                           const float *pos, const int32_t *n_edges_dev, const float *g_edge_attr,
+                                           float *g_pos, void *stream);
+DISTEGNN_API int distegnn_rollout_advance_bwd(int64_t n_nodes, int F, int speed_col, float tau, const float *x_next,
+                                              const float *x, const float *g_traj, const float *g_x_next,
+                                              const float *g_v_next, float *g_feat_next, float *g_pred, float *g_x,
+                                              void *stream);
 
 DISTEGNN_API int distegnn_kmeans_lloyd(int64_t n_nodes, int n_clusters, const float *pos, float *centers,
                                        int32_t *labels, double *sums, int32_t *state, float tol, int iters, void *stream);
