@@ -224,6 +224,13 @@ class CudaBackend:
         radius_graph_csr(pos, r, batch, loop=loop, edge_attr_nf=buf.edge_attr_nf, n_graphs=n_graphs, out=buf)
         self.launches += 7 if pos.shape[0] else 0            # ours; the cub scans and the radix sort come on top
 
+    def cutoff_into(self, buf, graph, pos: Tensor, rate: float, batch: Optional[Tensor], n_graphs: int) -> None:
+        """The kept edges of `graph` (the shortest int(E_b·(1 − rate)) of every graph) into the preallocated
+        `partition.RadiusGraphBuffers` `buf` (csrc/cutoff_csr.cu; no host sync)."""
+        from .partition import cutoff_edges_csr
+        cutoff_edges_csr(graph, pos, rate, batch, n_graphs, buf.edge_attr_nf, out=buf)
+        self.launches += (14 if graph.num_edges else 3) if pos.shape[0] else 0   # ours; two cub scans on top
+
     def edge_lengths(self, row: Tensor, col: Tensor, pos: Tensor, n_edges_dev: Optional[Tensor], ea: Tensor) -> None:
         """edge_attr[e, :] = ‖pos[row[e]] − pos[col[e]]‖ in CSR order, in place."""
         E, A = int(ea.shape[0]), int(ea.shape[1])

@@ -1,6 +1,7 @@
 """On-device graph partitioning and construction (SURVEY §8 f-2) — the device form of datasets/distribute_graphs.py.
 
     graph, edge_attr = radius_graph_csr(pos, r, batch=None)        # CSR by destination, int32, no int64 edge_index
+    graph, edge_attr = cutoff_edges_csr(graph, pos, 0.5, batch)      # FastEGNN's cutoff: the shortest half of each graph
     labels = kmeans_labels(pos, world_size)                          # == sklearn KMeans(random_state=0).fit_predict
     parts = split_large_graph(pos, x, target, vel, attr, r, P, split_mode="random" | "kmeans")
 
@@ -16,6 +17,7 @@ CUDA only; there is no CPU path.
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -62,7 +64,8 @@ def _build_into(buf: RadiusGraphBuffers, pos: Tensor, r: float, batch: Optional[
 
 def radius_graph_csr(pos: Tensor, r: float, batch: Optional[Tensor] = None, loop: bool = False, edge_attr_nf: int = 2,
                      capacity: Optional[int] = None, n_graphs: Optional[int] = None, table_cells: int = _TABLE_CELLS,
-                     out: Optional[RadiusGraphBuffers] = None) -> Tuple[CSRGraph, Optional[Tensor]]:
+                     out: Optional[RadiusGraphBuffers] = None,
+                     cutoff_rate: float = 0.0) -> Tuple[CSRGraph, Optional[Tensor]]:
     """All ordered pairs (i, j) of the same graph with ‖pos_i − pos_j‖ < r (j != i unless `loop`) as a CSRGraph grouped
     by destination i, plus edge_attr [E, edge_attr_nf] = the edge length in every column (distribute_graphs.py:43-44).
 
@@ -70,7 +73,15 @@ def radius_graph_csr(pos: Tensor, r: float, batch: Optional[Tensor] = None, loop
     buffers hold K entries, `graph.n_edges_dev` (int32 [1] on the device) says how many are valid, the kernels read it
     there, and `graph.overflowed()` (a sync) tells whether K was too small.  out=RadiusGraphBuffers: capacity mode into
     those buffers (capacity = out.capacity); returns `(out.graph, out.edge_attr)`.  `batch` int64, sorted (PyG
-    convention)."""
+    convention).
+
+    cutoff_rate > 0 (FastEGNN's cutoff_edges mode): the radius graph is the candidate set and `cutoff_edges_csr` keeps
+    the int(E_b * (1 - cutoff_rate)) shortest edges of every graph.  `capacity` / `out.capacity` count the CANDIDATES;
+    the returned graph holds the kept edges (count in `graph.n_edges_dev` in capacity mode).  0 runs no cutoff at all."""
+    _check_rate(cutoff_rate)
+    if cutoff_rate > 0:
+        return _radius_then_cut(pos, r, batch, loop, edge_attr_nf, capacity, n_graphs, table_cells, out,
+                                float(cutoff_rate))
     if pos.device.type != "cuda":
         raise _lib.DistEGNNError("distegnn_b200.radius_graph_csr runs only on CUDA tensors (no CPU path)")
     dev = pos.device
@@ -113,6 +124,115 @@ def _resized(buf: RadiusGraphBuffers, capacity: int) -> RadiusGraphBuffers:
     new.graph = CSRGraph(new.rowptr, new.col, new.row)
     new.graph.n_edges_dev, new.graph.info = new.info[0:1], new.info
     return new
+
+
+# ---- edge cutoff (FastEGNN's cutoff_edges mode; csrc/cutoff_csr.cu) ----------------------------------------------------
+def _check_rate(rate) -> None:
+    if isinstance(rate, bool) or not isinstance(rate, numbers.Real):
+        raise ValueError(f"cutoff_rate must be a real number in [0, 1] (got {rate!r})")
+    if not 0.0 <= float(rate) <= 1.0:                          # NaN fails too
+        raise ValueError(f"cutoff_rate must lie in [0, 1] (got {rate!r})")
+
+
+def _cut_workspace(out: RadiusGraphBuffers, n_graphs: int, capacity: int) -> Tensor:
+    """The cutoff's workspace, kept on the output buffers (allocated on first use, reused at a fixed address after)."""
+    key = (int(n_graphs), int(capacity))
+    if getattr(out, "cut_key", None) != key:
+        nbytes = C.c_int64(0)
+        check(_lib.load().distegnn_cutoff_csr_workspace_bytes(out.n_nodes, key[0], key[1], C.byref(nbytes)),
+              "cutoff_csr_workspace_bytes")
+        out.cut_ws = torch.empty(int(nbytes.value), dtype=torch.uint8, device=out.ws.device)
+        out.cut_key = key
+    return out.cut_ws
+
+
+def _cut_into(out: RadiusGraphBuffers, graph: CSRGraph, pos: Tensor, rate: float, batch: Optional[Tensor],
+              n_graphs: int) -> None:
+    """One C-ABI call: the kept edges of `graph` into `out` (no host synchronisation).  `pos` float32 contiguous,
+    `batch` int64 contiguous or None."""
+    cap = graph.num_edges
+    ws = _cut_workspace(out, n_graphs, cap)
+    overflow = graph.info[1:2] if graph.info is not None else None
+    rows = graph.rows().contiguous() if cap else None
+    with torch.cuda.device(pos.device):
+        check(_lib.load().distegnn_cutoff_csr(
+            out.n_nodes, n_graphs, ptr(pos), ptr(batch), float(rate), out.edge_attr_nf, ptr(graph.rowptr.contiguous()),
+            ptr(rows), ptr(graph.col.contiguous() if cap else None), ptr(graph.n_edges_dev), cap, ptr(overflow),
+            ptr(out.rowptr), ptr(out.row if cap else None), ptr(out.col if cap else None),
+            ptr(out.edge_attr if cap else None), ptr(out.info), ptr(ws), ws.numel(), _lib.stream_ptr(pos.device)),
+            "cutoff_csr")
+
+
+def cutoff_edges_csr(graph: CSRGraph, pos: Tensor, cutoff_rate: float, batch: Optional[Tensor] = None,
+                     n_graphs: Optional[int] = None, edge_attr_nf: int = 2, capacity: Optional[int] = None,
+                     out: Optional[RadiusGraphBuffers] = None) -> Tuple[CSRGraph, Optional[Tensor]]:
+    """FastEGNN's edge cutoff on the device (datasets/process_dataset.py:300-305, once per sample): of every graph of the
+    batch keep the int(E_b * (1 - cutoff_rate)) shortest edges of `graph` and drop the rest.
+
+    `graph` is any CSRGraph (built on the device, read from a shard, or `CSRGraph.from_edge_index`); its edges below
+    `graph.n_edges_dev` are the candidates.  The length is the fp32 ‖pos_i − pos_j‖ of the radius build; ties are broken by
+    CSR position (a stable selection), NaN sorts last.  Returns the kept edges as a CSRGraph in the candidates' order plus
+    edge_attr [E, edge_attr_nf] = the length in every column (:104).
+
+    capacity=None: exact (one host read of the kept count).  capacity=K (>= graph.num_edges): no host synchronisation —
+    buffers of K entries, the kept count in `graph.n_edges_dev` on the device.  out=RadiusGraphBuffers: into those
+    buffers (out.capacity >= graph.num_edges).  `batch` int64, sorted; pass `n_graphs` to avoid reading its last entry."""
+    _check_rate(cutoff_rate)
+    if not isinstance(graph, CSRGraph):
+        raise ValueError("graph must be a distegnn_b200.shards.CSRGraph")
+    if pos.device.type != "cuda" or graph.rowptr.device != pos.device:
+        raise _lib.DistEGNNError("distegnn_b200.cutoff_edges_csr runs only on CUDA tensors, graph and pos on one device "
+                                 "(no CPU path)")
+    dev = pos.device
+    N = int(pos.shape[0])
+    if graph.num_nodes != N:
+        raise ValueError(f"graph has {graph.num_nodes} nodes, pos has {N}")
+    E = graph.num_edges
+    B = 1 if batch is None else (int(n_graphs) if n_graphs is not None else int(batch[-1].item()) + 1)
+    p = pos.detach().to(torch.float32).contiguous()
+    b = None if batch is None else batch.to(torch.int64).contiguous()
+    if out is not None:
+        if out.n_nodes != N or out.edge_attr_nf != edge_attr_nf or out.ws.device != dev or out.capacity < E:
+            raise ValueError(f"RadiusGraphBuffers are for {out.n_nodes} nodes, {out.capacity} edges, edge_attr_nf="
+                             f"{out.edge_attr_nf} on {out.ws.device}; got {N}, {E} candidates, {edge_attr_nf} on {dev}")
+        if N:
+            _cut_into(out, graph, p, float(cutoff_rate), b, B)
+        return out.graph, out.edge_attr
+    if N == 0:
+        z = torch.zeros(0, dtype=torch.int32, device=dev)
+        return CSRGraph(torch.zeros(1, dtype=torch.int32, device=dev), z, z.clone()), torch.zeros(0, edge_attr_nf, device=dev)
+    if capacity is not None:
+        if int(capacity) < E:
+            raise ValueError(f"capacity {capacity} is below the candidate buffers' {E} entries")
+        buf = RadiusGraphBuffers(N, int(capacity), edge_attr_nf, dev, table_cells=27)
+        _cut_into(buf, graph, p, float(cutoff_rate), b, B)
+        return buf.graph, buf.edge_attr
+    buf = RadiusGraphBuffers(N, E, edge_attr_nf, dev, table_cells=27)
+    _cut_into(buf, graph, p, float(cutoff_rate), b, B)
+    kept, overflowed = buf.info[0:2].tolist()
+    if overflowed:
+        raise ValueError(f"the candidate graph overflowed its capacity {E} (its true edge count is "
+                         f"{int(buf.info[2].item())}): the candidates are incomplete")
+    ea = buf.edge_attr[:kept] if buf.edge_attr is not None else None
+    return CSRGraph(buf.rowptr, buf.col[:kept], buf.row[:kept]), ea
+
+
+def _radius_then_cut(pos, r, batch, loop, edge_attr_nf, capacity, n_graphs, table_cells, out, rate):
+    """radius_graph_csr(cutoff_rate > 0): the candidates (no edge_attr: the cutoff recomputes the lengths), then the cut."""
+    if pos.device.type != "cuda":
+        raise _lib.DistEGNNError("distegnn_b200.radius_graph_csr runs only on CUDA tensors (no CPU path)")
+    N = int(pos.shape[0])
+    B = 1 if batch is None else (int(n_graphs) if n_graphs is not None else int(batch[-1].item()) + 1)
+    if out is None and capacity is None:
+        g, _ = radius_graph_csr(pos, r, batch, loop=loop, edge_attr_nf=0, n_graphs=B, table_cells=table_cells)
+        return cutoff_edges_csr(g, pos, rate, batch, B, edge_attr_nf)
+    if out is None:
+        out = RadiusGraphBuffers(N, int(capacity), edge_attr_nf, pos.device, table_cells)
+    if getattr(out, "candidates", None) is None:
+        out.candidates = RadiusGraphBuffers(out.n_nodes, out.capacity, 0, out.ws.device, out.table_cells)
+    cg, _ = radius_graph_csr(pos, r, batch, loop=loop, edge_attr_nf=0, n_graphs=B, table_cells=table_cells,
+                             out=out.candidates)
+    return cutoff_edges_csr(cg, pos, rate, batch, B, edge_attr_nf, out=out)
 
 
 def kmeans_labels(pos: Tensor, n_clusters: int, random_state: int = 0, max_iter: int = 300, tol: float = 1e-4,

@@ -19,6 +19,10 @@ rerun from its saved start with the capacity grown to 1.25x the largest true edg
 check to `RolloutResult.check()`: the whole rollout is then enqueued without any host synchronisation.  With
 `model.cuda_graph = True` the step is captured once (after the eager step 0) and replayed.
 
+`cutoff_rate > 0` (FastEGNN's cutoff_edges mode, one device): each step's graph is the int(E_b·(1 − cutoff_rate))
+shortest edges of every graph of the candidates above (process_dataset.py:103, `partition.cutoff_edges_csr`), re-selected
+from the current lengths; the capacity and its regrowth count the candidates, `n_edges` the kept edges (DESIGN §16).
+
 `differentiable_rollout` (same arguments) runs the same steps and attaches `trajectory` and `virtual_locs` to autograd;
 its backward recomputes one step at a time in reverse (DESIGN §15).
 """
@@ -32,6 +36,7 @@ import torch
 
 from . import _lib
 from .fast_egnn import FastEGNN
+from .partition import _check_rate
 from .shards import CSRGraph
 
 Tensor = torch.Tensor
@@ -64,7 +69,7 @@ class RolloutResult:
         s = self.status.tolist()
         if s[1]:
             raise RuntimeError(f"rollout: the radius graph first outgrew the capacity {self.capacity} at step {s[2]} (the "
-                               f"largest edge count of any step was {s[3]}); the results from that step on are wrong — "
+                               f"largest edge count of any step was {max(s[3], s[6])}); the results from that step on are wrong — "
                                "pass a larger capacity or let rollout check (check_every > 0)")
         if s[5]:
             raise RuntimeError(f"differentiable_rollout: the backward rebuilt {s[5]} step graph(s) with another edge count "
@@ -79,8 +84,12 @@ def _unwrap(model) -> FastEGNN:
 
 
 def _validate(m: FastEGNN, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau,
-              speed_col, capacity, check_every) -> None:
+              speed_col, capacity, check_every, cutoff_rate=0.0) -> None:
     is_int = lambda v: isinstance(v, int) and not isinstance(v, bool)
+    _check_rate(cutoff_rate)
+    if cutoff_rate > 0 and m.world_size > 1:
+        raise ValueError("cutoff_rate > 0 is a single-device mode (the reference's cutoff_edges); with several ranks the "
+                         "partitions already drop their cross edges")
     if not is_int(steps) or steps < 1:
         raise ValueError(f"steps must be an int >= 1 (got {steps!r})")
     if not tau > 0:
@@ -130,7 +139,7 @@ class _Rollout:
     """State buffers at fixed addresses + the per-step enqueue (eager or CUDA-graph replay)."""
 
     def __init__(self, m: FastEGNN, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius,
-                 graph, loop, tau, speed_col, return_trajectory):
+                 graph, loop, tau, speed_col, return_trajectory, cutoff_rate=0.0):
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).clone().contiguous()
         self.m, self.be, self.dev = m, be, dev
         self.N, self.B = int(node_loc.shape[0]), int(loc_mean.shape[0])
@@ -154,6 +163,8 @@ class _Rollout:
         self.cuda_graph, self.graph_launches, self.replays = None, 0, 0
         self.bufs, self.capacity = None, None
         self.keep = None                                       # differentiable_rollout: per-step state for the backward
+        self.rate = float(cutoff_rate)
+        self.cut, self.cand = None, None                       # cutoff: kept-edge buffers, the candidate graph
         if graph is not None:                                  # fixed graph: only edge_attr changes
             graph.validate(dev)
             self.rowptr, self.row, self.col = graph.rowptr.contiguous(), graph.rows().contiguous(), graph.col.contiguous()
@@ -162,7 +173,10 @@ class _Rollout:
             self.edge_count = self.nE if self.nE is not None else \
                 torch.full((1,), self.E, dtype=torch.int32, device=dev)
             self.overflow = None
-            self.ea = torch.empty(self.E, self.A, dtype=torch.float32, device=dev) if self.A > 0 else None
+            self.ea = torch.empty(self.E, self.A, dtype=torch.float32, device=dev) if self.A > 0 and not self.rate else None
+            if self.rate > 0:                                  # the caller's graph is the candidate set
+                self.cand = graph
+                self._cut_buffers()
 
     # ---- graph buffers (radius mode) ----------------------------------------------------------------------------------
     def exact_capacity(self) -> int:
@@ -173,12 +187,29 @@ class _Rollout:
 
     def set_capacity(self, cap: int) -> None:
         self.capacity = int(cap)
-        self.bufs = self.be.graph_buffers(self.N, self.capacity, self.A, self.dev)
+        # with a cutoff the radius graph is only the candidate set: no edge_attr (the cutoff writes the kept lengths)
+        self.bufs = self.be.graph_buffers(self.N, self.capacity, 0 if self.rate > 0 else self.A, self.dev)
         g = self.bufs.graph
         self.rowptr, self.row, self.col, self.ea = g.rowptr, g.row, g.col, self.bufs.edge_attr
         self.E, self.nE = self.capacity, g.n_edges_dev
         self.edge_count, self.overflow = self.bufs.info[0:1], self.bufs.info[1:2]
+        if self.rate > 0:
+            self.cand = g
+            self._cut_buffers()
         self.cuda_graph = None                                 # captured addresses are stale
+
+    def _cut_buffers(self) -> None:
+        """Buffers of the kept edges (as many entries as the candidates): the model runs on them, and the advance records
+        their count."""
+        self.cut = self.be.graph_buffers(self.N, self.E, self.A, self.dev)
+        g = self.cut.graph
+        self.rowptr, self.row, self.col, self.ea, self.nE = g.rowptr, g.row, g.col, self.cut.edge_attr, g.n_edges_dev
+        self.edge_count = self.cut.info[0:1]
+
+    def cut_graph(self, x: Tensor) -> None:
+        """The kept edges of the candidates at positions x; counter[6] keeps the largest candidate count (regrowth)."""
+        self.be.cutoff_into(self.cut, self.cand, x, self.rate, self._gbatch(), self.B)
+        torch.maximum(self.counter[6:7], self.cut.info[2:3], out=self.counter[6:7])
 
     def _gbatch(self) -> Optional[Tensor]:
         return self.batch if self.B > 1 else None
@@ -201,8 +232,10 @@ class _Rollout:
                 self.keep["speed"].index_copy_(0, idx, self.feat[:, self.speed_col].unsqueeze(0))
         if self.bufs is not None:
             be.radius_graph_into(self.bufs, self.loc, self.radius, self._gbatch(), self.B, self.loop)
-        elif self.ea is not None:
+        elif self.ea is not None and self.cut is None:
             be.edge_lengths(self.row, self.col, self.loc, self.nE, self.ea)
+        if self.cut is not None:
+            self.cut_graph(self.loc)
         args = dict(node_feat=self.feat, node_loc=self.loc, node_vel=self.vel, loc_mean=self.loc_mean0, attr=self.attr,
                     data_batch=self.batch, rowptr=self.rowptr, row=self.row, col=self.col, ea=self.ea, nE=self.nE)
         m._run(be, self.pk, (self.N, self.E, self.B, self.K), args, self.ws, self.comm, init_centroid=init_centroid)
@@ -239,6 +272,8 @@ class _Rollout:
         """(any rank overflowed, this rank overflowed, this rank's largest true edge count): one host read, plus one
         MAX all-reduce of the flag with several ranks."""
         st = self.counter[1:4].clone()                         # [own flag, first step, largest count]
+        if self.cut is not None:                               # regrow from the candidates, not the kept edges
+            st[2:3] = self.counter[6:7]
         flag = st[0:1].clone()
         if self.m.world_size > 1:
             import torch.distributed as dist
@@ -261,30 +296,40 @@ def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_me
             node_attr: Optional[Tensor] = None, *, steps: int, radius: Optional[float] = None,
             graph: Optional[CSRGraph] = None, loop: bool = False, tau: float = 1.0, speed_col: Optional[int] = None,
             capacity: Optional[int] = None, check_every: Optional[int] = None,
-            return_trajectory: bool = False) -> RolloutResult:
+            return_trajectory: bool = False, cutoff_rate: float = 0.0) -> RolloutResult:
     """Roll `model` (a FastEGNN, or one wrapped in DistributedDataParallel) out for `steps` steps from the given state;
     see the module docstring for the update rules.  With several ranks every rank calls it with its own partition.
 
     capacity: edge capacity of the rebuilt graph (radius mode); None = count step 0's graph (one host sync) and take
     1.25x that.  check_every: steps per overflow check (default: all steps, one check at the end); 0 = no check inside
-    (call `RolloutResult.check()`).  Runs under no_grad; the caller's tensors are not modified."""
+    (call `RolloutResult.check()`).  Runs under no_grad; the caller's tensors are not modified.
+
+    cutoff_rate > 0 (FastEGNN's cutoff_edges mode, single device): every step keeps the int(E_b·(1 − cutoff_rate))
+    shortest edges of each graph's candidates (the rebuilt radius graph, or the caller's `graph`), re-selected from the
+    current lengths (`cutoff_edges_csr`).  `n_edges` then counts the kept edges; `capacity` and its regrowth count the
+    candidates.  0 runs no cutoff at all."""
     m = _unwrap(model)
     _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
-              capacity, check_every)
+              capacity, check_every, cutoff_rate)
     dev = node_loc.device
     be = m._get_backend(dev)                                    # raises on a CPU tensor (no CPU path)
     import contextlib
     guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
     with guard, torch.no_grad():
         r = _Rollout(m, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph,
-                     loop, tau, speed_col, return_trajectory)
+                     loop, tau, speed_col, return_trajectory, cutoff_rate)
         grown = _drive(r, capacity, check_every)
         loc_mean_out = r.finish()
         return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=loc_mean_out,
                              virtual_loc=r.ws["Xv"].clone(), trajectory=r.traj, n_edges=r.n_edges, capacity=r.capacity,
                              regrowths=grown, replays=r.replays, status=r.counter,
-                             graph=r.bufs.graph if r.bufs is not None else CSRGraph(r.rowptr, r.col, r.row),
-                             edge_attr=r.ea)
+                             graph=_result_graph(r), edge_attr=r.ea)
+
+
+def _result_graph(r: _Rollout) -> CSRGraph:
+    if r.cut is not None:
+        return r.cut.graph
+    return r.bufs.graph if r.bufs is not None else CSRGraph(r.rowptr, r.col, r.row)
 
 
 def _drive(r: _Rollout, capacity: Optional[int], check_every: Optional[int]) -> List[int]:
@@ -325,7 +370,7 @@ def differentiable_rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel:
                            data_batch: Tensor, node_attr: Optional[Tensor] = None, *, steps: int,
                            radius: Optional[float] = None, graph: Optional[CSRGraph] = None, loop: bool = False,
                            tau: float = 1.0, speed_col: Optional[int] = None, capacity: Optional[int] = None,
-                           check_every: Optional[int] = None) -> RolloutResult:
+                           check_every: Optional[int] = None, cutoff_rate: float = 0.0) -> RolloutResult:
     """`rollout()` with a backward: `trajectory` [steps,N,3] and `virtual_locs` [steps,B,3,C] are attached to autograd, so
     a loss on any steps back-propagates into the model's parameters (summed over the steps) and into each of node_feat,
     node_loc, node_vel, loc_mean and node_attr that requires grad.  Same arguments, checks, update rules and overflow
@@ -338,7 +383,9 @@ def differentiable_rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel:
     runs the backward kernels, the edge-length backward and the advance backward.  Peak memory is one step's training
     peak plus O(steps·N).  The graph is piecewise constant and gets no gradient; the edge lengths do.  loc_mean is read at
     step 0 only (later steps use the centroid of x_t, as in `rollout()`).  `model.input_grads` is not used or changed.
-    The backward reuses the rollout's graph buffers: after it, `graph` / `edge_attr` hold step 0's graph.
+    The backward reuses the rollout's graph buffers: after it, `graph` / `edge_attr` hold step 0's graph.  With
+    `cutoff_rate` the backward re-selects each step's kept edges from x_t (deterministic: the forward's); the selection
+    is piecewise constant and gets no gradient, the kept edges' lengths do.
 
     With several ranks (the model may be wrapped in DistributedDataParallel: its module is used) every rank calls this
     and then backward on its own partition.  The state gradients are exact on every rank (every cross-rank term goes
@@ -346,7 +393,7 @@ def differentiable_rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel:
     not see this call — so sum them over the ranks yourself, e.g. `dist.all_reduce(p.grad)` for every parameter."""
     m = _unwrap(model)
     _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
-              capacity, check_every)
+              capacity, check_every, cutoff_rate)
     dev = node_loc.device
     be = m._get_backend(dev)
     import contextlib
@@ -355,15 +402,14 @@ def differentiable_rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel:
         emb_wt, emb_b, hv0, lps = m._differentiable_params(dev)
         out = {}
         opts = dict(data_batch=data_batch, steps=steps, radius=radius, graph=graph, loop=loop, tau=tau,
-                    speed_col=speed_col, capacity=capacity, check_every=check_every)
+                    speed_col=speed_col, capacity=capacity, check_every=check_every, cutoff_rate=cutoff_rate)
         traj, vlocs = _RolloutFunction.apply(out, m, be, opts, emb_wt, emb_b, hv0, *lps, node_feat, node_loc, node_vel,
                                              loc_mean, node_attr)
     r = out["r"]
     return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=out["loc_mean"],
                          virtual_loc=r.ws["Xv"].clone(), trajectory=traj, n_edges=r.n_edges, capacity=r.capacity,
                          regrowths=out["grown"], replays=r.replays, status=r.counter,
-                         graph=r.bufs.graph if r.bufs is not None else CSRGraph(r.rowptr, r.col, r.row), edge_attr=r.ea,
-                         virtual_locs=vlocs)
+                         graph=_result_graph(r), edge_attr=r.ea, virtual_locs=vlocs)
 
 
 class _RolloutFunction(torch.autograd.Function):
@@ -376,7 +422,7 @@ class _RolloutFunction(torch.autograd.Function):
         node_feat, node_loc, node_vel, loc_mean, node_attr = rest[L:]
         o = opts
         r = _Rollout(m, be, node_loc.device, node_feat, node_loc, node_vel, loc_mean, o["data_batch"], node_attr,
-                     o["steps"], o["radius"], o["graph"], o["loop"], o["tau"], o["speed_col"], True)
+                     o["steps"], o["radius"], o["graph"], o["loop"], o["tau"], o["speed_col"], True, o["cutoff_rate"])
         r.keep_steps()
         out["grown"] = _drive(r, o["capacity"], o["check_every"])
         out["loc_mean"], out["r"] = r.finish(), r
@@ -415,9 +461,12 @@ class _RolloutFunction(torch.autograd.Function):
                 # 1. step t's graph from x_t: rebuilt (deterministic: the forward's graph) or the kept one's lengths
                 if r.bufs is not None:
                     be.radius_graph_into(r.bufs, x_t, r.radius, r._gbatch(), r.B, r.loop)
-                    r.counter[5:6] += (r.edge_count != r.n_edges[t:t + 1]).to(torch.int32)
-                elif r.ea is not None:
+                elif r.ea is not None and r.cut is None:
                     be.edge_lengths(r.row, r.col, x_t, r.nE, r.ea)
+                if r.cut is not None:                          # the kept edges, re-selected from x_t
+                    r.cut_graph(x_t)
+                if r.bufs is not None or r.cut is not None:    # the edge count the model ran on, against the forward's
+                    r.counter[5:6] += (r.edge_count != r.n_edges[t:t + 1]).to(torch.int32)
                 # 2. step t's forward again, with its activations
                 if sc is not None:
                     feat_t[:, sc] = r.keep["speed"][t]

@@ -297,6 +297,25 @@ DISTEGNN_API int distegnn_rollout_advance_bwd(int64_t n_nodes, int F, int speed_
                                               const float *g_v_next, float *g_feat_next, float *g_pred, float *g_x,
                                               void *stream);
 
+/* ---- edge cutoff (csrc/cutoff_csr.cu; FastEGNN's cutoff_edges mode, datasets/process_dataset.py:300-305) --------------
+ * Keeps the shortest edges of every graph of a CSR graph, on the device, without a host round trip.  Candidates: the edges
+ * of the input CSR (rowptr_in [N+1], row_in / col_in [capacity]) below *n_edges_in (NULL: rowptr_in[N]), never past
+ * `capacity`; graph b's candidates are the CSR range of its nodes (data_batch int64 [N] sorted, NULL for one graph).  Per
+ * graph, k_b = floor((double)E_b * (1.0 - cutoff_rate)) in fp64 (= Python's int(E * (1 - cutoff_rate))) and the kept set
+ * is the k_b smallest candidates by (fp32 length with the fill pass's arithmetic, CSR position): a stable selection, NaN
+ * last.  Output: a sub-sequence of the candidates in CSR order (row_out / col_out [capacity]), edge_attr_out
+ * [capacity, edge_attr_nf] = the length in every column, rowptr_out [N+1] = kept candidates before rowptr_in[i].
+ * info [4] (device): [0] kept edges (the output's n_edges_dev), [1] 1 if the candidate build overflowed (count above
+ * `capacity`, or *overflow_in nonzero; overflow_in may be NULL) — the output is then not valid, but nothing past the
+ * capacity is read, [2] candidate count, [3] 0.  cutoff_rate in [0, 1].  Deterministic bit for bit, capturable. */
+DISTEGNN_API int distegnn_cutoff_csr_workspace_bytes(int64_t n_nodes, int n_graphs, int64_t capacity, int64_t *bytes_host);
+DISTEGNN_API int distegnn_cutoff_csr(int64_t n_nodes, int n_graphs, const float *pos, const int64_t *data_batch,
+                                     double cutoff_rate, int edge_attr_nf, const int32_t *rowptr_in, const int32_t *row_in,
+                                     const int32_t *col_in, const int32_t *n_edges_in, int64_t capacity,
+                                     const int32_t *overflow_in, int32_t *rowptr_out, int32_t *row_out, int32_t *col_out,
+                                     float *edge_attr_out, int32_t *info, void *workspace, int64_t workspace_bytes,
+                                     void *stream);
+
 DISTEGNN_API int distegnn_kmeans_lloyd(int64_t n_nodes, int n_clusters, const float *pos, float *centers,
                                        int32_t *labels, double *sums, int32_t *state, float tol, int iters, void *stream);
 

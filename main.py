@@ -21,11 +21,21 @@ target (constant-velocity step).  It evaluates `--eval_steps` forward passes (gr
 weighted MSE x world_size, MMD regulariser on the virtual coordinates, gradient clipping 0.3, Adam) through the
 fused forward AND backward kernels under DDP — the epoch loop, loaders, checkpoints and wandb logging of
 utils/train.py stay with the reference (out of scope).
+
+`data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
+`batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
+graph, then `data.cutoff_rate` (`--cutoff_rate` overrides it, reference main.py:133-134) drops the longest edges of
+every graph on the device (`distegnn_b200.cutoff_edges_csr`, datasets/process_dataset.py:103,300-305).  The evaluation,
+`--train_steps` and `--rollout_steps` all run on the cut graph; a rollout re-selects the kept edges every step.  Under
+torchrun with more than one rank this mode exits with a message.  In `distribute` mode `--cutoff_rate` is ignored, as
+the reference ignores it there.
 """
 from __future__ import annotations
 
 import argparse
 import os
+import re
+import sys
 import time
 
 import torch
@@ -104,8 +114,19 @@ def main():
     if args.virtual_channels is not None:
         cfg["model"]["virtual_channels"] = args.virtual_channels
 
+    # FastEGNN's cutoff_edges mode (reference README.md:30-33): the cutoff rate applies; in distribute mode it does not
+    cutoff_mode = str(cfg["data"].get("accelerate_mode", "distribute")) == "cutoff_edges"
+    rate = None
+    if cutoff_mode:
+        rate = float(args.cutoff_rate if args.cutoff_rate is not None else cfg["data"].get("cutoff_rate", 0.0))
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            if int(os.environ.get("LOCAL_RANK", "0")) == 0:
+                print("accelerate_mode=cutoff_edges (FastEGNN) is a single-device mode, as in the reference; run it "
+                      "without torchrun or with one process (use accelerate_mode=distribute for several GPUs)", flush=True)
+            sys.exit(2)
     # options of the reference CLI that belong to its data pipeline / epoch loop (out of scope here): say so, loudly
-    ignored = [n for n, v in (("--wandb", args.wandb), ("--early_stop", args.early_stop), ("--cutoff_rate", args.cutoff_rate),
+    ignored = [n for n, v in (("--wandb", args.wandb), ("--early_stop", args.early_stop),
+                              ("--cutoff_rate", None if cutoff_mode else args.cutoff_rate),
                               ("--outer_radius", args.outer_radius)) if v]
     if ignored and int(os.environ.get("LOCAL_RANK", "0")) == 0:
         print(f"WARNING: {', '.join(ignored)} accepted for CLI compatibility but NOT used: logging, early stopping and "
@@ -136,10 +157,16 @@ def main():
 
     # ---- inputs: synthetic restatement of the configured dataset, partitioned like datasets/distribute_graphs.py ----
     d = cfg["data"]
-    name = DATASET_TO_WORKLOAD.get(str(d.get("dataset_name", "fluid113k")).lower(), "fluid113k")
-    base = synth.WORKLOADS[name]
+    ds = str(d.get("dataset_name", "fluid113k")).lower()
+    name = DATASET_TO_WORKLOAD.get(ds)
+    if name is None and cutoff_mode:                           # the FastEGNN configs name sized sets: nbody_100, ...
+        name = DATASET_TO_WORKLOAD.get(re.split(r"[_\-]", ds)[0])
+    base = synth.WORKLOADS[name or "fluid113k"]
     m = cfg["model"]
-    w = synth.Workload(base.name, args.nodes or base.n_nodes, d.get("inner_radius", d.get("radius", base.radius)),
+    radius = d.get("inner_radius", d.get("radius", base.radius))
+    if cutoff_mode and radius is not None and radius < 0:     # radius: -1 = fully connected (process_dataset.py:97-98)
+        radius = None
+    w = synth.Workload(base.name, args.nodes or base.n_nodes, radius,
                        base.degree, m["node_feat_nf"], m["node_attr_nf"], m["edge_attr_nf"], m["virtual_channels"],
                        m["normalize"])
     split = d.get("split_mode", "random")
@@ -148,10 +175,15 @@ def main():
             print(f"split_mode={split!r} needs METIS/spectral partitioners of the reference's data pipeline; "
                   "using 'random' for the synthetic graph")
         split = "random"
-    part = synth.make_partitions(w, world_size=world_size, split_mode=split, seed=cfg.get("seed", 0),
-                                 only_rank=local_rank)[local_rank]
-    inp = {k: (v.to(local_rank) if v is not None else None) for k, v in part.items()}
-    n_r, e_r = inp["node_loc"].shape[0], inp["edge_index"].shape[1]
+    cut = None
+    if cutoff_mode:
+        inp, cut = cutoff_inputs(w, int(d.get("batch_size", 1)), cfg.get("seed", 0), rate, local_rank)
+        n_r, e_r = inp["node_loc"].shape[0], cut["kept"]
+    else:
+        part = synth.make_partitions(w, world_size=world_size, split_mode=split, seed=cfg.get("seed", 0),
+                                     only_rank=local_rank)[local_rank]
+        inp = {k: (v.to(local_rank) if v is not None else None) for k, v in part.items()}
+        n_r, e_r = inp["node_loc"].shape[0], inp["edge_index"].shape[1]
 
     def forward():                                             # positional call as in utils/train.py:63-71
         node_attr = inp["node_attr"] if m["node_attr_nf"] > 0 else None
@@ -182,15 +214,38 @@ def main():
               f"edges(sum over partitions)={int(cnt[1])}  forward {dt * 1e3:.3f} ms  "
               f"{1.0 / dt:.2f} graph-steps/s  {cnt[1].item() / dt / 1e6:.1f} M edges/s  "
               f"mean squared displacement {se.item() / (3 * cnt[0].item()):.4e}  virtual_loc {tuple(X.shape)}")
+    if cut is not None and local_rank == 0:
+        print(f"[{w.name}] cutoff_edges: cutoff_rate={rate} kept {cut['kept']} of {cut['candidates']} candidate edges "
+              f"({cut['graphs']} graphs)")
     if args.rollout_steps > 0:
-        rollout_steps(args, model, inp, w, world_size, local_rank, distributed)
+        rollout_steps(args, model, inp, w, world_size, local_rank, distributed, cut)
     if args.train_steps > 0:
-        train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed)
+        train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed, cut)
     if distributed:
         dist.destroy_process_group()
 
 
-def rollout_steps(args, model, inp, w, world_size, local_rank, distributed):
+def cutoff_inputs(w, batch_size, seed, rate, device):
+    """`batch_size` synthetic graphs of the workload in one batch, their candidate graph as CSR, and its cut: FastEGNN's
+    cutoff_edges data (datasets/process_dataset.py:96-104, one cut per graph).  Returns (forward inputs, cut info)."""
+    from distegnn_b200 import cutoff_edges_csr
+    from distegnn_b200.shards import CSRGraph
+    parts = [synth.make_partitions(w, seed=seed + b)[0] for b in range(batch_size)]
+    cat = lambda k: None if parts[0][k] is None else torch.cat([p[k] for p in parts]).to(device)
+    n = [int(p["node_loc"].shape[0]) for p in parts]
+    off = [sum(n[:b]) for b in range(batch_size)]
+    ei = torch.cat([p["edge_index"] + off[b] for b, p in enumerate(parts)], 1).to(device)
+    batch = torch.arange(batch_size, device=device).repeat_interleave(torch.tensor(n, device=device))
+    inp = dict(node_feat=cat("node_feat"), node_loc=cat("node_loc"), node_vel=cat("node_vel"), node_attr=cat("node_attr"),
+               loc_mean=torch.stack([p["node_loc"].mean(0) for p in parts]).to(device), data_batch=batch)
+    cand, _ = CSRGraph.from_edge_index(ei, sum(n))
+    g, ea = cutoff_edges_csr(cand, inp["node_loc"], rate, batch, batch_size, w.edge_attr_nf)
+    inp["edge_index"], inp["edge_attr"] = g, ea
+    return inp, dict(candidates=cand.num_edges, kept=g.num_edges, graphs=batch_size, graph=cand, rate=rate,
+                     node_counts=n)
+
+
+def rollout_steps(args, model, inp, w, world_size, local_rank, distributed, cut=None):
     """K steps of `distegnn_b200.rollout` from the partition's state (radius graph rebuilt every step, or the fully
     connected graph kept when the dataset has no radius); ms/step from a host clock around a device synchronise, after
     one untimed rollout that also fixes the edge capacity."""
@@ -198,8 +253,12 @@ def rollout_steps(args, model, inp, w, world_size, local_rank, distributed):
     from distegnn_b200.shards import CSRGraph
     node = {k: inp[k] for k in ("node_feat", "node_loc", "node_vel", "loc_mean", "data_batch")}
     node["node_attr"] = inp["node_attr"] if w.node_attr_nf > 0 else None
-    kw = dict(radius=w.radius) if w.radius is not None else \
-        dict(graph=CSRGraph.from_edge_index(inp["edge_index"], inp["node_loc"].shape[0])[0])
+    if cut is not None:                                        # the candidates; each step keeps its shortest edges
+        kw = dict(radius=w.radius) if w.radius is not None else dict(graph=cut["graph"])
+        kw["cutoff_rate"] = cut["rate"]
+    else:
+        kw = dict(radius=w.radius) if w.radius is not None else \
+            dict(graph=CSRGraph.from_edge_index(inp["edge_index"], inp["node_loc"].shape[0])[0])
     K = args.rollout_steps
     # the synthetic features stand for the datasets' (|v|, ...) columns: column 0 is the speed, one frame per step
     kw.update(speed_col=0, tau=1.0)
@@ -221,7 +280,7 @@ def rollout_steps(args, model, inp, w, world_size, local_rank, distributed):
               f"{edges.item():.0f} edges/step (sum over partitions), capacity {res.capacity}")
 
 
-def train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed):
+def train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed, cut=None):
     """utils/train.py:98-158 on one (partitioned) synthetic graph: loss = n_r/Σn · MSE_r · world_size (DDP averages the
     gradients, the reference wants their sum) + MMD between the virtual coordinates and sampled target positions."""
     tc = cfg.get("train", {}) or {}
@@ -236,6 +295,8 @@ def train_steps(args, cfg, model, inp, forward, world_size, local_rank, distribu
     from distegnn_b200 import train_loss
     inner = model.module if distributed else model
     n_nodes = [int(target.shape[0])]                           # batch_size 1: one graph per rank
+    if cut is not None:                                        # cutoff_edges: batch_size graphs in one batch
+        n_nodes = cut["node_counts"]
 
     t_step = []
     for step in range(args.train_steps):
