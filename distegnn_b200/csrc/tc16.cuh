@@ -210,109 +210,6 @@ __device__ __forceinline__ void split16p(const f32x2 (&v)[8], float s, uint32_t 
         mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[j])));
     }
 }
-// Same contract as encode_row_s, for producers f(chunk, v[8 pairs], first_pass, flavour tag, qmax) that run their
-// SiLUs through silu4p<flavour>(…, qmax).  The hot pass uses the batched-reciprocal flavour; if its range guard
-// fires (or a row leaves the fp16 range) the warp redoes the row with the per-element flavour.  The first cold
-// pass is told first_pass = true again so that side effects (rows copied to shared memory) are rewritten with
-// valid values — producers must keep those side effects idempotent.
-template <class F>
-__device__ __forceinline__ float encode_row2_s(F&& f, uint32_t ta_hi, uint32_t ta_lo, float s_in) {
-    __half2 mx = __floats2half2_rn(0.f, 0.f);
-    float qmax = 0.f;
-    const bool pre_scaled = __any_sync(FULL, s_in != 1.0f);
-    if (!pre_scaled) {
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            f32x2 v[8];
-            uint32_t hi[8], lo[8];
-            f(c, v, true, kFast, qmax);
-            split16p<false>(v, 1.0f, hi, lo, mx);
-            tmma::tm_st8(ta_hi + 8 * c, hi);
-            tmma::tm_st8(ta_lo + 8 * c, lo);
-        }
-        if (!__any_sync(FULL, row_overflow(mx) || silu_q_overflow(qmax))) return 1.0f;
-    }
-    float fm = 0.f, sc, inv_unused;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-        f32x2 v[8];
-        f(c, v, true, kSafe, qmax);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            float v0, v1;
-            upk2(v[j], v0, v1);
-            fm = fmaxf(fm, fmaxf(fabsf(v0), fabsf(v1)));
-        }
-    }
-    range_scale(fm, sc, inv_unused);
-    sc = fminf(sc, s_in);
-    tmma::tm_st_fence();
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-        f32x2 v[8];
-        uint32_t hi[8], lo[8];
-        f(c, v, false, kSafe, qmax);
-        split16p<true>(v, sc, hi, lo, mx);
-        tmma::tm_st8(ta_hi + 8 * c, hi);
-        tmma::tm_st8(ta_lo + 8 * c, lo);
-    }
-    return sc;
-}
-// Same contract for stages whose input is a 64-column fp32 accumulator in tile memory at `t_src` (lane offset included):
-// the producer is f(chunk, d[16 raw accumulator words], v[8 pairs], first_pass, flavour tag, qmax).
-template <class F>
-__device__ __forceinline__ float encode_row2_tm(F&& f, uint32_t t_src, uint32_t ta_hi, uint32_t ta_lo) {
-    __half2 mx = __floats2half2_rn(0.f, 0.f);
-    float qmax = 0.f;
-    {
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            f32x2 v[8];
-            uint32_t hi[8], lo[8], d[16];
-            tmma::tm_ld16(t_src + 16 * c, d);
-            f(c, d, v, true, kFast, qmax);
-            split16p<false>(v, 1.0f, hi, lo, mx);
-            tmma::tm_st8(ta_hi + 8 * c, hi);
-            tmma::tm_st8(ta_lo + 8 * c, lo);
-        }
-        if (!__any_sync(FULL, row_overflow(mx) || silu_q_overflow(qmax))) return 1.0f;
-    }
-    float fm = 0.f, sc, inv_unused;                 // cold: per-row range rescue / per-element SiLU flavour
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-        f32x2 v[8];
-        uint32_t d[16];
-        tmma::tm_ld16(t_src + 16 * c, d);
-        f(c, d, v, true, kSafe, qmax);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            float v0, v1;
-            upk2(v[j], v0, v1);
-            fm = fmaxf(fm, fmaxf(fabsf(v0), fabsf(v1)));
-        }
-    }
-    range_scale(fm, sc, inv_unused);
-    sc = fminf(sc, 1.0f);
-    tmma::tm_st_fence();
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-        f32x2 v[8];
-        uint32_t hi[8], lo[8], d[16];
-        tmma::tm_ld16(t_src + 16 * c, d);
-        f(c, d, v, false, kSafe, qmax);
-        split16p<true>(v, sc, hi, lo, mx);
-        tmma::tm_st8(ta_hi + 8 * c, hi);
-        tmma::tm_st8(ta_lo + 8 * c, lo);
-    }
-    return sc == 1.0f ? 1.0f : 1.0f / sc;
-}
-
-template <class F>
-__device__ __forceinline__ float encode_row2(F&& f, uint32_t ta_hi, uint32_t ta_lo) {
-    const float sc = encode_row2_s(f, ta_hi, ta_lo, 1.0f);
-    return sc == 1.0f ? 1.0f : 1.0f / sc;
-}
-
 // Convenience: unscaled input, returns 1/scale for the epilogue.
 template <class F>
 __device__ __forceinline__ float encode_row(F&& f, uint32_t ta_hi, uint32_t ta_lo) {

@@ -1,19 +1,28 @@
-// Real<->virtual stage on the tensor cores — production kernel behind distegnn_virtual_layer_fwd (thread per row).
+// Real<->virtual stage on the tensor cores — production kernel behind distegnn_virtual_layer_fwd.
 // Replaces reference models/FastEGNN.py:252-253 (virtual geometry), 154-163 (edge_mode_virtual), 180, 191-193,
 // 207, 220-223 (virtual halves of coord_model_vel / coord_model_virtual / node_model / node_model_virtual) and
 // the global_mean_pool scatters at :193,:222.  Same math/outputs as testing/virtual_layer.cu (fp32-FMA twin).
 //
-// Rows of a tile are (node, channel) pairs: TN = 128 / C nodes per tile, row = n_local*C + c, one tile-memory row per
-// tile row.  One CTA per SM, 128 threads = 1 tile group = 1 warpgroup; thread r owns row r.
-// All three 64x64 layers run as wgmma tile GEMMs with the fp16 2-term split (tc16.cuh); tile memory per group
-// (tile_mma.cuh): A_hi 32 + A_lo 32 + D 64 columns (the two coordinate heads reuse D one after the other).
-//   stage 1  a1 = SiLU(Hn[node] + G[graph,c] + w_r·‖ΔX‖)  -> A              MMA 1: D = a1·W2vᵀ
-//            (the C x 64 G rows of the group's current graph are cached in shared memory: every (node, channel) row re-reads
-//             its G row, and shared memory leaves little L1)
-//   stage 2  mv = SiLU(D + b2v) -> shared tile + A                            MMA 2: D = mv·Wxvᵀ
-//            (then: agg_v[node] = mean_c mv, per-graph Σ_i mv accumulated in shared memory)
-//   stage 3a φ_xv = w3xv·SiLU(D + bxv)                                        MMA 3: D = mv·WXᵀ
-//   stage 3b φ_X  = w3x·SiLU(D + bx);  trans_v[node] = mean_c(−ΔX·φ_xv);  per-graph Σ_i ΔX·φ_X accumulated.
+// Rows of a tile are (node, channel) pairs: TN = 64 / C whole nodes per 64-row tile, row = n_local·C + c; rows past TN·C
+// (and past the last node) are padding and contribute nothing.  One CTA per SM, VW_WG warpgroups, each an independent
+// pipeline: a warpgroup grid-strides over its own tiles and, once set up, shares no barrier with the other warpgroups.
+// Warp w of a warpgroup owns rows 16w .. 16w+15 of its tile, which are exactly the rows of the m64n64 accumulator fragment
+// it holds (tile_mma.cuh); thread (g = lane/4, q = lane%4) owns rows g and g+8 of the warp, columns 8j + 2q + {0,1}.
+// The A operands and the accumulators stay in registers; the weights, the G rows of the warpgroup's current graph and the
+// fp32 mv rows (for the pools) are in shared memory.  Per tile (numerics as in the edge kernel: fp16 2-term split,
+// per-row power-of-two range rescue, one reciprocal per four SiLUs with a stage-level guard, cold paths per warp):
+//   stage 1  a1 = SiLU(Hn[node] + G[graph,c] + w_r·‖ΔX‖) -> fp16 hi/lo A fragments                 MMA 1: D = a1·W2vᵀ
+//   stage 2  mv = SiLU(D + b2v) -> fp32 staging rows + hi/lo A fragments (kept for both heads)        MMA 2: D = mv·Wxvᵀ
+//            while MMA 2 runs: agg_v[node] = mean_c mv, Σ_i mv per graph (lane <-> column pair)
+//   stage 3a φ_xv = w3xv·SiLU(D + bxv) per row (quad shuffles)                                        MMA 3: D = mv·WXᵀ
+//            while MMA 3 runs: trans_v[node] = mean_c(−ΔX·φ_xv)
+//   stage 3b φ_X = w3x·SiLU(D + bx) per row; Σ_i ΔX·φ_X per graph.
+// For C in {1, 2, 4, 8, 16} a node never straddles two warps and the pools are warp-local; for other C they read rows of
+// the other warps of the group behind a warpgroup barrier.  Per-graph sums are kept per warp in shared memory and flushed
+// to vsum (per warpgroup, one atomic per element) when the group's graph changes and at the end; tiles that straddle
+// graphs add their rows to vsum directly.  The next tile's Hn rows, coordinates and graph ids are prefetched towards L1.
+// Stages 2 and 3 run in the "t domain" (common.cuh silu4t): −log2(e) is folded into W2v and the biases, −ln 2 into the
+// head projections and the mv pools.
 #include "common.cuh"
 #include "tc16.cuh"
 #include "tile_mma.cuh"
@@ -36,64 +45,65 @@ struct VirtT16Args {
     float* agg_v;
     float* trans_v;
     float* vsum;
-    int g_smem;     // the launch reserved V16_GROUPS * C * 68 floats behind V16_SMEM_BYTES for the G rows of the current graph
 };
 
-constexpr int V16_THREADS = 128, V16_GROUPS = 1, V16_GROUP = 128;
-constexpr int V16_TM_COLS = 128;                  // per tile group: A_hi 32 | A_lo 32 | D 64
-constexpr int V16_ROW = 68;
-constexpr int V16_MAXC = DISTEGNN_MAX_CHANNELS;
-constexpr int V16_W = 4096;
-constexpr int V16_SMEM_BYTES = tmma::tm_bytes(V16_GROUPS * V16_TM_COLS)
-                               + 6 * V16_W * 2                         // W2v, Wxv, WX (hi+lo)
-                               + V16_GROUPS * TILE_M * V16_ROW * 4     // mv tile per group
-                               + V16_GROUPS * V16_MAXC * H * 4         // Σ mv accumulators per group
-                               + V16_GROUPS * 4 * V16_MAXC * 4         // Σ ΔX·φ_X accumulators per group
-                               + 6 * H * 4                             // w1r, b2v, bxv, w3xv, bx, w3x
-                               + V16_GROUPS * TILE_M * 4 * 4           // ΔX per row
-                               + V16_GROUPS * 2 * TILE_M * 4           // φ_xv, φ_X per row
-                               + V16_GROUPS * TILE_M * 4               // graph id per local node
-                               // + (launch time, if it fits) V16_GROUPS * C * V16_ROW * 4: G rows of the current graph
-                               + 128;
-constexpr uint32_t V16_LBO = 1024;
+// 4 warpgroups = 16 warps per SM
+constexpr int VW_WG = 4;
+constexpr int VW_THREADS = 128 * VW_WG, VW_WARPS = VW_THREADS / 32;
+constexpr int VW_TILE = 64;                    // rows per warpgroup tile
+// row pitch (floats) of the mv staging rows and the cached G rows: 72 = conflict-free LDS.64 / STS.64 in the accumulator
+// fragment pattern (rows g, columns 2q: banks 8g + 2q) and in the pools' row pattern
+constexpr int VW_ROW = 72;
+constexpr int VW_W = 64 * 64;                  // fp16 elements per weight matrix (8 KB)
+constexpr uint32_t VW_LBO = 1024;              // fp16 K-major no-swizzle, N = 64
+// shared memory (floats) for C channels: weights | w1r, b2v, bxv, w3xv, bx, w3x | mv rows per warp | ΔX, φ_xv, φ_X per
+// row and group | G rows of the current graph per group | Σ mv [C][64] per warp | Σ ΔX·φ_X [3][C] per warp (pitch 4C)
+__host__ __device__ constexpr int vw_smem_floats(int C) {
+    return 6 * VW_W / 2 + 6 * H + VW_WARPS * 16 * VW_ROW + VW_WG * VW_TILE * 6 + VW_WG * C * VW_ROW + VW_WARPS * C * H
+           + VW_WARPS * 4 * C;
+}
+__host__ __device__ constexpr int vw_smem_bytes(int C) { return vw_smem_floats(C) * 4; }
+using tc16::kFast;
+using tc16::kSafe;
 
-__global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const VirtT16Args a) {
+__global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const VirtT16Args a) {
     using namespace tmma;
-    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(V16_GROUPS * V16_TM_COLS);
-    __half* W2hi = reinterpret_cast<__half*>(smem_raw);
-    __half* W2lo = W2hi + V16_W;
-    __half* Wxvhi = W2lo + V16_W;
-    __half* Wxvlo = Wxvhi + V16_W;
-    __half* Wxhi = Wxvlo + V16_W;
-    __half* Wxlo = Wxhi + V16_W;
-    float* tiles = reinterpret_cast<float*>(Wxlo + V16_W);
-    float* accH_all = tiles + V16_GROUPS * TILE_M * V16_ROW;
-    float* accX_all = accH_all + V16_GROUPS * V16_MAXC * H;
-    float* w1rs = accX_all + V16_GROUPS * 4 * V16_MAXC;
+    const int C = a.C;
+    __half* W2hi = reinterpret_cast<__half*>(degnn_dyn_smem);
+    __half* W2lo = W2hi + VW_W;
+    __half* Wxvhi = W2lo + VW_W;
+    __half* Wxvlo = Wxvhi + VW_W;
+    __half* Wxhi = Wxvlo + VW_W;
+    __half* Wxlo = Wxhi + VW_W;
+    float* w1rs = reinterpret_cast<float*>(Wxlo + VW_W);
     float* b2s = w1rs + H;
     float* bxvs = b2s + H;
     float* w3xvs = bxvs + H;
     float* bxs = w3xvs + H;
     float* w3xs = bxs + H;
-    float* dX_all = w3xs + H;
-    float* phi_all = dX_all + V16_GROUPS * TILE_M * 4;
-    int* sgraph_all = reinterpret_cast<int*>(phi_all + V16_GROUPS * 2 * TILE_M);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sgraph_all + V16_GROUPS * TILE_M);
-    float* gs_all = reinterpret_cast<float*>(degnn_dyn_smem + V16_SMEM_BYTES);      // present iff a.g_smem
+    float* stage_all = w3xs + H;                                   // [warps][16][VW_ROW]
+    float* dX_all = stage_all + VW_WARPS * 16 * VW_ROW;            // [groups][64][4]
+    float* phi_all = dX_all + VW_WG * VW_TILE * 4;                 // [groups][2][64]: φ_xv, φ_X
+    float* gs_all = phi_all + VW_WG * VW_TILE * 2;                 // [groups][C][VW_ROW]
+    float* accH_all = gs_all + VW_WG * C * VW_ROW;                 // [warps][C][64]
+    float* accX_all = accH_all + VW_WARPS * C * H;                 // [warps][4C]: [3][C] used
 
     const int tid = threadIdx.x;
-    const int grp = tid / V16_GROUP, t = tid % V16_GROUP, wq = (tid >> 5) & 3;
-    const int C = a.C;
+    const int lane = tid & 31;
+    const int warp = tid >> 5;
+    const int wg = warp >> 2;              // warpgroup
+    const int w = warp & 3;                // warp inside the warpgroup: rows 16w .. 16w+15 of its tile
+    const int t = tid & 127;               // thread inside the warpgroup
+    const int g = lane >> 2, q = lane & 3; // fragment rows g, g+8 of the warp; columns 8j + 2q
     const int K = 4 + 3 * C + H * C;
     const bool need_feat = !(a.flags & DISTEGNN_FLAG_LAST);
-    const int TN = TILE_M / C;
-    const bool pow2C = (C & (C - 1)) == 0 && C <= 32;
-    const int lane = tid & 31;
+    const int TN = VW_TILE / C;
+    const bool warp_local = (16 % C) == 0;   // nodes never straddle warps: the pools need no warpgroup barrier
 
-    // ---- one-time setup ---------------------------------------------------------------------------
-    tc16::stage_weight<V16_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, SILU_T_IN);   // t2 = SILU_T_IN·(a1·W2vᵀ + b2v); mv' = SILU_T_IN·mv
-    tc16::stage_weight<V16_THREADS>(Wxvhi, Wxvlo, a.wxv, 0, 64, tid);
-    tc16::stage_weight<V16_THREADS>(Wxhi, Wxlo, a.wx, 0, 64, tid);
+    // ---- one-time setup -------------------------------------------------------------------------
+    tc16::stage_weight<VW_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, SILU_T_IN);   // t2 = SILU_T_IN·(a1·W2vᵀ + b2v); mv' = SILU_T_IN·mv
+    tc16::stage_weight<VW_THREADS>(Wxvhi, Wxvlo, a.wxv, 0, 64, tid);
+    tc16::stage_weight<VW_THREADS>(Wxhi, Wxlo, a.wx, 0, 64, tid);
     if (tid < H) {
         w1rs[tid] = a.w1r[tid];
         b2s[tid] = a.b2[tid] * SILU_T_IN;
@@ -102,285 +112,376 @@ __global__ void __launch_bounds__(V16_THREADS, 1) virtual_layer_t16_kernel(const
         bxs[tid] = a.bx[tid] * SILU_T_IN;
         w3xs[tid] = a.w3x[tid] * SILU_T_OUT;
     }
-    for (int i = tid; i < V16_GROUPS * (V16_MAXC * H + 4 * V16_MAXC); i += V16_THREADS) accH_all[i] = 0.f;
-    if (tid == 0) {
-        for (int i = 0; i < V16_GROUPS; ++i) mbar_init(&bars[i], 1);
-        fence_mbar_init();
-    }
+    for (int i = tid; i < VW_WARPS * (C * H + 4 * C); i += VW_THREADS) accH_all[i] = 0.f;   // accH and accX
     fence_proxy_async_smem();
     __syncthreads();
 
-    const uint32_t lane_off = ((uint32_t)(32 * wq)) << 16;
-    const uint32_t col0 = (uint32_t)(grp * V16_TM_COLS);
-    const uint32_t tA_hi = col0, tA_lo = col0 + 32, tD = col0 + 64;
-    auto desc = [&](const __half* p) { return make_b_desc(smem_u32(p), V16_LBO, 128); };
-    const uint64_t dW2hi = desc(W2hi), dW2lo = desc(W2lo), dWxvhi = desc(Wxvhi), dWxvlo = desc(Wxvlo),
-                   dWxhi = desc(Wxhi), dWxlo = desc(Wxlo);
-    float* tile_s = tiles + grp * TILE_M * V16_ROW;
-    float* myrow = tile_s + t * V16_ROW;
-    float* accH = accH_all + grp * V16_MAXC * H;
-    float* accX = accX_all + grp * 4 * V16_MAXC;
-    float* dXs = dX_all + grp * TILE_M * 4;
-    float* phis = phi_all + grp * 2 * TILE_M;
-    int* sgraph = sgraph_all + grp * TILE_M;
-    float* gs = gs_all + grp * a.C * V16_ROW;          // [C][68]: pitch 68 keeps the channel rows of a node on distinct banks
-    const bool g_smem = a.g_smem;
-    uint64_t* hbar = bars + grp;                  // Hn block landed (fetch_hn)
-    const uint32_t bar_id = 1 + grp;
-    int cur_graph = -1;
+    // descriptor of weight matrix k (W2v hi, lo, Wxv hi, lo, WX hi, lo): the matrices are 8 KB apart, and the start-address
+    // field (bits 0..13, address >> 4) of the first one has room for all six
+    const uint64_t bW0 = make_b_desc(smem_u32(W2hi), VW_LBO, 128);
+    auto bW = [&](int k) { return bW0 + (uint64_t)(k * (VW_W * 2 / 16)); };
+    float* tile_s = stage_all + wg * VW_TILE * VW_ROW;            // the group's 64 mv rows (warp w: rows 16w ..)
+    float* dXs = dX_all + wg * VW_TILE * 4;
+    float* phis = phi_all + wg * VW_TILE * 2;
+    float* gs = gs_all + wg * C * VW_ROW;
+    float* accH = accH_all + warp * C * H;
+    float* accX = accX_all + warp * 4 * C;
+    float* accH_g = accH_all + 4 * wg * C * H;                    // the four warps' sums of the group
+    float* accX_g = accX_all + 4 * wg * 4 * C;
+    const uint32_t bar_id = 1 + wg;
+    int cur_graph = -1;                                           // graph of the G cache and the per-warp sums (group-uniform)
 
-    auto flush = [&](int g) {                      // all threads of the group
-        if (g >= 0) {
-            float* dst = a.vsum + (size_t)g * K;
-            if (need_feat)
-                for (int i = t; i < C * H; i += V16_GROUP) {
-                    atomicAdd(dst + 4 + 3 * C + i, accH[i] * SILU_T_OUT);
-                    accH[i] = 0.f;
+    // the group's per-warp sums of graph gr -> vsum, one atomic per element; all threads of the group, behind a group barrier
+    auto flush = [&](int gr) {
+        if (gr < 0) return;
+        float* dst = a.vsum + (size_t)gr * K;
+        if (need_feat)
+            for (int i = t; i < C * H; i += 128) {
+                float s = 0.f;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    s += accH_g[k * C * H + i];
+                    accH_g[k * C * H + i] = 0.f;
                 }
-            if (t < 3 * C) {
-                atomicAdd(dst + 4 + t, accX[t]);
-                accX[t] = 0.f;
+                atomicAdd(dst + 4 + 3 * C + i, s * SILU_T_OUT);
             }
+        if (t < 3 * C) {
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                s += accX_g[k * 4 * C + t];
+                accX_g[k * 4 * C + t] = 0.f;
+            }
+            atomicAdd(dst + 4 + t, s);
         }
     };
-    auto a_ready = [&]() {
-        tm_st_fence();
-        named_bar(bar_id, V16_GROUP);
-    };
-    // D = A·Wᵀ over the whole tile by the group's warpgroup; mma_done() publishes D to every row thread
-    auto issue = [&](uint64_t bhi, uint64_t blo) { tc16::mma_f16x3<V16_LBO>(tD, tA_hi, tA_lo, bhi, blo, 1, false, 0, 2); };
-    auto mma_done = [&]() { named_bar(bar_id, V16_GROUP); };
 
-    const int64_t num_tiles = (a.N + TN - 1) / TN;
-    const int64_t tstride = (int64_t)gridDim.x * V16_GROUPS;
-    // Hn rows n0 .. n0+nvalid-1 of tile `tl` -> the start of the group's mv tile at the padded pitch V16_ROW (the channel rows
-    // of 4 different nodes that a warp reads together then sit on different banks): one 256-byte bulk copy per node, issued by
-    // the first `nvalid` threads of the group; thread 0 posts the byte count.
-    // Not called: stage 1 reads Hn with LDG behind an L1 prefetch.  Deleting even this unused lambda changes the kernel's
-    // SASS, so it goes together with the Hn mbarrier init above in a change that is benchmarked on its own.
-    [[maybe_unused]] auto fetch_hn = [&](int64_t tl) {
-        if (tl < num_tiles) {
-            const int64_t m0 = tl * TN;
-            const int nv = (int)min((int64_t)TN, a.N - m0);
-            if (t == 0) mbar_expect_tx(hbar, (uint32_t)nv * (H * 4));     // may land after the first bytes: the count just dips below 0
-            if (t < nv) bulk_g2s(tile_s + t * V16_ROW, a.Hn + (size_t)(m0 + t) * H, H * 4, hbar);
-        }
-    };
-    for (int64_t tile = (int64_t)blockIdx.x * V16_GROUPS + grp; tile < num_tiles; tile += tstride) {
-        const int64_t n0 = tile * TN;
+    const int num_tiles = (int)((a.N + TN - 1) / TN);            // < 2^31 (the launch checks)
+    const int stride = (int)gridDim.x * VW_WG;
+    const int ra = 16 * w + g, rb = ra + 8;            // the thread's tile rows
+    const float* colp = tile_s + 2 * lane;             // pools: lane <-> columns 2·lane, 2·lane + 1
+
+    for (int tile = (int)blockIdx.x * VW_WG + wg; tile < num_tiles; tile += stride) {
+        const int64_t n0 = (int64_t)tile * TN;
         const int nvalid = (int)min((int64_t)TN, a.N - n0);
         const int rows = nvalid * C;
-        {   // pull the next tile's small inputs (x4, graph ids) into L1 while this one computes
-            const int64_t nn0 = (tile + tstride) * TN;
+        {   // pull the next tile's inputs (Hn rows, x4, graph ids) into L1 while this one computes
+            const int64_t nn0 = (int64_t)(tile + stride) * TN;
             const int nnv = (int)min((int64_t)TN, a.N - nn0);
-            for (int i = t; i < 2 * nnv; i += V16_GROUP) prefetch_l1(a.Hn + (size_t)nn0 * H + 32 * i);
+            for (int i = t; i < 2 * nnv; i += 128) prefetch_l1(a.Hn + (size_t)nn0 * H + 32 * i);
             if (nnv > 0) {
                 if (t < (nnv * 16 + 127) / 128) prefetch_l1(a.x4 + (size_t)nn0 * 4 + 32 * t);
                 if (t == 127) prefetch_l1(a.batch + nn0);
                 if (t == 126) prefetch_l1(a.batch + nn0 + nnv - 1);
             }
         }
-        if (t < TN) sgraph[t] = (t < nvalid) ? __ldg(a.batch + n0 + t) : -1;
-        named_bar(bar_id, V16_GROUP);
-        const int g_first = sgraph[0], g_last = sgraph[nvalid - 1];
+        const int g_first = __ldg(a.batch + n0), g_last = __ldg(a.batch + n0 + nvalid - 1);
         const bool single = (g_first == g_last);
-        if (single && g_first != cur_graph) {
+        if (single && g_first != cur_graph) {          // group-uniform; rare: once per graph and group
+            named_bar(bar_id, 128);                    // every warp is done with the cache and its sums
             flush(cur_graph);
             cur_graph = g_first;
-            if (g_smem)
-                for (int i = t; i < C * (H / 4); i += V16_GROUP) {       // G[g_first] -> shared (rare: once per graph and group)
-                    const int c = i / (H / 4), q = i - c * (H / 4);
-                    *reinterpret_cast<float4*>(gs + c * V16_ROW + 4 * q) = ldg4(a.G + ((size_t)g_first * C + c) * H + 4 * q);
-                }
-            named_bar(bar_id, V16_GROUP);
+            for (int i = t; i < C * (H / 4); i += 128) {
+                const int c = i / (H / 4), q4 = i - c * (H / 4);
+                *reinterpret_cast<float4*>(gs + c * VW_ROW + 4 * q4) = ldg4(a.G + ((size_t)g_first * C + c) * H + 4 * q4);
+            }
+            named_bar(bar_id, 128);
         }
 
-        // ---- stage 1 ------------------------------------------------------------------------------
-        const bool rvalid = t < rows;
-        const int nl = rvalid ? t / C : 0;
-        const int ch = rvalid ? t - nl * C : 0;
-        const int g = rvalid ? sgraph[nl] : g_first;
-        const size_t node = (size_t)(n0 + nl);
-        float vr;
+        // ---- stage 1: a1 = SiLU(Hn + G + w_r·‖ΔX‖) for rows ra, rb -> fp16 hi/lo A fragments -----------------------
+        const bool va = ra < rows, vb = rb < rows;
+        const float* pa;
+        const float* pb;
+        const float* ga;
+        const float* gb;
+        float vra, vrb;
         {
-            const float4 xi = ldg4(a.x4 + node * 4);
-            const float* Xg = a.Xv + (size_t)g * 3 * C;
-            const float dx = __ldg(Xg + ch) - xi.x, dy = __ldg(Xg + C + ch) - xi.y, dz = __ldg(Xg + 2 * C + ch) - xi.z;
-            vr = sqrtf(dx * dx + dy * dy + dz * dz);
-            *reinterpret_cast<float4*>(dXs + 4 * t) = make_float4(dx, dy, dz, 0.f);
+            auto row_geo = [&](int r, bool v, const float*& hrow, const float*& grow) {
+                const int nl = v ? r / C : 0, ch = v ? r - nl * C : 0;
+                const size_t node = (size_t)(n0 + nl);
+                const int gr = single ? g_first : __ldg(a.batch + node);
+                const float4 xi = ldg4(a.x4 + node * 4);
+                const float* Xg = a.Xv + (size_t)gr * 3 * C;
+                const float dx = __ldg(Xg + ch) - xi.x, dy = __ldg(Xg + C + ch) - xi.y, dz = __ldg(Xg + 2 * C + ch) - xi.z;
+                if (q == 0) *reinterpret_cast<float4*>(dXs + 4 * r) = make_float4(dx, dy, dz, 0.f);
+                hrow = a.Hn + node * H + 2 * q;
+                // rows of the cached graph read shared memory, the others (tiles that straddle graphs) global memory
+                grow = (gr == cur_graph ? (const float*)(gs + ch * VW_ROW) : a.G + ((size_t)gr * C + ch) * H) + 2 * q;
+                return sqrtf(dx * dx + dy * dy + dz * dz);
+            };
+            vra = row_geo(ra, va, pa, ga);
+            vrb = row_geo(rb, vb, pb, gb);
         }
-        const float* hrow = a.Hn + node * H;
-        // rows of the cached graph read shared memory, the others (tiles that straddle graphs) global memory: generic loads
-        const float* grow = (g_smem && g == cur_graph) ? (const float*)(gs + ch * V16_ROW) : a.G + ((size_t)g * C + ch) * H;
-        const f32x2 vr2 = bc2(vr);
-        const float inv1 = tc16::encode_row2(
-            [&](int c, f32x2 (&v)[8], bool, auto safe, float& qmax) {
+        auto pre = [&](int j, const float* hrow, const float* grow, float vr) {
+            const f32x2 hh = __ldg(reinterpret_cast<const f32x2*>(hrow + 8 * j));
+            const f32x2 gg = *reinterpret_cast<const f32x2*>(grow + 8 * j);
+            return fma2(bc2(vr), *reinterpret_cast<const f32x2*>(w1rs + 8 * j + 2 * q), add2(hh, gg));
+        };
+        // register i = 2j + r of a fragment array <-> row g + 8r, columns 8j + 2q + {0,1} (= accumulator pair d[2i], d[2i+1])
+        uint32_t ahi[16], alo[16];
+        float inv1a = 1.0f, inv1b = 1.0f;  // 1 / the rows' range scales
+        {
+            __half2 mx = __floats2half2_rn(0.f, 0.f);
+            float qmax = 0.f;
 #pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                    const int cc = 16 * c + 4 * j4;
-                    const ulonglong2 hh = __ldg(reinterpret_cast<const ulonglong2*>(hrow + cc));
-                    const ulonglong2 gg = *reinterpret_cast<const ulonglong2*>(grow + cc);
-                    const ulonglong2 wr = *reinterpret_cast<const ulonglong2*>(w1rs + cc);
-                    f32x2 p0 = fma2(vr2, wr.x, add2(hh.x, gg.x)), p1 = fma2(vr2, wr.y, add2(hh.y, gg.y));
-                    silu4p<decltype(safe)::value>(p0, p1, qmax);
-                    if (!rvalid) p0 = p1 = 0ull;
-                    v[2 * j4] = p0;
-                    v[2 * j4 + 1] = p1;
+            for (int j = 0; j < 8; ++j) {
+                f32x2 xa = pre(j, pa, ga, vra), xb = pre(j, pb, gb, vrb);
+                silu4p<false>(xa, xb, qmax);
+                if (!va) xa = 0ull;
+                if (!vb) xb = 0ull;
+                tc16::split_pair(xa, ahi[2 * j], alo[2 * j]);
+                tc16::split_pair(xb, ahi[2 * j + 1], alo[2 * j + 1]);
+                // SiLU outputs are bounded below (−0.28): only the positive side can leave the fp16 range
+                mx = __hmax2(mx, __hmax2(*reinterpret_cast<const __half2*>(&ahi[2 * j]),
+                                         *reinterpret_cast<const __half2*>(&ahi[2 * j + 1])));
+            }
+            if (__any_sync(FULL, tc16::row_overflow(mx) || silu_q_overflow(qmax))) {
+                // cold: some row leaves the fp16 range, or the SiLU batch guard fired — per-element SiLU, row scales
+                float fa = 0.f, fb = 0.f, sa, sb;
+#pragma unroll 1
+                for (int j = 0; j < 8; ++j) {
+                    f32x2 xa = pre(j, pa, ga, vra), xb = pre(j, pb, gb, vrb);
+                    silu4p<true>(xa, xb, qmax);
+                    float v0, v1;
+                    upk2(xa, v0, v1);
+                    if (va) fa = fmaxf(fa, fmaxf(v0, v1));
+                    upk2(xb, v0, v1);
+                    if (vb) fb = fmaxf(fb, fmaxf(v0, v1));
                 }
-            },
-            lane_off + tA_hi, lane_off + tA_lo);
-        a_ready();
-        issue(dW2hi, dW2lo);
-        mma_done();
+                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 1));
+                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 2));
+                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 1));
+                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 2));
+                tc16::range_scale(fa, sa, inv1a);
+                tc16::range_scale(fb, sb, inv1b);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    f32x2 xa = pre(j, pa, ga, vra), xb = pre(j, pb, gb, vrb);
+                    silu4p<true>(xa, xb, qmax);
+                    if (!va) xa = 0ull;
+                    if (!vb) xb = 0ull;
+                    tc16::split_pair(mul2(xa, bc2(sa)), ahi[2 * j], alo[2 * j]);
+                    tc16::split_pair(mul2(xb, bc2(sb)), ahi[2 * j + 1], alo[2 * j + 1]);
+                }
+            }
+        }
 
-        // ---- stage 2: mv = SiLU(D + b2v) -> shared tile and A ---------------------------------------------
-        const float inv2 = tc16::encode_row2_tm(
-            [&](int c, const uint32_t (&d)[16], f32x2 (&v)[8], bool first, auto safe, float& qmax) {
-                const f32x2 is2 = bc2(inv1);
+        // ---- MMA 1 ----------------------------------------------------------------------------------------------
+        float d[32];
+        tc16::mma_f16x3_rA<VW_LBO>(d, ahi, alo, bW(0), bW(1));
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
+
+        // ---- stage 2: mv = SiLU(D/s + b2v) -> fp32 staging rows (pools) and fp16 hi/lo A fragments ----------------------
+        float inv2a = 1.0f, inv2b = 1.0f, s2a = 1.0f, s2b = 1.0f;     // 1 / the rows' range scales, the scales
+        auto m_pair = [&](int j, f32x2& ma, f32x2& mb) {
+            const f32x2 bb = *reinterpret_cast<const f32x2*>(b2s + 8 * j + 2 * q);
+            ma = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv1a), bb);
+            mb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv1b), bb);
+        };
+        // (ma, mb) = SILU_T_IN·mv -> the staging rows: the pools undo the factor, and MMA 3 re-splits its A operand from them
+        auto store_m = [&](int j, f32x2 ma, f32x2 mb) {
+            *reinterpret_cast<f32x2*>(tile_s + ra * VW_ROW + 8 * j + 2 * q) = ma;
+            *reinterpret_cast<f32x2*>(tile_s + rb * VW_ROW + 8 * j + 2 * q) = mb;
+        };
+        {
+            __half2 mx = __floats2half2_rn(0.f, 0.f);
+            float qmax = 0.f;
 #pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                    const int cc = 16 * c + 4 * j4;
-                    const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(b2s + cc);
-                    f32x2 m0 = fma2(pk2u(d[4 * j4 + 0], d[4 * j4 + 1]), is2, bb.x);
-                    f32x2 m1 = fma2(pk2u(d[4 * j4 + 2], d[4 * j4 + 3]), is2, bb.y);
-                    silu4t<decltype(safe)::value>(m0, m1, qmax);
-                    if (first && need_feat) *reinterpret_cast<ulonglong2*>(myrow + cc) = make_ulonglong2(m0, m1);
-                    v[2 * j4] = m0;
-                    v[2 * j4 + 1] = m1;
+            for (int j = 0; j < 8; ++j) {
+                f32x2 ma, mb;
+                m_pair(j, ma, mb);
+                silu4t<false>(ma, mb, qmax);
+                store_m(j, ma, mb);
+                tc16::split_pair(ma, ahi[2 * j], alo[2 * j]);
+                tc16::split_pair(mb, ahi[2 * j + 1], alo[2 * j + 1]);
+                // t-domain values: ≤ 0.41, unbounded below — track the minimum
+                mx = __hmin2(mx, __hmin2(*reinterpret_cast<const __half2*>(&ahi[2 * j]),
+                                         *reinterpret_cast<const __half2*>(&ahi[2 * j + 1])));
+            }
+            if (__any_sync(FULL, fminf(__low2float(mx), __high2float(mx)) < -tc16::RANGE || silu_q_overflow(qmax))) {
+                float fa = 0.f, fb = 0.f;      // cold (unrolled: d stays in registers)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    f32x2 ma, mb;
+                    m_pair(j, ma, mb);
+                    silu4t<true>(ma, mb, qmax);
+                    store_m(j, ma, mb);    // also rewrites the mv rows of the batch-guard case
+                    float v0, v1;
+                    upk2(ma, v0, v1);
+                    fa = fmaxf(fa, -fminf(v0, v1));
+                    upk2(mb, v0, v1);
+                    fb = fmaxf(fb, -fminf(v0, v1));
                 }
-            },
-            lane_off + tD, lane_off + tA_hi, lane_off + tA_lo);
-        a_ready();
-        issue(dWxvhi, dWxvlo);
-        // pools of mv (the tile in shared memory; MMA 2 wrote only D)
+                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 1));
+                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 2));
+                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 1));
+                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 2));
+                tc16::range_scale(fa, s2a, inv2a);
+                tc16::range_scale(fb, s2b, inv2b);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    f32x2 ma, mb;
+                    m_pair(j, ma, mb);
+                    silu4t<true>(ma, mb, qmax);
+                    tc16::split_pair(mul2(ma, bc2(s2a)), ahi[2 * j], alo[2 * j]);
+                    tc16::split_pair(mul2(mb, bc2(s2b)), ahi[2 * j + 1], alo[2 * j + 1]);
+                }
+            }
+        }
+
+        // the nodes whose per-node outputs (agg_v, trans_v) this warp writes: its own when nodes never straddle warps,
+        // else every fourth node of the tile (the rows of the other warps are read behind a group barrier)
+        const int nb = warp_local ? (16 * w) / C : w;
+        const int ne = warp_local ? min(nb + 16 / C, nvalid) : nvalid;
+        const int ns = warp_local ? 1 : 4;
+        const int r_end = min(16 * w + 16, rows);     // the warp's valid rows are 16w .. r_end − 1
+
+        // ---- MMA 2 (φ_xv head) overlapped with the pools of mv ------------------------------------------------------
+        tc16::mma_f16x3_rA<VW_LBO>(d, ahi, alo, bW(2), bW(3));
         if (need_feat) {
-            // thread <-> (column pair, quarter): one LDS.64 + one pair add per two elements, two chains per sum
-            const int c2 = 2 * (t & 31), q4 = t >> 5;
+            if (warp_local) __syncwarp();
+            else named_bar(bar_id, 128);
             auto ld2 = [](const float* p) { return *reinterpret_cast<const f32x2*>(p); };
-            const f32x2 invC2 = bc2(SILU_T_OUT / (float)C);     // the tile holds mv' = SILU_T_IN·mv
-            for (int n = q4; n < nvalid; n += 4) {          // mean over channels per node
-                const float* base = tile_s + (n * C) * V16_ROW + c2;
+            const f32x2 invC2 = bc2(SILU_T_OUT / (float)C);     // the rows hold mv' = SILU_T_IN·mv
+#pragma unroll 1
+            for (int n = nb; n < ne; n += ns) {                  // mean over channels per node
+                const float* base = colp + (n * C) * VW_ROW;
                 f32x2 s0 = 0ull, s1 = 0ull;
                 int c = 0;
+#pragma unroll 1
                 for (; c + 1 < C; c += 2) {
-                    s0 = add2(s0, ld2(base + c * V16_ROW));
-                    s1 = add2(s1, ld2(base + (c + 1) * V16_ROW));
+                    s0 = add2(s0, ld2(base + c * VW_ROW));
+                    s1 = add2(s1, ld2(base + (c + 1) * VW_ROW));
                 }
-                if (c < C) s0 = add2(s0, ld2(base + c * V16_ROW));
-                *reinterpret_cast<f32x2*>(a.agg_v + (size_t)(n0 + n) * H + c2) = mul2(add2(s0, s1), invC2);
+                if (c < C) s0 = add2(s0, ld2(base + c * VW_ROW));
+                *reinterpret_cast<f32x2*>(a.agg_v + (size_t)(n0 + n) * H + 2 * lane) = mul2(add2(s0, s1), invC2);
             }
-            if (single) {                                    // sum over nodes per channel
-                for (int c = q4; c < C; c += 4) {
-                    const float* base = tile_s + c * V16_ROW + c2;
-                    const int nstep = C * V16_ROW;
-                    f32x2 s0 = 0ull, s1 = 0ull;
-                    int n = 0;
-                    for (; n + 1 < nvalid; n += 2) {
-                        s0 = add2(s0, ld2(base + n * nstep));
-                        s1 = add2(s1, ld2(base + (n + 1) * nstep));
-                    }
-                    if (n < nvalid) s0 = add2(s0, ld2(base + n * nstep));
-                    f32x2* acc = reinterpret_cast<f32x2*>(accH + c * H + c2);
-                    *acc = add2(*acc, add2(s0, s1));
+            if (single) {                                        // sum of the warp's own rows per channel
+                const int cn = min(C, 16);
+#pragma unroll 1
+                for (int i = 0; i < cn; ++i) {
+                    const int r = 16 * w + i;
+                    if (r >= r_end) break;
+                    f32x2 s = ld2(colp + r * VW_ROW);
+#pragma unroll 1
+                    for (int r2 = r + C; r2 < r_end; r2 += C) s = add2(s, ld2(colp + r2 * VW_ROW));
+                    f32x2* acc = reinterpret_cast<f32x2*>(accH + (r % C) * H + 2 * lane);
+                    *acc = add2(*acc, s);
                 }
-            } else {
-                for (int n = q4; n < nvalid; n += 4) {
-                    float* dst = a.vsum + (size_t)sgraph[n] * K + 4 + 3 * C + c2;
-                    for (int c = 0; c < C; ++c) {
-                        float v0, v1;
-                        upk2(ld2(tile_s + (n * C + c) * V16_ROW + c2), v0, v1);
-                        atomicAdd(dst + c * H, v0 * SILU_T_OUT);
-                        atomicAdd(dst + c * H + 1, v1 * SILU_T_OUT);
-                    }
+            } else {                                             // straddling tile: the warp's rows straight to vsum
+#pragma unroll 1
+                for (int r = 16 * w; r < r_end; ++r) {
+                    const int n = r / C, c = r - n * C;
+                    float* dst = a.vsum + (size_t)__ldg(a.batch + n0 + n) * K + 4 + 3 * C + c * H + 2 * lane;
+                    float v0, v1;
+                    upk2(ld2(colp + r * VW_ROW), v0, v1);
+                    atomicAdd(dst, v0 * SILU_T_OUT);
+                    atomicAdd(dst + 1, v1 * SILU_T_OUT);
                 }
             }
         }
-        mma_done();
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
-        // ---- stage 3a: φ_xv = w3xv·SiLU(D + bxv) --------------------------------------------------------
-        auto head_pass = [&](const float* bs, const float* ws, auto safe, float& qmax) {
-            f32x2 ph01 = bc2(0.f), ph23 = bc2(0.f);
-            const f32x2 is2 = bc2(inv2);
-            auto head_math = [&](int c, const uint32_t (&d)[16]) {
+        // ---- stage 3: φ = w3·SiLU(D/s + b) per row (quad shuffles) ----------------------------------------------------
+        auto head = [&](const float* bs, const float* ws, float& phia, float& phib) {
+            // the pre-activations t = D/s + b replace D in place: both passes read them, and D is not needed again
 #pragma unroll
-                for (int j4 = 0; j4 < 4; ++j4) {
-                    const int cc = 16 * c + 4 * j4;
-                    const ulonglong2 bb = *reinterpret_cast<const ulonglong2*>(bs + cc);
-                    const ulonglong2 ww = *reinterpret_cast<const ulonglong2*>(ws + cc);
-                    f32x2 s0 = fma2(pk2u(d[4 * j4 + 0], d[4 * j4 + 1]), is2, bb.x);
-                    f32x2 s1 = fma2(pk2u(d[4 * j4 + 2], d[4 * j4 + 3]), is2, bb.y);
-                    silu4t<decltype(safe)::value>(s0, s1, qmax);
-                    ph01 = fma2(s0, ww.x, ph01);
-                    ph23 = fma2(s1, ww.y, ph23);
+            for (int j = 0; j < 8; ++j) {
+                const f32x2 bb = *reinterpret_cast<const f32x2*>(bs + 8 * j + 2 * q);
+                upk2(fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv2a), bb), d[4 * j + 0], d[4 * j + 1]);
+                upk2(fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv2b), bb), d[4 * j + 2], d[4 * j + 3]);
+            }
+            float qmax = 0.f;
+            f32x2 pha, phb;
+            auto pass = [&](auto safe) {
+                pha = phb = bc2(0.f);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const f32x2 ww = *reinterpret_cast<const f32x2*>(ws + 8 * j + 2 * q);
+                    f32x2 sa = pk2(d[4 * j + 0], d[4 * j + 1]), sb = pk2(d[4 * j + 2], d[4 * j + 3]);
+                    silu4t<decltype(safe)::value>(sa, sb, qmax);
+                    pha = fma2(sa, ww, pha);
+                    phb = fma2(sb, ww, phb);
                 }
             };
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                uint32_t d[16];
-                tm_ld16(lane_off + tD + 16 * c, d);
-                head_math(c, d);
+            pass(kFast);
+            if (__any_sync(FULL, silu_q_overflow(qmax))) pass(kSafe);      // cold (no scale)
+            float p0, p1;
+            upk2(pha, p0, p1);
+            phia = p0 + p1;
+            upk2(phb, p0, p1);
+            phib = p0 + p1;
+            phia += __shfl_xor_sync(FULL, phia, 1);
+            phia += __shfl_xor_sync(FULL, phia, 2);
+            phib += __shfl_xor_sync(FULL, phib, 1);
+            phib += __shfl_xor_sync(FULL, phib, 2);
+        };
+        {
+            float phia, phib;
+            head(bxvs, w3xvs, phia, phib);
+            if (q == 0) {
+                phis[ra] = phia;
+                phis[rb] = phib;
             }
-            float p0, p1, p2, p3;
-            upk2(ph01, p0, p1);
-            upk2(ph23, p2, p3);
-            return (p0 + p1) + (p2 + p3);
-        };
-        auto head = [&](const float* bs, const float* ws) {
-            float qmax = 0.f;
-            float phi = head_pass(bs, ws, tc16::kFast, qmax);
-            if (__any_sync(FULL, silu_q_overflow(qmax))) phi = head_pass(bs, ws, tc16::kSafe, qmax);   // cold
-            return phi;
-        };
-        phis[t] = head(bxvs, w3xvs);
-        named_bar(bar_id, V16_GROUP);                  // D fully read (A still holds mv); nobody reads the mv tile any more
-        issue(dWxhi, dWxlo);
-        // trans_v[node] = mean_c(−ΔX_c·φ_xv,c)
-        for (int i = t; i < nvalid * 3; i += V16_GROUP) {
-            const int n = i / 3, d = i - 3 * n;
-            float s = 0.f;
-            for (int c = 0; c < C; ++c) s = fmaf(-dXs[4 * (n * C + c) + d], phis[n * C + c], s);
-            a.trans_v[(size_t)(n0 + n) * 4 + d] = s / (float)C;
         }
-        mma_done();
 
-        // ---- stage 3b: φ_X = w3x·SiLU(D + bx); Σ_i ΔX_ic·φ_X,ic per graph [3][C] -----------------------------
-        const float phiX = head(bxs, w3xs);
-        if (single && pow2C) {
-            // rows of one channel sit C lanes apart: butterfly over the lane bits above log2(C), then one shared-memory atomic per
-            // (component, channel) and warp — no group barrier, no serial loop on the critical path of the tile
-            const float4 d4 = *reinterpret_cast<const float4*>(dXs + 4 * t);      // own ΔX, written by this thread in stage 1
-            float sx = rvalid ? d4.x * phiX : 0.f, sy = rvalid ? d4.y * phiX : 0.f, sz = rvalid ? d4.z * phiX : 0.f;
-            for (int o = C; o < 32; o <<= 1) {
-                sx += __shfl_xor_sync(FULL, sx, o);
-                sy += __shfl_xor_sync(FULL, sy, o);
-                sz += __shfl_xor_sync(FULL, sz, o);
+        // ---- MMA 3 (φ_X head) overlapped with trans_v[node] = mean_c(−ΔX_c·φ_xv,c) -----------------------------------------
+        // A = mv again, re-split from the thread's own staging rows (bit for bit the fragments of MMA 2, scale 1 exact): the
+        // fragments do not stay live across the φ_xv epilogue, which would not fit the register budget
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const f32x2 ma = *reinterpret_cast<const f32x2*>(tile_s + ra * VW_ROW + 8 * j + 2 * q);
+            const f32x2 mb = *reinterpret_cast<const f32x2*>(tile_s + rb * VW_ROW + 8 * j + 2 * q);
+            tc16::split_pair(mul2(ma, bc2(s2a)), ahi[2 * j], alo[2 * j]);
+            tc16::split_pair(mul2(mb, bc2(s2b)), ahi[2 * j + 1], alo[2 * j + 1]);
+        }
+        tc16::mma_f16x3_rA<VW_LBO>(d, ahi, alo, bW(4), bW(5));
+        if (warp_local) __syncwarp();
+        else named_bar(bar_id, 128);
+        for (int i = lane; i < (ne - nb + ns - 1) / ns * 3; i += 32) {
+            const int n = nb + (i / 3) * ns, dd = i - 3 * (i / 3);
+            float s = 0.f;
+            for (int c = 0; c < C; ++c) s = fmaf(-dXs[4 * (n * C + c) + dd], phis[n * C + c], s);
+            a.trans_v[(size_t)(n0 + n) * 4 + dd] = s / (float)C;
+        }
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
+
+        // ---- stage 3b: φ_X; Σ_i ΔX_ic·φ_X,ic over the warp's own rows, per graph [3][C] -------------------------------
+        {
+            float phia, phib;
+            head(bxs, w3xs, phia, phib);
+            if (q == 0) {
+                phis[VW_TILE + ra] = phia;
+                phis[VW_TILE + rb] = phib;
             }
-            if (lane < C) {
-                atomicAdd(accX + lane, sx);
-                atomicAdd(accX + C + lane, sy);
-                atomicAdd(accX + 2 * C + lane, sz);
+        }
+        __syncwarp();
+        const float* phx = phis + VW_TILE;
+        if (single) {
+            const int cn = min(C, 16);
+            for (int it = lane; it < 3 * cn; it += 32) {      // lane <-> (component, first row of a channel)
+                const int dd = it / cn, r = 16 * w + (it - dd * cn);
+                if (r < r_end) {
+                    float s = 0.f;
+                    for (int r2 = r; r2 < r_end; r2 += C) s = fmaf(dXs[4 * r2 + dd], phx[r2], s);
+                    accX[dd * C + r % C] += s;
+                }
             }
         } else {
-            phis[TILE_M + t] = phiX;
-            named_bar(bar_id, V16_GROUP);
-            if (t < 3 * C) {
-                const int d = t / C, c = t - d * C;
-                const float* phx = phis + TILE_M;
-                if (single) {
-                    float s = 0.f;
-                    for (int n = 0; n < nvalid; ++n) s = fmaf(dXs[4 * (n * C + c) + d], phx[n * C + c], s);
-                    accX[t] += s;
-                } else {
-                    for (int n = 0; n < nvalid; ++n)
-                        atomicAdd(a.vsum + (size_t)sgraph[n] * K + 4 + t, dXs[4 * (n * C + c) + d] * phx[n * C + c]);
+            for (int it = lane; it < 48; it += 32) {          // lane <-> (row, component)
+                const int r = 16 * w + it / 3, dd = it - 3 * (it / 3);
+                if (r < r_end) {
+                    const int n = r / C, c = r - n * C;
+                    atomicAdd(a.vsum + (size_t)__ldg(a.batch + n0 + n) * K + 4 + dd * C + c, dXs[4 * r + dd] * phx[r]);
                 }
             }
         }
-        // dXs / phis / the mv tile are rewritten by the next tile only after ITS first group barrier, which the threads of the
-        // loop above reach after their reads; sgraph is rewritten before that barrier, and read above only on the straddling path
-        if (!single) named_bar(bar_id, V16_GROUP);
+        // the staging rows, ΔX and φ are rewritten by the next tile: after the reads of this one (group-wide when the pools
+        // read other warps' rows)
+        if (warp_local) __syncwarp();
+        else named_bar(bar_id, 128);
     }
-    named_bar(bar_id, V16_GROUP);      // the last tile's shared-memory atomics into accX, before other threads flush them
+    named_bar(bar_id, 128);      // every warp's sums are complete
     flush(cur_graph);
 }
 
@@ -410,17 +511,14 @@ extern "C" int distegnn_virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, 
     a.bx = layer_params + L.off[DISTEGNN_P_V_BX];
     a.w3x = layer_params + L.off[DISTEGNN_P_V_W3X];
     a.agg_v = agg_v; a.trans_v = trans_v; a.vsum = vsum;
-    // the G cache is taken when it fits next to the fixed layout
-    const int g_bytes = V16_GROUPS * C * V16_ROW * 4;
-    a.g_smem = (V16_SMEM_BYTES + g_bytes <= 232448 - 1024) ? 1 : 0;
-    const int smem_bytes = V16_SMEM_BYTES + (a.g_smem ? g_bytes : 0);
-    static_assert(V16_SMEM_BYTES + V16_GROUPS * V16_MAXC * V16_ROW * 4 <= 232448, "G cache of the widest C must fit");
-    ensure_dynamic_smem((const void*)virtual_layer_t16_kernel, (int)V16_SMEM_BYTES + V16_GROUPS * V16_MAXC * V16_ROW * 4);
-    const int TN = TILE_M / C;
+    static_assert(vw_smem_bytes(DISTEGNN_MAX_CHANNELS) <= 232448, "the widest C must fit");
+    ensure_dynamic_smem((const void*)virtual_layer_t16_kernel, vw_smem_bytes(DISTEGNN_MAX_CHANNELS));
+    const int TN = VW_TILE / C;
     const int64_t tiles = (n_nodes + TN - 1) / TN;
-    int64_t grid = (tiles + V16_GROUPS - 1) / V16_GROUPS;
+    DEGNN_CHECK_ARG(tiles + (int64_t)sm_count() * VW_WG < ((int64_t)1 << 31), "too many nodes");
+    int64_t grid = (tiles + VW_WG - 1) / VW_WG;
     if (grid > sm_count()) grid = sm_count();
-    virtual_layer_t16_kernel<<<(unsigned)grid, V16_THREADS, smem_bytes, (cudaStream_t)stream>>>(a);
+    virtual_layer_t16_kernel<<<(unsigned)grid, VW_THREADS, vw_smem_bytes(C), (cudaStream_t)stream>>>(a);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }
