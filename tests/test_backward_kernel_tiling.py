@@ -19,20 +19,15 @@ import torch
 
 from distegnn_b200 import FastEGNN, _lib
 from oracle import fastegnn_oracle as orc
+from tests.helpers import FLOOR, check_bounds, rel, rowwise, within_rerun_bound
 
 pytestmark = pytest.mark.gpu
 
-TOL = 2e-5              # row-wise relative error against float64 autograd (the per-stage bound of the backward kernels)
 # g_x rows have three entries, each a signed sum over the node's edges (or channels), and whole rows cancel.  Measured on
 # an H100 80GB HBM3 (700 W): up to 4.6e-5 for the edge kernel (hub, FLAG_NORMALIZE) and 7.7e-5 for the virtual kernel
 # (2^k upstream, FLAG_LAST); the fp32-FMA twins reach 4.6e-5 on the same inputs.
 TOL_X = 1e-4
-# Where a case needs more than TOL, the tensor-core kernel must still be within this factor of the twin's error (its
-# operands are split into two fp16 terms with one power-of-two scale per row; the worst ratio measured is 9, on the
-# rescued rows of test_edge_bwd_rescued_and_guarded_rows).
-TWIN_FACTOR = 16
-FLOOR = 1e-30           # denominator floor of the row-wise error (the smallest rows here are about 1e-20)
-C_EDGE, NA = 3, 0       # virtual channels / node attributes of the layer whose edge stage is tested
+C_EDGE, NA = 3, 0      # virtual channels / node attributes of the layer whose edge stage is tested
 EDGE_FIELDS = ("E_W1R", "E_W1E", "E_W2", "E_B2", "E_WC", "E_BC", "E_W3")
 VIRT_FIELDS = ("V_W1R", "V_W2", "V_B2", "V_WXV", "V_BXV", "V_W3XV", "V_WX", "V_BX", "V_W3X")
 FLAG_SETS = [0, _lib.FLAG_NORMALIZE, _lib.FLAG_LAST, _lib.FLAG_NORMALIZE | _lib.FLAG_LAST]
@@ -63,20 +58,6 @@ def field_sizes(A):
             "V_BX": 64, "V_W3X": 64}
 
 
-def rowwise(got, ref, zero_rows=None):
-    """Largest row-wise relative error; rows flagged in `zero_rows` must be exactly zero in both."""
-    got = got.detach().double().reshape(got.shape[0], -1)
-    ref = ref.detach().double().reshape(ref.shape[0], -1)
-    assert torch.isfinite(got).all(), "non-finite output"
-    if zero_rows is not None and bool(zero_rows.any()):
-        assert float(ref[zero_rows].abs().max()) == 0.0
-        assert float(got[zero_rows].abs().max()) == 0.0, "structurally zero row is not exactly zero"
-        got, ref = got[~zero_rows], ref[~zero_rows]
-    if got.shape[0] == 0:
-        return 0.0
-    return float(((got - ref).abs().amax(1) / ref.abs().amax(1).clamp(min=FLOOR)).max())
-
-
 def edge_attr_rowwise(got, ref, terms, row, N):
     """g_edge_attr[e,k] = Σ_n g_z1[e,n]·W_e[k,n] can cancel to any magnitude, and g_z1 of one edge carries the fp32
     rounding of its gφ = g_aggx[row]·Δ (a three-term dot product).  So each edge's error is taken relative to the largest
@@ -85,27 +66,6 @@ def edge_attr_rowwise(got, ref, terms, row, N):
     err = (got.double() - ref.double()).abs().amax(1)
     scale = torch.zeros(N, dtype=torch.float64, device=got.device).scatter_reduce(0, row, terms.amax(1), "amax")
     return float((err / scale[row].clamp(min=FLOOR)).max())
-
-
-def check_bounds(errs, tols):
-    """errs: {kernel: {field: error}}.  Every field within its bound; a field above TOL in the tensor-core kernel within
-    TWIN_FACTOR of the twin's error."""
-    for kind, e in errs.items():
-        bad = {f: v for f, v in e.items() if v > tols.get(f, TOL)}
-        assert not bad, (kind, bad)
-    for f, v in errs["tc"].items():
-        if v > TOL and f in errs["twin"]:
-            assert v <= TWIN_FACTOR * max(errs["twin"][f], TOL), (f, v, errs["twin"][f])
-
-
-def rel(got, ref):
-    assert torch.isfinite(got).all(), "non-finite output"
-    return float((got.double() - ref.double()).abs().max()) / max(FLOOR, float(ref.abs().max()))
-
-
-def within_rerun_bound(a, b):
-    """Two launches that differ only in the order of their float atomics (DESIGN §5)."""
-    return float((a - b).abs().max()) <= 2e-6 * max(1.0, float(a.abs().max()))
 
 
 def param_errors(glp, rlp, names, A, offs):
