@@ -70,6 +70,12 @@ SIGNATURES = {
     "distegnn_loss_packed_floats": [_i32, _i32],
     "distegnn_loss_partials": [_i64, _i32, _i32, _i32, _i32, _i32, C.c_float] + [_vp] * 10,
     "distegnn_loss_finalize": [_i64, _i32, _i32, _i32, _i32, _i32, C.c_float, C.c_float, _i32] + [_vp] * 10,
+    "distegnn_deterministic_workspace_bytes": [_i64, _i64, _i32, C.POINTER(_i64)],
+    "distegnn_edge_layer_fwd_det": [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 11 + [_i64, _vp],
+    "distegnn_edge_combine_det": [_i64, _i64, _i32] + [_vp] * 5 + [_i64, _vp],
+    "distegnn_virtual_layer_fwd_det": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 10 + [_i64, _vp],
+    "distegnn_vsum_combine_det": [_i64, _i32, _i32, _u32] + [_vp] * 4 + [_i64, _vp],
+    "distegnn_rollout_centroid_det": [_i64, _i32] + [_vp] * 4,
 }
 ABI_VERSION = 2
 
@@ -120,6 +126,13 @@ def ptr(t: Optional[torch.Tensor]) -> Optional[int]:
 
 def stream_ptr(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
+
+
+def deterministic_workspace_bytes(N: int, E: int, Cn: int) -> int:
+    """Bytes of the deterministic mode's workspace for N nodes, an edge capacity E and Cn virtual channels."""
+    nbytes = _i64(0)
+    check(load().distegnn_deterministic_workspace_bytes(N, E, Cn, C.byref(nbytes)), "deterministic_workspace_bytes")
+    return int(nbytes.value)
 
 
 def param_layout(A: int, Cn: int, Na: int):

@@ -71,23 +71,42 @@ class CudaBackend:
 
     # ---- layer stages --------------------------------------------------------------------------
     def embed(self, dims, node_feat, node_loc, data_batch, emb_wt, emb_b, layer0, h, x4, batch32, P, Q,
-              Hn, vsum, n_invalid=None) -> None:
-        """`n_invalid`: zeroed int32 [1] device counter of data_batch entries that are unsorted / outside [0,B)."""
+              Hn, vsum, n_invalid=None, det_ws=None) -> None:
+        """`n_invalid`: zeroed int32 [1] device counter of data_batch entries that are unsorted / outside [0,B).  `det_ws`
+        (deterministic mode): the statistics in vsum are then recomputed from x4 in a fixed order."""
         N, B, F, A, Cn, Na = dims
         check(self.lib.distegnn_embed_fwd(N, B, F, A, Cn, Na, ptr(node_feat), ptr(node_loc),
                                           ptr(data_batch), ptr(emb_wt), ptr(emb_b), ptr(layer0), ptr(h),
                                           ptr(x4), ptr(batch32), ptr(P), ptr(Q), ptr(Hn), ptr(vsum),
                                           ptr(n_invalid), self._s(h)), "embed_fwd")
         self.launches += 1 if N else 0
+        if det_ws is not None:
+            self._vsum_combine(N, B, Cn, _lib.FLAG_INIT, batch32, x4, vsum, det_ws)
 
-    def edge_layer(self, dims, flags, row, col, ea, x4, P, Q, lp, agg_m, agg_x, n_edges_dev=None) -> None:
+    def edge_layer(self, dims, flags, row, col, ea, x4, P, Q, lp, agg_m, agg_x, n_edges_dev=None, det_ws=None) -> None:
         """`n_edges_dev`: int32 [1] on the device with the true edge count when E is only a capacity (CSRGraph built on the
-        device without a host round trip)."""
+        device without a host round trip).  `det_ws` (uint8, deterministic_workspace_bytes): the deterministic kernel and
+        its combine pass instead."""
         N, E, A, Cn, Na = dims
-        check(self.lib.distegnn_edge_layer_fwd(N, E, A, Cn, Na, flags, ptr(row), ptr(col), ptr(ea),
-                                               ptr(x4), ptr(P), ptr(Q), ptr(lp), ptr(agg_m), ptr(agg_x),
-                                               ptr(n_edges_dev), self._s(x4)), "edge_layer_fwd")
-        self.launches += 1 if E else 0
+        if det_ws is None:
+            check(self.lib.distegnn_edge_layer_fwd(N, E, A, Cn, Na, flags, ptr(row), ptr(col), ptr(ea),
+                                                   ptr(x4), ptr(P), ptr(Q), ptr(lp), ptr(agg_m), ptr(agg_x),
+                                                   ptr(n_edges_dev), self._s(x4)), "edge_layer_fwd")
+            self.launches += 1 if E else 0
+            return
+        check(self.lib.distegnn_edge_layer_fwd_det(N, E, A, Cn, Na, flags, ptr(row), ptr(col), ptr(ea), ptr(x4), ptr(P),
+                                                   ptr(Q), ptr(lp), ptr(agg_m), ptr(agg_x), ptr(n_edges_dev),
+                                                   ptr(det_ws), det_ws.numel(), self._s(x4)), "edge_layer_fwd_det")
+        check(self.lib.distegnn_edge_combine_det(N, E, Cn, ptr(row), ptr(n_edges_dev), ptr(agg_m), ptr(agg_x),
+                                                 ptr(det_ws), det_ws.numel(), self._s(x4)), "edge_combine_det")
+        self.launches += 2 if E else 0
+
+    def _vsum_combine(self, N, B, Cn, flags, batch32, x4, vsum, det_ws) -> None:
+        """Deterministic mode: vsum[:, 0:4] = Σ(x, 1) of x4 per graph in a fixed order; unless FLAG_INIT also the slots of
+        the deterministic real<->virtual kernel, in chunk order."""
+        check(self.lib.distegnn_vsum_combine_det(N, B, Cn, flags, ptr(batch32), ptr(x4), ptr(vsum), ptr(det_ws),
+                                                 det_ws.numel(), self._s(vsum)), "vsum_combine_det")
+        self.launches += 1
 
     def edge_layer_bwd(self, dims, flags, row, col, ea, x4, P, Q, lp, g_agg_m, g_agg_x, g_P, g_Q, g_x4, g_lp,
                        n_edges_dev=None, g_ea=None) -> None:
@@ -144,15 +163,22 @@ class CudaBackend:
                                             ptr(rowptr), ptr(row), ptr(col), ptr(dist), self._s(x4)), "radius_fill")
         self.launches += 1 if N else 0
 
-    def virtual_layer(self, dims, flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vsum) -> None:
+    def virtual_layer(self, dims, flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vsum, det_ws=None) -> None:
+        """`det_ws`: the deterministic kernel (vsum is complete only after vsum_combine)."""
         N, B, A, Cn, Na = dims
-        check(self.lib.distegnn_virtual_layer_fwd(N, B, A, Cn, Na, flags, ptr(batch32), ptr(x4), ptr(Hn),
-                                                  ptr(Xv), ptr(G), ptr(lp), ptr(agg_v), ptr(trans_v),
-                                                  ptr(vsum), self._s(x4)), "virtual_layer_fwd")
+        args = (N, B, A, Cn, Na, flags, ptr(batch32), ptr(x4), ptr(Hn), ptr(Xv), ptr(G), ptr(lp), ptr(agg_v), ptr(trans_v),
+                ptr(vsum))
+        if det_ws is None:
+            check(self.lib.distegnn_virtual_layer_fwd(*args, self._s(x4)), "virtual_layer_fwd")
+        else:
+            check(self.lib.distegnn_virtual_layer_fwd_det(*args, ptr(det_ws), det_ws.numel(), self._s(x4)),
+                  "virtual_layer_fwd_det")
         self.launches += 1 if N else 0
 
     def node_layer(self, dims, flags, rowptr, batch32, h, x4, vel, attr, agg_m, agg_x, agg_v, trans_v,
-                   lp, lp_next, h_out, x4_out, P, Q, Hn, loc_out, vsum) -> None:
+                   lp, lp_next, h_out, x4_out, P, Q, Hn, loc_out, vsum, det_ws=None) -> None:
+        """`det_ws` (deterministic mode): vsum is completed by the combine pass (Σ(x, 1) from x4_out in a fixed order, and
+        the slots of the deterministic real<->virtual kernel)."""
         N, B, A, Cn, Na = dims
         check(self.lib.distegnn_node_layer_fwd(N, B, A, Cn, Na, flags, ptr(rowptr), ptr(batch32), ptr(h),
                                                ptr(x4), ptr(vel), ptr(attr), ptr(agg_m), ptr(agg_x),
@@ -160,6 +186,8 @@ class CudaBackend:
                                                ptr(h_out), ptr(x4_out), ptr(P), ptr(Q), ptr(Hn),
                                                ptr(loc_out), ptr(vsum), self._s(x4)), "node_layer_fwd")
         self.launches += 1 if N else 0
+        if det_ws is not None:
+            self._vsum_combine(N, B, Cn, flags & _lib.FLAG_LAST, batch32, x4_out, vsum, det_ws)
 
     def node_layer_bwd(self, dims, flags, rowptr, batch32, h, vel, attr, agg_m, agg_v, lp, lp_next, g_x_out, g_vsum,
                        g_h_out, g_P, g_Q, g_Hn, g_h, g_x, g_agg_x, g_trans_v, g_agg_m, g_agg_v, g_lp, g_lp_next,
@@ -269,10 +297,10 @@ class CudaBackend:
               "rollout_advance_bwd")
         self.launches += 1 if N else 0
 
-    def rollout_centroid(self, pos: Tensor, batch: Optional[Tensor], sums: Tensor) -> None:
-        """sums float64 [B,4] += per-graph (Σx, Σy, Σz, count)."""
-        check(self.lib.distegnn_rollout_centroid(int(pos.shape[0]), int(sums.shape[0]), ptr(pos), ptr(batch), ptr(sums),
-                                                 self._s(pos)), "rollout_centroid")
+    def rollout_centroid(self, pos: Tensor, batch: Optional[Tensor], sums: Tensor, deterministic: bool = False) -> None:
+        """sums float64 [B,4] += per-graph (Σx, Σy, Σz, count); `deterministic`: in a fixed order."""
+        fn = self.lib.distegnn_rollout_centroid_det if deterministic else self.lib.distegnn_rollout_centroid
+        check(fn(int(pos.shape[0]), int(sums.shape[0]), ptr(pos), ptr(batch), ptr(sums), self._s(pos)), "rollout_centroid")
         self.launches += 1 if pos.shape[0] else 0
 
     def allreduce_packed(self, comm: "Comm", buf: Tensor) -> None:

@@ -28,6 +28,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "det.cuh"
 #include "tc16.cuh"
 #include "tile_mma.cuh"
 
@@ -53,6 +54,7 @@ struct EdgeCsArgs {
     const float* w3;
     float* agg_m;
     float* agg_x;
+    float* slots;   // deterministic mode: one DET_EDGE_SLOT-float slot per 16-edge slice (det.cuh)
 };
 
 // 4 warpgroups = 16 warps per SM: 128 registers per thread (ptxas: no spills), 196 KB of shared memory
@@ -75,7 +77,10 @@ constexpr uint32_t CS_LBO = 1024;                         // fp16 K-major no-swi
 using tc16::kFast;
 using tc16::kSafe;
 
-template <int AT, bool LASTL>
+// DET (deterministic mode, det.cuh): the partial of every run is stored, not added.  The run of a row whose first edge lies
+// in the warp's 16-edge slice goes to the row itself; the slice's head run, when it continues a row of the slice before,
+// goes to the slice's slot.  distegnn_edge_combine_det then adds the slots of each row in slice order.
+template <int AT, bool LASTL, bool DET>
 __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const EdgeCsArgs a) {
     using namespace tmma;
     constexpr int AMAX = AT >= 0 ? (AT > 0 ? AT : 1) : DISTEGNN_MAX_EDGE_ATTR;
@@ -189,6 +194,14 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         const int b = it & 1;
         float* qcur = qb + b * CS_WBUF;
 
+        int cont_row = -1;                     // DET: the row this slice continues from the slice before, if any
+        if constexpr (DET) {
+            const int64_t e0 = tile * CS_TILE + 16 * w;
+            const int r0 = __shfl_sync(FULL, row_c, 0);
+            if (r0 >= 0 && e0 > 0 && __ldg(a.row + e0 - 1) == r0) cont_row = r0;
+        }
+        float* const slot = DET ? a.slots + (size_t)(tile * 4 + w) * DET_EDGE_SLOT : nullptr;
+
         // ---- requests for the next tile (its staging buffer was released at the end of the previous tile) -------------
         if (ntile < num_tiles) fetch_q(ntile, b ^ 1, n_col, n_row >= 0);
         if (n_row >= 0) {
@@ -227,7 +240,11 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         const float* pb = a.P + (size_t)max(rb, 0) * H + 2 * q;
         const float* qa = qcur + g * CS_QROW + 2 * q;
         const float* qbr = qa + 8 * CS_QROW;
-        auto pre = [&](int j, const float* prow, const float* qrow, float rad, const float (&ea)[AMAX]) {
+        // DET: rows past the edge count are zero — their staging rows and attributes are left over from earlier tiles, and
+        // through the warp-wide cold-path tests they would make the bits of the valid rows depend on the tile order
+        const bool oka = !DET || ra >= 0, okb = !DET || rb >= 0;
+        auto pre = [&](int j, const float* prow, const float* qrow, float rad, const float (&ea)[AMAX], bool ok) {
+            if (DET && !ok) return bc2(0.f);
             const int c = 8 * j + 2 * q;
             const f32x2 pp = __ldg(reinterpret_cast<const f32x2*>(prow + 8 * j));
             const f32x2 qq = *reinterpret_cast<const f32x2*>(qrow + 8 * j);
@@ -248,7 +265,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             float qmax = 0.f;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                f32x2 va = pre(j, pa, qa, rada, eaa), vb = pre(j, pb, qbr, radb, eab);
+                f32x2 va = pre(j, pa, qa, rada, eaa, oka), vb = pre(j, pb, qbr, radb, eab, okb);
                 silu4p<false>(va, vb, qmax);
                 tc16::split_pair(va, ahi[2 * j], alo[2 * j]);
                 tc16::split_pair(vb, ahi[2 * j + 1], alo[2 * j + 1]);
@@ -261,7 +278,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 float fa = 0.f, fb = 0.f, sa, sb;
 #pragma unroll 1
                 for (int j = 0; j < 8; ++j) {
-                    f32x2 va = pre(j, pa, qa, rada, eaa), vb = pre(j, pb, qbr, radb, eab);
+                    f32x2 va = pre(j, pa, qa, rada, eaa, oka), vb = pre(j, pb, qbr, radb, eab, okb);
                     silu4p<true>(va, vb, qmax);
                     float v0, v1;
                     upk2(va, v0, v1);
@@ -277,7 +294,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 tc16::range_scale(fb, sb, inv1b);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    f32x2 va = pre(j, pa, qa, rada, eaa), vb = pre(j, pb, qbr, radb, eab);
+                    f32x2 va = pre(j, pa, qa, rada, eaa, oka), vb = pre(j, pb, qbr, radb, eab, okb);
                     silu4p<true>(va, vb, qmax);
                     tc16::split_pair(mul2(va, bc2(sa)), ahi[2 * j], alo[2 * j]);
                     tc16::split_pair(mul2(vb, bc2(sb)), ahi[2 * j + 1], alo[2 * j + 1]);
@@ -361,7 +378,11 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 if (rr >= 0) {
                     float v0, v1;
                     upk2(mul2(acc, bc2(SILU_T_OUT)), v0, v1);
-                    red_add_v2(a.agg_m + (size_t)rr * H + 2 * lane, v0, v1);
+                    if constexpr (DET)
+                        *reinterpret_cast<float2*>(rr == cont_row ? slot + 2 * lane : a.agg_m + (size_t)rr * H + 2 * lane) =
+                            make_float2(v0, v1);
+                    else
+                        red_add_v2(a.agg_m + (size_t)rr * H + 2 * lane, v0, v1);
                 }
             };
             f32x2 s0 = *reinterpret_cast<const f32x2*>(colp);
@@ -432,10 +453,17 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             }
             const int rnext = __shfl_down_sync(FULL, row_c, 1);
             if (row_c >= 0 && (lane == 15 || rnext != row_c)) {
-                float* dst = a.agg_x + (size_t)row_c * 4;
-                atomicAdd(dst + 0, sx);
-                atomicAdd(dst + 1, sy);
-                atomicAdd(dst + 2, sz);
+                if constexpr (DET) {
+                    float* dst = row_c == cont_row ? slot + H : a.agg_x + (size_t)row_c * 4;
+                    dst[0] = sx;
+                    dst[1] = sy;
+                    dst[2] = sz;
+                } else {
+                    float* dst = a.agg_x + (size_t)row_c * 4;
+                    atomicAdd(dst + 0, sx);
+                    atomicAdd(dst + 1, sy);
+                    atomicAdd(dst + 2, sz);
+                }
             }
         }
 
@@ -465,18 +493,26 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
 
 }  // namespace degnn
 
-extern "C" int distegnn_edge_layer_fwd(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags,
-                                       const int32_t* row, const int32_t* col, const float* edge_attr_sorted,
-                                       const float* x4, const float* P, const float* Q,
-                                       const float* layer_params, float* agg_m, float* agg_x,
-                                       const int32_t* n_edges_dev, void* stream) {
-    using namespace degnn;
+namespace degnn {
+
+template <bool DET>
+static int edge_layer_fwd(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags, const int32_t* row,
+                          const int32_t* col, const float* edge_attr_sorted, const float* x4, const float* P,
+                          const float* Q, const float* layer_params, float* agg_m, float* agg_x,
+                          const int32_t* n_edges_dev, void* workspace, int64_t workspace_bytes, void* stream,
+                          int max_ctas) {
     if (int rc = check_dims(A, C, Na)) return rc;
     if (n_edges == 0) return DISTEGNN_OK;
     DEGNN_CHECK_ARG(n_nodes > 0 && n_edges > 0, "negative size");
     DEGNN_CHECK_ARG(row && col && x4 && P && Q && layer_params && agg_x, "null pointer");
     DEGNN_CHECK_ARG(A == 0 || edge_attr_sorted, "null edge_attr with edge_attr_nf > 0");
     DEGNN_CHECK_ARG((flags & DISTEGNN_FLAG_LAST) || agg_m, "null agg_m");
+    float* slots = nullptr;
+    if (DET) {
+        if (int rc = det_check_workspace(n_nodes, n_edges, C, workspace, workspace_bytes, "distegnn_edge_layer_fwd_det"))
+            return rc;
+        slots = det_edge_slots(workspace, n_nodes, C);
+    }
     Layout L = make_layout(A, C, Na);
     EdgeCsArgs a;
     a.N = n_nodes; a.E = n_edges; a.E_dev = n_edges_dev; a.A = A; a.flags = flags & 0xffffu;
@@ -488,21 +524,51 @@ extern "C" int distegnn_edge_layer_fwd(int64_t n_nodes, int64_t n_edges, int A, 
     a.wc = layer_params + L.off[DISTEGNN_P_E_WC];
     a.bc = layer_params + L.off[DISTEGNN_P_E_BC];
     a.w3 = layer_params + L.off[DISTEGNN_P_E_W3];
-    a.agg_m = agg_m; a.agg_x = agg_x;
+    a.agg_m = agg_m; a.agg_x = agg_x; a.slots = slots;
     const int64_t tiles = (n_edges + CS_TILE - 1) / CS_TILE;
     int64_t grid = (tiles + CS_WG - 1) / CS_WG;
     if (grid > sm_count()) grid = sm_count();
+    if (DET) grid = det_grid(grid, max_ctas);
     auto launch = [&](auto kern) {
         ensure_dynamic_smem((const void*)kern, (int)CS_SMEM_BYTES);
         kern<<<(unsigned)grid, CS_THREADS, CS_SMEM_BYTES, (cudaStream_t)stream>>>(a);
     };
     const bool last = flags & DISTEGNN_FLAG_LAST;
     switch (A) {
-        case 0: last ? launch(edge_layer_cs_kernel<0, true>) : launch(edge_layer_cs_kernel<0, false>); break;
-        case 1: last ? launch(edge_layer_cs_kernel<1, true>) : launch(edge_layer_cs_kernel<1, false>); break;
-        case 2: last ? launch(edge_layer_cs_kernel<2, true>) : launch(edge_layer_cs_kernel<2, false>); break;
-        default: last ? launch(edge_layer_cs_kernel<-1, true>) : launch(edge_layer_cs_kernel<-1, false>); break;
+        case 0: last ? launch(edge_layer_cs_kernel<0, true, DET>) : launch(edge_layer_cs_kernel<0, false, DET>); break;
+        case 1: last ? launch(edge_layer_cs_kernel<1, true, DET>) : launch(edge_layer_cs_kernel<1, false, DET>); break;
+        case 2: last ? launch(edge_layer_cs_kernel<2, true, DET>) : launch(edge_layer_cs_kernel<2, false, DET>); break;
+        default: last ? launch(edge_layer_cs_kernel<-1, true, DET>) : launch(edge_layer_cs_kernel<-1, false, DET>); break;
     }
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
+}
+
+int edge_layer_fwd_det(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags, const int32_t* row,
+                       const int32_t* col, const float* edge_attr_sorted, const float* x4, const float* P, const float* Q,
+                       const float* layer_params, float* agg_m, float* agg_x, const int32_t* n_edges_dev,
+                       void* workspace, int64_t workspace_bytes, void* stream, int max_ctas) {
+    return edge_layer_fwd<true>(n_nodes, n_edges, A, C, Na, flags, row, col, edge_attr_sorted, x4, P, Q, layer_params,
+                                agg_m, agg_x, n_edges_dev, workspace, workspace_bytes, stream, max_ctas);
+}
+
+}  // namespace degnn
+
+extern "C" int distegnn_edge_layer_fwd(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags,
+                                       const int32_t* row, const int32_t* col, const float* edge_attr_sorted,
+                                       const float* x4, const float* P, const float* Q,
+                                       const float* layer_params, float* agg_m, float* agg_x,
+                                       const int32_t* n_edges_dev, void* stream) {
+    return degnn::edge_layer_fwd<false>(n_nodes, n_edges, A, C, Na, flags, row, col, edge_attr_sorted, x4, P, Q,
+                                        layer_params, agg_m, agg_x, n_edges_dev, nullptr, 0, stream, 0);
+}
+
+extern "C" int distegnn_edge_layer_fwd_det(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags,
+                                           const int32_t* row, const int32_t* col, const float* edge_attr_sorted,
+                                           const float* x4, const float* P, const float* Q,
+                                           const float* layer_params, float* agg_m, float* agg_x,
+                                           const int32_t* n_edges_dev, void* workspace, int64_t workspace_bytes,
+                                           void* stream) {
+    return degnn::edge_layer_fwd_det(n_nodes, n_edges, A, C, Na, flags, row, col, edge_attr_sorted, x4, P, Q,
+                                     layer_params, agg_m, agg_x, n_edges_dev, workspace, workspace_bytes, stream, 0);
 }

@@ -24,6 +24,7 @@
 // Stages 2 and 3 run in the "t domain" (common.cuh silu4t): −log2(e) is folded into W2v and the biases, −ln 2 into the
 // head projections and the mv pools.
 #include "common.cuh"
+#include "det.cuh"
 #include "tc16.cuh"
 #include "tile_mma.cuh"
 
@@ -45,6 +46,8 @@ struct VirtT16Args {
     float* agg_v;
     float* trans_v;
     float* vsum;
+    float* slots;   // deterministic mode: one K-float slot per chunk of 2^chunk_shift tiles (det.cuh)
+    int chunk_shift;
 };
 
 // 4 warpgroups = 16 warps per SM
@@ -66,6 +69,12 @@ __host__ __device__ constexpr int vw_smem_bytes(int C) { return vw_smem_floats(C
 using tc16::kFast;
 using tc16::kSafe;
 
+// DET (deterministic mode, det.cuh): a warpgroup takes whole chunks of 2^chunk_shift consecutive tiles, in tile order, and
+// the per-graph sums are walked node by node in row order by the thread that owns the element (accumulators in the
+// group's accH / accX, which DET does not use per warp); a graph's partial of the chunk is stored to vsum when the graph
+// starts in the chunk, else to the chunk's slot.
+static_assert(VW_TILE == DET_VTILE, "det.cuh sizes the slots from the tile");
+template <bool DET>
 __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const VirtT16Args a) {
     using namespace tmma;
     const int C = a.C;
@@ -158,15 +167,46 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
 
     const int num_tiles = (int)((a.N + TN - 1) / TN);            // < 2^31 (the launch checks)
     const int stride = (int)gridDim.x * VW_WG;
+    // DET: pipeline p takes the chunks p, p + stride, ...; inside a chunk the tiles follow each other
+    const int CH = 1 << a.chunk_shift;                 // DET: tiles per chunk
+    auto next_tile = [&](int tl) {
+        if constexpr (DET) return (tl + 1) % CH != 0 ? tl + 1 : tl + 1 + (stride - 1) * CH;
+        else return tl + stride;
+    };
+    float* accG = accH_all + 4 * wg * C * H;          // DET: the group's sums [C][64] and [3][C], thread-owned elements
+    float* accXG = accX_all + 4 * wg * 4 * C;
+    int curM = -1, curX = -1, cont = -1;               // DET: graphs of those sums; the graph continued into the chunk
+    auto det_dst = [&](int gr, int tl) {
+        return gr == cont ? a.slots + (size_t)(tl >> a.chunk_shift) * K : a.vsum + (size_t)gr * K;
+    };
+    auto det_flush_m = [&](int tl) {                   // thread t: columns 2(t & 31), +1 of channels t/32, t/32 + 4, ...
+        for (int c = t >> 5; c < C; c += 4) {
+            f32x2* acc = reinterpret_cast<f32x2*>(accG + c * H + 2 * (t & 31));
+            if (curM >= 0) {        // two scalar stores: rows of K = 4 + 67C floats are only 4-byte aligned for odd C
+                float* dst = det_dst(curM, tl) + 4 + 3 * C + c * H + 2 * (t & 31);
+                upk2(mul2(*acc, bc2(SILU_T_OUT)), dst[0], dst[1]);
+            }
+            *acc = 0ull;
+        }
+    };
+    auto det_flush_x = [&](int tl) {                   // thread t < 3C: entry t of [3][C]
+        if (t < 3 * C) {
+            if (curX >= 0) det_dst(curX, tl)[4 + t] = accXG[t];
+            accXG[t] = 0.f;
+        }
+    };
     const int ra = 16 * w + g, rb = ra + 8;            // the thread's tile rows
     const float* colp = tile_s + 2 * lane;             // pools: lane <-> columns 2·lane, 2·lane + 1
 
-    for (int tile = (int)blockIdx.x * VW_WG + wg; tile < num_tiles; tile += stride) {
+    for (int tile = DET ? ((int)blockIdx.x * VW_WG + wg) * CH : (int)blockIdx.x * VW_WG + wg; tile < num_tiles;
+         tile = next_tile(tile)) {
         const int64_t n0 = (int64_t)tile * TN;
+        if (DET && tile % CH == 0)
+            cont = (n0 > 0 && __ldg(a.batch + n0 - 1) == __ldg(a.batch + n0)) ? __ldg(a.batch + n0) : -1;
         const int nvalid = (int)min((int64_t)TN, a.N - n0);
         const int rows = nvalid * C;
         {   // pull the next tile's inputs (Hn rows, x4, graph ids) into L1 while this one computes
-            const int64_t nn0 = (int64_t)(tile + stride) * TN;
+            const int64_t nn0 = (int64_t)next_tile(tile) * TN;
             const int nnv = (int)min((int64_t)TN, a.N - nn0);
             for (int i = t; i < 2 * nnv; i += 128) prefetch_l1(a.Hn + (size_t)nn0 * H + 32 * i);
             if (nnv > 0) {
@@ -179,7 +219,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         const bool single = (g_first == g_last);
         if (single && g_first != cur_graph) {          // group-uniform; rare: once per graph and group
             named_bar(bar_id, 128);                    // every warp is done with the cache and its sums
-            flush(cur_graph);
+            if constexpr (!DET) flush(cur_graph);
             cur_graph = g_first;
             for (int i = t; i < C * (H / 4); i += 128) {
                 const int c = i / (H / 4), q4 = i - c * (H / 4);
@@ -339,7 +379,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         // ---- MMA 2 (φ_xv head) overlapped with the pools of mv ------------------------------------------------------
         tc16::mma_f16x3_rA<VW_LBO>(d, ahi, alo, bW(2), bW(3));
         if (need_feat) {
-            if (warp_local) __syncwarp();
+            if (warp_local && !DET) __syncwarp();
             else named_bar(bar_id, 128);
             auto ld2 = [](const float* p) { return *reinterpret_cast<const f32x2*>(p); };
             const f32x2 invC2 = bc2(SILU_T_OUT / (float)C);     // the rows hold mv' = SILU_T_IN·mv
@@ -356,7 +396,19 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
                 if (c < C) s0 = add2(s0, ld2(base + c * VW_ROW));
                 *reinterpret_cast<f32x2*>(a.agg_v + (size_t)(n0 + n) * H + 2 * lane) = mul2(add2(s0, s1), invC2);
             }
-            if (single) {                                        // sum of the warp's own rows per channel
+            if constexpr (DET) {                                 // every row of the tile, in row order
+                for (int n = 0; n < nvalid; ++n) {
+                    const int gr = single ? g_first : __ldg(a.batch + n0 + n);
+                    if (gr != curM) {
+                        det_flush_m(tile);
+                        curM = gr;
+                    }
+                    for (int c = t >> 5; c < C; c += 4) {
+                        f32x2* acc = reinterpret_cast<f32x2*>(accG + c * H + 2 * (t & 31));
+                        *acc = add2(*acc, ld2(tile_s + (n * C + c) * VW_ROW + 2 * (t & 31)));
+                    }
+                }
+            } else if (single) {                                 // sum of the warp's own rows per channel
                 const int cn = min(C, 16);
 #pragma unroll 1
                 for (int i = 0; i < cn; ++i) {
@@ -457,7 +509,20 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         }
         __syncwarp();
         const float* phx = phis + VW_TILE;
-        if (single) {
+        if constexpr (DET) {
+            named_bar(bar_id, 128);                              // φ_X of every row
+            if (t < 3 * C) {
+                const int dd = t / C, c = t - dd * C;
+                for (int n = 0; n < nvalid; ++n) {
+                    const int gr = single ? g_first : __ldg(a.batch + n0 + n);
+                    if (gr != curX) {
+                        det_flush_x(tile);
+                        curX = gr;
+                    }
+                    accXG[t] = fmaf(dXs[4 * (n * C + c) + dd], phx[n * C + c], accXG[t]);
+                }
+            }
+        } else if (single) {
             const int cn = min(C, 16);
             for (int it = lane; it < 3 * cn; it += 32) {      // lane <-> (component, first row of a channel)
                 const int dd = it / cn, r = 16 * w + (it - dd * cn);
@@ -478,25 +543,37 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         }
         // the staging rows, ΔX and φ are rewritten by the next tile: after the reads of this one (group-wide when the pools
         // read other warps' rows)
-        if (warp_local) __syncwarp();
+        if (warp_local && !DET) __syncwarp();
         else named_bar(bar_id, 128);
+        if (DET && ((tile + 1) % CH == 0 || tile + 1 >= num_tiles)) {     // end of the chunk
+            if (need_feat) det_flush_m(tile);
+            det_flush_x(tile);
+            curM = curX = -1;
+        }
     }
-    named_bar(bar_id, 128);      // every warp's sums are complete
-    flush(cur_graph);
+    if constexpr (!DET) {
+        named_bar(bar_id, 128);      // every warp's sums are complete
+        flush(cur_graph);
+    }
 }
 
 }  // namespace degnn
 
-extern "C" int distegnn_virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags,
-                                          const int32_t* batch32, const float* x4, const float* Hn,
-                                          const float* Xv, const float* G, const float* layer_params,
-                                          float* agg_v, float* trans_v, float* vsum, void* stream) {
-    using namespace degnn;
+namespace degnn {
+
+template <bool DET>
+static int virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags, const int32_t* batch32,
+                             const float* x4, const float* Hn, const float* Xv, const float* G, const float* layer_params,
+                             float* agg_v, float* trans_v, float* vsum, void* workspace, int64_t workspace_bytes,
+                             void* stream, int max_ctas) {
     if (int rc = check_dims(A, C, Na)) return rc;
     if (n_nodes == 0) return DISTEGNN_OK;
     DEGNN_CHECK_ARG(n_nodes > 0 && n_graphs > 0, "bad size");
     DEGNN_CHECK_ARG(batch32 && x4 && Hn && Xv && G && layer_params && trans_v && vsum, "null pointer");
     DEGNN_CHECK_ARG((flags & DISTEGNN_FLAG_LAST) || agg_v, "null agg_v");
+    if (DET)
+        if (int rc = det_check_workspace(n_nodes, -1, C, workspace, workspace_bytes, "distegnn_virtual_layer_fwd_det"))
+            return rc;
     Layout L = make_layout(A, C, Na);
     VirtT16Args a;
     a.N = n_nodes; a.B = n_graphs; a.C = C; a.flags = flags;
@@ -511,14 +588,46 @@ extern "C" int distegnn_virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, 
     a.bx = layer_params + L.off[DISTEGNN_P_V_BX];
     a.w3x = layer_params + L.off[DISTEGNN_P_V_W3X];
     a.agg_v = agg_v; a.trans_v = trans_v; a.vsum = vsum;
+    a.slots = DET ? det_vsum_slots(workspace) : nullptr;
+    a.chunk_shift = DET ? det_chunk_shift(n_nodes, C) : 0;
     static_assert(vw_smem_bytes(DISTEGNN_MAX_CHANNELS) <= 232448, "the widest C must fit");
-    ensure_dynamic_smem((const void*)virtual_layer_t16_kernel, vw_smem_bytes(DISTEGNN_MAX_CHANNELS));
+    ensure_dynamic_smem((const void*)virtual_layer_t16_kernel<DET>, vw_smem_bytes(DISTEGNN_MAX_CHANNELS));
     const int TN = VW_TILE / C;
     const int64_t tiles = (n_nodes + TN - 1) / TN;
-    DEGNN_CHECK_ARG(tiles + (int64_t)sm_count() * VW_WG < ((int64_t)1 << 31), "too many nodes");
-    int64_t grid = (tiles + VW_WG - 1) / VW_WG;
+    const int64_t units = DET ? det_chunks(n_nodes, C) : tiles;       // what the pipelines grid-stride over
+    DEGNN_CHECK_ARG(tiles + ((int64_t)sm_count() * VW_WG << (DET ? det_chunk_shift(n_nodes, C) : 0)) < ((int64_t)1 << 31),
+                    "too many nodes");
+    int64_t grid = (units + VW_WG - 1) / VW_WG;
     if (grid > sm_count()) grid = sm_count();
-    virtual_layer_t16_kernel<<<(unsigned)grid, VW_THREADS, vw_smem_bytes(C), (cudaStream_t)stream>>>(a);
+    if (DET) grid = det_grid(grid, max_ctas);
+    virtual_layer_t16_kernel<DET><<<(unsigned)grid, VW_THREADS, vw_smem_bytes(C), (cudaStream_t)stream>>>(a);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
+}
+
+int virtual_layer_fwd_det(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags, const int32_t* batch32,
+                          const float* x4, const float* Hn, const float* Xv, const float* G, const float* layer_params,
+                          float* agg_v, float* trans_v, float* vsum, void* workspace, int64_t workspace_bytes,
+                          void* stream, int max_ctas) {
+    return virtual_layer_fwd<true>(n_nodes, n_graphs, A, C, Na, flags, batch32, x4, Hn, Xv, G, layer_params, agg_v,
+                                   trans_v, vsum, workspace, workspace_bytes, stream, max_ctas);
+}
+
+}  // namespace degnn
+
+extern "C" int distegnn_virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags,
+                                          const int32_t* batch32, const float* x4, const float* Hn,
+                                          const float* Xv, const float* G, const float* layer_params,
+                                          float* agg_v, float* trans_v, float* vsum, void* stream) {
+    return degnn::virtual_layer_fwd<false>(n_nodes, n_graphs, A, C, Na, flags, batch32, x4, Hn, Xv, G, layer_params,
+                                           agg_v, trans_v, vsum, nullptr, 0, stream, 0);
+}
+
+extern "C" int distegnn_virtual_layer_fwd_det(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags,
+                                              const int32_t* batch32, const float* x4, const float* Hn,
+                                              const float* Xv, const float* G, const float* layer_params,
+                                              float* agg_v, float* trans_v, float* vsum, void* workspace,
+                                              int64_t workspace_bytes, void* stream) {
+    return degnn::virtual_layer_fwd_det(n_nodes, n_graphs, A, C, Na, flags, batch32, x4, Hn, Xv, G, layer_params,
+                                        agg_v, trans_v, vsum, workspace, workspace_bytes, stream, 0);
 }

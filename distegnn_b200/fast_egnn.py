@@ -219,11 +219,30 @@ class FastEGNN(nn.Module):
         self.process_group = None          # torch.distributed group for the virtual-node sync (None = WORLD)
         self.validate_inputs = True        # check edge ids / data_batch once per distinct tensor (one host sync each)
         self.input_grads = False           # opt-in: back-propagate into the floating inputs too (see _FastEGNNFunction)
+        self.deterministic = False         # opt-in: bitwise-reproducible forward (see the property)
         self._validated_batch = None       # (tensor, version, N, B) of the last data_batch that passed
         self._workspaces: Dict[tuple, Dict[str, Tensor]] = {}
         self._keep_state = None            # tests: a list that receives the training-path forward's saved state
         self._comm = None                  # backend.Comm | False (peer exchange unavailable: torch.distributed instead)
         self._comm_key = None
+
+    @property
+    def deterministic(self) -> bool:
+        """Opt-in deterministic mode (default False; DESIGN §17).  While it is on, the inference forward, the forward of the
+        training path, `rollout()` and the forward of `differentiable_rollout()` (trajectory and virtual_loc) are bitwise
+        reproducible: their bits depend only on the input tensors, N, B, C, A, Na, the layer flags and the library build
+        — not on the edge capacity, the grid, the stream, CUDA-graph capture or concurrent work.  Every per-destination
+        and per-graph sum is then taken in a fixed order instead of with atomics, at some cost in speed and a workspace
+        of about 17 bytes per edge of capacity.  Gradients are not covered: the backward keeps the existing
+        run-to-run bound.  Across ranks the per-rank values are deterministic and the peer-memory exchange adds them in
+        rank order; the torch.distributed fallback of that exchange is not covered."""
+        return self._deterministic
+
+    @deterministic.setter
+    def deterministic(self, on: bool) -> None:
+        if not isinstance(on, bool):
+            raise TypeError(f"deterministic must be a bool (got {type(on).__name__})")
+        self._deterministic = on
 
     # ---- runtime helpers -----------------------------------------------------------------------
     def _get_backend(self, device: torch.device):
@@ -463,8 +482,10 @@ class FastEGNN(nn.Module):
         vsum = zeros(B, K)
         comm = self._get_comm(be, dev, B, K)
         counter = None if self._batch_checked(a["data_batch"], N, B) else torch.zeros(1, dtype=torch.int32, device=dev)
+        det = self._det_workspace({}, dev, N, E) if self.deterministic and L else None
+        dk = {} if det is None else dict(det_ws=det)
         be.embed((N, B, F, A, Cn, Na), a["node_feat"], a["node_loc"], a["data_batch"], emb_wt, emb_b,
-                 layers[0] if L else None, h, x4, batch32, P, Q, Hn, vsum, counter)
+                 layers[0] if L else None, h, x4, batch32, P, Q, Hn, vsum, counter, **dk)
         self._check_batch(counter, a["data_batch"], N, B)
         st = dict(batch32=batch32, vsum_init=vsum, layers=[], comm=comm)
         if L == 0:
@@ -482,13 +503,14 @@ class FastEGNN(nn.Module):
             agg_x, trans_v, vs = zeros(N, 4), new(N, 4), zeros(B, K)
             agg_m = None if last else zeros(N, H)
             agg_v = None if last else new(N, H)
-            be.edge_layer((N, E, A, Cn, Na), flags, a["row"], a["col"], a["ea"], x4, P, Q, lp, agg_m, agg_x, a["nE"])
-            be.virtual_layer((N, B, A, Cn, Na), flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vs)
+            be.edge_layer((N, E, A, Cn, Na), flags, a["row"], a["col"], a["ea"], x4, P, Q, lp, agg_m, agg_x, a["nE"],
+                          **dk)
+            be.virtual_layer((N, B, A, Cn, Na), flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vs, **dk)
             x4n = new(N, 4)
             hn, Pn, Qn, Hnn = (None,) * 4 if last else (new(N, H), new(N, H), new(N, H), new(N, H))
             out = new(N, 3) if last else None
             be.node_layer((N, B, A, Cn, Na), flags, a["rowptr"], batch32, h, x4, a["node_vel"], a["attr"], agg_m,
-                          agg_x, agg_v, trans_v, lp, lp_next, hn, x4n, Pn, Qn, Hnn, out, vs)
+                          agg_x, agg_v, trans_v, lp, lp_next, hn, x4n, Pn, Qn, Hnn, out, vs, **dk)
             if comm is None:
                 self._sync_virtual(vs)
             st["layers"].append(dict(h=h, x4=x4, P=P, Q=Q, Hn=Hn, Xv=Xv, Hv=Hv, G=G, agg_m=agg_m, agg_x=agg_x,
@@ -503,6 +525,16 @@ class FastEGNN(nn.Module):
         return out, Xv, st
 
     # ---- device work ---------------------------------------------------------------------------
+    def _det_workspace(self, ws: Dict[str, Tensor], dev, N: int, E: int) -> Tensor:
+        """The deterministic mode's slots (csrc/det.cuh), kept in `ws` and grown to N nodes and E edges of capacity.  Growing
+        replaces the tensor: a captured graph that wrote to the old one holds its own reference (`_forward_graphed`,
+        `rollout`)."""
+        nbytes = max(_lib.deterministic_workspace_bytes(N, E, self.virtual_channels), 1)
+        det = ws.get("det")
+        if det is None or det.numel() < nbytes:
+            det = ws["det"] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        return det
+
     def _workspace(self, dev, N: int, B: int, K: int) -> Dict[str, Tensor]:
         """Per-shape buffers of the inference path, kept between calls.  `vsum`, `agg_m`, `agg_x` are accumulators: they
         start zeroed and every forward leaves them zeroed again (the consuming kernels clear them), so no memset is
@@ -546,8 +578,10 @@ class FastEGNN(nn.Module):
         if not self._batch_checked(a["data_batch"], N, B):
             counter = ws["counter"]
             counter.zero_()
+        det = self._det_workspace(ws, a["node_loc"].device, N, E) if self.deterministic and L else None
+        dk = {} if det is None else dict(det_ws=det)
         be.embed((N, B, F, A, Cn, Na), a["node_feat"], a["node_loc"], a["data_batch"], pk["emb_wt"], pk["emb_b"],
-                 layers[0] if L else None, h, x4, batch32, P, Q, Hn, vsum, counter)
+                 layers[0] if L else None, h, x4, batch32, P, Q, Hn, vsum, counter, **dk)
         self._check_batch(counter, a["data_batch"], N, B)
         if L == 0:
             vsum.zero_()
@@ -568,15 +602,15 @@ class FastEGNN(nn.Module):
             lp, lp_next = layers[i], (None if last else layers[i + 1])
             t0 = self._mark("edge")
             be.edge_layer((N, E, A, Cn, Na), flags, a["row"], a["col"], a["ea"], x4, P, Q, lp,
-                          None if last else agg_m, agg_x, a["nE"])
+                          None if last else agg_m, agg_x, a["nE"], **dk)
             t1 = self._mark("edge_end")
             be.virtual_layer((N, B, A, Cn, Na), flags, batch32, x4, Hn, Xv, G, lp,
-                             None if last else agg_v, trans_v, vsum)
+                             None if last else agg_v, trans_v, vsum, **dk)
             t2 = self._mark("virtual_end")
             be.node_layer((N, B, A, Cn, Na), flags | _lib.FLAG_ZERO_AGG, a["rowptr"], batch32, h, x4, a["node_vel"],
                           a["attr"], None if last else agg_m, agg_x, None if last else agg_v, trans_v, lp, lp_next,
                           None if last else h, x4, None if last else P, None if last else Q,
-                          None if last else Hn, out if last else None, vsum)
+                          None if last else Hn, out if last else None, vsum, **dk)
             t3 = self._mark("node_end")
             if sync:
                 self._sync_virtual(vsum)
@@ -595,7 +629,7 @@ class FastEGNN(nn.Module):
         and shapes of every tensor it reads, so it is valid for as long as the caller keeps passing the same (possibly
         in-place updated) tensors — inference loops, rollouts, benchmarks.  New tensors trigger a re-capture; after
         `_graph_max_captures` distinct keys the model falls back to eager launches for unseen keys."""
-        key = (dims, id(pk), id(comm)) + tuple((k, v.data_ptr(), tuple(v.shape)) for k, v in a.items() if v is not None)
+        key = (dims, id(pk), id(comm), self.deterministic) + tuple((k, v.data_ptr(), tuple(v.shape)) for k, v in a.items() if v is not None)
         ent = self._graph_cache.get(key)
         dev = a["node_loc"].device
         if ent is None:
@@ -614,7 +648,9 @@ class FastEGNN(nn.Module):
             n0 = be.launches
             with torch.cuda.graph(g):
                 self._run(be, pk, dims, a, ws, comm)
-            ent = (g, ws, be.launches - n0, a, pk)   # keep the keyed tensors alive: their addresses are baked in
+            # keep the keyed tensors alive: their addresses are baked in.  So is the deterministic workspace, which `ws`
+            # swaps for a larger one when a later call brings more edges: the entry keeps the one it captured
+            ent = (g, ws, be.launches - n0, a, pk, ws.get("det"))
             self._graph_cache[key] = ent
         ent[0].replay()
         be.launches += ent[2]

@@ -196,6 +196,8 @@ class _Rollout:
         if self.rate > 0:
             self.cand = g
             self._cut_buffers()
+        if self.m.deterministic:                               # sized here: the next step may be captured straight away
+            self.m._det_workspace(self.ws, self.dev, self.N, self.E)
         self.cuda_graph = None                                 # captured addresses are stale
 
     def _cut_buffers(self) -> None:
@@ -255,6 +257,7 @@ class _Rollout:
             with torch.cuda.graph(g):
                 self._enqueue(init_centroid=True)
             self.cuda_graph, self.graph_launches = g, self.be.launches - n0
+            self.graph_det_ws = self.ws.get("det")              # baked into the graph: keep it alive with it
             self.be.launches = n0
         self.cuda_graph.replay()
         self.be.launches += self.graph_launches
@@ -285,7 +288,7 @@ class _Rollout:
         """Per-graph centroid of the final positions over all partitions: one kernel (fp64 sums: exact count, no fp32
         rounding of Σx), one [B,4] fp64 all-reduce."""
         sums = torch.zeros(self.B, 4, dtype=torch.float64, device=self.dev)
-        self.be.rollout_centroid(self.loc, self._gbatch(), sums)
+        self.be.rollout_centroid(self.loc, self._gbatch(), sums, **(dict(deterministic=True) if self.m.deterministic else {}))
         if self.m.world_size > 1:                              # one fp64 SUM all-reduce (the peer exchange sums fp32)
             import torch.distributed as dist
             dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self.m.process_group)

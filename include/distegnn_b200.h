@@ -483,6 +483,52 @@ DISTEGNN_API int distegnn_loss_finalize(int64_t n_nodes, int n_graphs, int C, in
                                         const float *loc_mean, const float *acc, const float *packed, const float *gV_raw,
                                         float *g_pred, float *g_Xv, float *out, void *stream);
 
+/* ---- deterministic mode (csrc/deterministic.cu, csrc/det.cuh; DESIGN §17) ----------------------------------------------
+ * Bitwise-reproducible forward: every floating-point sum is taken in an order fixed by the sizes, never by the grid, the
+ * stream, concurrent work or the device-side edge count against the capacity.  The *_det entry points never allocate and
+ * never synchronise (capturable); they take one caller-owned workspace of distegnn_deterministic_workspace_bytes(n_nodes,
+ * edge_capacity, C) bytes (16-byte aligned; reused across layers and steps).  A forward layer in this mode is
+ *   distegnn_edge_layer_fwd_det, then distegnn_edge_combine_det      (agg_m / agg_x complete only after the combine)
+ *   distegnn_virtual_layer_fwd_det
+ *   distegnn_node_layer_fwd
+ *   distegnn_vsum_combine_det on the node layer's x4_out              (vsum complete only after the combine)
+ *   distegnn_virtual_update_fwd
+ * and the embedding is distegnn_embed_fwd followed by distegnn_vsum_combine_det with DISTEGNN_FLAG_INIT on its x4.
+ * distegnn_edge_layer_fwd_det: arguments as distegnn_edge_layer_fwd.  Stores, rather than adds, the partial sums of agg_m
+ *   and agg_x: rows whose first edge lies in a 16-edge slice get the slice's partial; later slices of a row fill their
+ *   slots.  Rows without an edge are not written (they keep the zeros of a cleared buffer).
+ * distegnn_edge_combine_det: adds the slots of every row spanning slices to the row, in slice order (agg_m NULL: last
+ *   layer, agg_x only).
+ * distegnn_virtual_layer_fwd_det: arguments as distegnn_virtual_layer_fwd.  vsum[:, 4:K] is stored per graph (the chunk
+ *   of 16 tiles that holds the graph's first node) and the later chunks' partials go to slots; vsum[:, 0:4] is left to the
+ *   combine.
+ * distegnn_vsum_combine_det: vsum[b, 0:3] = Σx of x4 over graph b, summed per chunk in node order and the chunks in
+ *   chunk order (replacing what the embedding / node kernel added), vsum[b, 3] = the node count; without
+ *   DISTEGNN_FLAG_INIT also vsum[b, 4:K] += the graph's slots, in chunk order.  data_batch sorted (int32, as the embedding
+ *   writes it).
+ *   With DISTEGNN_FLAG_LAST (after a last layer's real<->virtual kernel) only vsum[b, 4:4+3C] takes slots: the rest was
+ *   not written in that layer.
+ * distegnn_rollout_centroid_det: distegnn_rollout_centroid in a fixed order (no workspace). */
+DISTEGNN_API int distegnn_deterministic_workspace_bytes(int64_t n_nodes, int64_t edge_capacity, int C,
+                                                        int64_t *bytes_host);
+DISTEGNN_API int distegnn_edge_layer_fwd_det(int64_t n_nodes, int64_t n_edges, int A, int C, int Na, unsigned flags,
+                                             const int32_t *row, const int32_t *col, const float *edge_attr_sorted,
+                                             const float *x4, const float *P, const float *Q, const float *layer_params,
+                                             float *agg_m, float *agg_x, const int32_t *n_edges_dev, void *workspace,
+                                             int64_t workspace_bytes, void *stream);
+DISTEGNN_API int distegnn_edge_combine_det(int64_t n_nodes, int64_t n_edges, int C, const int32_t *row,
+                                           const int32_t *n_edges_dev, float *agg_m, float *agg_x, void *workspace,
+                                           int64_t workspace_bytes, void *stream);
+DISTEGNN_API int distegnn_virtual_layer_fwd_det(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags,
+                                                const int32_t *batch32, const float *x4, const float *Hn, const float *Xv,
+                                                const float *G, const float *layer_params, float *agg_v, float *trans_v,
+                                                float *vsum, void *workspace, int64_t workspace_bytes, void *stream);
+DISTEGNN_API int distegnn_vsum_combine_det(int64_t n_nodes, int n_graphs, int C, unsigned flags, const int32_t *batch32,
+                                           const float *x4, float *vsum, void *workspace, int64_t workspace_bytes,
+                                           void *stream);
+DISTEGNN_API int distegnn_rollout_centroid_det(int64_t n_nodes, int n_graphs, const float *pos,
+                                               const int64_t *data_batch, double *sums, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

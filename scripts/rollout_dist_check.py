@@ -7,8 +7,9 @@ Every rank rolls its random partition of one fluid graph out for `--steps` steps
 starts with half the edge capacity its graph needs, so it alone regrows while both ranks roll back, rerun and recapture.
 Rank 0 gathers every rank's trajectory and checks each step against `oracle.forward_partitions` in float64 on the state
 the rollout produced (each partition's graph rebuilt from its x_t, the global loc_mean of x_t), the velocity / speed /
-loc_mean rules, and that loc_mean and virtual_loc are bit-identical on the ranks.  Prints one JSON line and
-`ROLLOUT_DIST PASS|FAIL`.
+loc_mean rules, and that loc_mean and virtual_loc are bit-identical on the ranks.  With `--deterministic` the model runs in
+deterministic mode and every rank rolls out twice: the two runs (regrowth and rerun included) must be bitwise equal on
+each rank.  Prints one JSON line and `ROLLOUT_DIST PASS|FAIL`.
 """
 import argparse
 import json
@@ -28,6 +29,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--nodes", type=int, default=12000)
     ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--deterministic", action="store_true",
+                    help="model.deterministic = True; roll out twice and require bitwise equal runs on every rank")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     dev = torch.device("cuda", local)
@@ -42,13 +45,20 @@ def main():
     m.load_state_dict(sd)
     m = m.to(dev).eval()
     m.cuda_graph = True
+    m.deterministic = args.deterministic
     mine = {k: (v.to(dev) if v is not None else None) for k, v in parts[rank].items() if k not in ("edge_index", "edge_attr")}
     cap = int(parts[rank]["edge_index"].shape[1]) // 2 if rank == 0 else None
     K = args.steps
     res = rollout(m, **mine, steps=K, radius=w.radius, speed_col=0, capacity=cap, check_every=K, return_trajectory=True)
+    repeat_equal = None
+    if args.deterministic:
+        again = rollout(m, **mine, steps=K, radius=w.radius, speed_col=0, capacity=cap, check_every=K,
+                        return_trajectory=True)
+        repeat_equal = all(torch.equal(getattr(res, k), getattr(again, k))
+                           for k in ("trajectory", "node_vel", "node_feat", "loc_mean", "virtual_loc", "n_edges"))
     got = dict(traj=res.trajectory.cpu(), vel=res.node_vel.cpu(), feat=res.node_feat.cpu(), loc_mean=res.loc_mean.cpu(),
                X=res.virtual_loc.cpu(), n_edges=res.n_edges.cpu(), regrowths=res.regrowths, replays=res.replays,
-               peer=bool(m._comm))
+               peer=bool(m._comm), repeat_equal=repeat_equal)
     allg = [None] * world
     dist.all_gather_object(allg, got)
     ok, report = True, {}
@@ -91,12 +101,14 @@ def main():
         regrow = bool(allg[0]["regrowths"]) and not any(allg[r]["regrowths"] for r in range(1, world))
         # steps 1..K-1 replayed twice on every rank: the overflowed attempt and the rerun after rank 0 regrew
         graphed = all(a["replays"] == 2 * (K - 1) for a in allg) if all(a["peer"] for a in allg) else None
+        repeats = [a["repeat_equal"] for a in allg]
         ok &= eX <= 1e-5 * max(1.0, float(X.abs().max())) and elm <= 1e-6 and ev <= 1e-5 and ef <= 1e-5 and same \
-            and regrow and graphed is not False
+            and regrow and graphed is not False and (not args.deterministic or all(repeats))
         report = dict(world=world, nodes=args.nodes, steps=K, max_abs=worst, max_rel_disp=worst_rel, virtual_loc=eX,
                       loc_mean=elm, vel=ev, feat=ef, bit_identical=same, rank0_regrew=regrow,
                       regrowths=[a["regrowths"] for a in allg], peer_exchange=[a["peer"] for a in allg],
-                      replays=[a["replays"] for a in allg], pass_=bool(ok))
+                      replays=[a["replays"] for a in allg], deterministic=args.deterministic,
+                      repeat_bitwise_equal=repeats, pass_=bool(ok))
         print(json.dumps(report), flush=True)
         print("ROLLOUT_DIST", "PASS" if ok else "FAIL", flush=True)
     flag = torch.tensor([int(ok)], device=dev)
