@@ -3,15 +3,19 @@
 // (node_model) and emits the per-node operands of the NEXT layer's fused stages (P, Q, Hn; SURVEY §7 "W1 split").
 // Same math/outputs as node_layer.cu's fp32-FMA kernel (kept as ..._simt for cross-checks).
 //
-// One CTA per SM, 128 threads = 1 tile group = 1 warpgroup; thread r owns node r of the group's current 128-node tile.
-// All eight 64x64 layers run as wgmma tile GEMMs with the fp16 2-term split (tc16.cuh); weights (hi/lo, 128 KB) stay
-// resident in shared memory next to 64 KB of tile memory (tile_mma.cuh: A_hi [0,32)  A_lo [32,64)  D [64,128)).  Each
-// thread reads the 256-byte rows of h, agg_m, agg_v of its node straight from global memory (the kernel is bound by HBM
-// and has few tiles per SM).  Sequence per tile:
-//                      h -> A;                                MMA: D = h·Lᵀ (φ_v); x' and Σ(x',1) from φ_v
-//                      MMA: D = h·N1aᵀ;   agg_m/deg -> A; MMA: D += ·N1bᵀ;   agg_v -> A; MMA: D += ·N1cᵀ
+// One CTA per SM, NT_WG warpgroups, each an independent pipeline: a warpgroup grid-strides over its own 64-node tiles and,
+// once set up, shares no barrier with the other warpgroups.  Warp w of a warpgroup owns nodes 16w .. 16w+15 of its tile,
+// which are exactly the rows of the m64n64 accumulator fragment it holds (tile_mma.cuh); thread (g = lane/4, q = lane%4)
+// owns rows g and g+8 of the warp, columns 8j + 2q + {0,1}, and reads and writes the rows of h, agg_m, agg_v, h', P, Q, Hn
+// in that layout (a quad covers one 32-byte sector of a row per column block j).  All eight 64x64 GEMMs take their A
+// operand from registers (fp16 2-term split, tc16.cuh) and keep the accumulator there; the weights (hi/lo, 128 KB) stay
+// resident in shared memory, shared by the four pipelines.  Sequence per tile:
+//                      h -> A;                                MMA: D = h·Lᵀ;  φ_v per row (quad shuffles)
+//                      x' and Σ(x',1) from φ_v (lane q <-> coordinate q of the thread's rows)
+//                      MMA: D = h·N1aᵀ;   agg_m/deg -> A; MMA: D += ·N1bᵀ;   agg_v -> A; MMA: D += ·N1cᵀ  (one row scale)
 //                      t1 = SiLU(D + attr·N1d + b1) -> A;     MMA: D = t1·N2ᵀ
 //                      h' = h + D + b2 -> HBM, -> A;          3 x (MMA: D = h'·W'ᵀ, W' = W1a', W1b', W1vh'; D -> P / Q / Hn)
+// FLAG_LAST runs the first line and x' only.
 #include "common.cuh"
 #include "tc16.cuh"
 #include "tile_mma.cuh"
@@ -31,20 +35,179 @@ struct NodeTcArgs {
     float* h_out; float* x4_out; float* P; float* Q; float* Hn; float* loc_out; float* vsum;
 };
 
-constexpr int NT_THREADS = 128, NT_GROUPS = 1, NT_GROUP = 128;
-constexpr int NT_W = 4096;                                    // halfs per 64x64 matrix part
-constexpr int NT_TM_COLS = 128;                               // per tile group: A_hi 32 | A_lo 32 | D 64
-constexpr int NT_SMEM_BYTES = tmma::tm_bytes(NT_GROUPS * NT_TM_COLS)
-                              + (2 * NT_W + 6 * NT_W + 2 * NT_W + 2 * 3 * NT_W) * 2   // L, N1a-c, N2, NEXT (hi+lo)
-                              + (5 * H + DISTEGNN_MAX_NODE_ATTR * H) * 4             // lb, lw3, nb1, nb2, nxb1, N1d
-                              + NT_GROUPS * 8 * 4;                                   // accS[4] + sg[2] (+pad) per group
-constexpr uint32_t NT_LBO64 = 1024, NT_LBO192 = 3072;
+// 4 warpgroups = 16 warps per SM
+constexpr int NT_WG = 4;
+constexpr int NT_THREADS = 128 * NT_WG, NT_WARPS = NT_THREADS / 32;
+constexpr int NT_TILE = 64;                                   // nodes per warpgroup tile
+constexpr int NT_W = H * H;                                   // fp16 elements per 64x64 weight matrix
+constexpr uint32_t NT_LBO64 = tc16::lbo_bytes(64), NT_LBO192 = tc16::lbo_bytes(192);
 constexpr uint64_t NT_DESC_N64 = (64 / 8 * 128) >> 4;         // descriptor step to B row n + 64 (8-row groups 128 B apart)
+// weights L, N1a-c, N2, NEXT (hi+lo) | lb, lw3, nb1, nb2, nxb1, N1d [Na][64] | Σ(x,1) per warp
+constexpr int NT_SMEM_BYTES = 16 * NT_W * 2 + (5 * H + DISTEGNN_MAX_NODE_ATTR * H + NT_WARPS * 4) * 4;
+// weights NEXT (hi+lo) | embedding [F][64], bias, nxb1 | Σ(x,1) per warp
+constexpr int ET_SMEM_BYTES = 6 * NT_W * 2 + ((DISTEGNN_MAX_NODE_FEAT + 2) * H + NT_WARPS * 4) * 4;
+
+// The calling thread's two rows of its warpgroup's tile: a = row 16w + g, b = a + 8 (valid: < N), their node ids (a valid
+// node for rows past N, never read for them) and q = lane % 4: its column pairs are 8j + 2q, +1.
+struct Rows {
+    int q;
+    bool va, vb;
+    size_t na, nb;
+};
+__device__ __forceinline__ f32x2 ld_pair(const float* p) { return *reinterpret_cast<const f32x2*>(p); }
+__device__ __forceinline__ void st_pair(float* p, f32x2 v) { *reinterpret_cast<f32x2*>(p) = v; }
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(FULL, v, 1));
+    return fmaxf(v, __shfl_xor_sync(FULL, v, 2));
+}
+// Pull bytes [p, p + n) towards L2: one 128-byte line per thread of a warpgroup (t < 128) and step
+__device__ __forceinline__ void prefetch_l2_range(const void* p, size_t n, int t) {
+    const uintptr_t b = (uintptr_t)p, e = b + n;
+    for (uintptr_t l = (b & ~(uintptr_t)127) + 128u * (uintptr_t)t; l < e; l += 128u * 128u)
+        tmma::prefetch_l2((const void*)l);
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(FULL, v, 1);
+    return v + __shfl_xor_sync(FULL, v, 2);
+}
+
+// Encode the thread's rows a and b, produced as column pairs by f(j, xa, xb, first) (columns 8j + 2q, +1; first = false
+// on the cold passes), into the fp16 hi/lo A fragments (register 2j + r holds pair j of row a / b for r = 0 / 1).  sa / sb:
+// in, the power-of-two scales the rows already carry (1 normally); out, the scales used — smaller only where a row would
+// leave the fp16 range (cold path, per warp).  The passes are unrolled: f may read an accumulator that must stay in
+// registers.
+template <class F>
+__device__ __forceinline__ void encode_rows(F&& f, uint32_t (&hi)[16], uint32_t (&lo)[16], float& sa, float& sb) {
+    const bool pre_scaled = __any_sync(FULL, sa != 1.0f || sb != 1.0f);
+    if (!pre_scaled) {
+        __half2 mx = __floats2half2_rn(0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            f32x2 xa, xb;
+            f(j, xa, xb, true);
+            tc16::split_pair(xa, hi[2 * j], lo[2 * j]);
+            tc16::split_pair(xb, hi[2 * j + 1], lo[2 * j + 1]);
+            mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[2 * j])));
+            mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[2 * j + 1])));
+        }
+        if (!__any_sync(FULL, tc16::row_overflow(mx))) return;
+    }
+    // cold: some row of this warp carries a scale already or leaves the fp16 range
+    float fa = 0.f, fb = 0.f, ca, cb, unused;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        f32x2 xa, xb;
+        float v0, v1;
+        f(j, xa, xb, false);
+        upk2(xa, v0, v1);
+        fa = fmaxf(fa, fmaxf(fabsf(v0), fabsf(v1)));
+        upk2(xb, v0, v1);
+        fb = fmaxf(fb, fmaxf(fabsf(v0), fabsf(v1)));
+    }
+    tc16::range_scale(quad_max(fa), ca, unused);
+    tc16::range_scale(quad_max(fb), cb, unused);
+    sa = fminf(ca, sa);
+    sb = fminf(cb, sb);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        f32x2 xa, xb;
+        f(j, xa, xb, false);
+        tc16::split_pair(mul2(xa, bc2(sa)), hi[2 * j], lo[2 * j]);
+        tc16::split_pair(mul2(xb, bc2(sb)), hi[2 * j + 1], lo[2 * j + 1]);
+    }
+}
+
+// Σ(x, 1) per graph into vsum[:, 0:4].  Lane q of a quad holds entry q of its rows a and b.  Tiles inside one graph add to
+// per-warp sums in shared memory, flushed by the warpgroup (one atomic per entry) when its graph changes and at the end;
+// tiles that straddle graphs add their rows to vsum directly.
+struct XSum {
+    float* vsum;
+    int K;
+    float* acc_w;      // this warp's four sums
+    float* acc_g;      // the four warps' sums of the group
+    uint32_t bar;      // the group's named barrier
+    int t, lane;
+    int cur;           // graph of the sums (group-uniform)
+    __device__ __forceinline__ void flush() {
+        if (cur >= 0 && t < 4) {
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                s += acc_g[4 * k + t];
+                acc_g[4 * k + t] = 0.f;
+            }
+            atomicAdd(vsum + (size_t)cur * K + t, s);
+        }
+    }
+    __device__ __forceinline__ void start_tile(int g_first, bool single) {   // group-uniform; rare: once per graph
+        if (single && g_first != cur) {
+            tmma::named_bar(bar, 128);         // every warp is done with its sums
+            flush();
+            cur = g_first;
+            tmma::named_bar(bar, 128);
+        }
+    }
+    __device__ __forceinline__ void add(bool single, const Rows& r, float xa, float xb, int ga, int gb) {
+        if (single) {
+            float s = (r.va ? xa : 0.f) + (r.vb ? xb : 0.f);
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) s += __shfl_xor_sync(FULL, s, o);
+            if (lane < 4) acc_w[lane] += s;
+        } else {
+            if (r.va) atomicAdd(vsum + (size_t)ga * K + r.q, xa);
+            if (r.vb) atomicAdd(vsum + (size_t)gb * K + r.q, xb);
+        }
+    }
+    __device__ __forceinline__ void finish() {
+        tmma::named_bar(bar, 128);
+        flush();
+    }
+};
+
+// h rows -> h_out (rows < N) and A; P, Q, Hn = h·[W1a; W1b; W1vh]ᵀ, 64 columns at a time, with E_B1 added to P.
+// hrow(j, xa, xb) gives column pair j of rows a and b.  Rows out of the fp16 range are re-encoded from what was stored to
+// h_out (which may be the kernel's h input, so h cannot be read again).
+template <class Hrow>
+__device__ __forceinline__ void store_h_project(Hrow&& hrow, const Rows& r, float* h_out, float* P, float* Q, float* Hn,
+                                                uint64_t b_hi, uint64_t b_lo, const float* nxb1s, float (&d)[32],
+                                                uint32_t (&ahi)[16], uint32_t (&alo)[16]) {
+    float sa = 1.0f, sb = 1.0f;
+    encode_rows(
+        [&](int j, f32x2& xa, f32x2& xb, bool first) {
+            const int col = 8 * j + 2 * r.q;
+            if (first) {
+                hrow(j, xa, xb);
+                if (r.va) st_pair(h_out + r.na * H + col, xa);
+                if (r.vb) st_pair(h_out + r.nb * H + col, xb);
+            } else {
+                xa = r.va ? ld_pair(h_out + r.na * H + col) : 0ull;
+                xb = r.vb ? ld_pair(h_out + r.nb * H + col) : 0ull;
+            }
+        },
+        ahi, alo, sa, sb);
+    const float ia = sa == 1.0f ? 1.0f : 1.0f / sa, ib = sb == 1.0f ? 1.0f : 1.0f / sb;
+#pragma unroll 1
+    for (int o = 0; o < 3; ++o) {
+        tc16::mma_f16x3_rA<NT_LBO192>(d, ahi, alo, b_hi + o * NT_DESC_N64, b_lo + o * NT_DESC_N64);
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
+        float* dst = o == 0 ? P : (o == 1 ? Q : Hn);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int col = 8 * j + 2 * r.q;
+            float ya0 = d[4 * j + 0] * ia, ya1 = d[4 * j + 1] * ia, yb0 = d[4 * j + 2] * ib, yb1 = d[4 * j + 3] * ib;
+            if (o == 0) {
+                const float b0 = nxb1s[col], b1 = nxb1s[col + 1];
+                ya0 += b0; ya1 += b1; yb0 += b0; yb1 += b1;
+            }
+            if (r.va) st_pair(dst + r.na * H + col, pk2(ya0, ya1));
+            if (r.vb) st_pair(dst + r.nb * H + col, pk2(yb0, yb1));
+        }
+    }
+}
 
 __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const NodeTcArgs a) {
     using namespace tmma;
-    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(NT_GROUPS * NT_TM_COLS);
-    __half* Lhi = reinterpret_cast<__half*>(smem_raw);
+    __half* Lhi = reinterpret_cast<__half*>(degnn_dyn_smem);
     __half* Llo = Lhi + NT_W;
     __half* N1hi = Llo + NT_W;            // [3][4096]
     __half* N1lo = N1hi + 3 * NT_W;
@@ -58,10 +221,12 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
     float* nb2s = nb1s + H;
     float* nxb1s = nb2s + H;
     float* n1ds = nxb1s + H;              // [Na][64]
-    float* acc_all = n1ds + DISTEGNN_MAX_NODE_ATTR * H;          // per group: accS[4], sg[2] (as int), pad[2]
+    float* accx_all = n1ds + DISTEGNN_MAX_NODE_ATTR * H;          // [warps][4]: Σ(x',1)
 
     const int tid = threadIdx.x;
-    const int grp = tid / NT_GROUP, t = tid % NT_GROUP, lane = tid & 31, wq = (tid >> 5) & 3;
+    const int lane = tid & 31, warp = tid >> 5;
+    const int wg = warp >> 2, w = warp & 3, t = tid & 127;
+    const int q = lane & 3;
     const bool last = a.flags & DISTEGNN_FLAG_LAST;
     const bool zero_agg = a.flags & DISTEGNN_FLAG_ZERO_AGG;   // leave agg_m / agg_x zeroed for the next edge stage
     const int Na = a.Na;
@@ -86,246 +251,209 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
     }
     if (!last)
         for (int i = tid; i < Na * H; i += NT_THREADS) n1ds[i] = a.n1[(size_t)3 * H * H + i];
-    if (tid < NT_GROUPS * 8) acc_all[tid] = 0.f;
+    if (tid < NT_WARPS * 4) accx_all[tid] = 0.f;
     fence_proxy_async_smem();
     __syncthreads();
 
-    const uint32_t lane_off = ((uint32_t)(32 * wq)) << 16;
-    const uint32_t col0 = (uint32_t)(grp * NT_TM_COLS);
-    const uint32_t tA_hi = col0, tA_lo = col0 + 32, tD = col0 + 64;
     auto desc = [&](const __half* p, uint32_t lbo) { return make_b_desc(smem_u32(p), lbo, 128); };
     const uint64_t dLhi = desc(Lhi, NT_LBO64), dLlo = desc(Llo, NT_LBO64);
     const uint64_t dN2hi = desc(N2hi, NT_LBO64), dN2lo = desc(N2lo, NT_LBO64);
     const uint64_t dNXhi = desc(NXhi, NT_LBO192), dNXlo = desc(NXlo, NT_LBO192);
-    float* accS = acc_all + grp * 8;
-    int* sg = reinterpret_cast<int*>(accS + 4);
-    const uint32_t bar_id = 1 + grp;
-    int cur_graph = -1;
-    int it = 0;
+    XSum xs{a.vsum, a.K, accx_all + 4 * warp, accx_all + 16 * wg, 1u + (uint32_t)wg, t, lane, -1};
+    const int ra = 16 * w + (lane >> 2), rb = ra + 8;             // the thread's tile rows
 
-    const int64_t num_tiles = (a.N + TILE_M - 1) / TILE_M;
-    const int64_t tstride = (int64_t)gridDim.x * NT_GROUPS;
-    auto a_ready = [&]() {                           // A operand written by every thread of the group
-        tm_st_fence();
-        named_bar(bar_id, NT_GROUP);
-    };
-    // D = A·Wᵀ (or D += A·Wᵀ) over the whole tile by the group's warpgroup; the barrier publishes D to every row thread
-    auto mma = [&](uint64_t bhi, uint64_t blo, uint32_t lbo, bool accumulate) {
-        if (lbo == NT_LBO64) tc16::mma_f16x3<NT_LBO64>(tD, tA_hi, tA_lo, bhi, blo, 1, accumulate, 0, 2);
-        else tc16::mma_f16x3<NT_LBO192>(tD, tA_hi, tA_lo, bhi, blo, 1, accumulate, 0, 2);
-        named_bar(bar_id, NT_GROUP);
-    };
-    for (int64_t tile = (int64_t)blockIdx.x * NT_GROUPS + grp; tile < num_tiles; tile += tstride, ++it) {
-        int* sgp = sg + 2 * (it & 1);                // first/last graph id of the tile, double-buffered by tile parity
-        const int64_t n0 = tile * TILE_M;
-        const int nvalid = (int)min((int64_t)TILE_M, a.N - n0);
-        const bool valid = t < nvalid;
-        const size_t node = (size_t)(n0 + (valid ? t : 0));
-        // the own 64-wide row of a [N,64] array, 16 values per chunk (zeros past the last node).  Plain (coherent) loads:
-        // h is also this kernel's h_out in FastEGNN's layer loop, and agg_m is cleared by it
-        auto load_row16 = [&](const float* src, int c, float (&v)[16], float rs) {
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-                const float4 q = valid ? *reinterpret_cast<const float4*>(src + node * H + 16 * c + 4 * j4)
-                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-                v[4 * j4 + 0] = q.x * rs; v[4 * j4 + 1] = q.y * rs; v[4 * j4 + 2] = q.z * rs; v[4 * j4 + 3] = q.w * rs;
+    const int64_t num_tiles = (a.N + NT_TILE - 1) / NT_TILE;
+    for (int64_t tile = (int64_t)blockIdx.x * NT_WG + wg; tile < num_tiles; tile += (int64_t)gridDim.x * NT_WG) {
+        const int64_t n0 = tile * NT_TILE;
+        const int nvalid = (int)min((int64_t)NT_TILE, a.N - n0);
+        Rows r;
+        r.q = q;
+        r.va = ra < nvalid;
+        r.vb = rb < nvalid;
+        r.na = (size_t)(n0 + (r.va ? ra : 0));
+        r.nb = (size_t)(n0 + (r.vb ? rb : 0));
+        {   // pull the next tile's inputs towards L2: a tile takes many DRAM round trips, each of them waited for
+            const int64_t m0 = n0 + (int64_t)gridDim.x * NT_WG * NT_TILE;
+            if (m0 < a.N) {
+                const size_t mv = (size_t)min((int64_t)NT_TILE, a.N - m0), m = (size_t)m0;
+                prefetch_l2_range(a.h + m * H, mv * H * 4, t);
+                if (!last) {
+                    prefetch_l2_range(a.agg_m + m * H, mv * H * 4, t);
+                    prefetch_l2_range(a.agg_v + m * H, mv * H * 4, t);
+                    if (Na) prefetch_l2_range(a.attr + m * Na, mv * Na * 4, t);
+                }
+                prefetch_l2_range(a.x4 + m * 4, mv * 16, t);
+                prefetch_l2_range(a.agg_x + m * 4, mv * 16, t);
+                prefetch_l2_range(a.trans_v + m * 4, mv * 16, t);
+                prefetch_l2_range(a.vel + m * 3, mv * 12, t);
+                prefetch_l2_range(a.rowptr + m, (mv + 1) * 4, t);
+                prefetch_l2_range(a.batch + m, mv * 4, t);
             }
+        }
+        const int g_first = __ldg(a.batch + n0), g_last = __ldg(a.batch + n0 + nvalid - 1);
+        const bool single = g_first == g_last;
+        xs.start_tile(g_first, single);
+        // plain (coherent) loads of the rows: h is also this kernel's h_out in FastEGNN's layer loop, and agg_m is cleared
+        auto rows_of = [&](const float* src, int j, f32x2& xa, f32x2& xb) {
+            xa = r.va ? ld_pair(src + r.na * H + 8 * j + 2 * q) : 0ull;
+            xb = r.vb ? ld_pair(src + r.nb * H + 8 * j + 2 * q) : 0ull;
         };
-        auto zero_row = [&](const float* src) {      // after the last read of the own row
-            if (valid)
-#pragma unroll
-                for (int j4 = 0; j4 < 16; ++j4)
-                    *reinterpret_cast<float4*>(const_cast<float*>(src) + node * H + 4 * j4) = make_float4(0.f, 0.f, 0.f, 0.f);
-        };
 
-        int g = -1;
-        float invdeg = 0.f;
-        if (valid) {
-            g = __ldg(a.batch + node);
-            const int deg = __ldg(a.rowptr + node + 1) - __ldg(a.rowptr + node);
-            invdeg = 1.0f / (float)max(deg, 1);
-        }
-        if (t == 0) sgp[0] = g;
-        if (t == nvalid - 1) sgp[1] = g;
+        // ---- h -> A (fp16 hi/lo);  D = h·Lᵀ -------------------------------------------------------------------
+        uint32_t ahi[16], alo[16];
+        float sha = 1.0f, shb = 1.0f;
+        encode_rows([&](int j, f32x2& xa, f32x2& xb, bool) { rows_of(a.h, j, xa, xb); }, ahi, alo, sha, shb);
+        float d[32];
+        tc16::mma_f16x3_rA<NT_LBO64>(d, ahi, alo, dLhi, dLlo);
+        float inv_deg_a = 0.f, inv_deg_b = 0.f;
+        if (r.va) inv_deg_a = 1.0f / (float)max(__ldg(a.rowptr + r.na + 1) - __ldg(a.rowptr + r.na), 1);
+        if (r.vb) inv_deg_b = 1.0f / (float)max(__ldg(a.rowptr + r.nb + 1) - __ldg(a.rowptr + r.nb), 1);
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
-        // ---- h -> A (fp16 hi/lo) ---------------------------------------------------------------------------
-        const float s_h = tc16::encode_row_s([&](int c, float (&v)[16], bool) { load_row16(a.h, c, v, 1.0f); },
-                                             lane_off + tA_hi, lane_off + tA_lo, 1.0f);
-        const float inv_h = 1.0f / s_h;
-        a_ready();
-        mma(dLhi, dLlo, NT_LBO64, false);            // D = h·Lᵀ
+        // ---- φ_v(h) (FastEGNN.py:183: the OLD h) per row --------------------------------------------------------
+        float phia = 0.f, phib = 0.f;
+        {
+            const float iha = 1.0f / sha, ihb = 1.0f / shb;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = 8 * j + 2 * q + e;
+                    phia = fmaf(silu(fmaf(d[4 * j + e], iha, lbs[col])), lw3s[col], phia);
+                    phib = fmaf(silu(fmaf(d[4 * j + 2 + e], ihb, lbs[col])), lw3s[col], phib);
+                }
+            const float lb3 = __ldg(a.lb3);
+            phia = lb3 + quad_sum(phia);
+            phib = lb3 + quad_sum(phib);
+        }
 
-        // ---- per-node coordinate terms ------------------------------------------------------------------------
-        float4 x = make_float4(0.f, 0.f, 0.f, 0.f), ax = x, tv = x;
-        float v0 = 0.f, v1 = 0.f, v2 = 0.f;
-        if (valid) {
-            x = *reinterpret_cast<const float4*>(a.x4 + node * 4);        // plain loads: x4 may be x4_out, agg_x is cleared
-            ax = *reinterpret_cast<const float4*>(a.agg_x + node * 4);
-            if (zero_agg) *reinterpret_cast<float4*>(const_cast<float*>(a.agg_x) + node * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-            tv = ldg4(a.trans_v + node * 4);
-            v0 = __ldg(a.vel + node * 3);
-            v1 = __ldg(a.vel + node * 3 + 1);
-            v2 = __ldg(a.vel + node * 3 + 2);
-        }
-        const int g_first = sgp[0];                  // written before the barriers above
-        const bool single = g_first == sgp[1];
-        if (single && g_first != cur_graph) {        // group-uniform
-            if (cur_graph >= 0 && t < 4) {
-                atomicAdd(a.vsum + (size_t)cur_graph * a.K + t, accS[t]);
-                accS[t] = 0.f;
+        // ---- x' = x + agg_x/deg + trans_v + φ_v·v, entry q of the thread's rows (q = 3: x' has 0, Σ(x',1) counts 1) ------
+        {
+            // every load of both rows before the first store (the stores may alias the loaded rows)
+            const bool v[2] = {r.va, r.vb};
+            const size_t node[2] = {r.na, r.nb};
+            float x[2], ax[2], tv[2], vel[2], xn[2];
+            int gr[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                x[i] = ax[i] = tv[i] = vel[i] = 0.f;
+                gr[i] = g_first;
+                if (v[i]) {
+                    x[i] = a.x4[node[i] * 4 + q];                     // plain loads: x4 may be x4_out, agg_x is cleared
+                    ax[i] = a.agg_x[node[i] * 4 + q];
+                    tv[i] = __ldg(a.trans_v + node[i] * 4 + q);
+                    if (q < 3) vel[i] = __ldg(a.vel + node[i] * 3 + q);
+                    if (!single) gr[i] = __ldg(a.batch + node[i]);
+                }
             }
-            cur_graph = g_first;
-            named_bar(bar_id, NT_GROUP);             // flush complete before new contributions arrive
-        }
-        // φ_v(h) (FastEGNN.py:183: the OLD h), then x' = x + agg_x/deg + trans_v + φ_v·v
-        float phiv = __ldg(a.lb3);
+            const float phi[2] = {phia, phib}, inv_deg[2] = {inv_deg_a, inv_deg_b};
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            uint32_t d[16];
-            tm_ld16(lane_off + tD + 16 * c, d);
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-                phiv = fmaf(silu(fmaf(__uint_as_float(d[j]), inv_h, lbs[16 * c + j])), lw3s[16 * c + j], phiv);
-        }
-        float4 xn = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (valid) {
-            xn.x = x.x + ax.x * invdeg + tv.x + phiv * v0;
-            xn.y = x.y + ax.y * invdeg + tv.y + phiv * v1;
-            xn.z = x.z + ax.z * invdeg + tv.z + phiv * v2;
-            *reinterpret_cast<float4*>(a.x4_out + node * 4) = xn;
-            if (a.loc_out) {
-                a.loc_out[node * 3 + 0] = xn.x;
-                a.loc_out[node * 3 + 1] = xn.y;
-                a.loc_out[node * 3 + 2] = xn.z;
+            for (int i = 0; i < 2; ++i) {
+                xn[i] = q < 3 ? x[i] + ax[i] * inv_deg[i] + tv[i] + phi[i] * vel[i] : 0.f;
+                if (v[i]) {
+                    if (zero_agg) const_cast<float*>(a.agg_x)[node[i] * 4 + q] = 0.f;
+                    if (q < 3 && a.loc_out) a.loc_out[node[i] * 3 + q] = xn[i];
+                    a.x4_out[node[i] * 4 + q] = xn[i];
+                }
+                if (q == 3) xn[i] = 1.0f;
             }
+            xs.add(single, r, xn[0], xn[1], gr[0], gr[1]);
         }
-        if (single) {                                // Σ(x',1) of the tile -> group accumulator
-            float s4[4] = {xn.x, xn.y, xn.z, valid ? 1.f : 0.f};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) s4[j] += __shfl_xor_sync(FULL, s4[j], o);
-            }
-            if (lane == 0) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) atomicAdd(accS + j, s4[j]);
-            }
-        } else if (valid) {
-            float* dst = a.vsum + (size_t)g * a.K;
-            atomicAdd(dst + 0, xn.x);
-            atomicAdd(dst + 1, xn.y);
-            atomicAdd(dst + 2, xn.z);
-            atomicAdd(dst + 3, 1.0f);
-        }
-        named_bar(bar_id, NT_GROUP);                 // D fully read before the next GEMM overwrites it
         if (last) continue;
 
         // ---- node MLP layer 1: h·N1aᵀ + (agg_m / deg)·N1bᵀ + agg_v·N1cᵀ  (D accumulates with one row scale) -----------
-        mma(desc(N1hi, NT_LBO64), desc(N1lo, NT_LBO64), NT_LBO64, false);   // A still holds h (row scale s_h)
-        float s2 = s_h;                              // scale the D row currently carries
-        auto l1_chunk = [&](const float* src, float rs, uint64_t bhi, uint64_t blo, bool zero_src) {
-            const float sn = tc16::encode_row_s([&](int c, float (&v)[16], bool) { load_row16(src, c, v, rs); },
-                                                lane_off + tA_hi, lane_off + tA_lo, s2);
-            if (zero_src) zero_row(src);
-            if (__any_sync(FULL, sn != s2)) {        // cold: bring the partial sums in D to the new row scale
-                const float r = sn / s2;
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    uint32_t d[16];
-                    tm_ld16(lane_off + tD + 16 * c, d);
+        // The first GEMM is not issued before the coordinate update above: with it in flight there, ptxas serialises the
+        // kernel's wgmma (C7518).
+        tc16::mma_f16x3_rA<NT_LBO64>(d, ahi, alo, desc(N1hi, NT_LBO64), desc(N1lo, NT_LBO64));   // A still holds h
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
+        float s2a = sha, s2b = shb;                   // the scales the D rows currently carry
+        auto l1_chunk = [&](const float* src, float rsa, float rsb, int c, bool zero_src) {
+            float sna = s2a, snb = s2b;
+            encode_rows(
+                [&](int j, f32x2& xa, f32x2& xb, bool) {
+                    rows_of(src, j, xa, xb);
+                    xa = mul2(xa, bc2(rsa));
+                    xb = mul2(xb, bc2(rsb));
+                },
+                ahi, alo, sna, snb);
+            if (zero_src)                             // after the last read of the rows
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) d[j] = __float_as_uint(__uint_as_float(d[j]) * r);
-                    tm_st16(lane_off + tD + 16 * c, d);
+                for (int j = 0; j < 8; ++j) {
+                    if (r.va) st_pair(const_cast<float*>(src) + r.na * H + 8 * j + 2 * q, 0ull);
+                    if (r.vb) st_pair(const_cast<float*>(src) + r.nb * H + 8 * j + 2 * q, 0ull);
                 }
-                s2 = sn;
+            if (__any_sync(FULL, sna != s2a || snb != s2b)) {   // cold: bring the partial sums in D to the new row scales
+                const float fa = sna / s2a, fb = snb / s2b;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    d[4 * j + 0] *= fa; d[4 * j + 1] *= fa;
+                    d[4 * j + 2] *= fb; d[4 * j + 3] *= fb;
+                }
+                s2a = sna;
+                s2b = snb;
             }
-            a_ready();
-            mma(bhi, blo, NT_LBO64, true);
+            tc16::mma_f16x3_rA<NT_LBO64, true>(d, ahi, alo, desc(N1hi + c * NT_W, NT_LBO64), desc(N1lo + c * NT_W, NT_LBO64));
+            tc16::mma_f16x3_rA_wait(d, ahi, alo);
         };
-        l1_chunk(a.agg_m, invdeg, desc(N1hi + NT_W, NT_LBO64), desc(N1lo + NT_W, NT_LBO64), zero_agg);
-        l1_chunk(a.agg_v, 1.0f, desc(N1hi + 2 * NT_W, NT_LBO64), desc(N1lo + 2 * NT_W, NT_LBO64), false);
+        l1_chunk(a.agg_m, inv_deg_a, inv_deg_b, 1, zero_agg);
+        l1_chunk(a.agg_v, 1.0f, 1.0f, 2, false);
 
         // ---- t1 = SiLU(D/s + attr·N1d + b1) -> A;  D = t1·N2ᵀ ----------------------------------------------
-        float attrv[DISTEGNN_MAX_NODE_ATTR];
+        float attra[DISTEGNN_MAX_NODE_ATTR], attrb[DISTEGNN_MAX_NODE_ATTR];
 #pragma unroll
-        for (int k = 0; k < DISTEGNN_MAX_NODE_ATTR; ++k) attrv[k] = (k < Na && valid) ? __ldg(a.attr + node * Na + k) : 0.f;
-        const float inv_s2 = 1.0f / s2;
-        const float inv_t = tc16::encode_row(
-            [&](int c, float (&v)[16], bool) {
-                uint32_t d[16];
-                tm_ld16(lane_off + tD + 16 * c, d);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    float z = fmaf(__uint_as_float(d[j]), inv_s2, nb1s[16 * c + j]);
-#pragma unroll
-                    for (int k = 0; k < DISTEGNN_MAX_NODE_ATTR; ++k)
-                        if (k < Na) z = fmaf(attrv[k], n1ds[k * H + 16 * c + j], z);
-                    v[j] = silu(z);
-                }
-            },
-            lane_off + tA_hi, lane_off + tA_lo);
-        a_ready();
-        mma(dN2hi, dN2lo, NT_LBO64, false);
-
-        // ---- h' = h + D/s + b2 -> HBM and -> A;  P, Q, Hn = h'·[W1a';W1b';W1vh']ᵀ, 64 columns at a time -------------
-        // The first pass stores h' to h_out, which may be h itself; the cold passes of encode_row (rows out of the fp16
-        // range) therefore read h' back from h_out instead of recomputing it from h.
-        const float inv_n = tc16::encode_row(
-            [&](int c, float (&v)[16], bool first) {
-                if (!first && valid) {
-                    load_row16(a.h_out, c, v, 1.0f);
-                    return;
-                }
-                uint32_t d[16];
-                float h0[16];
-                tm_ld16(lane_off + tD + 16 * c, d);
-                load_row16(a.h, c, h0, 1.0f);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = h0[j] + fmaf(__uint_as_float(d[j]), inv_t, nb2s[16 * c + j]);
-                if (valid) {
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4)
-                        *reinterpret_cast<float4*>(a.h_out + node * H + 16 * c + 4 * j4) =
-                            make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-                }
-            },
-            lane_off + tA_hi, lane_off + tA_lo);
-        a_ready();
-#pragma unroll 1
-        for (int o = 0; o < 3; ++o) {
-            mma(dNXhi + o * NT_DESC_N64, dNXlo + o * NT_DESC_N64, NT_LBO192, false);
-            float* dst = (o == 0 ? a.P : (o == 1 ? a.Q : a.Hn)) + node * H;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                uint32_t d[16];
-                tm_ld16(lane_off + tD + 16 * c, d);
-                if (valid) {
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4) {
-                        float4 r;
-                        r.x = __uint_as_float(d[4 * j4 + 0]) * inv_n;
-                        r.y = __uint_as_float(d[4 * j4 + 1]) * inv_n;
-                        r.z = __uint_as_float(d[4 * j4 + 2]) * inv_n;
-                        r.w = __uint_as_float(d[4 * j4 + 3]) * inv_n;
-                        if (o == 0) {
-                            const float4 bb = *reinterpret_cast<const float4*>(nxb1s + 16 * c + 4 * j4);
-                            r.x += bb.x; r.y += bb.y; r.z += bb.z; r.w += bb.w;
-                        }
-                        *reinterpret_cast<float4*>(dst + 16 * c + 4 * j4) = r;
-                    }
-                }
-            }
-            named_bar(bar_id, NT_GROUP);             // D fully read before the next GEMM overwrites it
+        for (int k = 0; k < DISTEGNN_MAX_NODE_ATTR; ++k) {
+            attra[k] = (k < Na && r.va) ? __ldg(a.attr + r.na * Na + k) : 0.f;
+            attrb[k] = (k < Na && r.vb) ? __ldg(a.attr + r.nb * Na + k) : 0.f;
         }
+        float ta = 1.0f, tb = 1.0f;
+        {
+            const float i2a = 1.0f / s2a, i2b = 1.0f / s2b;
+            encode_rows(
+                [&](int j, f32x2& xa, f32x2& xb, bool) {
+                    float za[2], zb[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = 8 * j + 2 * q + e;
+                        za[e] = fmaf(d[4 * j + e], i2a, nb1s[col]);
+                        zb[e] = fmaf(d[4 * j + 2 + e], i2b, nb1s[col]);
+#pragma unroll
+                        for (int k = 0; k < DISTEGNN_MAX_NODE_ATTR; ++k)
+                            if (k < Na) {
+                                za[e] = fmaf(attra[k], n1ds[k * H + col], za[e]);
+                                zb[e] = fmaf(attrb[k], n1ds[k * H + col], zb[e]);
+                            }
+                    }
+                    xa = pk2(silu(za[0]), silu(za[1]));
+                    xb = pk2(silu(zb[0]), silu(zb[1]));
+                },
+                ahi, alo, ta, tb);
+        }
+        tc16::mma_f16x3_rA<NT_LBO64>(d, ahi, alo, dN2hi, dN2lo);
+        tc16::mma_f16x3_rA_wait(d, ahi, alo);
+
+        // ---- h' = h + D/s + b2 -> HBM and -> A;  P, Q, Hn = h'·[W1a';W1b';W1vh']ᵀ -----------------------------------
+        const float ita = ta == 1.0f ? 1.0f : 1.0f / ta, itb = tb == 1.0f ? 1.0f : 1.0f / tb;
+        store_h_project(
+            [&](int j, f32x2& xa, f32x2& xb) {
+                const int col = 8 * j + 2 * q;
+                f32x2 ha, hb;
+                rows_of(a.h, j, ha, hb);
+                float h0, h1;
+                upk2(ha, h0, h1);
+                xa = pk2(h0 + fmaf(d[4 * j + 0], ita, nb2s[col]), h1 + fmaf(d[4 * j + 1], ita, nb2s[col + 1]));
+                upk2(hb, h0, h1);
+                xb = pk2(h0 + fmaf(d[4 * j + 2], itb, nb2s[col]), h1 + fmaf(d[4 * j + 3], itb, nb2s[col + 1]));
+            },
+            r, a.h_out, a.P, a.Q, a.Hn, dNXhi, dNXlo, nxb1s, d, ahi, alo);
     }
-    named_bar(bar_id, NT_GROUP);
-    if (cur_graph >= 0 && t < 4) atomicAdd(a.vsum + (size_t)cur_graph * a.K + t, accS[t]);
+    xs.finish();
 }
 
 // =================================================================================================
 // embedding prologue on the tensor cores (FastEGNN.forward, reference models/FastEGNN.py:298-302):
-// h0 = embedding_in(node_feat) per node (F <= 16 inputs: plain FMAs), then P/Q/Hn of layer 0 as three N = 64 wgmma
-// tile GEMMs; also node_loc -> x4, data_batch -> int32, and Σ(x,1) per graph into vsum.  256 threads = 2 tile groups.
+// h0 = embedding_in(node_feat) per node (F <= 16 inputs: plain FMAs, straight into the A fragments), then P/Q/Hn of
+// layer 0 as three N = 64 GEMMs (store_h_project); also node_loc -> x4, data_batch -> int32, and Σ(x,1) per graph into
+// vsum.  Same CTA layout as the node kernel.
 // =================================================================================================
 struct EmbedTcArgs {
     int64_t N;
@@ -336,151 +464,113 @@ struct EmbedTcArgs {
     float* h; float* x4; int32_t* batch32; float* P; float* Q; float* Hn; float* vsum;
     int32_t* n_invalid;                                                   // device counter of bad data_batch entries (or null)
 };
-constexpr int ET_THREADS = 256, ET_GROUPS = 2, ET_GROUP = 128;
-constexpr int ET_SMEM_BYTES = tmma::tm_bytes(ET_GROUPS * NT_TM_COLS) + 2 * 3 * NT_W * 2 + (DISTEGNN_MAX_NODE_FEAT + 2) * H * 4
-                              + ET_GROUPS * 8 * 4;
 
-__global__ void __launch_bounds__(ET_THREADS, 1) embed_tc_kernel(const EmbedTcArgs a) {
+__global__ void __launch_bounds__(NT_THREADS, 1) embed_tc_kernel(const EmbedTcArgs a) {
     using namespace tmma;
-    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(ET_GROUPS * NT_TM_COLS);
-    __half* NXhi = reinterpret_cast<__half*>(smem_raw);
+    __half* NXhi = reinterpret_cast<__half*>(degnn_dyn_smem);
     __half* NXlo = NXhi + 3 * NT_W;
     float* wts = reinterpret_cast<float*>(NXlo + 3 * NT_W);     // [F][64]
     float* bs = wts + DISTEGNN_MAX_NODE_FEAT * H;
     float* nxb1s = bs + H;
-    float* acc_all = nxb1s + H;
+    float* accx_all = nxb1s + H;                                // [warps][4]: Σ(x,1)
     const int tid = threadIdx.x;
-    const int grp = tid / ET_GROUP, t = tid % ET_GROUP, lane = tid & 31, wq = (tid >> 5) & 3;
+    const int lane = tid & 31, warp = tid >> 5;
+    const int wg = warp >> 2, w = warp & 3, t = tid & 127;
+    const int q = lane & 3;
     const int F = a.F;
 
-    tc16::stage_weight<ET_THREADS>(NXhi, NXlo, a.nw1a, 0, 192, tid);
-    tc16::stage_weight<ET_THREADS>(NXhi, NXlo, a.nw1b, 64, 192, tid);
-    tc16::stage_weight<ET_THREADS>(NXhi, NXlo, a.nw1h, 128, 192, tid);
-    for (int i = tid; i < F * H; i += ET_THREADS) wts[i] = a.wt[i];
+    tc16::stage_weight<NT_THREADS>(NXhi, NXlo, a.nw1a, 0, 192, tid);
+    tc16::stage_weight<NT_THREADS>(NXhi, NXlo, a.nw1b, 64, 192, tid);
+    tc16::stage_weight<NT_THREADS>(NXhi, NXlo, a.nw1h, 128, 192, tid);
+    for (int i = tid; i < F * H; i += NT_THREADS) wts[i] = a.wt[i];
     if (tid < H) {
         bs[tid] = a.bias[tid];
         nxb1s[tid] = a.nxb1[tid];
     }
-    if (tid < ET_GROUPS * 8) acc_all[tid] = 0.f;
+    if (tid < NT_WARPS * 4) accx_all[tid] = 0.f;
     fence_proxy_async_smem();
     __syncthreads();
 
-    const uint32_t lane_off = ((uint32_t)(32 * wq)) << 16;
-    const uint32_t col0 = (uint32_t)(grp * NT_TM_COLS);
-    const uint32_t tA_hi = col0, tA_lo = col0 + 32, tD = col0 + 64;
     const uint64_t dNXhi = make_b_desc(smem_u32(NXhi), NT_LBO192, 128), dNXlo = make_b_desc(smem_u32(NXlo), NT_LBO192, 128);
-    float* accS = acc_all + grp * 8;
-    int* sg = reinterpret_cast<int*>(accS + 4);
-    const uint32_t bar_id = 1 + grp;
-    int cur_graph = -1, it = 0;
+    XSum xs{a.vsum, a.K, accx_all + 4 * warp, accx_all + 16 * wg, 1u + (uint32_t)wg, t, lane, -1};
+    const int ra = 16 * w + (lane >> 2), rb = ra + 8;
+    // precondition of every per-graph reduction downstream: ids sorted and inside [0,B) (PyG batches are; the reference
+    // takes B from data_batch[-1]+1, FastEGNN.py:298).  Violations are counted for the host and clamped.
+    auto graph_of = [&](size_t node) {
+        const int64_t gi = a.batch64[node];
+        return (int)(gi < 0 ? 0 : (gi >= a.B ? a.B - 1 : gi));
+    };
 
-    const int64_t num_tiles = (a.N + TILE_M - 1) / TILE_M;
-    for (int64_t tile = (int64_t)blockIdx.x * ET_GROUPS + grp; tile < num_tiles; tile += (int64_t)gridDim.x * ET_GROUPS, ++it) {
-        int* sgp = sg + 2 * (it & 1);
-        const int64_t n0 = tile * TILE_M;
-        const int nvalid = (int)min((int64_t)TILE_M, a.N - n0);
-        const bool valid = t < nvalid;
-        const size_t node = (size_t)(n0 + (valid ? t : 0));
-        int g = -1;
-        float4 xv = make_float4(0.f, 0.f, 0.f, 0.f);
-        float f[DISTEGNN_MAX_NODE_FEAT];
-#pragma unroll
-        for (int k = 0; k < DISTEGNN_MAX_NODE_FEAT; ++k) f[k] = (valid && k < F) ? __ldg(a.feat + node * F + k) : 0.f;
-        if (valid) {
-            // precondition of every per-graph reduction downstream: ids sorted and inside [0,B) (PyG batches are; the
-            // reference takes B from data_batch[-1]+1, FastEGNN.py:298).  Violations are counted for the host and clamped.
-            const int64_t gi = a.batch64[node];
-            const bool bad = gi < 0 || gi >= a.B || (node > 0 && a.batch64[node - 1] > gi);
-            if (bad && a.n_invalid) atomicAdd(a.n_invalid, 1);
-            g = (int)(gi < 0 ? 0 : (gi >= a.B ? a.B - 1 : gi));
-            a.batch32[node] = g;
-            const float* p = a.loc + node * 3;
-            xv = make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), 0.f);
-            *reinterpret_cast<float4*>(a.x4 + node * 4) = xv;
+    const int64_t num_tiles = (a.N + NT_TILE - 1) / NT_TILE;
+    for (int64_t tile = (int64_t)blockIdx.x * NT_WG + wg; tile < num_tiles; tile += (int64_t)gridDim.x * NT_WG) {
+        const int64_t n0 = tile * NT_TILE;
+        const int nvalid = (int)min((int64_t)NT_TILE, a.N - n0);
+        Rows r;
+        r.q = q;
+        r.va = ra < nvalid;
+        r.vb = rb < nvalid;
+        r.na = (size_t)(n0 + (r.va ? ra : 0));
+        r.nb = (size_t)(n0 + (r.vb ? rb : 0));
+        {   // pull the next tile's inputs towards L2
+            const int64_t m0 = n0 + (int64_t)gridDim.x * NT_WG * NT_TILE;
+            if (m0 < a.N) {
+                const size_t mv = (size_t)min((int64_t)NT_TILE, a.N - m0), m = (size_t)m0;
+                prefetch_l2_range(a.feat + m * F, mv * F * 4, t);
+                prefetch_l2_range(a.loc + m * 3, mv * 12, t);
+                prefetch_l2_range(a.batch64 + m, mv * 8, t);
+            }
         }
-        if (t == 0) sgp[0] = g;
-        if (t == nvalid - 1) sgp[1] = g;
+        const int g_first = graph_of((size_t)n0), g_last = graph_of((size_t)(n0 + nvalid - 1));
+        const bool single = g_first == g_last;
+        xs.start_tile(g_first, single);
 
-        // h0 row -> HBM and -> A
-        const float inv_n = tc16::encode_row(
-            [&](int c, float (&v)[16], bool first) {
+        // per node: graph id (lane 0 of the quad validates and stores it), coordinate q -> x4, Σ(x,1)
+        auto node_scalars = [&](bool v, size_t node, int& gr) {
+            gr = g_first;
+            if (!v) return 0.f;
+            gr = graph_of(node);
+            if (q == 0) {
+                const int64_t gi = a.batch64[node];
+                const bool bad = gi < 0 || gi >= a.B || (node > 0 && a.batch64[node - 1] > gi);
+                if (bad && a.n_invalid) atomicAdd(a.n_invalid, 1);
+                a.batch32[node] = gr;
+            }
+            const float x = q < 3 ? __ldg(a.loc + node * 3 + q) : 0.f;
+            a.x4[node * 4 + q] = x;
+            return q < 3 ? x : 1.0f;
+        };
+        int ga, gb;
+        const float xa = node_scalars(r.va, r.na, ga), xb = node_scalars(r.vb, r.nb, gb);
+        xs.add(single, r, xa, xb, ga, gb);
+
+        float fa[DISTEGNN_MAX_NODE_FEAT], fb[DISTEGNN_MAX_NODE_FEAT];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    float z = bs[16 * c + j];
+        for (int k = 0; k < DISTEGNN_MAX_NODE_FEAT; ++k) {
+            fa[k] = (r.va && k < F) ? __ldg(a.feat + r.na * F + k) : 0.f;
+            fb[k] = (r.vb && k < F) ? __ldg(a.feat + r.nb * F + k) : 0.f;
+        }
+        uint32_t ahi[16], alo[16];
+        float d[32];
+        store_h_project(
+            [&](int j, f32x2& ya, f32x2& yb) {
+                float za[2], zb[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = 8 * j + 2 * q + e;
+                    za[e] = zb[e] = bs[col];
 #pragma unroll
                     for (int k = 0; k < DISTEGNN_MAX_NODE_FEAT; ++k)
-                        if (k < F) z = fmaf(f[k], wts[k * H + 16 * c + j], z);
-                    v[j] = valid ? z : 0.f;
-                }
-                if (first && valid) {
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4)
-                        *reinterpret_cast<float4*>(a.h + node * H + 16 * c + 4 * j4) =
-                            make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-                }
-            },
-            lane_off + tA_hi, lane_off + tA_lo);
-        tm_st_fence();
-        named_bar(bar_id, ET_GROUP);
-        // Σ(x,1) per graph
-        const int g_first = sgp[0];
-        const bool single = g_first == sgp[1];
-        if (single && g_first != cur_graph) {
-            if (cur_graph >= 0 && t < 4) {
-                atomicAdd(a.vsum + (size_t)cur_graph * a.K + t, accS[t]);
-                accS[t] = 0.f;
-            }
-            cur_graph = g_first;
-            named_bar(bar_id, ET_GROUP);
-        }
-        if (single) {
-            float s4[4] = {xv.x, xv.y, xv.z, valid ? 1.f : 0.f};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) s4[j] += __shfl_xor_sync(FULL, s4[j], o);
-            }
-            if (lane == 0) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) atomicAdd(accS + j, s4[j]);
-            }
-        } else if (valid) {
-            float* dst = a.vsum + (size_t)g * a.K;
-            atomicAdd(dst + 0, xv.x);
-            atomicAdd(dst + 1, xv.y);
-            atomicAdd(dst + 2, xv.z);
-            atomicAdd(dst + 3, 1.0f);
-        }
-#pragma unroll 1
-        for (int o = 0; o < 3; ++o) {                // P, Q, Hn = h0·[W1a;W1b;W1vh]ᵀ, 64 columns at a time
-            tc16::mma_f16x3<NT_LBO192>(tD, tA_hi, tA_lo, dNXhi + o * NT_DESC_N64, dNXlo + o * NT_DESC_N64, 1, false, 0, 2);
-            named_bar(bar_id, ET_GROUP);
-            float* dst = (o == 0 ? a.P : (o == 1 ? a.Q : a.Hn)) + node * H;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                uint32_t d[16];
-                tm_ld16(lane_off + tD + 16 * c, d);
-                if (valid) {
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4) {
-                        float4 r;
-                        r.x = __uint_as_float(d[4 * j4 + 0]) * inv_n;
-                        r.y = __uint_as_float(d[4 * j4 + 1]) * inv_n;
-                        r.z = __uint_as_float(d[4 * j4 + 2]) * inv_n;
-                        r.w = __uint_as_float(d[4 * j4 + 3]) * inv_n;
-                        if (o == 0) {
-                            const float4 bb = *reinterpret_cast<const float4*>(nxb1s + 16 * c + 4 * j4);
-                            r.x += bb.x; r.y += bb.y; r.z += bb.z; r.w += bb.w;
+                        if (k < F) {
+                            za[e] = fmaf(fa[k], wts[k * H + col], za[e]);
+                            zb[e] = fmaf(fb[k], wts[k * H + col], zb[e]);
                         }
-                        *reinterpret_cast<float4*>(dst + 16 * c + 4 * j4) = r;
-                    }
                 }
-            }
-            named_bar(bar_id, ET_GROUP);             // D fully read before the next GEMM overwrites it
-        }
+                ya = r.va ? pk2(za[0], za[1]) : 0ull;
+                yb = r.vb ? pk2(zb[0], zb[1]) : 0ull;
+            },
+            r, a.h, a.P, a.Q, a.Hn, dNXhi, dNXlo, nxb1s, d, ahi, alo);
     }
-    named_bar(bar_id, ET_GROUP);
-    if (cur_graph >= 0 && t < 4) atomicAdd(a.vsum + (size_t)cur_graph * a.K + t, accS[t]);
+    xs.finish();
 }
 
 }  // namespace degnn
@@ -522,8 +612,8 @@ extern "C" int distegnn_node_layer_fwd(int64_t n_nodes, int n_graphs, int A, int
     a.nw1h = nx + L.off[DISTEGNN_P_V_W1H];
     a.h_out = h_out; a.x4_out = x4_out; a.P = P; a.Q = Q; a.Hn = Hn; a.loc_out = node_loc_out; a.vsum = vsum;
     ensure_dynamic_smem((const void*)node_layer_tc_kernel, (int)NT_SMEM_BYTES);
-    const int64_t tiles = (n_nodes + TILE_M - 1) / TILE_M;
-    int64_t grid = (tiles + NT_GROUPS - 1) / NT_GROUPS;
+    const int64_t tiles = (n_nodes + NT_TILE - 1) / NT_TILE;
+    int64_t grid = (tiles + NT_WG - 1) / NT_WG;
     if (grid > sm_count()) grid = sm_count();
     node_layer_tc_kernel<<<(unsigned)grid, NT_THREADS, NT_SMEM_BYTES, (cudaStream_t)stream>>>(a);
     DEGNN_CHECK_LAUNCH();
@@ -553,10 +643,10 @@ extern "C" int distegnn_embed_fwd(int64_t n_nodes, int n_graphs, int F, int A, i
     a.h = h; a.x4 = x4; a.batch32 = batch32; a.P = P; a.Q = Q; a.Hn = Hn; a.vsum = vsum;
     a.n_invalid = n_invalid;
     ensure_dynamic_smem((const void*)embed_tc_kernel, (int)ET_SMEM_BYTES);
-    const int64_t tiles = (n_nodes + TILE_M - 1) / TILE_M;
-    int64_t grid = (tiles + ET_GROUPS - 1) / ET_GROUPS;
+    const int64_t tiles = (n_nodes + NT_TILE - 1) / NT_TILE;
+    int64_t grid = (tiles + NT_WG - 1) / NT_WG;
     if (grid > sm_count()) grid = sm_count();
-    embed_tc_kernel<<<(unsigned)grid, ET_THREADS, ET_SMEM_BYTES, (cudaStream_t)stream>>>(a);
+    embed_tc_kernel<<<(unsigned)grid, NT_THREADS, ET_SMEM_BYTES, (cudaStream_t)stream>>>(a);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

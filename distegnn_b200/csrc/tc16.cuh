@@ -99,7 +99,8 @@ __device__ __forceinline__ void mma_f16x3(uint32_t d, uint32_t a_hi, uint32_t a_
 // N = 64.  a_hi / a_lo are the A fragments of the four k-steps (tile_mma.cuh wgmma_f16_m64n64k16_rA: registers 4ks ..
 // 4ks+3 for k-step ks), i.e. element (row, k) sits where an m64n64 accumulator keeps (row, column k).  Asynchronous:
 // issues the 12 wgmma and commits them; mma_f16x3_rA_wait completes the group before d is read or a_hi / a_lo reused.
-template <uint32_t LBO>
+// ACCUMULATE: D += instead of D =.
+template <uint32_t LBO, bool ACCUMULATE = false>
 __device__ __forceinline__ void mma_f16x3_rA(float (&d)[32], const uint32_t (&a_hi)[16], const uint32_t (&a_lo)[16],
                                              uint64_t b_hi, uint64_t b_lo) {
     constexpr uint64_t B_KSTEP = (2 * LBO) >> 4;
@@ -108,7 +109,7 @@ __device__ __forceinline__ void mma_f16x3_rA(float (&d)[32], const uint32_t (&a_
                                                             b + ks * B_KSTEP);
     };
     tmma::wgmma_fence();
-    mma(std::false_type{}, a_lo, 0, b_hi);
+    mma(std::integral_constant<bool, ACCUMULATE>{}, a_lo, 0, b_hi);
 #pragma unroll
     for (int ks = 1; ks < 4; ++ks) mma(std::true_type{}, a_lo, ks, b_hi);
 #pragma unroll
@@ -128,21 +129,6 @@ __device__ __forceinline__ void mma_f16x3_rA_wait(float (&d)[32], uint32_t (&a_h
     }
 }
 
-// 16 fp32 values (·s) -> 8 packed hi words + 8 packed lo words; `mx` tracks max |hi|
-template <bool SCALED>
-__device__ __forceinline__ void split16(const float (&v)[16], float s, uint32_t (&hi)[8], uint32_t (&lo)[8],
-                                        __half2& mx) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const float x0 = SCALED ? v[2 * j] * s : v[2 * j], x1 = SCALED ? v[2 * j + 1] * s : v[2 * j + 1];
-        const __half2 h = __floats2half2_rn(x0, x1);            // x0 -> low half (even k)
-        const float2 hf = __half22float2(h);
-        const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-        mx = __hmax2(mx, __habs2(h));
-        hi[j] = *reinterpret_cast<const uint32_t*>(&h);
-        lo[j] = *reinterpret_cast<const uint32_t*>(&l);
-    }
-}
 __device__ __forceinline__ bool row_overflow(__half2 mx) {
     return fmaxf(__low2float(mx), __high2float(mx)) > RANGE;
 }
@@ -154,50 +140,6 @@ __device__ __forceinline__ void range_scale(float rowmax, float& s, float& inv_s
     inv_s = 1.0f / s;
 }
 
-// Encode one 64-wide fp32 row, produced 16 values at a time by f(chunk, v, first_pass), into the A operand
-// (tile-memory columns ta_hi.. / ta_lo.., both including the warp's lane offset) with row scale `s_in` (a power of two
-// the row already carries, 1 normally).  Returns the scale actually used (<= s_in): smaller only if the row
-// would leave the fp16 range.  The caller issues tm_st_fence() afterwards and multiplies the accumulator row
-// by 1/scale in its epilogue.
-template <class F>
-__device__ __forceinline__ float encode_row_s(F&& f, uint32_t ta_hi, uint32_t ta_lo, float s_in) {
-    __half2 mx = __floats2half2_rn(0.f, 0.f);
-    const bool pre_scaled = __any_sync(FULL, s_in != 1.0f);
-    if (!pre_scaled) {
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-            float v[16];
-            uint32_t hi[8], lo[8];
-            f(c, v, true);
-            split16<false>(v, 1.0f, hi, lo, mx);
-            tmma::tm_st8(ta_hi + 8 * c, hi);
-            tmma::tm_st8(ta_lo + 8 * c, lo);
-        }
-        if (!__any_sync(FULL, row_overflow(mx))) return 1.0f;
-    }
-    // cold: some row of this warp carries a scale already or leaves the fp16 range
-    float fm = 0.f, sc, inv_unused;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-        float v[16];
-        f(c, v, pre_scaled && true);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) fm = fmaxf(fm, fabsf(v[j]));
-    }
-    range_scale(fm, sc, inv_unused);
-    sc = fminf(sc, s_in);
-    tmma::tm_st_fence();
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-        float v[16];
-        uint32_t hi[8], lo[8];
-        f(c, v, false);
-        split16<true>(v, sc, hi, lo, mx);
-        tmma::tm_st8(ta_hi + 8 * c, hi);
-        tmma::tm_st8(ta_lo + 8 * c, lo);
-    }
-    return sc;
-}
 // ---- register-pair flavour (fp32 pairs, common.cuh) ------------------------------------------------------------
 constexpr std::false_type kFast{};   // silu4p flavour tags
 constexpr std::true_type kSafe{};
@@ -209,12 +151,6 @@ __device__ __forceinline__ void split16p(const f32x2 (&v)[8], float s, uint32_t 
         split_pair(SCALED ? mul2(v[j], bc2(s)) : v[j], hi[j], lo[j]);
         mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[j])));
     }
-}
-// Convenience: unscaled input, returns 1/scale for the epilogue.
-template <class F>
-__device__ __forceinline__ float encode_row(F&& f, uint32_t ta_hi, uint32_t ta_lo) {
-    const float sc = encode_row_s(f, ta_hi, ta_lo, 1.0f);
-    return sc == 1.0f ? 1.0f : 1.0f / sc;
 }
 
 }  // namespace tc16

@@ -80,6 +80,7 @@ __device__ __forceinline__ void tm_ld16(uint32_t taddr, uint32_t (&r)[16]) {
     for (int i = 0; i < 4; ++i) tm_ld4(taddr + 4 * i, &r[4 * i]);
 }
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // ---- wgmma: one 64-row block of a tile, N = 64, fp16 operands, fp32 accumulators in registers ---------------------------
 // Accumulator fragment of m64n64 (thread = lane l of warp w of the warpgroup): d[4j+0], d[4j+1] = row 16w + l/4,
