@@ -6,17 +6,20 @@
 // the graph in the form the edge kernels consume: int32 CSR by destination row (rowptr / row / col) and edge_attr in CSR
 // order.  Everything the host used to decide is decided on the device, so the call neither synchronises nor needs the
 // edge count in advance (the caller passes a CAPACITY; the true count lands in info[0], an overflow flag in info[1]):
-//   1. bounding box of the positions (block reduction + ordered-int atomics)
-//   2. uniform grid: cell size = radius, grown x1.5 until the dense cell table fits the caller's table_cells
+//   1. bounding box of the finite coordinates (block reduction + ordered-int atomics)
+//   2. uniform grid (radius_grid.cuh): cell size = radius·(1 + 2^-10), grown x1.5 until the dense cell table fits the
+//      caller's table_cells; every key lies inside the table for any position, ±inf and NaN included
 //   3. cell key per node + histogram; exclusive scan of the histogram = first position of every cell (cub)
 //   4. node ids sorted by key (cub radix sort), so that a warp scans neighbouring cells together
 //   5. count pass (27 cells as 9 contiguous key ranges) -> degrees -> exclusive scan = rowptr (cub)
 //   6. fill pass: col, row, edge length into edge_attr columns, at rowptr offsets
-// `dist < r` as torch_cluster (strict), j != i unless `loop`, same graph id only.
+// `dist < r` as torch_cluster (strict, the fp32 `d2 < r2`), j != i unless `loop`, same graph id only.  A node with a
+// non-finite coordinate has an inf or NaN d2 to every node, itself included, so it gets no edges.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "radius_grid.cuh"
 
 namespace degnn {
 
@@ -68,8 +71,10 @@ __global__ void __launch_bounds__(256) rcsr_bounds_kernel(const RcsrArgs a) {
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
             const float v = __ldg(a.pos + i * 3 + d);
-            lo[d] = fminf(lo[d], v);
-            hi[d] = fmaxf(hi[d], v);
+            if (isfinite(v)) {                            // an inf would stretch the grid over nothing
+                lo[d] = fminf(lo[d], v);
+                hi[d] = fmaxf(hi[d], v);
+            }
         }
     }
 #pragma unroll
@@ -89,34 +94,33 @@ __global__ void __launch_bounds__(256) rcsr_bounds_kernel(const RcsrArgs a) {
 __global__ void rcsr_grid_kernel(const RcsrArgs a) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
     GridDev g;
-    const float lo[3] = {ord2f(a.bounds[0]), ord2f(a.bounds[1]), ord2f(a.bounds[2])};
-    const float ext[3] = {ord2f(a.bounds[3]) - lo[0], ord2f(a.bounds[4]) - lo[1], ord2f(a.bounds[5]) - lo[2]};
-    float cell = a.radius;
-    int d[3];
-    for (int it = 0; it < 200; ++it) {                // grow the cell until the dense table fits
-        bool ok = true;
-        double cells = (double)a.B;
-        for (int k = 0; k < 3; ++k) {
-            const float q = ext[k] / cell;
-            d[k] = q < 1.0e6f ? (int)q + 1 : 1000001;
-            if (d[k] > 1024) ok = false;
-            cells *= (double)d[k];
-        }
-        if (ok && cells + 1.0 <= (double)a.table_cells) break;
-        cell *= 1.5f;
+    float lo[3], ext[3];
+    for (int k = 0; k < 3; ++k) {
+        lo[k] = ord2f(a.bounds[k]);
+        float hi = ord2f(a.bounds[3 + k]);
+        if (!(lo[k] <= hi)) lo[k] = hi = 0.f;        // no finite coordinate on this axis
+        ext[k] = hi - lo[k];                          // +inf if the finite range exceeds FLT_MAX: one slab on that axis
     }
+    const RadiusGridSize s = radius_grid_size(ext, a.radius, a.B, a.table_cells);
     g.ox = lo[0]; g.oy = lo[1]; g.oz = lo[2];
-    g.inv_cell = 1.0f / cell;
-    g.nx = d[0]; g.ny = d[1]; g.nz = d[2];
-    g.ncell = d[0] * d[1] * d[2];
+    g.inv_cell = 1.0f / s.cell;
+    g.nx = s.dims[0]; g.ny = s.dims[1]; g.nz = s.dims[2];
+    g.ncell = s.ncell;
     *a.grid = g;
     a.info[2] = g.ncell * a.B;
 }
 
+// Cell index along one axis, in [0, n) for any coordinate: below the origin -> 0, beyond the last cell (+inf included)
+// -> n - 1, NaN -> 0.  Monotone in x, so clamping only merges end cells, which the 27-cell scan still covers.
+__device__ __forceinline__ int axis_cell(float x, float o, float inv_cell, int n) {
+    const float q = (x - o) * inv_cell;
+    return q > 0.f ? (q < (float)n ? (int)q : n - 1) : 0;
+}
+
 __device__ __forceinline__ void cell_of(const GridDev& g, float x, float y, float z, int& ix, int& iy, int& iz) {
-    ix = min(max((int)((x - g.ox) * g.inv_cell), 0), g.nx - 1);
-    iy = min(max((int)((y - g.oy) * g.inv_cell), 0), g.ny - 1);
-    iz = min(max((int)((z - g.oz) * g.inv_cell), 0), g.nz - 1);
+    ix = axis_cell(x, g.ox, g.inv_cell, g.nx);
+    iy = axis_cell(y, g.oy, g.inv_cell, g.ny);
+    iz = axis_cell(z, g.oz, g.inv_cell, g.nz);
 }
 
 __global__ void __launch_bounds__(256) rcsr_keys_kernel(const RcsrArgs a) {
@@ -265,6 +269,7 @@ extern "C" int distegnn_radius_graph_csr(int64_t n_nodes, int n_graphs, const fl
     DEGNN_CHECK_ARG(capacity >= 0 && capacity < INT32_MAX && (capacity == 0 || (row && col)), "bad capacity / null edge buffers");
     DEGNN_CHECK_ARG(radius > 0.f && edge_attr_nf >= 0 && edge_attr_nf <= DISTEGNN_MAX_EDGE_ATTR, "bad radius / edge_attr_nf");
     DEGNN_CHECK_ARG(n_graphs == 1 || data_batch, "data_batch needed for more than one graph");
+    DEGNN_CHECK_ARG((int64_t)n_graphs + 1 <= table_cells, "table_cells must hold one cell per graph plus one");
     int64_t need = 0;
     if (int rc = distegnn_radius_csr_workspace_bytes(n_nodes, table_cells, &need)) return rc;
     if (workspace_bytes < need) {

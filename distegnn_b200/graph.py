@@ -17,6 +17,7 @@ from . import _lib
 Tensor = torch.Tensor
 _MAX_DIM = 1024            # cells per axis
 _MAX_TABLE = 1 << 27       # entries of the dense cell table (graphs x cells)
+_FLT_MAX = float(torch.finfo(torch.float32).max)
 
 
 def radius_graph(pos: Tensor, r: float, batch: Optional[Tensor] = None, loop: bool = False,
@@ -39,15 +40,25 @@ def radius_graph(pos: Tensor, r: float, batch: Optional[Tensor] = None, loop: bo
     be = cuda_backend()
     x4 = torch.zeros(N, 4, dtype=torch.float32, device=dev)
     x4[:, :3] = pos.detach().to(torch.float32)
+    if not bool(torch.isfinite(x4[:, :3]).all()):
+        raise ValueError("radius_graph: positions must be finite (partition.radius_graph_csr gives nodes with an inf or "
+                         "NaN coordinate no edges instead)")
     batch32 = None if batch is None else batch.to(torch.int32).contiguous()
     B = 1 if batch is None else int(batch.max().item()) + 1
+    if B + 1 > _MAX_TABLE:
+        raise ValueError(f"radius_graph: {B} graphs exceed the cell table ({_MAX_TABLE} entries)")
     lo, hi = x4[:, :3].amin(0), x4[:, :3].amax(0)
     lo_h = [float(v) for v in lo.tolist()]
-    ext = [float(v) for v in (hi - lo).tolist()]
-    cell = float(r)
+    ext = [h - l for h, l in zip(hi.tolist(), lo_h)]          # float64: finite even where the fp32 difference overflows
+    # first cell r·(1 + 2^-10) in fp32, the margin that keeps pairs closer than r within adjacent cells despite the
+    # rounding of the fp32 cell index (csrc/radius_grid.cuh)
+    cell = float(torch.tensor(float(r), dtype=torch.float32) * (1.0 + 2.0 ** -10))
     while True:                                               # grow the cell until the dense table fits
         dims = [min(int(e / cell) + 1, 1 << 30) for e in ext]
         if max(dims) <= _MAX_DIM and B * dims[0] * dims[1] * dims[2] + 1 <= _MAX_TABLE:
+            break
+        if cell * 1.5 > _FLT_MAX:                             # r tiny against an extent near FLT_MAX: one cell per graph
+            dims = [1, 1, 1]
             break
         cell *= 1.5
     inv_cell = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(cell, dtype=torch.float32)   # the kernel's 1/cell

@@ -225,7 +225,8 @@ DISTEGNN_API int distegnn_virtual_layer_bwd(int64_t n_nodes, int n_graphs, int A
 /* On-device radius graph (SURVEY §8 f-2): replaces the host-side `radius_graph(pos_i, r=radius, max_num_neighbors=N)`
  * + `edge_attr = |dx|` of the reference's partitioners (datasets/distribute_graphs.py:43-44; PyG / torch_cluster).
  * Uniform-grid cell list; the caller sorts the nodes' cell keys (key = graph*ncell + (ix*ny + iy)*nz + iz, cell size >=
- * radius, ix = (int)((x - origin_x) * (1/cell)) clamped to the grid) and passes `order` (node ids in key order) and the
+ * radius — take radius*(1 + 2^-10) or more: with exactly radius the rounding of the fp32 index can put two nodes closer
+ * than radius two cells apart — ix = (int)((x - origin_x) * (1/cell)) clamped to the grid) and passes `order` (node ids in key order) and the
  * dense table cell_start[n_graphs*ncell + 1] (first position of every key).  origin_host[3] / dims_host[3] are HOST
  * arrays.  Two phases because the edge count is only known after the first:
  *   distegnn_radius_count -> deg[i] = number of j (same graph, j != i unless loop) with |x_i - x_j| < radius
@@ -244,9 +245,11 @@ DISTEGNN_API int distegnn_radius_fill(int64_t n_nodes, const float* x4, const in
  * reference-boundary tensors in (pos [N,3] fp32, data_batch int64 [N] sorted, may be NULL for one graph), int32 CSR by
  * destination out (rowptr [N+1], row / col [capacity]) plus edge_attr [capacity, edge_attr_nf] = the edge length in every
  * column (datasets/distribute_graphs.py:43-44).  Pairs with |x_i - x_j| < radius (strict, as torch_cluster), j != i unless
- * `loop`, same graph only.  Bounding box, grid sizing (cell >= radius, grown until graphs x cells <= table_cells), cell
- * keys, sort, counts and prefix sums all happen on the device; info [4] (device): [0] edges found, [1] 1 if that exceeds
- * `capacity` (then only rowptr is complete), [2] cells used.  capacity = 0 runs the count only (row/col may be NULL). */
+ * `loop`, same graph only.  Bounding box, grid sizing (cell >= radius*(1 + 2^-10), grown until graphs x cells + 1 <=
+ * table_cells; needs n_graphs + 1 <= table_cells), cell keys, sort, counts and prefix sums all happen on the device;
+ * info [4] (device): [0] edges found, [1] 1 if that exceeds `capacity` (then only rowptr is complete), [2] cells used.
+ * capacity = 0 runs the count only (row/col may be NULL).  Any position is accepted: a node with an inf or NaN
+ * coordinate gets no edges, the others their normal ones. */
 DISTEGNN_API int distegnn_radius_csr_workspace_bytes(int64_t n_nodes, int64_t table_cells, int64_t *bytes_host);
 DISTEGNN_API int distegnn_radius_graph_csr(int64_t n_nodes, int n_graphs, const float *pos, const int64_t *data_batch,
                                            float radius, int loop, int edge_attr_nf, int64_t capacity,
