@@ -60,6 +60,15 @@ def rowwise(got, ref, zero_rows=None):
     return float(((got - ref).abs().amax(1) / ref.abs().amax(1).clamp(min=FLOOR)).max())
 
 
+def terms_rowwise(got, ref, terms):
+    """Row-wise error of a short signed sum, relative to the largest magnitude of the terms summed into the row."""
+    assert torch.isfinite(got).all(), "non-finite output"
+    if got.shape[0] == 0:
+        return 0.0
+    err = (got.double() - ref.double()).abs().amax(1)
+    return float((err / terms.amax(1).clamp(min=FLOOR)).max())
+
+
 def rel(got, ref):
     assert torch.isfinite(got).all(), "non-finite output"
     return float((got.double() - ref.double()).abs().max()) / max(FLOOR, float(ref.abs().max()))

@@ -23,7 +23,7 @@ import torch
 
 from distegnn_b200 import FastEGNN, _lib
 from oracle import fastegnn_oracle as orc
-from tests.helpers import FLOOR, check_bounds, rel, rowwise, within_rerun_bound
+from tests.helpers import FLOOR, check_bounds, rel, rowwise, terms_rowwise, within_rerun_bound
 from tests.shadow_backend import ShadowBackend, _fields
 
 pytestmark = pytest.mark.gpu
@@ -65,13 +65,6 @@ def packed(F, Na, C):
 
 def K_of(C):
     return 4 + 3 * C + H * C
-
-
-def terms_rowwise(got, ref, terms):
-    """Row-wise error of a short signed sum, relative to the largest magnitude of the terms summed into the row."""
-    assert torch.isfinite(got).all(), "non-finite output"
-    err = (got.double() - ref.double()).abs().amax(1)
-    return float((err / terms.amax(1).clamp(min=FLOOR)).max())
 
 
 def fmt(errs):
