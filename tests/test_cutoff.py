@@ -18,6 +18,7 @@ import pytest
 import torch
 
 from distegnn_b200 import FastEGNN, _lib, cutoff_edges_csr, differentiable_rollout, radius_graph_csr, rollout, synth
+from distegnn_b200.backend import CudaBackend
 from distegnn_b200.shards import CSRGraph
 from oracle import cutoff_oracle as co
 from oracle import fastegnn_oracle as orc
@@ -250,8 +251,10 @@ def _check_against_oracle(cand, out, ea, pos, rate, batch=None, B=1, exact_lengt
     crp, crow, ccol = _valid(cand)
     rp, row, col = _valid(out)
     p = pos.cpu().numpy()
-    l32 = (pos[torch.from_numpy(crow).long().to(pos.device)] - pos[torch.from_numpy(ccol).long().to(pos.device)]
-           ).norm(dim=1).cpu().numpy()
+    ea32 = torch.empty(crow.shape[0], 1, dtype=torch.float32, device=pos.device)  # the kernel's own fp32 lengths
+    CudaBackend().edge_lengths(torch.from_numpy(crow).to(pos.device), torch.from_numpy(ccol).to(pos.device), pos, None,
+                               ea32)
+    l32 = ea32[:, 0].cpu().numpy()
     lengths = co.lengths64(p, crow, ccol) if exact_lengths else l32
     orp, orow, ocol, _, mask = co.cutoff_csr(crp, crow, ccol, p, rate, None if batch is None else batch.cpu().numpy(), B,
                                              lengths=lengths)
