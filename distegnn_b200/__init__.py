@@ -4,11 +4,10 @@ Public surface mirrors the reference: ``from distegnn_b200 import FastEGNN`` is 
 ``from models.FastEGNN import FastEGNN``.
 """
 from .fast_egnn import E_GCL_vel, FastEGNN  # noqa: F401
-from .graph import radius_graph, split_large_graph_random  # noqa: F401  (on-device graph construction, SURVEY §8 f-2)
 from .loss import train_loss  # noqa: F401  (fused weighted-MSE + MMD loss of the training step, SURVEY §8 f-3)
-from .partition import cutoff_edges_csr, kmeans_labels, radius_graph_csr, split_large_graph  # noqa: F401  (CSR out, no host round trip)
+from .partition import cutoff_edges_csr, kmeans_labels, radius_graph, radius_graph_csr, split_large_graph  # noqa: F401  (CSR out, no host round trip)
 from .rollout import RolloutResult, differentiable_rollout, rollout  # noqa: F401  (multi-step, on the device)
 
 __all__ = ["FastEGNN", "E_GCL_vel", "radius_graph", "radius_graph_csr", "kmeans_labels", "split_large_graph",
-           "split_large_graph_random", "train_loss", "rollout", "RolloutResult",
+           "train_loss", "rollout", "RolloutResult",
            "differentiable_rollout", "cutoff_edges_csr"]

@@ -49,8 +49,6 @@ SIGNATURES = {
     "distegnn_kmeans_lloyd": [_i64, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp],
     "distegnn_virtual_layer_bwd": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 16,
     "distegnn_virtual_bwd_prepare": [_i32, _i32, _i32, _vp, _vp, _vp],
-    "distegnn_radius_count": [_i64, _vp, _vp, _vp, _vp, _vp, C.c_float, _vp, C.c_float, _i32, _vp, _vp],
-    "distegnn_radius_fill": [_i64, _vp, _vp, _vp, _vp, _vp, C.c_float, _vp, C.c_float, _i32, _vp, _vp, _vp, _vp, _vp],
     "distegnn_virtual_layer_fwd": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 10,
     "distegnn_node_layer_fwd": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 20,
     "distegnn_virtual_update_fwd": [_i32, _i32, _i32, _i32, _u32] + [_vp] * 10,
@@ -77,7 +75,7 @@ SIGNATURES = {
     "distegnn_vsum_combine_det": [_i64, _i32, _i32, _u32] + [_vp] * 4 + [_i64, _vp],
     "distegnn_rollout_centroid_det": [_i64, _i32] + [_vp] * 4,
 }
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 _lib: Optional[C.CDLL] = None
 

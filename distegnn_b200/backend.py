@@ -140,29 +140,6 @@ class CudaBackend:
               "virtual_layer_bwd")
         self.launches += 1 if N else 0
 
-    @staticmethod
-    def _grid_host(grid):
-        import ctypes as C
-        origin, cell, dims = grid
-        return (C.c_float * 3)(*origin), float(cell), (C.c_int32 * 3)(*dims)
-
-    def radius_count(self, N, x4, batch32, order32, cell_start, grid, r, loop, deg) -> None:
-        """Neighbour counts of the on-device radius graph (csrc/radius_graph.cu)."""
-        import ctypes as C
-        o, cell, d = self._grid_host(grid)
-        check(self.lib.distegnn_radius_count(N, ptr(x4), ptr(batch32), ptr(order32), ptr(cell_start),
-                                             C.cast(o, C.c_void_p), cell, C.cast(d, C.c_void_p), float(r), int(loop),
-                                             ptr(deg), self._s(x4)), "radius_count")
-        self.launches += 1 if N else 0
-
-    def radius_fill(self, N, x4, batch32, order32, cell_start, grid, r, loop, rowptr, row, col, dist) -> None:
-        import ctypes as C
-        o, cell, d = self._grid_host(grid)
-        check(self.lib.distegnn_radius_fill(N, ptr(x4), ptr(batch32), ptr(order32), ptr(cell_start),
-                                            C.cast(o, C.c_void_p), cell, C.cast(d, C.c_void_p), float(r), int(loop),
-                                            ptr(rowptr), ptr(row), ptr(col), ptr(dist), self._s(x4)), "radius_fill")
-        self.launches += 1 if N else 0
-
     def virtual_layer(self, dims, flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vsum, det_ws=None) -> None:
         """`det_ws`: the deterministic kernel (vsum is complete only after vsum_combine)."""
         N, B, A, Cn, Na = dims

@@ -159,6 +159,17 @@ __device__ __forceinline__ void silu4t(f32x2& a, f32x2& b, float& qmax) {
 __device__ __forceinline__ float4 ldg4(const float* p) {
     return __ldg(reinterpret_cast<const float4*>(p));
 }
+// The fp32 squared edge length, the one expression behind every edge length on the device: the radius build's fill pass
+// (d2 < r2, edge_attr = sqrtf(d2)), the rollout's edge lengths and their backward, and the cutoff's keys.  They must
+// agree bit for bit: the differentiable rollout's backward rebuilds each step's graph and checks its edge count, and the
+// cutoff ranks edges by keys that must equal the build's edge_attr.
+__device__ __forceinline__ float edge_len2(float dx, float dy, float dz) { return dx * dx + dy * dy + dz * dz; }
+// pos[i] − pos[j] of pos [N,3]
+__device__ __forceinline__ void edge_delta(const float* pos, int i, int j, float& dx, float& dy, float& dz) {
+    dx = __ldg(pos + (int64_t)i * 3) - __ldg(pos + (int64_t)j * 3);
+    dy = __ldg(pos + (int64_t)i * 3 + 1) - __ldg(pos + (int64_t)j * 3 + 1);
+    dz = __ldg(pos + (int64_t)i * 3 + 2) - __ldg(pos + (int64_t)j * 3 + 2);
+}
 __device__ __forceinline__ float4 fma4(float s, float4 w, float4 a) {
     return make_float4(fmaf(s, w.x, a.x), fmaf(s, w.y, a.y), fmaf(s, w.z, a.z), fmaf(s, w.w, a.w));
 }

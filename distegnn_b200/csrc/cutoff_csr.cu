@@ -115,11 +115,9 @@ __global__ void __launch_bounds__(256) cut_keys_kernel(const CutArgs a) {
     const int64_t valid = cut_valid(a);
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < valid; e += (int64_t)gridDim.x * blockDim.x) {
         const int i = __ldg(a.row_in + e), j = __ldg(a.col_in + e);
-        // the arithmetic of distegnn_radius_graph_csr's fill pass and distegnn_edge_lengths_csr
-        const float ddx = __ldg(a.pos + (int64_t)i * 3) - __ldg(a.pos + (int64_t)j * 3);
-        const float ddy = __ldg(a.pos + (int64_t)i * 3 + 1) - __ldg(a.pos + (int64_t)j * 3 + 1);
-        const float ddz = __ldg(a.pos + (int64_t)i * 3 + 2) - __ldg(a.pos + (int64_t)j * 3 + 2);
-        const float dd = sqrtf(ddx * ddx + ddy * ddy + ddz * ddz);
+        float ddx, ddy, ddz;
+        edge_delta(a.pos, i, j, ddx, ddy, ddz);
+        const float dd = sqrtf(edge_len2(ddx, ddy, ddz));
         a.keys[e] = isnan(dd) ? NAN_KEY : __float_as_uint(dd);     // dd >= 0: the bits order as the values
     }
 }

@@ -173,7 +173,7 @@ __global__ void __launch_bounds__(256) rcsr_scan_kernel(const RcsrArgs a) {
                 if (j == i && !a.loop) continue;
                 const float4 pj = ldg4(a.x4 + (size_t)j * 4);
                 const float ddx = p.x - pj.x, ddy = p.y - pj.y, ddz = p.z - pj.z;
-                const float d2 = ddx * ddx + ddy * ddy + ddz * ddz;
+                const float d2 = edge_len2(ddx, ddy, ddz);
                 if (d2 < r2) {
                     if (FILL) {
                         if (w < a.capacity) {

@@ -78,11 +78,9 @@ __global__ void __launch_bounds__(256) edge_lengths_kernel(int64_t E, int A, con
     const int64_t nE = n_edges_dev ? min((int64_t)__ldg(n_edges_dev), E) : E;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nE; e += (int64_t)gridDim.x * blockDim.x) {
         const int i = __ldg(row + e), j = __ldg(col + e);
-        // same arithmetic as the fill pass of distegnn_radius_graph_csr: a rebuilt and a kept graph agree bit for bit
-        const float ddx = __ldg(pos + (int64_t)i * 3) - __ldg(pos + (int64_t)j * 3);
-        const float ddy = __ldg(pos + (int64_t)i * 3 + 1) - __ldg(pos + (int64_t)j * 3 + 1);
-        const float ddz = __ldg(pos + (int64_t)i * 3 + 2) - __ldg(pos + (int64_t)j * 3 + 2);
-        const float dd = sqrtf(ddx * ddx + ddy * ddy + ddz * ddz);
+        float ddx, ddy, ddz;
+        edge_delta(pos, i, j, ddx, ddy, ddz);
+        const float dd = sqrtf(edge_len2(ddx, ddy, ddz));
         for (int c = 0; c < A; ++c) ea[e * A + c] = dd;
     }
 }
@@ -136,11 +134,9 @@ __global__ void __launch_bounds__(256) edge_lengths_bwd_kernel(int64_t E, int A,
         if (e < nE) {
             i = __ldg(row + e);
             const int j = __ldg(col + e);
-            // the forward's arithmetic (edge_lengths_kernel and the radius fill pass)
-            const float ddx = __ldg(pos + (int64_t)i * 3) - __ldg(pos + (int64_t)j * 3);
-            const float ddy = __ldg(pos + (int64_t)i * 3 + 1) - __ldg(pos + (int64_t)j * 3 + 1);
-            const float ddz = __ldg(pos + (int64_t)i * 3 + 2) - __ldg(pos + (int64_t)j * 3 + 2);
-            const float dd = sqrtf(ddx * ddx + ddy * ddy + ddz * ddz);
+            float ddx, ddy, ddz;
+            edge_delta(pos, i, j, ddx, ddy, ddz);
+            const float dd = sqrtf(edge_len2(ddx, ddy, ddz));
             if (dd > 0.f) {
                 float g = 0.f;
                 for (int k = 0; k < A; ++k) g += __ldg(g_ea + e * A + k);

@@ -1,6 +1,7 @@
 """On-device graph partitioning and construction (SURVEY §8 f-2) — the device form of datasets/distribute_graphs.py.
 
     graph, edge_attr = radius_graph_csr(pos, r, batch=None)        # CSR by destination, int32, no int64 edge_index
+    edge_index, edge_attr = radius_graph(pos, r, batch=None)         # the same graph as PyG's int64 edge_index
     graph, edge_attr = cutoff_edges_csr(graph, pos, 0.5, batch)      # FastEGNN's cutoff: the shortest half of each graph
     labels = kmeans_labels(pos, world_size)                          # == sklearn KMeans(random_state=0).fit_predict
     parts = split_large_graph(pos, x, target, vel, attr, r, P, split_mode="random" | "kmeans")
@@ -124,6 +125,36 @@ def _resized(buf: RadiusGraphBuffers, capacity: int) -> RadiusGraphBuffers:
     new.graph = CSRGraph(new.rowptr, new.col, new.row)
     new.graph.n_edges_dev, new.graph.info = new.info[0:1], new.info
     return new
+
+
+def radius_graph(pos: Tensor, r: float, batch: Optional[Tensor] = None, loop: bool = False,
+                 max_num_neighbors: Optional[int] = None, edge_attr_nf: int = 2) -> Tuple[Tensor, Tensor]:
+    """`radius_graph_csr` in the call shape of `torch_geometric.nn.radius_graph` as the reference's partitioners use it
+    (datasets/distribute_graphs.py:43-44: `radius_graph(pos_i, r=radius, max_num_neighbors=pos_i.size(0))` followed by
+    `edge_attr = ‖Δx‖` repeated twice).
+
+    Returns (edge_index [2,E] int64 with edge_index[0] = i ascending, edge_attr [E, edge_attr_nf] fp32 = the edge length
+    in every column).  `max_num_neighbors` is accepted for signature compatibility; the reference always passes the node
+    count (no cap), a smaller cap raises.  Non-finite positions raise.  Counts in int32 as `radius_graph_csr` does, so
+    E < 2^31."""
+    if pos.device.type != "cuda":
+        raise _lib.DistEGNNError("distegnn_b200.radius_graph runs only on CUDA tensors (no CPU path)")
+    N = int(pos.shape[0])
+    if max_num_neighbors is not None and max_num_neighbors < N - 1:
+        raise NotImplementedError("max_num_neighbors below the node count is not supported (the reference never caps)")
+    if N == 0:
+        return (torch.zeros(2, 0, dtype=torch.int64, device=pos.device),
+                torch.zeros(0, edge_attr_nf, device=pos.device))
+    p = pos.detach().to(torch.float32).contiguous()
+    if not bool(torch.isfinite(p).all()):
+        raise ValueError("radius_graph: positions must be finite (radius_graph_csr gives nodes with an inf or NaN "
+                         "coordinate no edges instead)")
+    B = 1 if batch is None else int(batch.max().item()) + 1
+    g, ea = radius_graph_csr(p, r, batch, loop=loop, edge_attr_nf=min(edge_attr_nf, 1), n_graphs=B,
+                             table_cells=max(_TABLE_CELLS, B + 1))
+    edge_index = torch.stack([g.row, g.col]).to(torch.int64)
+    edge_attr = ea.repeat(1, edge_attr_nf) if edge_attr_nf > 0 else p.new_zeros(g.num_edges, 0)
+    return edge_index, edge_attr
 
 
 # ---- edge cutoff (FastEGNN's cutoff_edges mode; csrc/cutoff_csr.cu) ----------------------------------------------------

@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define DISTEGNN_ABI_VERSION 2
+#define DISTEGNN_ABI_VERSION 3
 
 #if defined(__GNUC__)
 #define DISTEGNN_API __attribute__((visibility("default")))
@@ -221,25 +221,6 @@ DISTEGNN_API int distegnn_virtual_layer_bwd(int64_t n_nodes, int n_graphs, int A
                                             const float* g_agg_v, const float* g_trans_v, const float* g_vsum,
                                             float* g_Hn, float* g_xv, float* g_G, float* g_Xv, float* g_layer_params,
                                             void* stream);
-
-/* On-device radius graph (SURVEY §8 f-2): replaces the host-side `radius_graph(pos_i, r=radius, max_num_neighbors=N)`
- * + `edge_attr = |dx|` of the reference's partitioners (datasets/distribute_graphs.py:43-44; PyG / torch_cluster).
- * Uniform-grid cell list; the caller sorts the nodes' cell keys (key = graph*ncell + (ix*ny + iy)*nz + iz, cell size >=
- * radius — take radius*(1 + 2^-10) or more: with exactly radius the rounding of the fp32 index can put two nodes closer
- * than radius two cells apart — ix = (int)((x - origin_x) * (1/cell)) clamped to the grid) and passes `order` (node ids in key order) and the
- * dense table cell_start[n_graphs*ncell + 1] (first position of every key).  origin_host[3] / dims_host[3] are HOST
- * arrays.  Two phases because the edge count is only known after the first:
- *   distegnn_radius_count -> deg[i] = number of j (same graph, j != i unless loop) with |x_i - x_j| < radius
- *   caller: rowptr = exclusive prefix sum of deg (int64 [N+1]), allocates E = rowptr[N] entries
- *   distegnn_radius_fill  -> row[e] = i, col[e] = j for e in [rowptr[i], rowptr[i+1]), dist[e] = |x_i - x_j| (dist may be
- *                            NULL): edges grouped by destination row, rows ascending. */
-DISTEGNN_API int distegnn_radius_count(int64_t n_nodes, const float* x4, const int32_t* batch32, const int32_t* order,
-                                       const int64_t* cell_start, const float* origin_host, float cell_size,
-                                       const int32_t* dims_host, float radius, int loop, int32_t* deg, void* stream);
-DISTEGNN_API int distegnn_radius_fill(int64_t n_nodes, const float* x4, const int32_t* batch32, const int32_t* order,
-                                      const int64_t* cell_start, const float* origin_host, float cell_size,
-                                      const int32_t* dims_host, float radius, int loop, const int64_t* rowptr,
-                                      int32_t* row, int32_t* col, float* dist, void* stream);
 
 /* On-device radius graph, CSR out, in ONE call and without a host round trip (csrc/radius_csr.cu; SURVEY §8 f-2): the
  * reference-boundary tensors in (pos [N,3] fp32, data_batch int64 [N] sorted, may be NULL for one graph), int32 CSR by

@@ -50,7 +50,7 @@ def test_python_binding_table_matches_header():
 
 def test_host_only_entry_points():
     lib = _lib.load()
-    assert lib.distegnn_abi_version() == 2 == _lib.ABI_VERSION
+    assert lib.distegnn_abi_version() == 3 == _lib.ABI_VERSION
     offs, total = _lib.param_layout(2, 8, 2)
     assert total > 0 and offs["E_W1A"] == 0
     # error convention: negative code + message, ValueError on the Python side for bad arguments
@@ -75,12 +75,9 @@ def test_backend_has_every_method_the_host_code_calls():
     from distegnn_b200 import backend
     from tests.shadow_backend import ShadowBackend
     root = os.path.dirname(os.path.abspath(backend.__file__))
-    used = set()
-    for f in ("fast_egnn.py", "graph.py"):
-        used |= set(re.findall(r"\bbe\.(\w+)\(", open(os.path.join(root, f)).read()))
+    used = set(re.findall(r"\bbe\.(\w+)\(", open(os.path.join(root, "fast_egnn.py")).read()))
     cls = [v for v in vars(backend).values() if isinstance(v, type) and v.__name__.endswith("Backend")][0]
     missing = sorted(m for m in used if not hasattr(cls, m))
     assert not missing, f"CudaBackend lacks {missing}"
-    model_only = {m for m in used if m not in ("radius_count", "radius_fill")}      # graph.py is CUDA-only
-    missing = sorted(m for m in model_only if not hasattr(ShadowBackend, m))
+    missing = sorted(m for m in used if not hasattr(ShadowBackend, m))
     assert not missing, f"ShadowBackend lacks {missing}"

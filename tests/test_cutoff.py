@@ -111,7 +111,7 @@ def test_cabi_argument_checks():
     nb = C.c_int64(0)
     assert lib.distegnn_cutoff_csr_workspace_bytes(10, 0, 100, C.byref(nb)) == -1
     assert lib.distegnn_cutoff_csr_workspace_bytes(10, 1, -1, C.byref(nb)) == -1
-    assert lib.distegnn_abi_version() == 2
+    assert lib.distegnn_abi_version() == 3
 
 
 def test_python_validation():

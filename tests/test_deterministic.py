@@ -184,7 +184,7 @@ def test_cabi_argument_rejection():
     assert lib.distegnn_vsum_combine_det(N, 3, Cn, 0, p, p, p, None, 0, None) == -1
     assert lib.distegnn_rollout_centroid_det(N, 2, p, None, p, None) == -1 and "data_batch" in err()
     assert lib.distegnn_rollout_centroid_det(N, 1, None, None, p, None) == -1
-    assert lib.distegnn_abi_version() == 2
+    assert lib.distegnn_abi_version() == 3
     # the grid cap is a testing-library argument, not part of the product's ABI
     assert not hasattr(lib, "distegnn_set_deterministic_grid_cap")
     t = _testing()

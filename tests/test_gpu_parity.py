@@ -59,7 +59,7 @@ def check_close(out, X, ref, refX, pos, what=""):
 
 def test_library_loaded_and_abi():
     lib = _lib.load()
-    assert lib.distegnn_abi_version() == 2
+    assert lib.distegnn_abi_version() == 3
 
 
 def test_edge_kernel_tensor_core_vs_fma_twin():
@@ -896,26 +896,26 @@ def test_training_path_gradients_batched_nbody():
 
 @pytest.mark.gpu
 def test_random_partitioner_on_device_matches_host_restatement():
-    """split_large_graph_random (device) against the host restatement of distribute_graphs.py:17-51 in synth.py:
-    same chunks from the same seed, same edge sets and edge lengths per partition, global loc_mean everywhere."""
-    from distegnn_b200 import split_large_graph_random
+    """split_large_graph(split_mode="random") (device) against the host restatement of distribute_graphs.py:17-51 in
+    synth.py: same chunks from the same seed, same edge sets and edge lengths per partition, global loc_mean everywhere."""
+    from distegnn_b200 import split_large_graph
     w = synth.WORKLOADS["fluid113k"]
     n, P, seed = 30_000, 4, 7
     pts = synth.make_points(w, seed, n)
     host = synth.make_partitions(w, world_size=P, split_mode="random", seed=seed, n_nodes=n)
     d = dev()
     t = lambda a: torch.from_numpy(a).to(d)
-    parts = split_large_graph_random(t(pts["pos"]), t(pts["feat"]), t(pts["pos"]), t(pts["vel"]), t(pts["attr"]), w.radius, P,
-                                     generator=torch.Generator().manual_seed(seed))
+    parts = split_large_graph(t(pts["pos"]), t(pts["feat"]), t(pts["pos"]), t(pts["vel"]), t(pts["attr"]), w.radius, P,
+                              split_mode="random", generator=torch.Generator().manual_seed(seed))
     assert len(parts) == P
     for mine, ref in zip(parts, host):
         assert torch.equal(mine["pos"].cpu(), ref["node_loc"]) and torch.equal(mine["x"].cpu(), ref["node_feat"])
         assert float((mine["loc_mean"].cpu() - ref["loc_mean"]).abs().max()) <= 1e-5
-        a, b = _edge_set(mine["edge_index"]), _edge_set(ref["edge_index"])
+        (a, E), b = _csr_edge_set(mine["edge_index"]), _edge_set(ref["edge_index"])
         border = {e for e in (a ^ b)
                   if abs(float(np.linalg.norm(ref["node_loc"][e[0]].double().numpy() - ref["node_loc"][e[1]].double().numpy())) - w.radius) < 1e-6}
         assert (a ^ b) == border, (len(a), len(b))
-        assert mine["edge_attr"].shape == (mine["edge_index"].shape[1], 2)
+        assert mine["edge_attr"].shape == (E, 2)
 
 
 @pytest.mark.gpu

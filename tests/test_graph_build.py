@@ -1,5 +1,5 @@
-"""The radius-graph builders (DESIGN §10) against a float64 brute force: `partition.radius_graph_csr`
-(csrc/radius_csr.cu) and the older `graph.radius_graph` (csrc/radius_graph.cu).
+"""The radius-graph builder (DESIGN §10) against a float64 brute force, through both of its outputs:
+`partition.radius_graph_csr` (csrc/radius_csr.cu, a CSRGraph) and `partition.radius_graph` (the int64 edge_index over it).
 
 The reference classifies every same-graph pair of the fp32 positions in float64 against r2 = fp32(r·r): required if
 d² < r2·(1 − 2^-20), forbidden if d² ≥ r2·(1 + 2^-20), either way in between; a node with a non-finite coordinate has
@@ -146,7 +146,7 @@ def check_graph(g, ea, pos, batch, r, loop):
     return keys
 
 
-# ---- the two builders ---------------------------------------------------------------------------------------------------
+# ---- the two outputs -----------------------------------------------------------------------------------------------------
 def build_csr(pos, batch, r, loop=False, n_graphs=None, **kw):
     from distegnn_b200.partition import radius_graph_csr
     pd = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).to(dev())
@@ -154,7 +154,7 @@ def build_csr(pos, batch, r, loop=False, n_graphs=None, **kw):
     return radius_graph_csr(pd, r, bd, loop=loop, n_graphs=n_graphs, **kw)
 
 
-def build_legacy(pos, batch, r, loop=False):
+def build_coo(pos, batch, r, loop=False):
     from distegnn_b200 import radius_graph
     from distegnn_b200.shards import CSRGraph
     pd = torch.from_numpy(np.ascontiguousarray(pos, dtype=np.float32)).to(dev())
@@ -166,10 +166,10 @@ def build_legacy(pos, batch, r, loop=False):
     return CSRGraph(rowptr, ei[1].to(torch.int32).contiguous(), ei[0].to(torch.int32).contiguous()), ea
 
 
-BUILDERS = {"csr": build_csr, "legacy": build_legacy}
+BUILDERS = {"csr": build_csr, "coo": build_coo}
 
 
-def check_both(pos, batch, r, loop=False, builders=("csr", "legacy")):
+def check_both(pos, batch, r, loop=False, builders=("csr", "coo")):
     for name in builders:
         g, ea = BUILDERS[name](pos, batch, r, loop)
         check_graph(g, ea, pos, batch, r, loop)
@@ -251,7 +251,7 @@ def test_emulated_cell_of_exactly_r_splits_pairs_and_the_margin_does_not(r):
 
 # ---- GPU: 1. far from the grid origin -----------------------------------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("builder", ["csr", "legacy"])
+@pytest.mark.parametrize("builder", ["csr", "coo"])
 @pytest.mark.parametrize("r", [0.035, 0.075, 0.1, 0.3])
 def test_no_missed_edges_far_from_the_grid_origin(builder, r):
     """Pairs closer than r that a cell of exactly r splits over two cells are found, on every axis."""
@@ -266,7 +266,7 @@ def test_no_missed_edges_far_from_the_grid_origin(builder, r):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("builder", ["csr", "legacy"])
+@pytest.mark.parametrize("builder", ["csr", "coo"])
 @pytest.mark.parametrize("offset", [1e3, -1e3, 1e4, -1e4])
 def test_clouds_at_large_offsets(builder, offset):
     """Random clouds 1000 cells long at coordinates ±1e3 and ±1e4, where the fp32 spacing of the coordinates (up to 1e-3)
@@ -280,7 +280,7 @@ def test_clouds_at_large_offsets(builder, offset):
 
 # ---- GPU: 2. lattices at the boundary -----------------------------------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("builder", ["csr", "legacy"])
+@pytest.mark.parametrize("builder", ["csr", "coo"])
 @pytest.mark.parametrize("s,offset", [(0.125, 0.0), (0.1015625, 1e3), (0.03515625, -1e4), (0.375, 1e4)])
 def test_lattice_at_spacing_r_and_just_below(builder, s, offset):
     """A 10³ lattice of exact fp32 spacing s at an offset: with r = s the neighbours at d = r are absent (strict), with
@@ -376,7 +376,7 @@ def test_twenty_thousand_tiny_graphs():
     for loop in (False, True):
         g, ea = build_csr(pos, batch, 0.6, loop, n_graphs=20_000)
         check_graph(g, ea, pos, batch, 0.6, loop)
-    check_both(pos, batch, 0.6, False, builders=("legacy",))
+    check_both(pos, batch, 0.6, False, builders=("coo",))
 
 
 @pytest.mark.gpu
@@ -388,7 +388,7 @@ def test_graph_ids_without_nodes():
     for n_graphs in (5, 9, 64):
         g, ea = build_csr(pos, batch, 0.15, n_graphs=n_graphs)
         check_graph(g, ea, pos, batch, 0.15, False)
-    check_both(pos, batch, 0.15, False, builders=("legacy",))
+    check_both(pos, batch, 0.15, False, builders=("coo",))
 
 
 @pytest.mark.gpu
@@ -505,17 +505,17 @@ def test_extent_near_float_max(r, scale):
     assert g.num_edges > 0
     gc, _ = build_csr(pos, batch, r, n_graphs=B, capacity=g.num_edges)
     assert int(gc.info[2].item()) <= DEFAULT_TABLE
-    check_both(pos, batch, r, builders=("legacy",))
+    check_both(pos, batch, r, builders=("coo",))
 
 
 @pytest.mark.gpu
-def test_legacy_builder_rejects_non_finite_positions():
+def test_coo_builder_rejects_non_finite_positions():
     pos = np.random.default_rng(10).uniform(0, 1, size=(100, 3)).astype(np.float32)
     for v in (np.inf, -np.inf, np.nan):
         p = pos.copy()
         p[17, 1] = v
         with pytest.raises(ValueError, match="finite"):
-            build_legacy(p, None, 0.1)
+            build_coo(p, None, 0.1)
 
 
 # ---- GPU: 8. on top of the builders -------------------------------------------------------------------------------------

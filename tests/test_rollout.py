@@ -114,7 +114,7 @@ def test_rollout_symbols_in_library():
     lib = _lib.load()
     for name in ("distegnn_rollout_advance", "distegnn_edge_lengths_csr", "distegnn_rollout_centroid"):
         assert hasattr(lib, name)
-    assert lib.distegnn_abi_version() == 2 and _lib.FLAG_INIT_CENTROID == 32
+    assert lib.distegnn_abi_version() == 3 and _lib.FLAG_INIT_CENTROID == 32
 
 
 def test_rollout_argument_validation():

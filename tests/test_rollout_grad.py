@@ -157,7 +157,7 @@ def _cpu_case(n=160, seed=0, world=1, rank=0):
 
 def test_new_symbols_and_their_argument_checks():
     lib = _lib.load()
-    assert lib.distegnn_abi_version() == 2
+    assert lib.distegnn_abi_version() == 3
     p = 256                                                    # any non-null pointer: never dereferenced
     bwd = lib.distegnn_edge_lengths_bwd
     assert bwd(-1, 2, p, p, p, None, p, p, None) == -1         # bad size
