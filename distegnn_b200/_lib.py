@@ -74,7 +74,9 @@ SIGNATURES = {
     "distegnn_virtual_layer_fwd_det": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 10 + [_i64, _vp],
     "distegnn_vsum_combine_det": [_i64, _i32, _i32, _u32] + [_vp] * 4 + [_i64, _vp],
     "distegnn_rollout_centroid_det": [_i64, _i32] + [_vp] * 4,
+    "distegnn_frames_assemble": [_i32, _i32, _i64, _i64] + [_vp] * 14,
 }
+FRAMES_NBODY, FRAMES_WATER3D, FRAMES_LARGEFLUID = 0, 1, 2
 ABI_VERSION = 3
 
 _lib: Optional[C.CDLL] = None

@@ -1,0 +1,147 @@
+// Frame assembly: the per-sample arithmetic of the reference's data pipeline on the device (distegnn_b200/frames.py).
+//
+// The reference builds every training sample once on the host (datasets/process_dataset.py:61-115 N-body, :239-277 and
+// :334-347 Water-3D, :480-557 Fluid113K) and caches it.  Here the loader stages the raw frames a batch needs and
+//   distegnn_frames_assemble   per scene: loc_mean (fp64 sums over the WHOLE frame, fixed order) and the max of the
+//                              normalised static column, both before any split (distribute_graphs.py:32, :346 then :348);
+//                              per node of this rank: the gathers, v, ‖v‖ and the normalised column, data_batch
+// builds this rank's node arrays in two launches, without allocating or synchronising (capturable).
+#include "common.cuh"
+
+namespace degnn {
+
+constexpr int RED_THREADS = 512;
+
+struct FramesArgs {
+    int recipe, B, S;
+    int64_t n_frame, n_out;
+    const float* x0;            // [n_frame,3] pos[f]
+    const float* x1;            // [n_frame,3] pos[f+1] (Water-3D) or vel[f]
+    const float* xt;            // [n_frame,3] pos[f+Δ]
+    const float* stat;          // [n_frame,S]
+    const int64_t* scene_ptr;   // [B+1]
+    const int64_t* out_ptr;     // [B+1]
+    const int32_t* index;       // [n_out] or null
+    float *feat, *loc, *vel, *attr, *target;
+    int64_t* batch;
+    float *loc_mean, *scene_max;
+};
+
+// One block per scene: Σx in fp64 by a fixed per-thread stride and a fixed tree, so the result does not depend on
+// scheduling; the max of static column 0 (order-independent).
+__global__ void __launch_bounds__(RED_THREADS) frames_scene_kernel(const FramesArgs a) {
+    __shared__ double ssum[3][RED_THREADS];
+    __shared__ float smax[RED_THREADS];
+    const int b = blockIdx.x, t = threadIdx.x;
+    const int64_t lo = a.scene_ptr[b], hi = a.scene_ptr[b + 1];
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+    float m = -INFINITY;
+    for (int64_t i = lo + t; i < hi; i += RED_THREADS) {
+        s0 += (double)__ldg(a.x0 + i * 3);
+        s1 += (double)__ldg(a.x0 + i * 3 + 1);
+        s2 += (double)__ldg(a.x0 + i * 3 + 2);
+        m = fmaxf(m, __ldg(a.stat + i * a.S));
+    }
+    ssum[0][t] = s0; ssum[1][t] = s1; ssum[2][t] = s2; smax[t] = m;
+    __syncthreads();
+    for (int w = RED_THREADS / 2; w > 0; w >>= 1) {
+        if (t < w) {
+#pragma unroll
+            for (int d = 0; d < 3; ++d) ssum[d][t] += ssum[d][t + w];
+            smax[t] = fmaxf(smax[t], smax[t + w]);
+        }
+        __syncthreads();
+    }
+    if (t == 0) {
+        const double n = (double)(hi - lo);
+#pragma unroll
+        for (int d = 0; d < 3; ++d) a.loc_mean[b * 3 + d] = __double2float_rn(ssum[d][0] / n);
+        a.scene_max[b] = smax[0];
+    }
+}
+
+__device__ __forceinline__ int sample_of(const int64_t* ptr, int B, int64_t k) {
+    int lo = 0, hi = B - 1;                    // last b with ptr[b] <= k
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(ptr + mid) <= k) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// One thread per output node.  Gathers are copies; v, ‖v‖ and the division are round-to-nearest fp32 operations in the
+// reference's order (no contraction): ‖v‖ = sqrt((vx·vx + vy·vy) + vz·vz).
+__global__ void __launch_bounds__(256) frames_node_kernel(const FramesArgs a) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.n_out; k += (int64_t)gridDim.x * blockDim.x) {
+        const int b = sample_of(a.out_ptr, a.B, k);
+        const int64_t base = __ldg(a.scene_ptr + b), n = __ldg(a.scene_ptr + b + 1) - base;
+        const int64_t li = a.index ? (int64_t)__ldg(a.index + k) : k - __ldg(a.out_ptr + b);
+        const bool ok = li >= 0 && li < n;     // the host validates the index lists; never read outside the scene
+        const int64_t g = base + (ok ? li : 0);
+        const float nan = __int_as_float(0x7fc00000);
+        float x[3], v[3], y[3];
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            x[d] = ok ? __ldg(a.x0 + g * 3 + d) : nan;
+            y[d] = ok ? __ldg(a.xt + g * 3 + d) : nan;
+            const float w = ok ? __ldg(a.x1 + g * 3 + d) : nan;
+            v[d] = a.recipe == DISTEGNN_FRAMES_WATER3D ? __fsub_rn(w, x[d]) : w;
+        }
+        const float speed = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])),
+                                                 __fmul_rn(v[2], v[2])));
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            a.loc[k * 3 + d] = x[d];
+            a.vel[k * 3 + d] = v[d];
+            a.target[k * 3 + d] = y[d];
+        }
+        if (a.recipe == DISTEGNN_FRAMES_LARGEFLUID) {         // [viscosity, mass, ‖v‖] / [viscosity, mass]
+            const float s0 = ok ? __ldg(a.stat + g * 2) : nan, s1 = ok ? __ldg(a.stat + g * 2 + 1) : nan;
+            a.feat[k * 3] = s0; a.feat[k * 3 + 1] = s1; a.feat[k * 3 + 2] = speed;
+            a.attr[k * 2] = s0; a.attr[k * 2 + 1] = s1;
+        } else {                                              // [‖v‖, s / max(s)] / [s]
+            const float s = ok ? __ldg(a.stat + g) : nan;
+            a.feat[k * 2] = speed;
+            a.feat[k * 2 + 1] = __fdiv_rn(s, __ldg(a.scene_max + b));
+            a.attr[k] = s;
+        }
+        a.batch[k] = b;
+    }
+}
+
+static unsigned node_grid(int64_t n) {
+    const int64_t cap = 8 * (int64_t)sm_count();
+    const int64_t g = (n + 255) / 256;
+    return (unsigned)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+}  // namespace degnn
+
+extern "C" int distegnn_frames_assemble(int recipe, int n_samples, int64_t n_frame_nodes, int64_t n_out,
+                                        const float* frames, const float* statics, const int64_t* scene_ptr,
+                                        const int64_t* out_ptr, const int32_t* index, float* node_feat, float* node_loc,
+                                        float* node_vel, float* node_attr, float* target, int64_t* data_batch,
+                                        float* loc_mean, float* scene_max, void* stream) {
+    using namespace degnn;
+    DEGNN_CHECK_ARG(recipe == DISTEGNN_FRAMES_NBODY || recipe == DISTEGNN_FRAMES_WATER3D ||
+                        recipe == DISTEGNN_FRAMES_LARGEFLUID, "unknown recipe");
+    DEGNN_CHECK_ARG(n_samples >= 1 && n_frame_nodes >= 0 && n_out >= 0, "bad size");
+    DEGNN_CHECK_ARG(index || n_out == n_frame_nodes, "without an index list every node is assembled (n_out == n_frame_nodes)");
+    DEGNN_CHECK_ARG(scene_ptr && out_ptr && loc_mean && scene_max, "null pointer");
+    DEGNN_CHECK_ARG(n_frame_nodes == 0 || (frames && statics), "null pointer");
+    DEGNN_CHECK_ARG(n_out == 0 || (node_feat && node_loc && node_vel && node_attr && target && data_batch), "null pointer");
+    FramesArgs a;
+    a.recipe = recipe; a.B = n_samples; a.S = recipe == DISTEGNN_FRAMES_LARGEFLUID ? 2 : 1;
+    a.n_frame = n_frame_nodes; a.n_out = n_out;
+    a.x0 = frames; a.x1 = frames + n_frame_nodes * 3; a.xt = frames + n_frame_nodes * 6; a.stat = statics;
+    a.scene_ptr = scene_ptr; a.out_ptr = out_ptr; a.index = index;
+    a.feat = node_feat; a.loc = node_loc; a.vel = node_vel; a.attr = node_attr; a.target = target; a.batch = data_batch;
+    a.loc_mean = loc_mean; a.scene_max = scene_max;
+    frames_scene_kernel<<<n_samples, RED_THREADS, 0, (cudaStream_t)stream>>>(a);
+    DEGNN_CHECK_LAUNCH();
+    if (n_out > 0) {
+        frames_node_kernel<<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a);
+        DEGNN_CHECK_LAUNCH();
+    }
+    return DISTEGNN_OK;
+}

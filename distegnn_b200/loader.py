@@ -19,7 +19,7 @@ from __future__ import annotations
 
 import queue
 import threading
-from typing import Dict, Iterator, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -103,13 +103,7 @@ class ShardLoader:
         self.generator.manual_seed(seed)
 
     def __len__(self) -> int:
-        n = len(self.paths)
-        return n // self.batch_size if self.drop_last else (n + self.batch_size - 1) // self.batch_size
-
-    def _order(self) -> List[int]:
-        if self.shuffle:
-            return torch.randperm(len(self.paths), generator=self.generator).tolist()     # RandomSampler(replacement=False)
-        return list(range(len(self.paths)))
+        return n_batches(len(self.paths), self.batch_size, self.drop_last)
 
     def _host_batch(self, idx: Sequence[int]) -> Dict[str, Tensor]:
         host = collate([read_shard(self.paths[i]) for i in idx])
@@ -118,51 +112,78 @@ class ShardLoader:
         return host
 
     def __iter__(self) -> Iterator[Tuple[Dict[str, object], Dict[str, object]]]:
-        order = self._order()
-        batches = [order[i:i + self.batch_size] for i in range(0, len(order), self.batch_size)]
-        if self.drop_last and batches and len(batches[-1]) < self.batch_size:
-            batches.pop()
+        batches = sampler_batches(len(self.paths), self.batch_size, self.shuffle, self.generator, self.drop_last)
         if self.device is None or self.device.type != "cuda":
             for b in batches:
                 yield batch_to_device(self._host_batch(b), self.device or "cpu", non_blocking=False)
             return
-        if self.prefetch <= 0:
+        yield from staged(batches, self._host_batch, lambda host: batch_to_device(host, self.device), self.device,
+                          self.prefetch)
+
+
+def n_batches(n: int, batch_size: int, drop_last: bool) -> int:
+    return n // batch_size if drop_last else (n + batch_size - 1) // batch_size
+
+
+def sampler_batches(n: int, batch_size: int, shuffle: bool, generator: torch.Generator,
+                    drop_last: bool) -> List[List[int]]:
+    """One epoch's batches of item indices: `RandomSampler(replacement=False)` order drawn from `generator` (every rank
+    seeds it alike and walks the items in the same order) or index order, cut into `batch_size` batches, `drop_last`."""
+    order = torch.randperm(n, generator=generator).tolist() if shuffle else list(range(n))
+    batches = [order[i:i + batch_size] for i in range(0, len(order), batch_size)]
+    if drop_last and batches and len(batches[-1]) < batch_size:
+        batches.pop()
+    return batches
+
+
+def _record_on(v, stream) -> None:
+    if isinstance(v, torch.Tensor):
+        v.record_stream(stream)
+    elif isinstance(v, CSRGraph):
+        for t in (v.rowptr, v.col, v.row, v.info):
+            if t is not None:
+                t.record_stream(stream)
+
+
+def staged(batches: Sequence, make_host: Callable, to_device: Callable, device: torch.device,
+           prefetch: int) -> Iterator[Tuple[Dict[str, object], Dict[str, object]]]:
+    """The loaders' staging pipeline on a CUDA device: a background thread builds each batch on the host
+    (`make_host(batch)`, pinned buffers) and runs `to_device(host)` -> (kwargs, extras) on a side stream, so the H2D copy
+    (and whatever device work `to_device` enqueues) of batch i+1 overlaps the step on batch i; one CUDA event per batch
+    orders the consumer's stream after it.  prefetch = batches staged ahead (0 = synchronous, no thread)."""
+    if prefetch <= 0:
+        for b in batches:
+            yield to_device(make_host(b))
+        return
+    copy_stream = torch.cuda.Stream(device=device)
+    q: "queue.Queue" = queue.Queue(maxsize=prefetch)
+
+    def worker():
+        try:
+            torch.cuda.set_device(device)
             for b in batches:
-                yield batch_to_device(self._host_batch(b), self.device)
-            return
-        copy_stream = torch.cuda.Stream(device=self.device)
-        q: "queue.Queue" = queue.Queue(maxsize=self.prefetch)
+                host = make_host(b)
+                with torch.cuda.stream(copy_stream):
+                    item = to_device(host)
+                    ev = torch.cuda.Event()
+                    ev.record(copy_stream)
+                q.put((item, ev, host))                      # `host` rides along: pinned memory must outlive the copy
+            q.put(None)
+        except BaseException as e:                           # noqa: BLE001 — surfaced on the consumer side
+            q.put(e)
 
-        def worker():
-            try:
-                torch.cuda.set_device(self.device)
-                for b in batches:
-                    host = self._host_batch(b)
-                    with torch.cuda.stream(copy_stream):
-                        item = batch_to_device(host, self.device)
-                        ev = torch.cuda.Event()
-                        ev.record(copy_stream)
-                    q.put((item, ev, host))                  # `host` rides along: pinned memory must outlive the copy
-                q.put(None)
-            except BaseException as e:                       # noqa: BLE001 — surfaced on the consumer side
-                q.put(e)
-
-        th = threading.Thread(target=worker, daemon=True)
-        th.start()
-        while True:
-            got = q.get()
-            if got is None:
-                break
-            if isinstance(got, BaseException):
-                raise got
-            (kwargs, extras), ev, _host = got
-            cur = torch.cuda.current_stream(self.device)
-            cur.wait_event(ev)
-            for v in list(kwargs.values()) + [extras.get("target")]:
-                if isinstance(v, torch.Tensor):
-                    v.record_stream(cur)
-                elif isinstance(v, CSRGraph):
-                    v.rowptr.record_stream(cur)
-                    v.col.record_stream(cur)
-            yield kwargs, extras
-        th.join()
+    th = threading.Thread(target=worker, daemon=True)
+    th.start()
+    while True:
+        got = q.get()
+        if got is None:
+            break
+        if isinstance(got, BaseException):
+            raise got
+        (kwargs, extras), ev, _host = got
+        cur = torch.cuda.current_stream(device)
+        cur.wait_event(ev)
+        for v in list(kwargs.values()) + [extras.get("target")]:
+            _record_on(v, cur)
+        yield kwargs, extras
+    th.join()

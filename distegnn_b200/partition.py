@@ -301,6 +301,25 @@ def kmeans_labels(pos: Tensor, n_clusters: int, random_state: int = 0, max_iter:
     return labels.to(torch.int64)
 
 
+def node_chunks(n_nodes: int, world_size: int, split_mode: str = "random", pos: Optional[Tensor] = None,
+                generator=None) -> List[Tensor]:
+    """The node sets of the reference's partitioners, one int64 index tensor per rank: "random" = a host `randperm(n)` cut
+    into P−1 chunks of ⌊n/P⌋ plus the remainder, in permutation order (distribute_graphs.py:26-30; host tensors);
+    "kmeans" = `nonzero(kmeans_labels(pos) == i)`, nodes in index order (:188-198; on `pos.device`, needs `pos`)."""
+    n = int(n_nodes)
+    if split_mode == "random":
+        idx = torch.randperm(n, generator=generator)             # on the host, as the reference (device == 'cpu')
+        sizes = [n // world_size] * (world_size - 1)
+        sizes.append(n - sum(sizes))
+        return list(torch.split(idx, sizes))
+    if split_mode == "kmeans":
+        if pos is None:
+            raise ValueError("split_mode='kmeans' needs the positions")
+        labels = kmeans_labels(pos, world_size)
+        return [torch.nonzero(labels == i, as_tuple=False).flatten() for i in range(world_size)]
+    raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans)")
+
+
 def split_large_graph(pos: Tensor, x: Tensor, target: Tensor, vel: Tensor, attr: Optional[Tensor], radius: float,
                       world_size: int, split_mode: str = "random", special_nodes: Optional[Tensor] = None, generator=None,
                       edge_attr_nf: int = 2) -> List[Dict[str, Tensor]]:
@@ -310,16 +329,7 @@ def split_large_graph(pos: Tensor, x: Tensor, target: Tensor, vel: Tensor, attr:
     `edge_attr_nf` columns (:44) and the GLOBAL `loc_mean` (:32).  Returns dicts with the reference's `Data` field names,
     `edge_index` being a `CSRGraph` (what `FastEGNN.forward` consumes directly)."""
     n = int(pos.shape[0])
-    if split_mode == "random":
-        idx = torch.randperm(n, generator=generator)             # on the host, as the reference (device == 'cpu')
-        sizes = [n // world_size] * (world_size - 1)
-        sizes.append(n - sum(sizes))
-        chunks = [c.to(pos.device) for c in torch.split(idx, sizes)]
-    elif split_mode == "kmeans":
-        labels = kmeans_labels(pos, world_size)
-        chunks = [torch.nonzero(labels == i, as_tuple=False).flatten() for i in range(world_size)]
-    else:
-        raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans)")
+    chunks = [c.to(pos.device) for c in node_chunks(n, world_size, split_mode, pos=pos, generator=generator)]
     loc_mean = pos.mean(dim=0, keepdim=True)
     if special_nodes is None:
         special_nodes = torch.ones(n, dtype=torch.bool, device=pos.device)

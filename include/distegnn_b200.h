@@ -513,6 +513,31 @@ DISTEGNN_API int distegnn_vsum_combine_det(int64_t n_nodes, int n_graphs, int C,
 DISTEGNN_API int distegnn_rollout_centroid_det(int64_t n_nodes, int n_graphs, const float *pos,
                                                const int64_t *data_batch, double *sums, void *stream);
 
+/* ---- frame assembly (csrc/frames.cu; distegnn_b200/frames.py: training batches from raw trajectories) ----------------
+ * For a batch of n_samples samples, from the staged frames of each sample's WHOLE scene — frames float32 [3, n_frame_nodes,
+ * 3] = (pos[f], x1, pos[f+Δ]) with x1 = pos[f+1] for DISTEGNN_FRAMES_WATER3D and vel[f] otherwise, scenes concatenated at
+ * scene_ptr int64 [n_samples+1] — and the static fields statics float32 [n_frame_nodes, S] (S = 1: particle type or
+ * charge; S = 2 for DISTEGNN_FRAMES_LARGEFLUID: viscosity, mass), writes this rank's nodes: output node k of sample b
+ * (out_ptr int64 [n_samples+1]) is scene node index[k] (int32, scene-local; NULL = every node in order, then n_out ==
+ * n_frame_nodes):
+ *   node_loc = pos[f], target = pos[f+Δ], node_vel = x1 − pos[f] (Water-3D) or x1   (copies / one fp32 subtraction)
+ *   NBODY, WATER3D:  node_feat [n_out,2] = [‖v‖, s / scene_max[b]], node_attr [n_out,1] = s
+ *   LARGEFLUID:      node_feat [n_out,3] = [viscosity, mass, ‖v‖], node_attr [n_out,2] = [viscosity, mass]
+ *   data_batch int64 [n_out] = b;  ‖v‖ = sqrt((vx·vx + vy·vy) + vz·vz), every operation round-to-nearest, no contraction
+ * and per sample, over the whole scene before any split: loc_mean [n_samples,3] = fp32(Σx / n) with Σx in fp64 in a fixed
+ * order (deterministic bit for bit), scene_max [n_samples] = max of static column 0.  An index outside its scene yields NaN
+ * rows (nothing outside the scene is read).  No workspace, no allocation, no host synchronisation; capturable. */
+enum {
+    DISTEGNN_FRAMES_NBODY = 0,
+    DISTEGNN_FRAMES_WATER3D = 1,
+    DISTEGNN_FRAMES_LARGEFLUID = 2,
+};
+DISTEGNN_API int distegnn_frames_assemble(int recipe, int n_samples, int64_t n_frame_nodes, int64_t n_out,
+                                          const float *frames, const float *statics, const int64_t *scene_ptr,
+                                          const int64_t *out_ptr, const int32_t *index, float *node_feat,
+                                          float *node_loc, float *node_vel, float *node_attr, float *target,
+                                          int64_t *data_batch, float *loc_mean, float *scene_max, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

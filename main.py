@@ -22,6 +22,11 @@ weighted MSE x world_size, MMD regulariser on the virtual coordinates, gradient 
 fused forward AND backward kernels under DDP — the epoch loop, loaders, checkpoints and wandb logging of
 utils/train.py stay with the reference (out of scope).
 
+`--trajectory PATH` trains and evaluates on real frames instead (distegnn_b200.frames.FrameLoader, DESIGN §18): the
+config's recipe (N-body, Water-3D, Fluid113K), radius / inner_radius, delta_t (N-body: frame_0, frame_T), split_mode and
+cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  Without the flag the
+synthetic path below runs unchanged.
+
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
 `batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
 graph, then `data.cutoff_rate` (`--cutoff_rate` overrides it, reference main.py:133-134) drops the longest edges of
@@ -91,6 +96,8 @@ def parse():
                    "(distegnn_b200.rollout): graph rebuilt on the device every step; prints ms/step and edges/step")
     p.add_argument("--train_steps", type=int, default=0, help="(new) optimisation steps of the reference's training "
                    "step (utils/train.py:98-158) on the synthetic target")
+    p.add_argument("--trajectory", type=str, default=None, help="(new) train and evaluate on raw frames under this "
+                   "directory (distegnn_b200.frames): N-body .npy files, or train/ and valid/ folders of .npz scenes")
     return p.parse_args()
 
 
@@ -154,6 +161,11 @@ def main():
     if distributed:                                            # reference main.py:194-196
         model = DistributedDataParallel(model, device_ids=[local_rank], find_unused_parameters=True)
     model.eval()
+    if args.trajectory:
+        trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate)
+        if distributed:
+            dist.destroy_process_group()
+        return
 
     # ---- inputs: synthetic restatement of the configured dataset, partitioned like datasets/distribute_graphs.py ----
     d = cfg["data"]
@@ -223,6 +235,109 @@ def main():
         train_steps(args, cfg, model, inp, forward, world_size, local_rank, distributed, cut)
     if distributed:
         dist.destroy_process_group()
+
+
+def frame_loaders(path, cfg, world_size, rank, device, rate):
+    """FrameLoaders over the raw trajectories under `path` with the config's recipe (datasets/process_dataset.py):
+    N-body (`dataset_name: nbody*`, the reference's loc_/vel_/charges_ .npy files, frame_0 / frame_T), Water-3D or
+    Fluid113K (`path`/train/*.npz, `path`/valid/*.npz).  cutoff_edges mode: one graph per sample, radius = data.radius
+    (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
+    sample split over the ranks by split_mode (metis / spectral fall back to random), a radius graph per partition with
+    inner_radius.  Returns (recipe name, {"train": loader, "valid": loader or None})."""
+    import glob
+    from distegnn_b200.frames import FrameLoader, load_nbody, load_scenes, sample_list
+    d = cfg["data"]
+    ds = str(d.get("dataset_name", "")).lower()
+    recipe = "nbody" if ds.startswith("nbody") else "water3d" if ds.startswith("water") else "largefluid"
+    cutoff_mode = rate is not None
+    if recipe == "nbody":
+        frame_0, frame_T = int(d.get("frame_0", 30)), int(d.get("frame_T", 40))
+        delta = frame_T - frame_0
+    else:
+        frame_0, delta = 0, int(d.get("delta_t", 1))
+    if cutoff_mode:
+        radius = 0.035 if recipe == "water3d" else d.get("radius", -1)
+    else:
+        radius = d.get("inner_radius")
+    split = str(d.get("split_mode", "random"))
+    if split not in ("random", "kmeans"):
+        split = "random"
+    seed, bs = int(cfg.get("seed", 0)), int(d.get("batch_size", 1))
+    out = {}
+    for part in ("train", "valid"):
+        if recipe == "nbody":
+            if not os.path.exists(os.path.join(path, f"loc_{part}_charged100_0_0_1.npy")):
+                out[part] = None
+                continue
+            traj = load_nbody(path, part)
+        else:
+            files = sorted(glob.glob(os.path.join(path, part, "*.npz")))
+            if not files:
+                out[part] = None
+                continue
+            traj = load_scenes(files, recipe)
+        kw = {} if recipe == "nbody" else dict(max_frame=min(traj.recipe.max_frame,
+                                                             min(sc.n_frames for sc in traj.scenes) - 1 - max(delta, 1)))
+        samples = sample_list(traj, seed=seed, max_samples=d.get("max_samples"), delta_t=delta, frame_0=frame_0, **kw)
+        out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
+                                seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
+                                cutoff_rate=rate or 0.0)
+    if out["train"] is None:
+        raise SystemExit(f"--trajectory {path}: no training data for recipe {recipe!r}")
+    return recipe, out
+
+
+def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate):
+    """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
+    reference's training step on batches from FrameLoader, then the mean MSE over the validation batches."""
+    from distegnn_b200 import train_loss
+    recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, torch.device("cuda", local_rank), rate)
+    tc = cfg.get("train", {}) or {}
+    mmd = tc.get("mmd", {}) or {}
+    lr = args.lr if args.lr is not None else float(tc.get("learning_rate", tc.get("lr", 5e-4)))
+    opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=float(tc.get("weight_decay", 1e-12)))
+    inner = model.module if distributed else model
+    use_attr = cfg["model"]["node_attr_nf"] > 0
+
+    def forward(kw):                                           # positional call as in utils/train.py:63-71
+        return model(kw["node_feat"], kw["node_loc"], kw["node_vel"], kw["loc_mean"], kw["edge_index"],
+                     kw["data_batch"], kw["edge_attr"], kw["node_attr"] if use_attr else None)
+
+    def loss_of(kw, ex):
+        pred, X = forward(kw)
+        return train_loss(pred, ex["target"], X, kw["data_batch"], world_size=world_size,
+                          mmd_samples=int(mmd.get("samples", 50)), mmd_sigma=float(mmd.get("sigma", 3)),
+                          mmd_weight=float(mmd.get("weight", 0.01)), loc_mean=kw["loc_mean"],
+                          node_counts=ex["node_counts"], model=inner)
+
+    steps = args.train_steps or len(loaders["train"])
+    model.train()
+    done, t0 = 0, time.perf_counter()
+    while done < steps:
+        for kw, ex in loaders["train"]:
+            opt.zero_grad()
+            loss, info = loss_of(kw, ex)
+            loss.backward()
+            torch.nn.utils.clip_grad_norm_(model.parameters(), max_norm=0.3)
+            opt.step()
+            done += 1
+            if local_rank == 0 and (done % 10 == 0 or done == steps):
+                print(f"[{recipe}] train step {done}: MSE {info['logged'].item():.6e}", flush=True)
+            if done == steps:
+                break
+    torch.cuda.synchronize()
+    if local_rank == 0:
+        print(f"[{recipe}] {steps} train steps on raw frames: {(time.perf_counter() - t0) / steps * 1e3:.2f} ms/step")
+    ev = loaders["valid"] or loaders["train"]
+    model.eval()
+    tot, n = 0.0, 0
+    with torch.no_grad():
+        for kw, ex in ev:
+            _, info = loss_of(kw, ex)
+            tot, n = tot + float(info["logged"]), n + 1
+    if local_rank == 0:
+        print(f"[{recipe}] evaluation over {n} batches ({'valid' if loaders['valid'] else 'train'}): mean MSE "
+              f"{tot / max(n, 1):.6e}")
 
 
 def cutoff_inputs(w, batch_size, seed, rate, device):
