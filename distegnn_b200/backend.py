@@ -280,6 +280,21 @@ class CudaBackend:
         check(fn(int(pos.shape[0]), int(sums.shape[0]), ptr(pos), ptr(batch), ptr(sums), self._s(pos)), "rollout_centroid")
         self.launches += 1 if pos.shape[0] else 0
 
+    def rollout_sq_err(self, pred: Tensor, targets: Tensor, batch: Optional[Tensor], counter: Tensor, sq_err: Tensor,
+                       ws: Tensor) -> None:
+        """sq_err float64 [steps,B] row counter[0] = per-graph Σ‖pred − targets[counter[0]]‖² (see
+        distegnn_rollout_sq_err; `ws` from rollout_sq_err_workspace, zeroed)."""
+        N = int(pred.shape[0])
+        check(self.lib.distegnn_rollout_sq_err(N, int(sq_err.shape[1]), int(sq_err.shape[0]), ptr(pred), ptr(targets),
+                                               ptr(batch), ptr(counter), ptr(sq_err), ptr(ws), ws.numel(),
+                                               self._s(pred)), "rollout_sq_err")
+        self.launches += 1 if N else 0
+
+    def rollout_sq_err_workspace(self, n_nodes: int, device) -> Tensor:
+        nbytes = C.c_int64(0)
+        check(self.lib.distegnn_rollout_sq_err_workspace_bytes(n_nodes, C.byref(nbytes)), "rollout_sq_err_workspace_bytes")
+        return torch.zeros(int(nbytes.value), dtype=torch.uint8, device=device)
+
     def allreduce_packed(self, comm: "Comm", buf: Tensor) -> None:
         """In-place SUM of `buf` over the partitions through the communicator's peer-mapped segments."""
         check(self.lib.distegnn_allreduce_packed(comm.handle, ptr(buf), buf.numel(), self._s(buf)), "allreduce_packed")

@@ -5,7 +5,9 @@
 //   distegnn_frames_assemble   per scene: loc_mean (fp64 sums over the WHOLE frame, fixed order) and the max of the
 //                              normalised static column, both before any split (distribute_graphs.py:32, :346 then :348);
 //                              per node of this rank: the gathers, v, ‖v‖ and the normalised column, data_batch
-// builds this rank's node arrays in two launches, without allocating or synchronising (capturable).
+// builds this rank's node arrays in two launches, without allocating or synchronising (capturable).  With a horizon K > 1
+//   distegnn_frames_targets    gathers the staged frames pos[f + 2Δ] .. pos[f + KΔ] into targets[1:] the same way
+// (one more launch; targets[0] is the assembly's target).
 #include "common.cuh"
 
 namespace degnn {
@@ -109,6 +111,27 @@ __global__ void __launch_bounds__(256) frames_node_kernel(const FramesArgs a) {
     }
 }
 
+// One thread per (horizon step t >= 1, output node): targets[t] = frame 2 + t of the staged block (pos[f + (t+1)Δ]),
+// by the node kernel's scene offsets and index.  Copies only.
+__global__ void __launch_bounds__(256) frames_targets_kernel(int B, int64_t n_frame, int64_t n_out, int K,
+                                                             const float* frames, const int64_t* scene_ptr,
+                                                             const int64_t* out_ptr, const int32_t* index,
+                                                             float* targets) {
+    const int64_t total = (int64_t)(K - 1) * n_out;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t t = q / n_out + 1, k = q - (t - 1) * n_out;
+        const int b = sample_of(out_ptr, B, k);
+        const int64_t base = __ldg(scene_ptr + b), n = __ldg(scene_ptr + b + 1) - base;
+        const int64_t li = index ? (int64_t)__ldg(index + k) : k - __ldg(out_ptr + b);
+        const bool ok = li >= 0 && li < n;
+        const float* src = frames + ((2 + t) * n_frame + base + (ok ? li : 0)) * 3;
+        float* dst = targets + (t * n_out + k) * 3;
+        const float nan = __int_as_float(0x7fc00000);
+#pragma unroll
+        for (int d = 0; d < 3; ++d) dst[d] = ok ? __ldg(src + d) : nan;
+    }
+}
+
 static unsigned node_grid(int64_t n) {
     const int64_t cap = 8 * (int64_t)sm_count();
     const int64_t g = (n + 255) / 256;
@@ -143,5 +166,19 @@ extern "C" int distegnn_frames_assemble(int recipe, int n_samples, int64_t n_fra
         frames_node_kernel<<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a);
         DEGNN_CHECK_LAUNCH();
     }
+    return DISTEGNN_OK;
+}
+
+extern "C" int distegnn_frames_targets(int n_samples, int64_t n_frame_nodes, int64_t n_out, int horizon,
+                                       const float* frames, const int64_t* scene_ptr, const int64_t* out_ptr,
+                                       const int32_t* index, float* targets, void* stream) {
+    using namespace degnn;
+    DEGNN_CHECK_ARG(n_samples >= 1 && n_frame_nodes >= 0 && n_out >= 0 && horizon >= 1, "bad size");
+    DEGNN_CHECK_ARG(index || n_out == n_frame_nodes, "without an index list every node is gathered (n_out == n_frame_nodes)");
+    if (horizon == 1 || n_out == 0) return DISTEGNN_OK;
+    DEGNN_CHECK_ARG(frames && scene_ptr && out_ptr && targets, "null pointer");
+    frames_targets_kernel<<<node_grid((int64_t)(horizon - 1) * n_out), 256, 0, (cudaStream_t)stream>>>(
+        n_samples, n_frame_nodes, n_out, horizon, frames, scene_ptr, out_ptr, index, targets);
+    DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

@@ -208,16 +208,25 @@ def sample_list(traj: Trajectories, seed: int = 0, max_samples: Optional[int] = 
     return out
 
 
-def check_samples(traj: Trajectories, samples: Sequence[Tuple[int, int]], delta_t: int) -> None:
+def check_samples(traj: Trajectories, samples: Sequence[Tuple[int, int]], delta_t: int, horizon: int = 1) -> None:
+    """Raise ValueError naming the first sample whose frames f, f+1 (Water-3D's velocity) or f + tΔ for t = 1..horizon
+    fall outside its scene."""
+    if not isinstance(horizon, int) or isinstance(horizon, bool) or horizon < 1:
+        raise ValueError(f"horizon must be an int >= 1 (got {horizon!r})")
     need_next = not traj.recipe.needs_velocity                   # v = pos[f+1] − pos[f]
     for s, f in samples:
         if not 0 <= s < len(traj):
             raise ValueError(f"sample ({s}, {f}): no scene {s} (there are {len(traj)})")
         T = traj.scenes[s].n_frames
-        last = max(f + delta_t, f + 1 if need_next else f)
-        if f < 0 or f + delta_t < 0 or last >= T:
+        ends = (f + delta_t, f + horizon * delta_t)
+        last = max(*ends, f + 1 if need_next else f)
+        if f < 0 or min(ends) < 0 or last >= T:
+            fit = (T - 1 - f) // delta_t if delta_t > 0 and 0 <= f < T else 0
+            more = "" if horizon == 1 else \
+                f"; horizon={horizon} needs frame {f + horizon * delta_t}, and only {max(fit, 0)} step(s) of {delta_t} " \
+                f"frames fit after frame {f} (at most horizon {max(fit, 0)})"
             raise ValueError(f"sample ({s}, {f}): frames {f}..{last} fall outside scene {s} of {T} frames "
-                             f"(delta_t={delta_t})")
+                             f"(delta_t={delta_t}){more}")
 
 
 def complete_graph_edges(n: int) -> Tensor:
@@ -240,15 +249,19 @@ class FrameLoader:
     cutoff_rate     > 0: keep the int(E_b·(1 − rate)) shortest edges of every graph
     capacity        None: exact graph allocation (the edge counts are read back every batch).  K: edge buffers of K
                     entries and no host synchronisation at all; `check()` raises if a batch overflowed them
+    horizon         K >= 1 target frames per sample: extras["targets"] float32 [K,M,3] holds this rank's nodes at frames
+                    f + tΔ, t = 1..K (targets[0] is extras["target"] itself), for `rollout(targets=...)` or a loss on a
+                    differentiable rollout.  2 + K frames per sample are staged; K = 1 stages and launches as without it
     """
 
     def __init__(self, traj: Trajectories, samples: Sequence[Tuple[int, int]], delta_t: int = 1,
                  radius: Optional[float] = None, batch_size: int = 1, shuffle: bool = False, seed: int = 0,
                  drop_last: bool = True, device=None, prefetch: int = 2, world_size: int = 1, rank: int = 0,
                  split_mode: str = "random", split_seed: Optional[int] = None, cutoff_rate: float = 0.0,
-                 capacity: Optional[int] = None, edge_attr_nf: int = 2, loop: bool = False):
+                 capacity: Optional[int] = None, edge_attr_nf: int = 2, loop: bool = False, horizon: int = 1):
         self.traj, self.samples, self.delta_t = traj, [(int(s), int(f)) for s, f in samples], int(delta_t)
-        check_samples(traj, self.samples, self.delta_t)
+        check_samples(traj, self.samples, self.delta_t, horizon)
+        self.horizon = horizon
         if world_size < 1 or not 0 <= rank < world_size:
             raise ValueError(f"rank {rank} outside world_size {world_size}")
         if world_size > 1 and split_mode not in ("random", "kmeans"):
@@ -313,7 +326,7 @@ class FrameLoader:
         scenes = [self.traj.scenes[self.samples[i][0]] for i in idx]
         ns = [sc.n_nodes for sc in scenes]
         N = sum(ns)
-        frames = torch.empty(3, N, 3, dtype=torch.float32, pin_memory=pin)
+        frames = torch.empty(2 + self.horizon, N, 3, dtype=torch.float32, pin_memory=pin)
         statics = torch.empty(N, len(rc.static_keys), dtype=torch.float32, pin_memory=pin)
         fr, st = frames.numpy(), statics.numpy()
         parts, counts, off = [], [], 0
@@ -321,7 +334,8 @@ class FrameLoader:
             f = self.samples[i][1]
             fr[0, off:off + n] = sc.position[f]
             fr[1, off:off + n] = sc.velocity[f] if rc.needs_velocity else sc.position[f + 1]
-            fr[2, off:off + n] = sc.position[f + self.delta_t]
+            for t in range(1, self.horizon + 1):                 # pos[f + tΔ]
+                fr[1 + t, off:off + n] = sc.position[f + t * self.delta_t]
             st[off:off + n] = sc.static
             chunk, cnt = self.partition(i)
             parts.append(chunk)
@@ -350,6 +364,11 @@ class FrameLoader:
             self._complete[counts] = g
         return self._complete[counts]
 
+    def complete_graph(self, counts: Sequence[int]) -> CSRGraph:
+        """The fully connected graph of a batch with these per-graph node counts (kept per tuple; the candidates of a
+        fully connected recipe's cutoff, e.g. for `rollout(graph=..., cutoff_rate=...)`)."""
+        return self._complete_graph(tuple(int(c) for c in counts), self.device)
+
     def _to_device(self, host: Dict[str, object]) -> Tuple[Dict[str, object], Dict[str, object]]:
         rc, dev, A = self.traj.recipe, self.device, self.edge_attr_nf
         counts: List[int] = host["node_counts"]
@@ -360,7 +379,9 @@ class FrameLoader:
         index = host["index"].to(dev, non_blocking=True) if "index" in host else None
         f32 = dict(dtype=torch.float32, device=dev)
         feat, loc, vel = torch.empty(M, rc.node_feat_nf, **f32), torch.empty(M, 3, **f32), torch.empty(M, 3, **f32)
-        attr, target = torch.empty(M, rc.node_attr_nf, **f32), torch.empty(M, 3, **f32)
+        K = self.horizon
+        attr, targets = torch.empty(M, rc.node_attr_nf, **f32), torch.empty(K, M, 3, **f32)
+        target = targets[0]
         batch = torch.empty(M, dtype=torch.int64, device=dev)
         loc_mean, scene_max = torch.empty(B, 3, **f32), torch.empty(B, **f32)
         with torch.cuda.device(dev):
@@ -368,11 +389,16 @@ class FrameLoader:
                 rc.code, B, host["n_frame"], M, ptr(frames), ptr(statics), ptr(meta[:B + 1]), ptr(meta[B + 1:]),
                 ptr(index), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(target), ptr(batch), ptr(loc_mean),
                 ptr(scene_max), _lib.stream_ptr(dev)), "frames_assemble")
+            if K > 1:
+                check(_lib.load().distegnn_frames_targets(B, host["n_frame"], M, K, ptr(frames), ptr(meta[:B + 1]),
+                                                          ptr(meta[B + 1:]), ptr(index), ptr(targets),
+                                                          _lib.stream_ptr(dev)), "frames_targets")
         graph, edge_attr = self._graph(loc, batch, tuple(counts))
         kwargs = dict(node_feat=feat, node_loc=loc, node_vel=vel, loc_mean=loc_mean, edge_index=graph,
                       data_batch=batch, edge_attr=edge_attr, node_attr=attr)
         ptr_ = [0] + np.cumsum(counts).tolist()
-        extras = dict(target=target, ptr=ptr_, n_graphs=B, node_counts=list(counts), scene_max=scene_max)
+        extras = dict(target=target, targets=targets, ptr=ptr_, n_graphs=B, node_counts=list(counts),
+                      scene_max=scene_max)
         return kwargs, extras
 
     def _graph(self, loc: Tensor, batch: Tensor, counts: Tuple[int, ...]) -> Tuple[CSRGraph, Optional[Tensor]]:

@@ -2,7 +2,7 @@
 
     res = rollout(model, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr=None, *,
                   steps, radius=None, graph=None, loop=False, tau=1.0, speed_col=None,
-                  capacity=None, check_every=None, return_trajectory=False)
+                  capacity=None, check_every=None, return_trajectory=False, targets=None)
 
 Step t -> t+1 restates the reference's data pipeline on predicted positions (DESIGN §14):
   x_{t+1} = the model's output;  v_{t+1} = (x_{t+1} − x_t) / tau (process_dataset.py:345);  node_feat[:, speed_col] =
@@ -23,7 +23,10 @@ check to `RolloutResult.check()`: the whole rollout is then enqueued without any
 shortest edges of every graph of the candidates above (process_dataset.py:103, `partition.cutoff_edges_csr`), re-selected
 from the current lengths; the capacity and its regrowth count the candidates, `n_edges` the kept edges (DESIGN §16).
 
-`differentiable_rollout` (same arguments) runs the same steps and attaches `trajectory` and `virtual_locs` to autograd;
+`targets` [steps,N,3] (recorded positions, e.g. from `FrameLoader(horizon=steps)`) adds the per-step, per-graph squared
+error against them, computed inside the step (DESIGN §19): `sq_err`, `graph_nodes` and `mse` of the result.
+
+`differentiable_rollout` (same arguments, without `targets`) runs the same steps and attaches `trajectory` and `virtual_locs` to autograd;
 its backward recomputes one step at a time in reverse (DESIGN §15).
 """
 from __future__ import annotations
@@ -62,6 +65,10 @@ class RolloutResult:
     graph: Optional[CSRGraph] = None   # the last step's graph (radius mode: capacity-sized, count in graph.n_edges_dev)
     edge_attr: Optional[Tensor] = None  # its edge_attr, in CSR order
     virtual_locs: Optional[Tensor] = None   # [steps,B,3,C] each step's virtual_loc (differentiable_rollout only)
+    # with `targets` (rollout only), on the device:
+    sq_err: Optional[Tensor] = None    # float64 [steps,B]: Σ over graph b's nodes of ‖x_{t+1} − targets[t]‖², all ranks
+    graph_nodes: Optional[Tensor] = None   # int64 [B]: node counts over all ranks
+    mse: Optional[Tensor] = None       # float64 [steps]: Σ_b sq_err[t] / (3 Σ_b graph_nodes), the training loss's MSE
 
     def check(self) -> None:
         """Raise if a graph build overflowed its capacity, or if the backward of a differentiable rollout rebuilt a graph
@@ -135,11 +142,25 @@ def _validate(m: FastEGNN, node_feat, node_loc, node_vel, loc_mean, data_batch, 
             raise ValueError(f"{name} must be a floating tensor")
 
 
+def _check_targets(targets, steps: int, node_loc: Tensor) -> None:
+    if targets is None:
+        return
+    N = int(node_loc.shape[0])
+    if not isinstance(targets, torch.Tensor):
+        raise ValueError(f"targets must be a tensor (got {type(targets).__name__})")
+    if targets.dtype != torch.float32:
+        raise ValueError(f"targets must be float32 (got {targets.dtype})")
+    if tuple(targets.shape) != (steps, N, 3):
+        raise ValueError(f"targets must be [steps, N, 3] = [{steps}, {N}, 3] (got {list(targets.shape)})")
+    if targets.device != node_loc.device:
+        raise ValueError(f"targets is on {targets.device}, node_loc on {node_loc.device}")
+
+
 class _Rollout:
     """State buffers at fixed addresses + the per-step enqueue (eager or CUDA-graph replay)."""
 
     def __init__(self, m: FastEGNN, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius,
-                 graph, loop, tau, speed_col, return_trajectory, cutoff_rate=0.0):
+                 graph, loop, tau, speed_col, return_trajectory, cutoff_rate=0.0, targets=None):
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).clone().contiguous()
         self.m, self.be, self.dev = m, be, dev
         self.N, self.B = int(node_loc.shape[0]), int(loc_mean.shape[0])
@@ -155,6 +176,11 @@ class _Rollout:
         self.counter[2:3].fill_(-1)
         self.traj = torch.empty(steps, self.N, 3, dtype=torch.float32, device=dev) if return_trajectory else None
         self.n_edges = torch.zeros(steps, dtype=torch.int32, device=dev)
+        self.targets = self.sq_err = self.sq_ws = None
+        if targets is not None:                                # per-step error: row counter[0] of sq_err, every step
+            self.targets = targets.detach().contiguous()
+            self.sq_err = torch.zeros(steps, self.B, dtype=torch.float64, device=dev)
+            self.sq_ws = be.rollout_sq_err_workspace(self.N, dev)
         self.pk = m._packed_params(dev)
         self.ws = m._workspace(dev, self.N, self.B, self.K)
         self.comm = m._get_comm(be, dev, self.B, self.K)       # collective on first use
@@ -243,6 +269,8 @@ class _Rollout:
         m._run(be, self.pk, (self.N, self.E, self.B, self.K), args, self.ws, self.comm, init_centroid=init_centroid)
         if self.keep is not None:
             self.keep["Xv"].index_copy_(0, idx, self.ws["Xv"].unsqueeze(0))
+        if self.targets is not None:                           # reads the step counter before the advance moves it
+            be.rollout_sq_err(self.ws["out"], self.targets, self._gbatch(), self.counter, self.sq_err, self.sq_ws)
         be.rollout_advance(self.speed_col, self.tau, self.ws["out"], self.loc, self.vel,
                            self.feat if self.speed_col is not None else None, self.traj, self.edge_count, self.overflow,
                            self.n_edges, self.counter)
@@ -286,20 +314,37 @@ class _Rollout:
 
     def finish(self) -> Tensor:
         """Per-graph centroid of the final positions over all partitions: one kernel (fp64 sums: exact count, no fp32
-        rounding of Σx), one [B,4] fp64 all-reduce."""
+        rounding of Σx), one [B,4] fp64 all-reduce.  With targets the [steps,B] error sums ride in the same all-reduce,
+        and `graph_nodes` takes the node counts from the centroid sums."""
         sums = torch.zeros(self.B, 4, dtype=torch.float64, device=self.dev)
         self.be.rollout_centroid(self.loc, self._gbatch(), sums, **(dict(deterministic=True) if self.m.deterministic else {}))
         if self.m.world_size > 1:                              # one fp64 SUM all-reduce (the peer exchange sums fp32)
             import torch.distributed as dist
-            dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self.m.process_group)
+            if self.sq_err is None:
+                dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self.m.process_group)
+            else:
+                packed = torch.cat([sums.reshape(-1), self.sq_err.reshape(-1)])
+                dist.all_reduce(packed, op=dist.ReduceOp.SUM, group=self.m.process_group)
+                sums = packed[:sums.numel()].view(self.B, 4)
+                self.sq_err = packed[sums.numel():].view(self.steps, self.B)
+        if self.sq_err is not None:
+            self.graph_nodes = sums[:, 3].round().long()
         return (sums[:, :3] / sums[:, 3:4].clamp(min=1.0)).float()
+
+    def errors(self) -> dict:
+        """sq_err, graph_nodes and mse of RolloutResult (all None without targets)."""
+        if self.sq_err is None:
+            return {}
+        mse = self.sq_err.sum(1) / (3.0 * self.graph_nodes.sum().double()).clamp(min=1.0)
+        return dict(sq_err=self.sq_err, graph_nodes=self.graph_nodes, mse=mse)
 
 
 def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_mean: Tensor, data_batch: Tensor,
             node_attr: Optional[Tensor] = None, *, steps: int, radius: Optional[float] = None,
             graph: Optional[CSRGraph] = None, loop: bool = False, tau: float = 1.0, speed_col: Optional[int] = None,
             capacity: Optional[int] = None, check_every: Optional[int] = None,
-            return_trajectory: bool = False, cutoff_rate: float = 0.0) -> RolloutResult:
+            return_trajectory: bool = False, cutoff_rate: float = 0.0,
+            targets: Optional[Tensor] = None) -> RolloutResult:
     """Roll `model` (a FastEGNN, or one wrapped in DistributedDataParallel) out for `steps` steps from the given state;
     see the module docstring for the update rules.  With several ranks every rank calls it with its own partition.
 
@@ -310,23 +355,30 @@ def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_me
     cutoff_rate > 0 (FastEGNN's cutoff_edges mode, single device): every step keeps the int(E_b·(1 − cutoff_rate))
     shortest edges of each graph's candidates (the rebuilt radius graph, or the caller's `graph`), re-selected from the
     current lengths (`cutoff_edges_csr`).  `n_edges` then counts the kept edges; `capacity` and its regrowth count the
-    candidates.  0 runs no cutoff at all."""
+    candidates.  0 runs no cutoff at all.
+
+    targets: float32 [steps,N,3] on node_loc's device, this rank's rows of the recorded positions after each step (e.g.
+    `FrameLoader(horizon=steps)`'s extras["targets"]).  Each step then adds one launch, between the forward and the
+    advance, that stores sq_err[t, b] = Σ_{i in graph b} ‖x_{t+1,i} − targets[t,i]‖² (fp32 differences, fp64 sums in a
+    fixed order: bitwise reproducible in deterministic mode); the result's `sq_err`, `graph_nodes` and `mse` hold it,
+    summed over the ranks in the end-of-rollout all-reduce (DESIGN §19)."""
     m = _unwrap(model)
     _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
               capacity, check_every, cutoff_rate)
+    _check_targets(targets, steps, node_loc)
     dev = node_loc.device
     be = m._get_backend(dev)                                    # raises on a CPU tensor (no CPU path)
     import contextlib
     guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
     with guard, torch.no_grad():
         r = _Rollout(m, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph,
-                     loop, tau, speed_col, return_trajectory, cutoff_rate)
+                     loop, tau, speed_col, return_trajectory, cutoff_rate, targets)
         grown = _drive(r, capacity, check_every)
         loc_mean_out = r.finish()
         return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=loc_mean_out,
                              virtual_loc=r.ws["Xv"].clone(), trajectory=r.traj, n_edges=r.n_edges, capacity=r.capacity,
                              regrowths=grown, replays=r.replays, status=r.counter,
-                             graph=_result_graph(r), edge_attr=r.ea)
+                             graph=_result_graph(r), edge_attr=r.ea, **r.errors())
 
 
 def _result_graph(r: _Rollout) -> CSRGraph:

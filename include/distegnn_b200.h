@@ -512,6 +512,20 @@ DISTEGNN_API int distegnn_vsum_combine_det(int64_t n_nodes, int n_graphs, int C,
                                            void *stream);
 DISTEGNN_API int distegnn_rollout_centroid_det(int64_t n_nodes, int n_graphs, const float *pos,
                                                const int64_t *data_batch, double *sums, void *stream);
+/* distegnn_rollout_sq_err: a rollout step's error against recorded targets, between the forward and
+ * distegnn_rollout_advance.  With t = counter[0] (the advance's step counter, see distegnn_rollout_advance; nothing is
+ * written unless 0 <= t < steps):
+ *   sq_err[t, b] = Σ_{i in graph b} ‖pred_i − targets[t, i]‖²     (sq_err float64 [steps, n_graphs], targets [steps, N, 3])
+ * with the differences in fp32 (round-to-nearest) and the squares and sums in fp64, in an order fixed by n_nodes and the
+ * graph sizes alone: chunks of 2048 rows, each graph's rows in a chunk summed as distegnn_rollout_centroid_det sums, the
+ * chunks added in order.  Every entry of row t is stored (0 for a graph without nodes), never accumulated, so a rerun step
+ * overwrites its row.  data_batch int64 [N] sorted (NULL for one graph).  One launch, no allocation, no host
+ * synchronisation; capturable.  The workspace (distegnn_rollout_sq_err_workspace_bytes, 16-byte aligned) must be zeroed
+ * once before the first call; the kernel leaves it fit for the next.  n_nodes 0: nothing is launched. */
+DISTEGNN_API int distegnn_rollout_sq_err_workspace_bytes(int64_t n_nodes, int64_t *bytes_host);
+DISTEGNN_API int distegnn_rollout_sq_err(int64_t n_nodes, int n_graphs, int steps, const float *pred,
+                                         const float *targets, const int64_t *data_batch, const int32_t *counter,
+                                         double *sq_err, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---- frame assembly (csrc/frames.cu; distegnn_b200/frames.py: training batches from raw trajectories) ----------------
  * For a batch of n_samples samples, from the staged frames of each sample's WHOLE scene — frames float32 [3, n_frame_nodes,
@@ -537,6 +551,15 @@ DISTEGNN_API int distegnn_frames_assemble(int recipe, int n_samples, int64_t n_f
                                           const int64_t *out_ptr, const int32_t *index, float *node_feat,
                                           float *node_loc, float *node_vel, float *node_attr, float *target,
                                           int64_t *data_batch, float *loc_mean, float *scene_max, void *stream);
+/* distegnn_frames_targets: multi-step targets.  frames float32 [2 + horizon, n_frame_nodes, 3] = (pos[f], x1, pos[f+Δ],
+ * pos[f+2Δ], .., pos[f+horizon·Δ]) per scene (the first three as for distegnn_frames_assemble, which reads only those);
+ * writes targets float32 [horizon, n_out, 3] rows 1..horizon−1: targets[t, k] = pos[f+(t+1)Δ] of output node k, with the
+ * assembly's scene_ptr, out_ptr and index (NULL = every node in order; an index outside its scene yields NaN rows).
+ * Row 0 is not written: pass targets[0] as the assembly's `target`.  Copies only; horizon 1 launches nothing.  No
+ * workspace, no allocation, no host synchronisation; capturable. */
+DISTEGNN_API int distegnn_frames_targets(int n_samples, int64_t n_frame_nodes, int64_t n_out, int horizon,
+                                         const float *frames, const int64_t *scene_ptr, const int64_t *out_ptr,
+                                         const int32_t *index, float *targets, void *stream);
 
 #ifdef __cplusplus
 }

@@ -24,8 +24,10 @@ utils/train.py stay with the reference (out of scope).
 
 `--trajectory PATH` trains and evaluates on real frames instead (distegnn_b200.frames.FrameLoader, DESIGN §18): the
 config's recipe (N-body, Water-3D, Fluid113K), radius / inner_radius, delta_t (N-body: frame_0, frame_T), split_mode and
-cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  Without the flag the
-synthetic path below runs unchanged.
+cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  With `--rollout_steps K`
+it then rolls the trained model out K steps from every validation batch and prints the per-step MSE against the recorded
+frames f + Δ .. f + KΔ (DESIGN §19; `--rollout_tau` sets the velocity's time step, Water-3D defaults to Δ).  Without the
+flag the synthetic path below runs unchanged.
 
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
 `batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
@@ -97,7 +99,11 @@ def parse():
     p.add_argument("--train_steps", type=int, default=0, help="(new) optimisation steps of the reference's training "
                    "step (utils/train.py:98-158) on the synthetic target")
     p.add_argument("--trajectory", type=str, default=None, help="(new) train and evaluate on raw frames under this "
-                   "directory (distegnn_b200.frames): N-body .npy files, or train/ and valid/ folders of .npz scenes")
+                   "directory (distegnn_b200.frames): N-body .npy files, or train/ and valid/ folders of .npz scenes; "
+                   "with --rollout_steps K also a K-step rollout from every validation batch against the recorded frames")
+    p.add_argument("--rollout_tau", type=float, default=None, help="(new) time step of a --trajectory rollout's "
+                   "velocity v = (x' − x)/tau; default Δ for Water-3D (one-frame differences), required for N-body and "
+                   "Fluid113K (physical velocities; the frame time is not in the files)")
     return p.parse_args()
 
 
@@ -237,24 +243,30 @@ def main():
         dist.destroy_process_group()
 
 
-def frame_loaders(path, cfg, world_size, rank, device, rate):
+def recipe_of_config(cfg):
+    """(recipe name, frame_0, Δ) of the config's dataset (N-body: frame_T − frame_0; else data.delta_t)."""
+    d = cfg["data"]
+    ds = str(d.get("dataset_name", "")).lower()
+    recipe = "nbody" if ds.startswith("nbody") else "water3d" if ds.startswith("water") else "largefluid"
+    if recipe == "nbody":
+        frame_0, frame_T = int(d.get("frame_0", 30)), int(d.get("frame_T", 40))
+        return recipe, frame_0, frame_T - frame_0
+    return recipe, 0, int(d.get("delta_t", 1))
+
+
+def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("train", "valid")):
     """FrameLoaders over the raw trajectories under `path` with the config's recipe (datasets/process_dataset.py):
     N-body (`dataset_name: nbody*`, the reference's loc_/vel_/charges_ .npy files, frame_0 / frame_T), Water-3D or
     Fluid113K (`path`/train/*.npz, `path`/valid/*.npz).  cutoff_edges mode: one graph per sample, radius = data.radius
     (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
     sample split over the ranks by split_mode (metis / spectral fall back to random), a radius graph per partition with
-    inner_radius.  Returns (recipe name, {"train": loader, "valid": loader or None})."""
+    inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
+    N-body frame_0 that cannot hold them exits with a message).  Returns (recipe name, {part: loader or None})."""
     import glob
     from distegnn_b200.frames import FrameLoader, load_nbody, load_scenes, sample_list
     d = cfg["data"]
-    ds = str(d.get("dataset_name", "")).lower()
-    recipe = "nbody" if ds.startswith("nbody") else "water3d" if ds.startswith("water") else "largefluid"
+    recipe, frame_0, delta = recipe_of_config(cfg)
     cutoff_mode = rate is not None
-    if recipe == "nbody":
-        frame_0, frame_T = int(d.get("frame_0", 30)), int(d.get("frame_T", 40))
-        delta = frame_T - frame_0
-    else:
-        frame_0, delta = 0, int(d.get("delta_t", 1))
     if cutoff_mode:
         radius = 0.035 if recipe == "water3d" else d.get("radius", -1)
     else:
@@ -264,7 +276,7 @@ def frame_loaders(path, cfg, world_size, rank, device, rate):
         split = "random"
     seed, bs = int(cfg.get("seed", 0)), int(d.get("batch_size", 1))
     out = {}
-    for part in ("train", "valid"):
+    for part in parts:
         if recipe == "nbody":
             if not os.path.exists(os.path.join(path, f"loc_{part}_charged100_0_0_1.npy")):
                 out[part] = None
@@ -276,13 +288,18 @@ def frame_loaders(path, cfg, world_size, rank, device, rate):
                 out[part] = None
                 continue
             traj = load_scenes(files, recipe)
-        kw = {} if recipe == "nbody" else dict(max_frame=min(traj.recipe.max_frame,
-                                                             min(sc.n_frames for sc in traj.scenes) - 1 - max(delta, 1)))
+        kw = {}
+        if recipe != "nbody":
+            shortest = min(sc.n_frames for sc in traj.scenes)
+            kw["max_frame"] = min(traj.recipe.max_frame, shortest - 1 - max(horizon * delta, 1))
+            if horizon > 1 and kw["max_frame"] < 0:
+                raise SystemExit(f"--trajectory {path}/{part}: the shortest scene has {shortest} frames; it cannot hold "
+                                 f"{horizon} step(s) of delta_t={delta} frames after any frame")
         samples = sample_list(traj, seed=seed, max_samples=d.get("max_samples"), delta_t=delta, frame_0=frame_0, **kw)
         out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
                                 seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
-                                cutoff_rate=rate or 0.0)
-    if out["train"] is None:
+                                cutoff_rate=rate or 0.0, horizon=horizon)
+    if "train" in parts and out["train"] is None:
         raise SystemExit(f"--trajectory {path}: no training data for recipe {recipe!r}")
     return recipe, out
 
@@ -291,6 +308,14 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate):
     """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
     reference's training step on batches from FrameLoader, then the mean MSE over the validation batches."""
     from distegnn_b200 import train_loss
+    recipe, _, delta = recipe_of_config(cfg)
+    K = args.rollout_steps
+    tau = args.rollout_tau if args.rollout_tau is not None else (float(delta) if recipe == "water3d" else None)
+    if K > 0 and tau is None:                                  # before any training: the rollout could not run
+        if local_rank == 0:
+            print(f"--rollout_steps with --trajectory on {recipe!r} needs --rollout_tau: its velocities are physical and "
+                  "the frame time is not in the files (Water-3D defaults to delta_t)", flush=True)
+        sys.exit(2)
     recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, torch.device("cuda", local_rank), rate)
     tc = cfg.get("train", {}) or {}
     mmd = tc.get("mmd", {}) or {}
@@ -338,6 +363,52 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate):
     if local_rank == 0:
         print(f"[{recipe}] evaluation over {n} batches ({'valid' if loaders['valid'] else 'train'}): mean MSE "
               f"{tot / max(n, 1):.6e}")
+    if K > 0:
+        rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau)
+
+
+# the |v| column of each recipe's node features (distegnn_b200/frames.py): N-body, Water-3D [‖v‖, ·], Fluid113K [·, ·, ‖v‖]
+SPEED_COL = {"nbody": 0, "water3d": 0, "largefluid": 2}
+
+
+def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau):
+    """--trajectory with --rollout_steps K: a K-step `rollout(targets=...)` from every batch of the valid split (the
+    train split without one), through a FrameLoader with horizon K and the config's radius and cutoff rate; prints the
+    per-step MSE averaged over the batches, each weighted by its graph count (utils/train.py:112-114, 166)."""
+    from distegnn_b200 import rollout
+    K = args.rollout_steps
+    dev = torch.device("cuda", local_rank)
+    part = "valid"
+    try:
+        _, lds = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=K, parts=(part,))
+        if lds[part] is None:
+            part = "train"
+            _, lds = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=K, parts=(part,))
+    except ValueError as e:                                    # a sample that cannot hold K steps
+        if local_rank == 0:
+            print(f"--rollout_steps {K}: {e}", flush=True)
+        sys.exit(2)
+    ld = lds[part]
+    use_attr = cfg["model"]["node_attr_nf"] > 0
+    tot, graphs, n = torch.zeros(K, dtype=torch.float64, device=dev), 0, 0
+    t0 = time.perf_counter()
+    for kw, ex in ld:
+        if ld.radius is not None:
+            g = dict(radius=ld.radius)
+        else:                                                  # fully connected: the candidates, cut again every step
+            g = dict(graph=ld.complete_graph(tuple(ex["node_counts"])) if ld.cutoff_rate > 0 else kw["edge_index"])
+        res = rollout(model, kw["node_feat"], kw["node_loc"], kw["node_vel"], kw["loc_mean"], kw["data_batch"],
+                      kw["node_attr"] if use_attr else None, steps=K, tau=tau, speed_col=SPEED_COL[recipe],
+                      cutoff_rate=ld.cutoff_rate, targets=ex["targets"], **g)
+        tot += res.mse * ex["n_graphs"]
+        graphs, n = graphs + ex["n_graphs"], n + 1
+    mse = (tot / max(graphs, 1)).tolist()
+    dt = time.perf_counter() - t0
+    if local_rank == 0:
+        print(f"[{recipe}] rollout evaluation over {n} batches ({part}), {K} steps, tau={tau:g}: "
+              f"{dt / max(n * K, 1) * 1e3:.2f} ms/step", flush=True)
+        for t, v in enumerate(mse):
+            print(f"[{recipe}] rollout step {t + 1}: MSE {v:.6e}", flush=True)
 
 
 def cutoff_inputs(w, batch_size, seed, rate, device):
