@@ -78,6 +78,8 @@ SIGNATURES = {
     "distegnn_frames_targets": [_i32, _i64, _i64, _i32] + [_vp] * 6,
     "distegnn_rollout_sq_err_workspace_bytes": [_i64, C.POINTER(_i64)],
     "distegnn_rollout_sq_err": [_i64, _i32, _i32] + [_vp] * 6 + [_i64, _vp],
+    "distegnn_rollout_chamfer_workspace_bytes": [_i64, _i32, C.POINTER(_i64)],
+    "distegnn_rollout_chamfer": [_i64, _i32, _i32] + [_vp] * 6 + [_i64, _vp],
 }
 FRAMES_NBODY, FRAMES_WATER3D, FRAMES_LARGEFLUID = 0, 1, 2
 ABI_VERSION = 3

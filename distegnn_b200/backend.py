@@ -295,6 +295,22 @@ class CudaBackend:
         check(self.lib.distegnn_rollout_sq_err_workspace_bytes(n_nodes, C.byref(nbytes)), "rollout_sq_err_workspace_bytes")
         return torch.zeros(int(nbytes.value), dtype=torch.uint8, device=device)
 
+    def rollout_chamfer(self, pred: Tensor, targets: Tensor, batch: Optional[Tensor], counter: Tensor, chamfer: Tensor,
+                        ws: Tensor) -> None:
+        """chamfer float64 [steps,B,2] row counter[0] = per-graph Chamfer sums of pred against targets[counter[0]], both
+        directions (see distegnn_rollout_chamfer; `ws` from rollout_chamfer_workspace)."""
+        N = int(pred.shape[0])
+        check(self.lib.distegnn_rollout_chamfer(N, int(chamfer.shape[1]), int(chamfer.shape[0]), ptr(pred),
+                                                ptr(targets), ptr(batch), ptr(counter), ptr(chamfer), ptr(ws),
+                                                ws.numel(), self._s(pred)), "rollout_chamfer")
+        self.launches += 7 if N else 0                         # ours; the cub scan comes on top
+
+    def rollout_chamfer_workspace(self, n_nodes: int, n_graphs: int, device) -> Tensor:
+        nbytes = C.c_int64(0)
+        check(self.lib.distegnn_rollout_chamfer_workspace_bytes(n_nodes, n_graphs, C.byref(nbytes)),
+              "rollout_chamfer_workspace_bytes")
+        return torch.empty(int(nbytes.value), dtype=torch.uint8, device=device)
+
     def allreduce_packed(self, comm: "Comm", buf: Tensor) -> None:
         """In-place SUM of `buf` over the partitions through the communicator's peer-mapped segments."""
         check(self.lib.distegnn_allreduce_packed(comm.handle, ptr(buf), buf.numel(), self._s(buf)), "allreduce_packed")

@@ -4,6 +4,7 @@
 // not enter the result.
 #include "common.cuh"
 #include "det.cuh"
+#include "rollout_err.cuh"
 
 namespace degnn {
 
@@ -16,17 +17,6 @@ int det_check_workspace(int64_t n_nodes, int64_t n_edges, int C, const void* ws,
         return DISTEGNN_EWORKSPACE;
     }
     return DISTEGNN_OK;
-}
-
-template <typename I>
-__device__ int64_t lower_bound_dev(const I* v, int64_t n, int64_t key) {
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if ((int64_t)__ldg(v + mid) < key) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
 }
 
 // One warp per 16-edge slice; the slice that holds a row's first edge and whose last run goes on into the next slice adds
@@ -56,28 +46,6 @@ __global__ void __launch_bounds__(256) edge_combine_det_kernel(int64_t E, const 
         if (agg_m) *reinterpret_cast<float2*>(agg_m + (size_t)r * H + 2 * lane) = m;
         if (lane < 3) agg_x[(size_t)r * 4 + lane] = x;
     }
-}
-
-constexpr int DET_RED = 256;   // threads of the per-graph reductions: part of the summation order
-
-// Σ over rows [lo, hi) of v(i) (NV components) in a fixed order: thread t takes rows lo + t, lo + t + DET_RED, ..., then a
-// fixed tree over the threads.  Result in red[k][0].
-template <typename T, int NV, typename F>
-__device__ void det_row_sum(int64_t lo, int64_t hi, F v, T (*red)[DET_RED]) {
-    const int t = threadIdx.x;
-    T s[NV];
-#pragma unroll
-    for (int k = 0; k < NV; ++k) s[k] = T(0);
-    for (int64_t i = lo + t; i < hi; i += DET_RED) v(i, s);
-#pragma unroll
-    for (int k = 0; k < NV; ++k) red[k][t] = s[k];
-    for (int o = DET_RED / 2; o > 0; o >>= 1) {
-        __syncthreads();
-        if (t < o)
-#pragma unroll
-            for (int k = 0; k < NV; ++k) red[k][t] += red[k][t + o];
-    }
-    __syncthreads();
 }
 
 // One thread per vsum chunk (the real<->virtual kernel's chunks, det.cuh): Σx of the chunk's nodes in node order per graph,
@@ -158,8 +126,6 @@ __global__ void __launch_bounds__(DET_RED) centroid_det_kernel(int64_t N, int B,
 // with det_row_sum, the centroid's reduction.  A graph's first chunk stores its partial to sq_err[t, b], each later chunk
 // to its own slot; the last block to finish adds every graph's slots in chunk order.  So the order depends on N and the
 // graph sizes alone, and every value is a plain store (a rerun step overwrites its row).
-constexpr int64_t SQERR_CHUNK = 2048;   // rows per block: part of the summation order
-
 __global__ void __launch_bounds__(DET_RED) rollout_sq_err_kernel(int64_t N, int B, int steps, const float* pred,
                                                                  const float* targets, const int64_t* batch,
                                                                  const int32_t* counter, double* sq_err, double* slots,
@@ -175,10 +141,8 @@ __global__ void __launch_bounds__(DET_RED) rollout_sq_err_kernel(int64_t N, int 
         const int64_t b = batch ? __ldg(batch + i) : 0;
         const int64_t j = batch ? i + lower_bound_dev(batch + i, r1 - i, b + 1) : r1;
         det_row_sum<double, 1>(i, j, [&](int64_t k, double (&s)[1]) {
-            const float dx = __fsub_rn(__ldg(pred + k * 3), __ldg(tg + k * 3));
-            const float dy = __fsub_rn(__ldg(pred + k * 3 + 1), __ldg(tg + k * 3 + 1));
-            const float dz = __fsub_rn(__ldg(pred + k * 3 + 2), __ldg(tg + k * 3 + 2));
-            s[0] += ((double)dx * dx + (double)dy * dy) + (double)dz * dz;
+            s[0] += target_sq_dist([&](int d) { return __ldg(pred + k * 3 + d); },
+                                   [&](int d) { return __ldg(tg + k * 3 + d); });
         }, red);
         if (threadIdx.x == 0 && b >= 0 && b < B) {
             const bool first = i > r0 || r0 == 0 || (batch && __ldg(batch + r0 - 1) != b);   // starts in this chunk

@@ -2,7 +2,7 @@
 
     res = rollout(model, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr=None, *,
                   steps, radius=None, graph=None, loop=False, tau=1.0, speed_col=None,
-                  capacity=None, check_every=None, return_trajectory=False, targets=None)
+                  capacity=None, check_every=None, return_trajectory=False, targets=None, chamfer=False)
 
 Step t -> t+1 restates the reference's data pipeline on predicted positions (DESIGN §14):
   x_{t+1} = the model's output;  v_{t+1} = (x_{t+1} − x_t) / tau (process_dataset.py:345);  node_feat[:, speed_col] =
@@ -25,6 +25,8 @@ from the current lengths; the capacity and its regrowth count the candidates, `n
 
 `targets` [steps,N,3] (recorded positions, e.g. from `FrameLoader(horizon=steps)`) adds the per-step, per-graph squared
 error against them, computed inside the step (DESIGN §19): `sq_err`, `graph_nodes` and `mse` of the result.
+`chamfer=True` adds the per-step, per-graph Chamfer distance to them, which does not pair node i with node i (DESIGN
+§20): `chamfer` and `chamfer_mse` of the result.
 
 `differentiable_rollout` (same arguments, without `targets`) runs the same steps and attaches `trajectory` and `virtual_locs` to autograd;
 its backward recomputes one step at a time in reverse (DESIGN §15).
@@ -69,6 +71,9 @@ class RolloutResult:
     sq_err: Optional[Tensor] = None    # float64 [steps,B]: Σ over graph b's nodes of ‖x_{t+1} − targets[t]‖², all ranks
     graph_nodes: Optional[Tensor] = None   # int64 [B]: node counts over all ranks
     mse: Optional[Tensor] = None       # float64 [steps]: Σ_b sq_err[t] / (3 Σ_b graph_nodes), the training loss's MSE
+    # with `targets` and chamfer=True: [t, b, 0] prediction -> record, [t, b, 1] record -> prediction
+    chamfer: Optional[Tensor] = None   # float64 [steps,B,2]: Σ of nearest-neighbour d per graph, partition-local, all ranks
+    chamfer_mse: Optional[Tensor] = None   # float64 [steps,2]: Σ_b chamfer[t,b,k] / (3 Σ_b graph_nodes) <= mse
 
     def check(self) -> None:
         """Raise if a graph build overflowed its capacity, or if the backward of a differentiable rollout rebuilt a graph
@@ -142,8 +147,12 @@ def _validate(m: FastEGNN, node_feat, node_loc, node_vel, loc_mean, data_batch, 
             raise ValueError(f"{name} must be a floating tensor")
 
 
-def _check_targets(targets, steps: int, node_loc: Tensor) -> None:
+def _check_targets(targets, steps: int, node_loc: Tensor, chamfer: bool = False) -> None:
+    if not isinstance(chamfer, bool):
+        raise ValueError(f"chamfer must be a bool (got {type(chamfer).__name__})")
     if targets is None:
+        if chamfer:
+            raise ValueError("chamfer=True needs targets: the Chamfer distance is taken against the recorded frames")
         return
     N = int(node_loc.shape[0])
     if not isinstance(targets, torch.Tensor):
@@ -160,7 +169,7 @@ class _Rollout:
     """State buffers at fixed addresses + the per-step enqueue (eager or CUDA-graph replay)."""
 
     def __init__(self, m: FastEGNN, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius,
-                 graph, loop, tau, speed_col, return_trajectory, cutoff_rate=0.0, targets=None):
+                 graph, loop, tau, speed_col, return_trajectory, cutoff_rate=0.0, targets=None, chamfer=False):
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).clone().contiguous()
         self.m, self.be, self.dev = m, be, dev
         self.N, self.B = int(node_loc.shape[0]), int(loc_mean.shape[0])
@@ -181,6 +190,10 @@ class _Rollout:
             self.targets = targets.detach().contiguous()
             self.sq_err = torch.zeros(steps, self.B, dtype=torch.float64, device=dev)
             self.sq_ws = be.rollout_sq_err_workspace(self.N, dev)
+        self.chamfer = self.ch_ws = None
+        if chamfer:                                            # and row counter[0] of chamfer, after sq_err
+            self.chamfer = torch.zeros(steps, self.B, 2, dtype=torch.float64, device=dev)
+            self.ch_ws = be.rollout_chamfer_workspace(self.N, self.B, dev)
         self.pk = m._packed_params(dev)
         self.ws = m._workspace(dev, self.N, self.B, self.K)
         self.comm = m._get_comm(be, dev, self.B, self.K)       # collective on first use
@@ -271,6 +284,8 @@ class _Rollout:
             self.keep["Xv"].index_copy_(0, idx, self.ws["Xv"].unsqueeze(0))
         if self.targets is not None:                           # reads the step counter before the advance moves it
             be.rollout_sq_err(self.ws["out"], self.targets, self._gbatch(), self.counter, self.sq_err, self.sq_ws)
+        if self.chamfer is not None:
+            be.rollout_chamfer(self.ws["out"], self.targets, self._gbatch(), self.counter, self.chamfer, self.ch_ws)
         be.rollout_advance(self.speed_col, self.tau, self.ws["out"], self.loc, self.vel,
                            self.feat if self.speed_col is not None else None, self.traj, self.edge_count, self.overflow,
                            self.n_edges, self.counter)
@@ -314,8 +329,9 @@ class _Rollout:
 
     def finish(self) -> Tensor:
         """Per-graph centroid of the final positions over all partitions: one kernel (fp64 sums: exact count, no fp32
-        rounding of Σx), one [B,4] fp64 all-reduce.  With targets the [steps,B] error sums ride in the same all-reduce,
-        and `graph_nodes` takes the node counts from the centroid sums."""
+        rounding of Σx), one [B,4] fp64 all-reduce.  With targets the [steps,B] error sums (and the [steps,B,2]
+        partition-local Chamfer sums) ride in the same all-reduce, and `graph_nodes` takes the node counts from the
+        centroid sums."""
         sums = torch.zeros(self.B, 4, dtype=torch.float64, device=self.dev)
         self.be.rollout_centroid(self.loc, self._gbatch(), sums, **(dict(deterministic=True) if self.m.deterministic else {}))
         if self.m.world_size > 1:                              # one fp64 SUM all-reduce (the peer exchange sums fp32)
@@ -323,20 +339,28 @@ class _Rollout:
             if self.sq_err is None:
                 dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self.m.process_group)
             else:
-                packed = torch.cat([sums.reshape(-1), self.sq_err.reshape(-1)])
+                parts = [sums, self.sq_err] + ([self.chamfer] if self.chamfer is not None else [])
+                packed = torch.cat([p.reshape(-1) for p in parts])
                 dist.all_reduce(packed, op=dist.ReduceOp.SUM, group=self.m.process_group)
-                sums = packed[:sums.numel()].view(self.B, 4)
-                self.sq_err = packed[sums.numel():].view(self.steps, self.B)
+                sums, self.sq_err, *rest = packed.split([p.numel() for p in parts])
+                sums = sums.view(self.B, 4)
+                self.sq_err = self.sq_err.view(self.steps, self.B)
+                if rest:
+                    self.chamfer = rest[0].view(self.steps, self.B, 2)
         if self.sq_err is not None:
             self.graph_nodes = sums[:, 3].round().long()
         return (sums[:, :3] / sums[:, 3:4].clamp(min=1.0)).float()
 
     def errors(self) -> dict:
-        """sq_err, graph_nodes and mse of RolloutResult (all None without targets)."""
+        """sq_err, graph_nodes and mse of RolloutResult (all None without targets), and chamfer and chamfer_mse (None
+        without chamfer=True)."""
         if self.sq_err is None:
             return {}
-        mse = self.sq_err.sum(1) / (3.0 * self.graph_nodes.sum().double()).clamp(min=1.0)
-        return dict(sq_err=self.sq_err, graph_nodes=self.graph_nodes, mse=mse)
+        denom = (3.0 * self.graph_nodes.sum().double()).clamp(min=1.0)
+        out = dict(sq_err=self.sq_err, graph_nodes=self.graph_nodes, mse=self.sq_err.sum(1) / denom)
+        if self.chamfer is not None:
+            out.update(chamfer=self.chamfer, chamfer_mse=self.chamfer.sum(1) / denom)
+        return out
 
 
 def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_mean: Tensor, data_batch: Tensor,
@@ -344,7 +368,7 @@ def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_me
             graph: Optional[CSRGraph] = None, loop: bool = False, tau: float = 1.0, speed_col: Optional[int] = None,
             capacity: Optional[int] = None, check_every: Optional[int] = None,
             return_trajectory: bool = False, cutoff_rate: float = 0.0,
-            targets: Optional[Tensor] = None) -> RolloutResult:
+            targets: Optional[Tensor] = None, chamfer: bool = False) -> RolloutResult:
     """Roll `model` (a FastEGNN, or one wrapped in DistributedDataParallel) out for `steps` steps from the given state;
     see the module docstring for the update rules.  With several ranks every rank calls it with its own partition.
 
@@ -361,18 +385,26 @@ def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_me
     `FrameLoader(horizon=steps)`'s extras["targets"]).  Each step then adds one launch, between the forward and the
     advance, that stores sq_err[t, b] = Σ_{i in graph b} ‖x_{t+1,i} − targets[t,i]‖² (fp32 differences, fp64 sums in a
     fixed order: bitwise reproducible in deterministic mode); the result's `sq_err`, `graph_nodes` and `mse` hold it,
-    summed over the ranks in the end-of-rollout all-reduce (DESIGN §19)."""
+    summed over the ranks in the end-of-rollout all-reduce (DESIGN §19).
+
+    chamfer=True (needs `targets`): each step also stores, after the sq_err launch and before the advance,
+    chamfer[t, b, 0] = Σ_{i in graph b} min_j d(x_{t+1,i}, targets[t,j]) and chamfer[t, b, 1] = Σ_j min_i d(targets[t,j],
+    x_{t+1,i}) over graph b's nodes of this rank, d the sq_err term: exact nearest neighbours on a device cell grid, a
+    fixed number of launches per step, no host read (DESIGN §20).  The result's `chamfer` [steps,B,2] and `chamfer_mse`
+    [steps,2] (normalised like `mse`, and never above it) hold it.  With several ranks each rank's partition-local sums
+    are added in the end-of-rollout all-reduce: the result lies between the whole-cloud Chamfer sum and sq_err.  The
+    trajectory, sq_err and mse do not change with it."""
     m = _unwrap(model)
     _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
               capacity, check_every, cutoff_rate)
-    _check_targets(targets, steps, node_loc)
+    _check_targets(targets, steps, node_loc, chamfer)
     dev = node_loc.device
     be = m._get_backend(dev)                                    # raises on a CPU tensor (no CPU path)
     import contextlib
     guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
     with guard, torch.no_grad():
         r = _Rollout(m, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph,
-                     loop, tau, speed_col, return_trajectory, cutoff_rate, targets)
+                     loop, tau, speed_col, return_trajectory, cutoff_rate, targets, chamfer)
         grown = _drive(r, capacity, check_every)
         loc_mean_out = r.finish()
         return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=loc_mean_out,

@@ -526,6 +526,21 @@ DISTEGNN_API int distegnn_rollout_sq_err_workspace_bytes(int64_t n_nodes, int64_
 DISTEGNN_API int distegnn_rollout_sq_err(int64_t n_nodes, int n_graphs, int steps, const float *pred,
                                          const float *targets, const int64_t *data_batch, const int32_t *counter,
                                          double *sq_err, void *workspace, int64_t workspace_bytes, void *stream);
+/* distegnn_rollout_chamfer: the Chamfer distance of a rollout step against its recorded frame (DESIGN §20), launched
+ * beside distegnn_rollout_sq_err.  With t = counter[0] (nothing is written unless 0 <= t < steps) and, for graph b, its
+ * rows I_b:
+ *   chamfer[t, b, 0] = Σ_{i in I_b} min_{j in I_b} d(pred_i, targets[t, j])      (prediction -> record)
+ *   chamfer[t, b, 1] = Σ_{j in I_b} min_{i in I_b} d(targets[t, j], pred_i)      (record -> prediction)
+ * (chamfer float64 [steps, n_graphs, 2]), d the per-node term of distegnn_rollout_sq_err, every minimum exact.  The sums
+ * take that entry point's order, so chamfer[t, b, k] <= sq_err[t, b] bit for bit.  A graph without nodes gets 0, a graph
+ * with a non-finite coordinate in pred or targets[t] NaN in both entries.  Row t is stored, never accumulated.
+ * data_batch int64 [N] sorted (NULL for one graph); n_nodes + n_graphs <= 2^29.  A fixed number of launches, no
+ * allocation, no host synchronisation; capturable.  The workspace (distegnn_rollout_chamfer_workspace_bytes, 16-byte
+ * aligned) needs no initialisation.  n_nodes 0: nothing is launched. */
+DISTEGNN_API int distegnn_rollout_chamfer_workspace_bytes(int64_t n_nodes, int n_graphs, int64_t *bytes_host);
+DISTEGNN_API int distegnn_rollout_chamfer(int64_t n_nodes, int n_graphs, int steps, const float *pred,
+                                          const float *targets, const int64_t *data_batch, const int32_t *counter,
+                                          double *chamfer, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---- frame assembly (csrc/frames.cu; distegnn_b200/frames.py: training batches from raw trajectories) ----------------
  * For a batch of n_samples samples, from the staged frames of each sample's WHOLE scene — frames float32 [3, n_frame_nodes,

@@ -1,6 +1,6 @@
 /*
- * distegnn_b200_testing_grid.h — the radius build's grid sizing on the host, exported by libdistegnn_b200_testing.so
- * (csrc/testing/radius_grid.cu).  NOT part of the product: only tests call it, on machines without a device.
+ * distegnn_b200_testing_grid.h — the grid sizing of the radius build and of the rollout's Chamfer search on the host,
+ * exported by libdistegnn_b200_testing.so (csrc/testing/radius_grid.cu).  NOT part of the product: only tests call it, on machines without a device.
  */
 #ifndef DISTEGNN_B200_TESTING_GRID_H
 #define DISTEGNN_B200_TESTING_GRID_H
@@ -16,6 +16,10 @@ extern "C" {
  * dims[3] and ncell = dims[0]*dims[1]*dims[2] per graph (csrc/radius_grid.cuh).  No device needed. */
 DISTEGNN_API int distegnn_radius_grid_size(const float *ext, float radius, int n_graphs, int64_t table_cells,
                                            float *cell, int32_t *dims, int64_t *ncell);
+/* Host-only: the grid distegnn_rollout_chamfer sizes for one graph of bounding-box extents ext[3] (as above) and a budget
+ * of `budget` cells per cloud (the graph's node count + 1): cell edge, dims[3] and ncell (csrc/chamfer_grid.cuh). */
+DISTEGNN_API int distegnn_chamfer_grid_size(const float *ext, int64_t budget, float *cell, int32_t *dims,
+                                            int64_t *ncell);
 
 #ifdef __cplusplus
 }

@@ -26,7 +26,8 @@ utils/train.py stay with the reference (out of scope).
 config's recipe (N-body, Water-3D, Fluid113K), radius / inner_radius, delta_t (N-body: frame_0, frame_T), split_mode and
 cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  With `--rollout_steps K`
 it then rolls the trained model out K steps from every validation batch and prints the per-step MSE against the recorded
-frames f + Δ .. f + KΔ (DESIGN §19; `--rollout_tau` sets the velocity's time step, Water-3D defaults to Δ).  Without the
+frames f + Δ .. f + KΔ (DESIGN §19; `--rollout_tau` sets the velocity's time step, Water-3D defaults to Δ);
+`--rollout_chamfer` adds both directions of the normalised Chamfer distance to every step's line (DESIGN §20).  Without the
 flag the synthetic path below runs unchanged.
 
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
@@ -101,6 +102,9 @@ def parse():
     p.add_argument("--trajectory", type=str, default=None, help="(new) train and evaluate on raw frames under this "
                    "directory (distegnn_b200.frames): N-body .npy files, or train/ and valid/ folders of .npz scenes; "
                    "with --rollout_steps K also a K-step rollout from every validation batch against the recorded frames")
+    p.add_argument("--rollout_chamfer", action="store_true", help="(new) with --trajectory and --rollout_steps: also "
+                   "print each step's Chamfer distance to the recorded frame (prediction -> record, record -> "
+                   "prediction), normalised like the MSE; independent of particle identity")
     p.add_argument("--rollout_tau", type=float, default=None, help="(new) time step of a --trajectory rollout's "
                    "velocity v = (x' − x)/tau; default Δ for Water-3D (one-frame differences), required for N-body and "
                    "Fluid113K (physical velocities; the frame time is not in the files)")
@@ -374,7 +378,8 @@ SPEED_COL = {"nbody": 0, "water3d": 0, "largefluid": 2}
 def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau):
     """--trajectory with --rollout_steps K: a K-step `rollout(targets=...)` from every batch of the valid split (the
     train split without one), through a FrameLoader with horizon K and the config's radius and cutoff rate; prints the
-    per-step MSE averaged over the batches, each weighted by its graph count (utils/train.py:112-114, 166)."""
+    per-step MSE averaged over the batches, each weighted by its graph count (utils/train.py:112-114, 166).  With
+    --rollout_chamfer each line also carries the two directions of `chamfer_mse`, averaged the same way."""
     from distegnn_b200 import rollout
     K = args.rollout_steps
     dev = torch.device("cuda", local_rank)
@@ -391,6 +396,7 @@ def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau):
     ld = lds[part]
     use_attr = cfg["model"]["node_attr_nf"] > 0
     tot, graphs, n = torch.zeros(K, dtype=torch.float64, device=dev), 0, 0
+    ch_tot = torch.zeros(K, 2, dtype=torch.float64, device=dev)
     t0 = time.perf_counter()
     for kw, ex in ld:
         if ld.radius is not None:
@@ -399,16 +405,20 @@ def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau):
             g = dict(graph=ld.complete_graph(tuple(ex["node_counts"])) if ld.cutoff_rate > 0 else kw["edge_index"])
         res = rollout(model, kw["node_feat"], kw["node_loc"], kw["node_vel"], kw["loc_mean"], kw["data_batch"],
                       kw["node_attr"] if use_attr else None, steps=K, tau=tau, speed_col=SPEED_COL[recipe],
-                      cutoff_rate=ld.cutoff_rate, targets=ex["targets"], **g)
+                      cutoff_rate=ld.cutoff_rate, targets=ex["targets"], chamfer=args.rollout_chamfer, **g)
         tot += res.mse * ex["n_graphs"]
+        if args.rollout_chamfer:
+            ch_tot += res.chamfer_mse * ex["n_graphs"]
         graphs, n = graphs + ex["n_graphs"], n + 1
     mse = (tot / max(graphs, 1)).tolist()
+    ch = (ch_tot / max(graphs, 1)).tolist()
     dt = time.perf_counter() - t0
     if local_rank == 0:
         print(f"[{recipe}] rollout evaluation over {n} batches ({part}), {K} steps, tau={tau:g}: "
               f"{dt / max(n * K, 1) * 1e3:.2f} ms/step", flush=True)
         for t, v in enumerate(mse):
-            print(f"[{recipe}] rollout step {t + 1}: MSE {v:.6e}", flush=True)
+            extra = f", Chamfer pred->rec {ch[t][0]:.6e}, rec->pred {ch[t][1]:.6e}" if args.rollout_chamfer else ""
+            print(f"[{recipe}] rollout step {t + 1}: MSE {v:.6e}{extra}", flush=True)
 
 
 def cutoff_inputs(w, batch_size, seed, rate, device):
