@@ -6,39 +6,36 @@
 //   1. init: zero the histogram, the per-graph bounds and flags, the ticket
 //   2. per-graph bounding box of the finite coordinates of P ∪ Q (ordered-int atomics), and a flag for a graph with a
 //      non-finite coordinate
-//   3. per-graph grid (chamfer_grid.cuh): at most n_b + 1 cells per cloud, so graph b's cells of cloud c occupy the keys
+//   3. per-graph grid (cell_grid.cuh): at most n_b + 1 cells per cloud, so graph b's cells of cloud c occupy the keys
 //      c·(N + B) + lo_b + b .. + n_b (lo_b its first row): no scan over the graphs, and every key inside the table
 //   4. cell key per point, and its rank in the cell (atomicAdd); 5. exclusive scan of the histogram (cub)
 //   6. points scattered to start[key] + rank: each cell's points of one cloud are contiguous, in some order
 //   7. one thread per point (in cell order), best = d to its matched node: rings of growing Chebyshev radius around its
 //      cell in the other cloud's table until the stop rule below holds; past kChamferRingCap rings (an outlier), the
 //      whole warp scans the graph's whole other cloud for it
-//   8. per-graph sums of the minima with det_row_sum over the sq_err kernel's 2048-row chunks, combined by the last block
+//   8. per-graph sums of the minima, both directions at once, with the sq_err kernel's graph_chunk_sum (rollout_err.cuh)
 // A minimum does not depend on the order its candidates are visited in, so the atomics' order never reaches a value.
 // Every term of a sum is at most the sq_err term of its row (the matched node is a candidate), and the two sums add in
-// the same fixed order, so chamfer[t, b, k] <= sq_err[t, b] bit for bit.
+// the same fixed order (one function), so chamfer[t, b, k] <= sq_err[t, b] bit for bit.
 //
-// Stop rule.  For an axis with n > 1 cells the computed index of a coordinate x is min(⌊u⌋, n − 1), u = fl(fl(x − o) ·
-// fl(1/c)) >= 0, with the exact e = (x − o)/c <= 1025: three roundings leave |u − e| < 3·1025·2^-24 < 1.84e-4.  After
-// rings 0..R, a point p not scanned has index distance >= R + 1 to the query q along some axis; clamping only shrinks
-// index distances, so |u_p − u_q| > R there and |x_p − x_q| > c·(R − 3.7e-4).  Its d is at least the fp64 square of the
-// fp32 difference on that axis, >= (c·(R − 3.7e-4)·(1 − 2^-24))² > (c·R·(1 − 2^-10))² for R >= 1.  So the search stops
-// once best <= (c·R·(1 − 2^-10))² (R = 0: best = 0), or once the rings cover the grid: no point left can beat best.  An
-// axis with one cell (extent 0, or past FLT_MAX) never separates two points.  This is the radius build's cell margin
-// (DESIGN §10) read the other way round.
+// Stop rule.  For an axis with n > 1 cells the computed index of a coordinate x is min(⌊u⌋, n − 1) with u within 1.9e-4
+// of the exact (x − o)/c, and two points' u within 3.7e-4 of their exact index difference (the rounding bound of
+// `axis_cell`, cell_grid.cuh).  After rings 0..R, a point p not scanned has index distance >= R + 1 to the query q along
+// some axis; clamping only shrinks index distances, so |u_p − u_q| > R there and |x_p − x_q| > c·(R − 3.7e-4).  Its d is
+// at least the fp64 square of the fp32 difference on that axis, >= (c·(R − 3.7e-4)·(1 − 2^-24))² > (c·R·(1 − 2^-10))²
+// for R >= 1.  So the search stops once best <= (c·R·(1 − 2^-10))² (R = 0: best = 0), or once the rings cover the grid:
+// no point left can beat best.  An axis with one cell (extent 0, or past FLT_MAX) never separates two points.  This is
+// the radius build's cell margin (kRadiusCellMargin, DESIGN §10) read the other way round.
 #include <cub/device/device_scan.cuh>
 
-#include "chamfer_grid.cuh"
+#include "cell_grid.cuh"
 #include "common.cuh"
 #include "rollout_err.cuh"
 
 namespace degnn {
 
-struct ChamferGrid {
-    float ox, oy, oz, inv_cell;
-    int nx, ny, nz, base;      // base = lo_b + b: the graph's first key in either cloud's table
-    float cell;
-    int ncell;
+struct ChamferGrid : CellGrid {
+    int base;                  // lo_b + b: the graph's first key in either cloud's table
 };
 
 struct ChamferArgs {
@@ -61,27 +58,15 @@ struct ChamferArgs {
     unsigned* ticket;
 };
 
-__device__ __forceinline__ int chf_ord(float f) {      // order-preserving float -> int
-    const int i = __float_as_int(f);
-    return i >= 0 ? i : i ^ 0x7fffffff;
-}
-__device__ __forceinline__ float chf_unord(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
 __device__ __forceinline__ const float* chf_frame(const ChamferArgs& a) {   // targets[t]; row 0 outside [0, steps)
     const int t = __ldcg(a.counter);
     return a.targets + (t >= 0 && t < a.steps ? (int64_t)t * a.N * 3 : 0);
 }
 
-__device__ __forceinline__ int chf_graph(const ChamferArgs& a, int64_t i) {
-    if (!a.batch) return 0;
-    const int64_t b = __ldg(a.batch + i);
-    return (int)(b < 0 ? 0 : (b >= a.B ? a.B - 1 : b));
-}
-
 __global__ void chamfer_init_kernel(const ChamferArgs a) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i <= 2 * a.T) a.cell_start[i] = 0;
-    if (i < (int64_t)a.B * 6) a.bounds[i] = chf_ord(i % 6 < 3 ? INFINITY : -INFINITY);
+    if (i < (int64_t)a.B * 6) a.bounds[i] = ordered_int(i % 6 < 3 ? INFINITY : -INFINITY);
     if (i < a.B) a.flags[i] = 0;
     if (i == 0) *a.ticket = 0;
 }
@@ -97,8 +82,8 @@ __global__ void __launch_bounds__(256) chamfer_bounds_kernel(const ChamferArgs a
     if (r0 >= a.N) return;
     const int64_t r1 = min(a.N, r0 + CHF_WARP_ROWS);
     const float* tg = chf_frame(a);
-    const int g0 = chf_graph(a, r0);
-    const bool one = chf_graph(a, r1 - 1) == g0;                // batch sorted: the whole range is graph g0
+    const int g0 = graph_id(a.batch, r0, a.B);
+    const bool one = graph_id(a.batch, r1 - 1, a.B) == g0;                // batch sorted: the whole range is graph g0
     float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
     int bad = 0;
     for (int64_t i = r0 + lane; i < r1; i += 32) {
@@ -106,44 +91,24 @@ __global__ void __launch_bounds__(256) chamfer_bounds_kernel(const ChamferArgs a
         int nf = 0;
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
-            const float p = __ldg(a.pred + i * 3 + d), q = __ldg(tg + i * 3 + d);
-            if (isfinite(p)) { l[d] = fminf(l[d], p); h[d] = fmaxf(h[d], p); } else nf = 1;
-            if (isfinite(q)) { l[d] = fminf(l[d], q); h[d] = fmaxf(h[d], q); } else nf = 1;
+            if (!bound_add(l[d], h[d], __ldg(a.pred + i * 3 + d))) nf = 1;
+            if (!bound_add(l[d], h[d], __ldg(tg + i * 3 + d))) nf = 1;
         }
         if (one) {
 #pragma unroll
             for (int d = 0; d < 3; ++d) { lo[d] = fminf(lo[d], l[d]); hi[d] = fmaxf(hi[d], h[d]); }
             bad |= nf;
         } else {
-            const int b = chf_graph(a, i);
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                if (l[d] <= h[d]) {
-                    atomicMin(a.bounds + (int64_t)b * 6 + d, chf_ord(l[d]));
-                    atomicMax(a.bounds + (int64_t)b * 6 + 3 + d, chf_ord(h[d]));
-                }
-            }
+            const int b = graph_id(a.batch, i, a.B);
+            bound_flush(a.bounds + (int64_t)b * 6, l, h);
             if (nf) atomicOr(a.flags + b, 1);
         }
     }
     if (!one) return;                                           // warp-uniform
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo[d] = fminf(lo[d], __shfl_xor_sync(FULL, lo[d], o));
-            hi[d] = fmaxf(hi[d], __shfl_xor_sync(FULL, hi[d], o));
-        }
-    }
+    bound_warp_reduce(lo, hi);
     bad = __any_sync(FULL, bad);
     if (lane == 0) {
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-            if (lo[d] <= hi[d]) {
-                atomicMin(a.bounds + (int64_t)g0 * 6 + d, chf_ord(lo[d]));
-                atomicMax(a.bounds + (int64_t)g0 * 6 + 3 + d, chf_ord(hi[d]));
-            }
-        }
+        bound_flush(a.bounds + (int64_t)g0 * 6, lo, hi);
         if (bad) atomicOr(a.flags + g0, 1);
     }
 }
@@ -151,36 +116,11 @@ __global__ void __launch_bounds__(256) chamfer_bounds_kernel(const ChamferArgs a
 __global__ void chamfer_grid_kernel(const ChamferArgs a) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.B) return;
-    const int64_t lo = a.batch ? lower_bound_dev(a.batch, a.N, b) : 0;
-    const int64_t hi = a.batch ? lower_bound_dev(a.batch, a.N, (int64_t)b + 1) : a.N;   // lo <= hi for any batch
+    int64_t lo, hi;
+    graph_rows(a.batch, a.N, b, lo, hi);
     float o[3], ext[3];
-    for (int k = 0; k < 3; ++k) {
-        o[k] = chf_unord(a.bounds[(int64_t)b * 6 + k]);
-        float h = chf_unord(a.bounds[(int64_t)b * 6 + 3 + k]);
-        if (!(o[k] <= h)) o[k] = h = 0.f;                       // no finite coordinate on this axis
-        ext[k] = h - o[k];                                      // +inf past FLT_MAX: one slab on that axis
-    }
-    const RadiusGridSize s = chamfer_grid_size(ext, hi - lo + 1);
-    ChamferGrid g;
-    g.ox = o[0]; g.oy = o[1]; g.oz = o[2];
-    g.inv_cell = 1.0f / s.cell;
-    g.nx = s.dims[0]; g.ny = s.dims[1]; g.nz = s.dims[2];
-    g.base = (int)(lo + b);
-    g.cell = s.cell;
-    g.ncell = s.ncell;
-    a.grid[b] = g;
-}
-
-// Cell index along one axis, in [0, n) for any coordinate (NaN -> 0, +inf -> n − 1); monotone in x.
-__device__ __forceinline__ int chf_axis(float x, float o, float inv_cell, int n) {
-    const float q = (x - o) * inv_cell;
-    return q > 0.f ? (q < (float)n ? (int)q : n - 1) : 0;
-}
-
-__device__ __forceinline__ void chf_cell(const ChamferGrid& g, float x, float y, float z, int& ix, int& iy, int& iz) {
-    ix = chf_axis(x, g.ox, g.inv_cell, g.nx);
-    iy = chf_axis(y, g.oy, g.inv_cell, g.ny);
-    iz = chf_axis(z, g.oz, g.inv_cell, g.nz);
+    bounds_origin_extent(a.bounds + (int64_t)b * 6, o, ext);
+    a.grid[b] = ChamferGrid{make_cell_grid(o, chamfer_grid_size(ext, hi - lo + 1)), (int)(lo + b)};
 }
 
 __device__ __forceinline__ float4 chf_point(const ChamferArgs& a, const float* tg, int64_t k, int64_t& i, int& c) {
@@ -196,9 +136,9 @@ __global__ void __launch_bounds__(256) chamfer_keys_kernel(const ChamferArgs a) 
     int64_t i;
     int c;
     const float4 p = chf_point(a, chf_frame(a), k, i, c);
-    const ChamferGrid g = a.grid[chf_graph(a, i)];
+    const ChamferGrid g = a.grid[graph_id(a.batch, i, a.B)];
     int ix, iy, iz;
-    chf_cell(g, p.x, p.y, p.z, ix, iy, iz);
+    cell_of(g, p.x, p.y, p.z, ix, iy, iz);
     const int key = (int)(c * a.T) + g.base + (ix * g.ny + iy) * g.nz + iz;
     a.keyrank[k] = make_int2(key, atomicAdd(a.cell_start + key, 1));
 }
@@ -226,7 +166,7 @@ __global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a
     const float4 q = live ? a.sorted[s] : make_float4(0.f, 0.f, 0.f, 0.f);
     const int c = s >= a.N;                                    // the query's cloud; it searches the other one
     const int64_t i = __float_as_int(q.w);
-    const int b = live ? chf_graph(a, i) : 0;
+    const int b = live ? graph_id(a.batch, i, a.B) : 0;
     const bool search = live && !__ldg(a.flags + b);           // a non-finite coordinate in the graph: NaN sums
     const ChamferGrid g = a.grid[b];
     const int* start = a.cell_start + (1 - c) * a.T + g.base;
@@ -240,7 +180,7 @@ __global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a
         const float* m = (c ? a.pred : chf_frame(a)) + i * 3;
         best = dist(make_float4(__ldg(m), __ldg(m + 1), __ldg(m + 2), 0.f));
         int ix, iy, iz;
-        chf_cell(g, q.x, q.y, q.z, ix, iy, iz);
+        cell_of(g, q.x, q.y, q.z, ix, iy, iz);
         const int reach = max(max(max(ix, g.nx - 1 - ix), max(iy, g.ny - 1 - iy)), max(iz, g.nz - 1 - iz));
         auto scan = [&](int k0, int k1) {                      // the points of cells k0 .. k1 − 1
             const int e = __ldg(start + k1);
@@ -286,65 +226,17 @@ __global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a
     if (live) a.minima[c * a.N + i] = search ? best : __longlong_as_double(0x7ff8000000000000ll);
 }
 
-// distegnn_rollout_sq_err's reduction on the per-node minima, both directions at once: block c sums its chunk's rows of
-// each graph with det_row_sum, stores a graph's first chunk to chamfer[t, b, :] and every later chunk to its slot; the
-// last block adds the slots in chunk order.
+// distegnn_rollout_sq_err's reduction on the per-node minima, both directions at once.  The workspace is not
+// initialised: the init kernel zeroes the ticket.
 __global__ void __launch_bounds__(DET_RED) chamfer_sum_kernel(const ChamferArgs a) {
-    __shared__ double red[2][DET_RED];
-    __shared__ bool last;
-    const int64_t N = a.N;
-    const int B = a.B;
     const int t = __ldcg(a.counter);
     const bool keep = t >= 0 && t < a.steps;
-    const int64_t c = blockIdx.x, r0 = c * SQERR_CHUNK, r1 = min(N, r0 + SQERR_CHUNK);
-    double* out = a.chamfer + (keep ? (int64_t)t * B * 2 : 0);
-    for (int64_t i = r0; keep && i < r1;) {
-        const int64_t b = a.batch ? __ldg(a.batch + i) : 0;
-        const int64_t j = a.batch ? i + lower_bound_dev(a.batch + i, r1 - i, b + 1) : r1;
-        det_row_sum<double, 2>(i, j, [&](int64_t k, double (&s)[2]) {
-            s[0] += __ldg(a.minima + k);
-            s[1] += __ldg(a.minima + N + k);
-        }, red);
-        if (threadIdx.x == 0 && b >= 0 && b < B) {
-            const bool first = i > r0 || r0 == 0 || (a.batch && __ldg(a.batch + r0 - 1) != b);
-            double* dst = first ? out + b * 2 : a.slots + c * 2;
-            dst[0] = red[0][0];
-            dst[1] = red[1][0];
-        }
-        __syncthreads();
-        i = j;
-    }
-    if (threadIdx.x == 0) {
-        __threadfence();
-        last = atomicAdd(a.ticket, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!last || !keep) return;
-    __threadfence();
-    for (int u = threadIdx.x; u < 2 * B; u += DET_RED) {
-        const int b = u >> 1, d = u & 1;
-        const int64_t lo = a.batch ? lower_bound_dev(a.batch, N, b) : 0;
-        const int64_t hi = a.batch ? lower_bound_dev(a.batch, N, (int64_t)b + 1) : N;
-        double acc = 0.0;
-        if (hi > lo) {
-            acc = __ldcg(out + u);
-            int64_t k = lo / SQERR_CHUNK + 1;
-            const int64_t k1 = (hi - 1) / SQERR_CHUNK;
-            for (; k + 8 <= k1 + 1; k += 8) {                  // eight independent loads in flight, added in chunk order
-                double v[8];
-#pragma unroll
-                for (int w = 0; w < 8; ++w) v[w] = __ldcg(a.slots + (k + w) * 2 + d);
-#pragma unroll
-                for (int w = 0; w < 8; ++w) acc += v[w];
-            }
-            for (; k <= k1; ++k) acc += __ldcg(a.slots + k * 2 + d);
-        }
-        out[u] = acc;
-    }
+    graph_chunk_sum<2>(a.N, a.B, a.batch, keep, a.chamfer + (keep ? (int64_t)t * a.B * 2 : 0), a.slots, a.ticket,
+                       [&](int64_t k, double (&s)[2]) {
+                           s[0] += __ldg(a.minima + k);
+                           s[1] += __ldg(a.minima + a.N + k);
+                       });
 }
-
-static size_t chf_al(size_t x) { return (x + 255) / 256 * 256; }
-static int64_t chf_chunks(int64_t N) { return (N + SQERR_CHUNK - 1) / SQERR_CHUNK; }
 
 struct ChamferLayout {
     size_t bounds, flags, grid, keyrank, cell_start, sorted, minima, slots, ticket, tmp, tmp_bytes, total;
@@ -356,20 +248,19 @@ static int chamfer_layout(int64_t N, int B, ChamferLayout& L) {
     if (cub::DeviceScan::ExclusiveSum(nullptr, scan, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(2 * T + 1)) !=
         cudaSuccess)
         return DISTEGNN_ECUDA;
-    size_t o = 0;
-    auto put = [&](size_t& field, size_t bytes) { field = o; o += chf_al(bytes); };
-    put(L.bounds, (size_t)B * 6 * 4);
-    put(L.flags, (size_t)B * 4);
-    put(L.grid, (size_t)B * sizeof(ChamferGrid));
-    put(L.keyrank, (size_t)N * 2 * sizeof(int2));
-    put(L.cell_start, (size_t)(2 * T + 1) * 4);
-    put(L.sorted, (size_t)N * 2 * sizeof(float4));
-    put(L.minima, (size_t)N * 2 * 8);
-    put(L.slots, (size_t)chf_chunks(N) * 2 * 8);
-    put(L.ticket, 4);
+    WorkspaceCursor ws;
+    L.bounds = ws.take((size_t)B * 6 * 4);
+    L.flags = ws.take((size_t)B * 4);
+    L.grid = ws.take((size_t)B * sizeof(ChamferGrid));
+    L.keyrank = ws.take((size_t)N * 2 * sizeof(int2));
+    L.cell_start = ws.take((size_t)(2 * T + 1) * 4);
+    L.sorted = ws.take((size_t)N * 2 * sizeof(float4));
+    L.minima = ws.take((size_t)N * 2 * 8);
+    L.slots = ws.take((size_t)err_chunks(N) * 2 * 8);
+    L.ticket = ws.take(4);
     L.tmp_bytes = scan;
-    put(L.tmp, scan);
-    L.total = o;
+    L.tmp = ws.take(scan);
+    L.total = ws.end;
     return DISTEGNN_OK;
 }
 
@@ -440,7 +331,7 @@ int distegnn_rollout_chamfer(int64_t n_nodes, int n_graphs, int steps, const flo
     }
     chamfer_scatter_kernel<<<nb2, 256, 0, stream>>>(a);
     chamfer_search_kernel<<<nb2, 256, 0, stream>>>(a);
-    chamfer_sum_kernel<<<(unsigned)chf_chunks(n_nodes), DET_RED, 0, stream>>>(a);
+    chamfer_sum_kernel<<<(unsigned)err_chunks(n_nodes), DET_RED, 0, stream>>>(a);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

@@ -42,6 +42,17 @@ int check_dims(int A, int C, int Na);
         }                                                                                \
     } while (0)
 
+// Workspace carving: the parts of a caller-owned workspace are 256-byte aligned and laid out in the order they are taken.
+inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+struct WorkspaceCursor {
+    size_t end = 0;            // bytes taken so far
+    size_t take(size_t bytes) {
+        const size_t at = end;
+        end += align256(bytes);
+        return at;
+    }
+};
+
 int sm_count();   // cached multiprocessor count of the current device
 // Opt `kernel` in to `bytes` of dynamic shared memory, once per (device, kernel).  Not a stream operation, so it is
 // done on the first (eager) call and never again — nothing but launches happens under CUDA-graph capture.
@@ -169,6 +180,12 @@ __device__ __forceinline__ void edge_delta(const float* pos, int i, int j, float
     dx = __ldg(pos + (int64_t)i * 3) - __ldg(pos + (int64_t)j * 3);
     dy = __ldg(pos + (int64_t)i * 3 + 1) - __ldg(pos + (int64_t)j * 3 + 1);
     dz = __ldg(pos + (int64_t)i * 3 + 2) - __ldg(pos + (int64_t)j * 3 + 2);
+}
+// graph id of node i from data_batch, clamped into [0, B); 0 without a batch (one graph)
+__device__ __forceinline__ int graph_id(const int64_t* batch, int64_t i, int B) {
+    if (!batch) return 0;
+    const int64_t b = __ldg(batch + i);
+    return (int)(b < 0 ? 0 : (b >= B ? B - 1 : b));
 }
 __device__ __forceinline__ float4 fma4(float s, float4 w, float4 a) {
     return make_float4(fmaf(s, w.x, a.x), fmaf(s, w.y, a.y), fmaf(s, w.z, a.z), fmaf(s, w.w, a.w));

@@ -60,12 +60,6 @@ __device__ __forceinline__ int64_t cut_valid(const CutArgs& a) {
     return max((int64_t)0, min(nc, a.capacity));
 }
 
-__device__ __forceinline__ int clamp_graph(const CutArgs& a, int64_t i) {
-    if (!a.batch64) return 0;
-    const int64_t bb = a.batch64[i];
-    return (int)(bb < 0 ? 0 : (bb >= a.B ? a.B - 1 : bb));
-}
-
 // the graph holding candidate edge e (estart is non-decreasing; the graph found is non-empty)
 __device__ __forceinline__ int graph_of_edge(const int32_t* estart, int lo, int hi, int64_t e) {
     while (lo < hi) {               // last b in [lo, hi] with estart[b] <= e
@@ -77,8 +71,8 @@ __device__ __forceinline__ int graph_of_edge(const int32_t* estart, int lo, int 
 
 __global__ void __launch_bounds__(256) cut_graph_starts_kernel(const CutArgs a) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= a.N; i += (int64_t)gridDim.x * blockDim.x) {
-        const int prev = i == 0 ? -1 : clamp_graph(a, i - 1);
-        const int cur = i == a.N ? a.B : clamp_graph(a, i);
+        const int prev = i == 0 ? -1 : graph_id(a.batch64, i - 1, a.B);
+        const int cur = i == a.N ? a.B : graph_id(a.batch64, i, a.B);
         for (int b = prev + 1; b <= cur; ++b) a.gstart[b] = (int32_t)i;
     }
 }
@@ -262,14 +256,12 @@ __global__ void __launch_bounds__(256) cut_rowptr_kernel(const CutArgs a) {
             a.info[3] = 0;
             continue;
         }
-        const int g = clamp_graph(a, i);
+        const int g = graph_id(a.batch64, i, a.B);
         const int64_t s = __ldg(a.estart + g), e = __ldg(a.estart + g + 1);
         const int64_t p = min(max(min((int64_t)__ldg(a.rowptr_in + i), valid), s), e);
         a.rowptr_out[i] = (int32_t)kept_before(a, g, p);
     }
 }
-
-static size_t al256(size_t x) { return (x + 255) / 256 * 256; }
 
 struct CutLayout {
     size_t gstart, estart, kcount, kb, thr, rem, need, hist, keys, flags, tmp, tmp_bytes, total;
@@ -281,21 +273,20 @@ static int cut_layout(int64_t N, int B, int64_t capacity, CutLayout& L) {
     if (capacity > 0 && cub::DeviceScan::ExclusiveSum(nullptr, scan2, (unsigned long long*)nullptr,
                                                       (unsigned long long*)nullptr, (int)capacity) != cudaSuccess)
         return DISTEGNN_ECUDA;
-    size_t o = 0;
-    auto put = [&](size_t& field, size_t bytes) { field = o; o += al256(bytes); };
-    put(L.gstart, (size_t)(B + 1) * 4);
-    put(L.estart, (size_t)(B + 1) * 4);
-    put(L.kcount, (size_t)(B + 1) * 4);
-    put(L.kb, (size_t)B * 4);
-    put(L.thr, (size_t)B * 4);
-    put(L.rem, (size_t)B * 4);
-    put(L.need, (size_t)B * 4);
-    put(L.hist, (size_t)B * 256 * 4);
-    put(L.keys, (size_t)capacity * 4);
-    put(L.flags, (size_t)capacity * 8);
+    WorkspaceCursor ws;
+    L.gstart = ws.take((size_t)(B + 1) * 4);
+    L.estart = ws.take((size_t)(B + 1) * 4);
+    L.kcount = ws.take((size_t)(B + 1) * 4);
+    L.kb = ws.take((size_t)B * 4);
+    L.thr = ws.take((size_t)B * 4);
+    L.rem = ws.take((size_t)B * 4);
+    L.need = ws.take((size_t)B * 4);
+    L.hist = ws.take((size_t)B * 256 * 4);
+    L.keys = ws.take((size_t)capacity * 4);
+    L.flags = ws.take((size_t)capacity * 8);
     L.tmp_bytes = scan1 > scan2 ? scan1 : scan2;
-    put(L.tmp, L.tmp_bytes);
-    L.total = o + 256;
+    L.tmp = ws.take(L.tmp_bytes);
+    L.total = ws.end + 256;              // the caller's pointer is aligned up
     (void)N;
     return DISTEGNN_OK;
 }
@@ -352,7 +343,7 @@ extern "C" int distegnn_cutoff_csr(int64_t n_nodes, int n_graphs, const float* p
     }
     CutLayout L;
     cut_layout(n_nodes, n_graphs, capacity, L);
-    char* ws = (char*)(((uintptr_t)workspace + 255) / 256 * 256);
+    char* ws = (char*)align256((uintptr_t)workspace);
     CutArgs a;
     a.N = n_nodes; a.capacity = capacity; a.B = n_graphs; a.A = edge_attr_nf; a.keep_frac = 1.0 - cutoff_rate;
     a.pos = pos; a.batch64 = n_graphs > 1 ? data_batch : nullptr;

@@ -30,7 +30,6 @@ constexpr int DET_MIN_CHUNK = 16;      // real<->virtual tiles per chunk, at lea
 constexpr int64_t DET_MAX_CHUNKS = 4096;   // bounds the in-order combine (and the slots) per graph
 constexpr int DET_VTILE = 64;          // rows per real<->virtual tile (VW_TILE)
 
-inline int64_t det_align(int64_t b) { return (b + 255) / 256 * 256; }
 __host__ __device__ inline int det_nodes_per_tile(int C) { return DET_VTILE / C; }
 inline int64_t det_tiles(int64_t N, int C) { return (N + det_nodes_per_tile(C) - 1) / det_nodes_per_tile(C); }
 // log2 of the tiles per chunk: the smallest power of two >= DET_MIN_CHUNK that leaves at most DET_MAX_CHUNKS chunks
@@ -44,8 +43,8 @@ inline int64_t det_chunks(int64_t N, int C) {
     return (det_tiles(N, C) + (1ll << s) - 1) >> s;
 }
 inline int det_K(int C) { return 4 + 3 * C + H * C; }
-inline int64_t det_vsum_bytes(int64_t N, int C) { return det_align(det_chunks(N, C) * det_K(C) * 4); }
-inline int64_t det_edge_bytes(int64_t E) { return det_align((E + 15) / 16 * DET_EDGE_SLOT * 4); }
+inline int64_t det_vsum_bytes(int64_t N, int C) { return (int64_t)align256(det_chunks(N, C) * det_K(C) * 4); }
+inline int64_t det_edge_bytes(int64_t E) { return (int64_t)align256((E + 15) / 16 * DET_EDGE_SLOT * 4); }
 inline float* det_vsum_slots(void* ws) { return reinterpret_cast<float*>(ws); }
 inline float* det_edge_slots(void* ws, int64_t N, int C) {
     return reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + det_vsum_bytes(N, C));

@@ -1,5 +1,4 @@
-// Deterministic mode (det.cuh, DESIGN §17): workspace sizing, the two combine passes, and the fixed-order rollout centroid;
-// with the centroid's reduction, the rollout's per-step error against recorded targets (DESIGN §19), fixed-order always.
+// Deterministic mode (det.cuh, DESIGN §17): workspace sizing, the two combine passes, and the fixed-order rollout centroid.
 // Each output element of these kernels is computed by one thread in an order fixed by the input sizes, so their grids do
 // not enter the result.
 #include "common.cuh"
@@ -110,8 +109,8 @@ __global__ void __launch_bounds__(DET_RED) centroid_det_kernel(int64_t N, int B,
                                                                double* sums) {
     __shared__ double red[3][DET_RED];
     for (int b = blockIdx.x; b < B; b += gridDim.x) {
-        const int64_t lo = batch ? lower_bound_dev(batch, N, b) : 0;
-        const int64_t hi = batch ? lower_bound_dev(batch, N, (int64_t)b + 1) : N;
+        int64_t lo, hi;
+        graph_rows(batch, N, b, lo, hi);
         det_row_sum<double, 3>(lo, hi, [&](int64_t i, double (&s)[3]) {
             s[0] += (double)__ldg(pos + i * 3); s[1] += (double)__ldg(pos + i * 3 + 1); s[2] += (double)__ldg(pos + i * 3 + 2);
         }, red);
@@ -120,70 +119,6 @@ __global__ void __launch_bounds__(DET_RED) centroid_det_kernel(int64_t N, int B,
         __syncthreads();
     }
 }
-
-// The per-step error of a rollout against recorded targets (distegnn_rollout_sq_err).  Block c takes the rows [c·CH,
-// (c+1)·CH) and sums Σ_d (pred − target)² (fp32 differences, fp64 squares and sums) over each graph's rows in the chunk
-// with det_row_sum, the centroid's reduction.  A graph's first chunk stores its partial to sq_err[t, b], each later chunk
-// to its own slot; the last block to finish adds every graph's slots in chunk order.  So the order depends on N and the
-// graph sizes alone, and every value is a plain store (a rerun step overwrites its row).
-__global__ void __launch_bounds__(DET_RED) rollout_sq_err_kernel(int64_t N, int B, int steps, const float* pred,
-                                                                 const float* targets, const int64_t* batch,
-                                                                 const int32_t* counter, double* sq_err, double* slots,
-                                                                 unsigned* ticket) {
-    __shared__ double red[1][DET_RED];
-    __shared__ bool last;
-    const int t = __ldcg(counter);             // this step: the advance moves the counter on after this launch
-    const bool keep = t >= 0 && t < steps;
-    const int64_t c = blockIdx.x, r0 = c * SQERR_CHUNK, r1 = min(N, r0 + SQERR_CHUNK);
-    const float* tg = targets + (keep ? (int64_t)t * N * 3 : 0);
-    double* out = sq_err + (keep ? (int64_t)t * B : 0);
-    for (int64_t i = r0; keep && i < r1;) {    // the graphs of the chunk, one after the other (batch sorted)
-        const int64_t b = batch ? __ldg(batch + i) : 0;
-        const int64_t j = batch ? i + lower_bound_dev(batch + i, r1 - i, b + 1) : r1;
-        det_row_sum<double, 1>(i, j, [&](int64_t k, double (&s)[1]) {
-            s[0] += target_sq_dist([&](int d) { return __ldg(pred + k * 3 + d); },
-                                   [&](int d) { return __ldg(tg + k * 3 + d); });
-        }, red);
-        if (threadIdx.x == 0 && b >= 0 && b < B) {
-            const bool first = i > r0 || r0 == 0 || (batch && __ldg(batch + r0 - 1) != b);   // starts in this chunk
-            if (first) out[b] = red[0][0];
-            else slots[c] = red[0][0];
-        }
-        __syncthreads();
-        i = j;
-    }
-    if (threadIdx.x == 0) {
-        __threadfence();
-        last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!last) return;
-    __threadfence();
-    if (threadIdx.x == 0) *ticket = 0;
-    if (!keep) return;
-    for (int b = threadIdx.x; b < B; b += DET_RED) {
-        const int64_t lo = batch ? lower_bound_dev(batch, N, b) : 0;
-        const int64_t hi = batch ? lower_bound_dev(batch, N, (int64_t)b + 1) : N;
-        double acc = 0.0;
-        if (hi > lo) {
-            acc = __ldcg(out + b);
-            int64_t k = lo / SQERR_CHUNK + 1;
-            const int64_t k1 = (hi - 1) / SQERR_CHUNK;
-            for (; k + 8 <= k1 + 1; k += 8) {  // eight independent loads in flight, added in chunk order
-                double v[8];
-#pragma unroll
-                for (int u = 0; u < 8; ++u) v[u] = __ldcg(slots + k + u);
-#pragma unroll
-                for (int u = 0; u < 8; ++u) acc += v[u];
-            }
-            for (; k <= k1; ++k) acc += __ldcg(slots + k);
-        }
-        out[b] = acc;
-    }
-}
-
-static int64_t sq_err_chunks(int64_t N) { return (N + SQERR_CHUNK - 1) / SQERR_CHUNK; }
-static int64_t sq_err_workspace(int64_t N) { return det_align(sq_err_chunks(N) * 8) + 256; }
 
 static unsigned det_blocks(int64_t units, int64_t per_sm, int max_ctas) {
     const int64_t cap = per_sm * sm_count();
@@ -258,37 +193,6 @@ int distegnn_rollout_centroid_det(int64_t n_nodes, int n_graphs, const float* po
     DEGNN_CHECK_ARG(pos && sums, "null pointer");
     centroid_det_kernel<<<det_blocks(n_graphs, 8, 0), DET_RED, 0, (cudaStream_t)stream>>>(n_nodes, n_graphs, pos,
                                                                                        data_batch, sums);
-    DEGNN_CHECK_LAUNCH();
-    return DISTEGNN_OK;
-}
-
-int distegnn_rollout_sq_err_workspace_bytes(int64_t n_nodes, int64_t* bytes_host) {
-    using namespace degnn;
-    DEGNN_CHECK_ARG(bytes_host, "null output pointer");
-    DEGNN_CHECK_ARG(n_nodes >= 0, "negative size");
-    *bytes_host = sq_err_workspace(n_nodes);
-    return DISTEGNN_OK;
-}
-
-int distegnn_rollout_sq_err(int64_t n_nodes, int n_graphs, int steps, const float* pred, const float* targets,
-                            const int64_t* data_batch, const int32_t* counter, double* sq_err, void* workspace,
-                            int64_t workspace_bytes, void* stream) {
-    using namespace degnn;
-    DEGNN_CHECK_ARG(n_nodes >= 0 && n_graphs > 0 && steps >= 1, "bad size");
-    DEGNN_CHECK_ARG(n_graphs == 1 || data_batch, "data_batch needed for more than one graph");
-    DEGNN_CHECK_ARG(counter && sq_err, "null pointer");
-    if (n_nodes == 0) return DISTEGNN_OK;
-    DEGNN_CHECK_ARG(pred && targets && workspace, "null pointer");
-    DEGNN_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "workspace not 16-byte aligned");
-    if (workspace_bytes < sq_err_workspace(n_nodes)) {
-        set_error("distegnn_rollout_sq_err: workspace %lld < %lld bytes", (long long)workspace_bytes,
-                  (long long)sq_err_workspace(n_nodes));
-        return DISTEGNN_EWORKSPACE;
-    }
-    double* slots = reinterpret_cast<double*>(workspace);
-    unsigned* ticket = reinterpret_cast<unsigned*>(reinterpret_cast<char*>(workspace) + det_align(sq_err_chunks(n_nodes) * 8));
-    rollout_sq_err_kernel<<<(unsigned)sq_err_chunks(n_nodes), DET_RED, 0, (cudaStream_t)stream>>>(
-        n_nodes, n_graphs, steps, pred, targets, data_batch, counter, sq_err, slots, ticket);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

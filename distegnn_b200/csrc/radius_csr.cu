@@ -7,7 +7,7 @@
 // order.  Everything the host used to decide is decided on the device, so the call neither synchronises nor needs the
 // edge count in advance (the caller passes a CAPACITY; the true count lands in info[0], an overflow flag in info[1]):
 //   1. bounding box of the finite coordinates (block reduction + ordered-int atomics)
-//   2. uniform grid (radius_grid.cuh): cell size = radius·(1 + 2^-10), grown x1.5 until the dense cell table fits the
+//   2. uniform grid (cell_grid.cuh): cell size = radius·(1 + 2^-10), grown x1.5 until the dense cell table fits the
 //      caller's table_cells; every key lies inside the table for any position, ±inf and NaN included
 //   3. cell key per node + histogram; exclusive scan of the histogram = first position of every cell (cub)
 //   4. node ids sorted by key (cub radix sort), so that a warp scans neighbouring cells together
@@ -18,15 +18,10 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include "cell_grid.cuh"
 #include "common.cuh"
-#include "radius_grid.cuh"
 
 namespace degnn {
-
-struct GridDev {
-    float ox, oy, oz, inv_cell;
-    int nx, ny, nz, ncell;     // ncell = nx*ny*nz (per graph)
-};
 
 struct RcsrArgs {
     int64_t N, capacity, table_cells;
@@ -35,7 +30,7 @@ struct RcsrArgs {
     const float* pos;          // [N,3]
     const int64_t* batch64;    // [N] or null
     int* bounds;               // [6] ordered-int encoded min xyz / max xyz
-    GridDev* grid;
+    CellGrid* grid;            // one grid; graph b's cells take the keys b·ncell + [0, ncell)
     float* x4;                 // [N,4]
     int32_t* batch32;          // [N]
     int32_t* keys;             // [N]
@@ -51,17 +46,10 @@ struct RcsrArgs {
     int32_t* info;             // [4]: edges found, overflow flag, cells used, reserved
 };
 
-__device__ __forceinline__ int f2ord(float f) {      // order-preserving float -> int
-    const int i = __float_as_int(f);
-    return i >= 0 ? i : i ^ 0x7fffffff;
-}
-__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
 __global__ void rcsr_init_kernel(const RcsrArgs a) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i <= a.table_cells) a.cell_cnt[i] = 0;
-    if (i < 3) a.bounds[i] = f2ord(INFINITY);
-    if (i >= 3 && i < 6) a.bounds[i] = f2ord(-INFINITY);
+    if (i < 6) a.bounds[i] = ordered_int(i < 3 ? INFINITY : -INFINITY);
     if (i < 4) a.info[i] = 0;
 }
 
@@ -69,75 +57,32 @@ __global__ void __launch_bounds__(256) rcsr_bounds_kernel(const RcsrArgs a) {
     float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.N; i += (int64_t)gridDim.x * blockDim.x) {
 #pragma unroll
-        for (int d = 0; d < 3; ++d) {
-            const float v = __ldg(a.pos + i * 3 + d);
-            if (isfinite(v)) {                            // an inf would stretch the grid over nothing
-                lo[d] = fminf(lo[d], v);
-                hi[d] = fmaxf(hi[d], v);
-            }
-        }
+        for (int d = 0; d < 3; ++d) bound_add(lo[d], hi[d], __ldg(a.pos + i * 3 + d));
     }
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo[d] = fminf(lo[d], __shfl_xor_sync(FULL, lo[d], o));
-            hi[d] = fmaxf(hi[d], __shfl_xor_sync(FULL, hi[d], o));
-        }
-        if ((threadIdx.x & 31) == 0) {
-            atomicMin(a.bounds + d, f2ord(lo[d]));
-            atomicMax(a.bounds + 3 + d, f2ord(hi[d]));
-        }
-    }
+    bound_warp_reduce(lo, hi);
+    if ((threadIdx.x & 31) == 0) bound_flush(a.bounds, lo, hi);
 }
 
 __global__ void rcsr_grid_kernel(const RcsrArgs a) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    GridDev g;
-    float lo[3], ext[3];
-    for (int k = 0; k < 3; ++k) {
-        lo[k] = ord2f(a.bounds[k]);
-        float hi = ord2f(a.bounds[3 + k]);
-        if (!(lo[k] <= hi)) lo[k] = hi = 0.f;        // no finite coordinate on this axis
-        ext[k] = hi - lo[k];                          // +inf if the finite range exceeds FLT_MAX: one slab on that axis
-    }
-    const RadiusGridSize s = radius_grid_size(ext, a.radius, a.B, a.table_cells);
-    g.ox = lo[0]; g.oy = lo[1]; g.oz = lo[2];
-    g.inv_cell = 1.0f / s.cell;
-    g.nx = s.dims[0]; g.ny = s.dims[1]; g.nz = s.dims[2];
-    g.ncell = s.ncell;
+    float o[3], ext[3];
+    bounds_origin_extent(a.bounds, o, ext);
+    const CellGrid g = make_cell_grid(o, radius_grid_size(ext, a.radius, a.B, a.table_cells));
     *a.grid = g;
     a.info[2] = g.ncell * a.B;
-}
-
-// Cell index along one axis, in [0, n) for any coordinate: below the origin -> 0, beyond the last cell (+inf included)
-// -> n - 1, NaN -> 0.  Monotone in x, so clamping only merges end cells, which the 27-cell scan still covers.
-__device__ __forceinline__ int axis_cell(float x, float o, float inv_cell, int n) {
-    const float q = (x - o) * inv_cell;
-    return q > 0.f ? (q < (float)n ? (int)q : n - 1) : 0;
-}
-
-__device__ __forceinline__ void cell_of(const GridDev& g, float x, float y, float z, int& ix, int& iy, int& iz) {
-    ix = axis_cell(x, g.ox, g.inv_cell, g.nx);
-    iy = axis_cell(y, g.oy, g.inv_cell, g.ny);
-    iz = axis_cell(z, g.oz, g.inv_cell, g.nz);
 }
 
 __global__ void __launch_bounds__(256) rcsr_keys_kernel(const RcsrArgs a) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0) a.deg[a.N] = 0;
     if (i >= a.N) return;
-    const GridDev g = *a.grid;
+    const CellGrid g = *a.grid;
     const float x = __ldg(a.pos + i * 3), y = __ldg(a.pos + i * 3 + 1), z = __ldg(a.pos + i * 3 + 2);
     *reinterpret_cast<float4*>(a.x4 + i * 4) = make_float4(x, y, z, 0.f);
-    int b = 0;
-    if (a.batch64) {
-        const int64_t bb = a.batch64[i];
-        b = (int)(bb < 0 ? 0 : (bb >= a.B ? a.B - 1 : bb));
-    }
+    const int b = graph_id(a.batch64, i, a.B);
     a.batch32[i] = b;
     int ix, iy, iz;
-    cell_of(g, x, y, z, ix, iy, iz);
+    cell_of(g, x, y, z, ix, iy, iz);     // clamping only merges end cells, which the 27-cell scan still covers
     const int key = b * g.ncell + (ix * g.ny + iy) * g.nz + iz;
     a.keys[i] = key;
     a.ids[i] = (int32_t)i;
@@ -148,7 +93,7 @@ template <bool FILL>
 __global__ void __launch_bounds__(256) rcsr_scan_kernel(const RcsrArgs a) {
     const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.N) return;
-    const GridDev g = *a.grid;
+    const CellGrid g = *a.grid;
     const int i = __ldg(a.order + k);
     const float4 p = ldg4(a.x4 + (size_t)i * 4);
     const int b = __ldg(a.batch32 + i);
@@ -203,7 +148,6 @@ __global__ void rcsr_info_kernel(const RcsrArgs a) {
     }
 }
 
-static size_t al256(size_t x) { return (x + 255) / 256 * 256; }
 static int bits_for(int64_t n) {
     int b = 1;
     while (b < 31 && ((int64_t)1 << b) < n) ++b;
@@ -223,22 +167,21 @@ static int rcsr_layout(int64_t N, int64_t table_cells, RcsrLayout& L) {
         return DISTEGNN_ECUDA;
     if (cub::DeviceScan::ExclusiveSum(nullptr, scan2, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(N + 1)) != cudaSuccess)
         return DISTEGNN_ECUDA;
-    size_t o = 0;
-    auto put = [&](size_t& field, size_t bytes) { field = o; o += al256(bytes); };
-    put(L.bounds, 6 * 4);
-    put(L.grid, sizeof(GridDev));
-    put(L.x4, (size_t)N * 16);
-    put(L.batch32, (size_t)N * 4);
-    put(L.keys, (size_t)N * 4);
-    put(L.ids, (size_t)N * 4);
-    put(L.skeys, (size_t)N * 4);
-    put(L.order, (size_t)N * 4);
-    put(L.cell_cnt, (size_t)(table_cells + 1) * 4);
-    put(L.deg, (size_t)(N + 1) * 4);
+    WorkspaceCursor ws;
+    L.bounds = ws.take(6 * 4);
+    L.grid = ws.take(sizeof(CellGrid));
+    L.x4 = ws.take((size_t)N * 16);
+    L.batch32 = ws.take((size_t)N * 4);
+    L.keys = ws.take((size_t)N * 4);
+    L.ids = ws.take((size_t)N * 4);
+    L.skeys = ws.take((size_t)N * 4);
+    L.order = ws.take((size_t)N * 4);
+    L.cell_cnt = ws.take((size_t)(table_cells + 1) * 4);
+    L.deg = ws.take((size_t)(N + 1) * 4);
     L.tmp_bytes = sort_b > scan1 ? sort_b : scan1;
     if (scan2 > L.tmp_bytes) L.tmp_bytes = scan2;
-    put(L.tmp, L.tmp_bytes);
-    L.total = o + 256;
+    L.tmp = ws.take(L.tmp_bytes);
+    L.total = ws.end + 256;              // the caller's pointer is aligned up
     return DISTEGNN_OK;
 }
 
@@ -278,11 +221,11 @@ extern "C" int distegnn_radius_graph_csr(int64_t n_nodes, int n_graphs, const fl
     }
     RcsrLayout L;
     rcsr_layout(n_nodes, table_cells, L);
-    char* ws = (char*)(((uintptr_t)workspace + 255) / 256 * 256);
+    char* ws = (char*)align256((uintptr_t)workspace);
     RcsrArgs a;
     a.N = n_nodes; a.capacity = capacity; a.table_cells = table_cells; a.B = n_graphs; a.A = edge_attr_nf; a.loop = loop;
     a.radius = radius; a.pos = pos; a.batch64 = data_batch;
-    a.bounds = (int*)(ws + L.bounds); a.grid = (GridDev*)(ws + L.grid); a.x4 = (float*)(ws + L.x4);
+    a.bounds = (int*)(ws + L.bounds); a.grid = (CellGrid*)(ws + L.grid); a.x4 = (float*)(ws + L.x4);
     a.batch32 = (int32_t*)(ws + L.batch32); a.keys = (int32_t*)(ws + L.keys); a.ids = (int32_t*)(ws + L.ids);
     a.skeys = (int32_t*)(ws + L.skeys); a.order = (int32_t*)(ws + L.order); a.cell_cnt = (int32_t*)(ws + L.cell_cnt);
     a.deg = (int32_t*)(ws + L.deg);

@@ -92,11 +92,7 @@ __global__ void __launch_bounds__(256) centroid_kernel(int64_t N, int B, const f
     for (int64_t base = (int64_t)blockIdx.x * blockDim.x; base < N; base += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i = base + threadIdx.x;
         const bool ok = i < N;
-        int b = 0;
-        if (ok && batch) {
-            const int64_t bb = batch[i];
-            b = (int)(bb < 0 ? 0 : (bb >= B ? B - 1 : bb));
-        }
+        const int b = ok ? graph_id(batch, i, B) : 0;
         double s[4] = {0.0, 0.0, 0.0, 0.0};
         if (ok) {
             s[0] = __ldg(pos + i * 3); s[1] = __ldg(pos + i * 3 + 1); s[2] = __ldg(pos + i * 3 + 2); s[3] = 1.0;

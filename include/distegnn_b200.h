@@ -512,8 +512,8 @@ DISTEGNN_API int distegnn_vsum_combine_det(int64_t n_nodes, int n_graphs, int C,
                                            void *stream);
 DISTEGNN_API int distegnn_rollout_centroid_det(int64_t n_nodes, int n_graphs, const float *pos,
                                                const int64_t *data_batch, double *sums, void *stream);
-/* distegnn_rollout_sq_err: a rollout step's error against recorded targets, between the forward and
- * distegnn_rollout_advance.  With t = counter[0] (the advance's step counter, see distegnn_rollout_advance; nothing is
+/* distegnn_rollout_sq_err (csrc/rollout_err.cu): a rollout step's error against recorded targets, between the forward
+ * and distegnn_rollout_advance.  With t = counter[0] (the advance's step counter, see distegnn_rollout_advance; nothing is
  * written unless 0 <= t < steps):
  *   sq_err[t, b] = Σ_{i in graph b} ‖pred_i − targets[t, i]‖²     (sq_err float64 [steps, n_graphs], targets [steps, N, 3])
  * with the differences in fp32 (round-to-nearest) and the squares and sums in fp64, in an order fixed by n_nodes and the

@@ -13,11 +13,11 @@ extern "C" {
 
 /* Host-only: the grid distegnn_radius_graph_csr sizes for bounding-box extents ext[3] (hi - lo over the finite
  * coordinates; +inf, -inf or NaN allowed), `radius`, `n_graphs` graphs and a table of `table_cells` entries: cell edge,
- * dims[3] and ncell = dims[0]*dims[1]*dims[2] per graph (csrc/radius_grid.cuh).  No device needed. */
+ * dims[3] and ncell = dims[0]*dims[1]*dims[2] per graph (csrc/cell_grid.cuh).  No device needed. */
 DISTEGNN_API int distegnn_radius_grid_size(const float *ext, float radius, int n_graphs, int64_t table_cells,
                                            float *cell, int32_t *dims, int64_t *ncell);
 /* Host-only: the grid distegnn_rollout_chamfer sizes for one graph of bounding-box extents ext[3] (as above) and a budget
- * of `budget` cells per cloud (the graph's node count + 1): cell edge, dims[3] and ncell (csrc/chamfer_grid.cuh). */
+ * of `budget` cells per cloud (the graph's node count + 1): cell edge, dims[3] and ncell (csrc/cell_grid.cuh). */
 DISTEGNN_API int distegnn_chamfer_grid_size(const float *ext, int64_t budget, float *cell, int32_t *dims,
                                             int64_t *ncell);
 

@@ -18,7 +18,7 @@ import pytest
 import torch
 
 F32 = np.float32
-MARGIN = F32(1.0) + F32(2.0 ** -10)        # the first cell edge is fp32(r) * MARGIN (csrc/radius_grid.cuh)
+MARGIN = F32(1.0) + F32(2.0 ** -10)        # the first cell edge is fp32(r) * MARGIN (csrc/cell_grid.cuh)
 DEFAULT_TABLE = 1 << 22
 
 
