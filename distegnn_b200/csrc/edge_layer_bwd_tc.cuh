@@ -134,12 +134,12 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
     // after the group barrier that publishes the A operand: D = A·Wᵀ over the whole tile by the group's warpgroup, written
     // over A; mma_done() publishes D to every row thread
     auto issue = [&](const __half* whi, const __half* wlo) {
-        tc16::mma_f16x3<BT_LBO>(col0, col0, col0 + 32u, make_b_desc(smem_u32(whi), BT_LBO, 128),
-                                make_b_desc(smem_u32(wlo), BT_LBO, 128), 1, false, 0, 2);
+        tc16::mma_f16x3<BT_LBO>(col0, col0, col0 + 32u, make_desc(smem_u32(whi), BT_LBO, 128),
+                                make_desc(smem_u32(wlo), BT_LBO, 128), 1, false, 0, 2);
     };
     auto mma_done = [&]() { named_bar(bar_id, BT_GROUP); };
     auto a_ready = [&]() {
-        tm_st_fence();
+        fence_proxy_async_smem();
         named_bar(bar_id, BT_GROUP);
     };
     // column sums of the gradient tile into a shared accumulator: thread <-> (column, half of the rows)

@@ -9,7 +9,7 @@
 // q = lane%4) owns rows g and g+8 of the warp, columns 8j + 2q + {0,1} (j = 0..7).  The A operands and the accumulators
 // stay in registers; only the weights (W2, Wc hi/lo) and the neighbour rows Q[col] are in shared memory.  Per tile
 // (numerics as in the other tensor-core kernels: fp16 2-term split, per-row power-of-two range rescue, one reciprocal
-// per four SiLUs with a stage-level guard):
+// per four SiLUs with a stage-level guard; the rescue and the guard are tc16.cuh encode_rows, the φ head phi_head_t):
 //   stage 1  a1 = SiLU(P[row] + Q[col] + w_r·r + W_e·a) -> fp16 hi/lo A fragments                MMA 1: D = a1·W2ᵀ
 //   stage 2  m = SiLU(D + b2) -> fp32 into the warp's staging rows (segment sum) + hi/lo A fragments   MMA 2: D = m·Wcᵀ
 //            segment sum of m over destination rows while MMA 2 runs (lane <-> column pair, one RED.v2 per run)
@@ -74,8 +74,6 @@ constexpr int CS_SMEM_BYTES = 4 * CS_W * 2                // W2 hi/lo, Wc hi/lo
                               + CS_WARPS * CS_IDX * 4                     // indices of the tile after next
                               + CS_WARPS * 16 * 8 * 4;                    // x[row], x[col] of the next tile
 constexpr uint32_t CS_LBO = 1024;                         // fp16 K-major no-swizzle, N = 64
-using tc16::kFast;
-using tc16::kSafe;
 
 // DET (deterministic mode, det.cuh): the partial of every run is stored, not added.  The run of a row whose first edge lies
 // in the warp's 16-edge slice goes to the row itself; the slice's head run, when it continues a row of the slice before,
@@ -133,8 +131,8 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
     int* nidx = idx_all + warp * CS_IDX;
     float* xs = xs_all + warp * 16 * 8 + 8 * (lane & 15);     // (x_row, x_col) of edge `lane` of the next tile
     uint64_t* qbar = bars + 2 * warp;
-    const uint64_t bW2hi = make_b_desc(smem_u32(W2hi), CS_LBO, 128), bW2lo = make_b_desc(smem_u32(W2lo), CS_LBO, 128);
-    const uint64_t bWchi = make_b_desc(smem_u32(Wchi), CS_LBO, 128), bWclo = make_b_desc(smem_u32(Wclo), CS_LBO, 128);
+    const uint64_t bW2hi = make_desc(smem_u32(W2hi), CS_LBO, 128), bW2lo = make_desc(smem_u32(W2lo), CS_LBO, 128);
+    const uint64_t bWchi = make_desc(smem_u32(Wchi), CS_LBO, 128), bWclo = make_desc(smem_u32(Wclo), CS_LBO, 128);
 
     const int64_t nE = a.E_dev ? min((int64_t)__ldg(a.E_dev), a.E) : a.E;     // valid edges (<= the host-side bound)
     const int64_t num_tiles = (nE + CS_TILE - 1) / CS_TILE;
@@ -258,49 +256,17 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         };
         // register i = 2j + r of a fragment array <-> row g + 8r, columns 8j + 2q + {0,1} (= accumulator pair d[2i], d[2i+1])
         uint32_t ahi[16], alo[16];
-        float inv1a = 1.0f, inv1b = 1.0f;  // 1 / the rows' range scales
+        float qmax = 0.f;
+        auto silu_guard = [&] { return silu_q_overflow(qmax); };
+        tc16::RowScales s1;
         mbar_wait(qbar + b, (uint32_t)((it >> 1) & 1));
-        {
-            __half2 mx = __floats2half2_rn(0.f, 0.f);
-            float qmax = 0.f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                f32x2 va = pre(j, pa, qa, rada, eaa, oka), vb = pre(j, pb, qbr, radb, eab, okb);
-                silu4p<false>(va, vb, qmax);
-                tc16::split_pair(va, ahi[2 * j], alo[2 * j]);
-                tc16::split_pair(vb, ahi[2 * j + 1], alo[2 * j + 1]);
-                // SiLU outputs are bounded below (−0.28): only the positive side can leave the fp16 range
-                mx = __hmax2(mx, __hmax2(*reinterpret_cast<const __half2*>(&ahi[2 * j]),
-                                         *reinterpret_cast<const __half2*>(&ahi[2 * j + 1])));
-            }
-            if (__any_sync(FULL, tc16::row_overflow(mx) || silu_q_overflow(qmax))) {
-                // cold: some row leaves the fp16 range, or the SiLU batch guard fired — per-element SiLU, row scales
-                float fa = 0.f, fb = 0.f, sa, sb;
-#pragma unroll 1
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 va = pre(j, pa, qa, rada, eaa, oka), vb = pre(j, pb, qbr, radb, eab, okb);
-                    silu4p<true>(va, vb, qmax);
-                    float v0, v1;
-                    upk2(va, v0, v1);
-                    fa = fmaxf(fa, fmaxf(v0, v1));
-                    upk2(vb, v0, v1);
-                    fb = fmaxf(fb, fmaxf(v0, v1));
-                }
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 1));
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 2));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 1));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 2));
-                tc16::range_scale(fa, sa, inv1a);
-                tc16::range_scale(fb, sb, inv1b);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 va = pre(j, pa, qa, rada, eaa, oka), vb = pre(j, pb, qbr, radb, eab, okb);
-                    silu4p<true>(va, vb, qmax);
-                    tc16::split_pair(mul2(va, bc2(sa)), ahi[2 * j], alo[2 * j]);
-                    tc16::split_pair(mul2(vb, bc2(sb)), ahi[2 * j + 1], alo[2 * j + 1]);
-                }
-            }
-        }
+        tc16::encode_rows<false, true>(
+            [&](int j, f32x2& va, f32x2& vb, auto pass) {
+                va = pre(j, pa, qa, rada, eaa, oka);
+                vb = pre(j, pb, qbr, radb, eab, okb);
+                silu4p<decltype(pass)::value != tc16::FAST_PASS>(va, vb, qmax);
+            },
+            ahi, alo, s1, silu_guard);
 
         // ---- MMA 1; the run-start mask of the warp's edges while it runs --------------------------------------------
         float d[32];
@@ -311,61 +277,22 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
         // ---- stage 2: m = SiLU(D/s + b2) -> fp32 staging rows (segment sum) and fp16 hi/lo A fragments ----------------
-        float inv2a = 1.0f, inv2b = 1.0f;
-        auto m_pair = [&](int j, f32x2& ma, f32x2& mb) {
-            const f32x2 bb = *reinterpret_cast<const f32x2*>(b2s + 8 * j + 2 * q);
-            ma = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv1a), bb);
-            mb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv1b), bb);
-        };
-        auto store_m = [&](int j, f32x2 ma, f32x2 mb) {     // (ma, mb) = SILU_T_IN·m: the flush and Wc's consumer undo it
-            *reinterpret_cast<f32x2*>(qcur + g * CS_QROW + 8 * j + 2 * q) = ma;
-            *reinterpret_cast<f32x2*>(qcur + (g + 8) * CS_QROW + 8 * j + 2 * q) = mb;
-        };
-        {
-            __half2 mx = __floats2half2_rn(0.f, 0.f);
-            float qmax = 0.f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                f32x2 ma, mb;
-                m_pair(j, ma, mb);
-                silu4t<false>(ma, mb, qmax);
-                if (need_m) store_m(j, ma, mb);
-                tc16::split_pair(ma, ahi[2 * j], alo[2 * j]);
-                tc16::split_pair(mb, ahi[2 * j + 1], alo[2 * j + 1]);
-                // t-domain values: ≤ 0.41, unbounded below — track the minimum
-                mx = __hmin2(mx, __hmin2(*reinterpret_cast<const __half2*>(&ahi[2 * j]),
-                                         *reinterpret_cast<const __half2*>(&ahi[2 * j + 1])));
-            }
-            if (__any_sync(FULL, fminf(__low2float(mx), __high2float(mx)) < -tc16::RANGE || silu_q_overflow(qmax))) {
-                float fa = 0.f, fb = 0.f, sa, sb;      // cold (unrolled: d stays in registers)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 ma, mb;
-                    m_pair(j, ma, mb);
-                    silu4t<true>(ma, mb, qmax);
-                    if (need_m) store_m(j, ma, mb);    // also rewrites the m rows of the batch-guard case
-                    float v0, v1;
-                    upk2(ma, v0, v1);
-                    fa = fmaxf(fa, -fminf(v0, v1));
-                    upk2(mb, v0, v1);
-                    fb = fmaxf(fb, -fminf(v0, v1));
+        // (ma, mb) = SILU_T_IN·m: the flush and Wc's consumer undo it.  The rows are stored by the pass whose values are
+        // final: the fast pass, and again by the row-max pass when the warp takes the cold path (batch guard included).
+        qmax = 0.f;
+        tc16::RowScales s2;
+        tc16::encode_rows<false>(
+            [&](int j, f32x2& ma, f32x2& mb, auto pass) {
+                const f32x2 bb = *reinterpret_cast<const f32x2*>(b2s + 8 * j + 2 * q);
+                ma = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(s1.inv_a), bb);
+                mb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(s1.inv_b), bb);
+                silu4t<decltype(pass)::value != tc16::FAST_PASS>(ma, mb, qmax);
+                if (need_m && decltype(pass)::value != tc16::ENCODE_PASS) {
+                    *reinterpret_cast<f32x2*>(qcur + g * CS_QROW + 8 * j + 2 * q) = ma;
+                    *reinterpret_cast<f32x2*>(qcur + (g + 8) * CS_QROW + 8 * j + 2 * q) = mb;
                 }
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 1));
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 2));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 1));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 2));
-                tc16::range_scale(fa, sa, inv2a);
-                tc16::range_scale(fb, sb, inv2b);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 ma, mb;
-                    m_pair(j, ma, mb);
-                    silu4t<true>(ma, mb, qmax);
-                    tc16::split_pair(mul2(ma, bc2(sa)), ahi[2 * j], alo[2 * j]);
-                    tc16::split_pair(mul2(mb, bc2(sb)), ahi[2 * j + 1], alo[2 * j + 1]);
-                }
-            }
-        }
+            },
+            ahi, alo, s2, silu_guard);
 
         // ---- MMA 2 (φ head) overlapped with the segment sum of m ----------------------------------------------
         tc16::mma_f16x3_rA<CS_LBO>(d, ahi, alo, bWchi, bWclo);
@@ -414,32 +341,8 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
         // ---- stage 3: φ = w3·SiLU(D/s + bc) per row; Δx·φ summed per destination row ------------------------------
-        float qmax = 0.f;
-        f32x2 pha, phb;
-        auto phi_pass = [&](auto safe) {
-            pha = phb = bc2(0.f);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const f32x2 bb = *reinterpret_cast<const f32x2*>(bcs + 8 * j + 2 * q);
-                const f32x2 ww = *reinterpret_cast<const f32x2*>(w3s + 8 * j + 2 * q);
-                f32x2 sa = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv2a), bb);
-                f32x2 sb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv2b), bb);
-                silu4t<decltype(safe)::value>(sa, sb, qmax);
-                pha = fma2(sa, ww, pha);
-                phb = fma2(sb, ww, phb);
-            }
-        };
-        phi_pass(kFast);
-        if (__any_sync(FULL, silu_q_overflow(qmax))) phi_pass(kSafe);      // cold (no scale)
-        float p0, p1;
-        upk2(pha, p0, p1);
-        float phia = p0 + p1;
-        upk2(phb, p0, p1);
-        float phib = p0 + p1;
-        phia += __shfl_xor_sync(FULL, phia, 1);
-        phia += __shfl_xor_sync(FULL, phia, 2);
-        phib += __shfl_xor_sync(FULL, phib, 1);
-        phib += __shfl_xor_sync(FULL, phib, 2);
+        float phia, phib;
+        tc16::phi_head_t(d, s2.inv_a, s2.inv_b, bcs, w3s, q, phia, phib);
         {   // lane e < 16 <-> edge e = fragment row (e & 7) + 8·(e >> 3), held by quad e & 7
             const float fa = __shfl_sync(FULL, phia, 4 * (lane & 7)), fb = __shfl_sync(FULL, phib, 4 * (lane & 7));
             const float phi = (lane & 8) ? fb : fa;

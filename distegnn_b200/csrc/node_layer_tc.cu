@@ -56,65 +56,11 @@ struct Rows {
 };
 __device__ __forceinline__ f32x2 ld_pair(const float* p) { return *reinterpret_cast<const f32x2*>(p); }
 __device__ __forceinline__ void st_pair(float* p, f32x2 v) { *reinterpret_cast<f32x2*>(p) = v; }
-__device__ __forceinline__ float quad_max(float v) {
-    v = fmaxf(v, __shfl_xor_sync(FULL, v, 1));
-    return fmaxf(v, __shfl_xor_sync(FULL, v, 2));
-}
 // Pull bytes [p, p + n) towards L2: one 128-byte line per thread of a warpgroup (t < 128) and step
 __device__ __forceinline__ void prefetch_l2_range(const void* p, size_t n, int t) {
     const uintptr_t b = (uintptr_t)p, e = b + n;
     for (uintptr_t l = (b & ~(uintptr_t)127) + 128u * (uintptr_t)t; l < e; l += 128u * 128u)
         tmma::prefetch_l2((const void*)l);
-}
-__device__ __forceinline__ float quad_sum(float v) {
-    v += __shfl_xor_sync(FULL, v, 1);
-    return v + __shfl_xor_sync(FULL, v, 2);
-}
-
-// Encode the thread's rows a and b, produced as column pairs by f(j, xa, xb, first) (columns 8j + 2q, +1; first = false
-// on the cold passes), into the fp16 hi/lo A fragments (register 2j + r holds pair j of row a / b for r = 0 / 1).  sa / sb:
-// in, the power-of-two scales the rows already carry (1 normally); out, the scales used — smaller only where a row would
-// leave the fp16 range (cold path, per warp).  The passes are unrolled: f may read an accumulator that must stay in
-// registers.
-template <class F>
-__device__ __forceinline__ void encode_rows(F&& f, uint32_t (&hi)[16], uint32_t (&lo)[16], float& sa, float& sb) {
-    const bool pre_scaled = __any_sync(FULL, sa != 1.0f || sb != 1.0f);
-    if (!pre_scaled) {
-        __half2 mx = __floats2half2_rn(0.f, 0.f);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            f32x2 xa, xb;
-            f(j, xa, xb, true);
-            tc16::split_pair(xa, hi[2 * j], lo[2 * j]);
-            tc16::split_pair(xb, hi[2 * j + 1], lo[2 * j + 1]);
-            mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[2 * j])));
-            mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[2 * j + 1])));
-        }
-        if (!__any_sync(FULL, tc16::row_overflow(mx))) return;
-    }
-    // cold: some row of this warp carries a scale already or leaves the fp16 range
-    float fa = 0.f, fb = 0.f, ca, cb, unused;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        f32x2 xa, xb;
-        float v0, v1;
-        f(j, xa, xb, false);
-        upk2(xa, v0, v1);
-        fa = fmaxf(fa, fmaxf(fabsf(v0), fabsf(v1)));
-        upk2(xb, v0, v1);
-        fb = fmaxf(fb, fmaxf(fabsf(v0), fabsf(v1)));
-    }
-    tc16::range_scale(quad_max(fa), ca, unused);
-    tc16::range_scale(quad_max(fb), cb, unused);
-    sa = fminf(ca, sa);
-    sb = fminf(cb, sb);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        f32x2 xa, xb;
-        f(j, xa, xb, false);
-        tc16::split_pair(mul2(xa, bc2(sa)), hi[2 * j], lo[2 * j]);
-        tc16::split_pair(mul2(xb, bc2(sb)), hi[2 * j + 1], lo[2 * j + 1]);
-    }
 }
 
 // Σ(x, 1) per graph into vsum[:, 0:4].  Lane q of a quad holds entry q of its rows a and b.  Tiles inside one graph add to
@@ -171,11 +117,11 @@ template <class Hrow>
 __device__ __forceinline__ void store_h_project(Hrow&& hrow, const Rows& r, float* h_out, float* P, float* Q, float* Hn,
                                                 uint64_t b_hi, uint64_t b_lo, const float* nxb1s, float (&d)[32],
                                                 uint32_t (&ahi)[16], uint32_t (&alo)[16]) {
-    float sa = 1.0f, sb = 1.0f;
-    encode_rows(
-        [&](int j, f32x2& xa, f32x2& xb, bool first) {
+    tc16::RowScales s;
+    tc16::encode_rows<true>(
+        [&](int j, f32x2& xa, f32x2& xb, auto pass) {
             const int col = 8 * j + 2 * r.q;
-            if (first) {
+            if constexpr (decltype(pass)::value == tc16::FAST_PASS) {
                 hrow(j, xa, xb);
                 if (r.va) st_pair(h_out + r.na * H + col, xa);
                 if (r.vb) st_pair(h_out + r.nb * H + col, xb);
@@ -184,8 +130,8 @@ __device__ __forceinline__ void store_h_project(Hrow&& hrow, const Rows& r, floa
                 xb = r.vb ? ld_pair(h_out + r.nb * H + col) : 0ull;
             }
         },
-        ahi, alo, sa, sb);
-    const float ia = sa == 1.0f ? 1.0f : 1.0f / sa, ib = sb == 1.0f ? 1.0f : 1.0f / sb;
+        ahi, alo, s);
+    const float ia = s.a == 1.0f ? 1.0f : 1.0f / s.a, ib = s.b == 1.0f ? 1.0f : 1.0f / s.b;
 #pragma unroll 1
     for (int o = 0; o < 3; ++o) {
         tc16::mma_f16x3_rA<NT_LBO192>(d, ahi, alo, b_hi + o * NT_DESC_N64, b_lo + o * NT_DESC_N64);
@@ -255,7 +201,7 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
     fence_proxy_async_smem();
     __syncthreads();
 
-    auto desc = [&](const __half* p, uint32_t lbo) { return make_b_desc(smem_u32(p), lbo, 128); };
+    auto desc = [&](const __half* p, uint32_t lbo) { return make_desc(smem_u32(p), lbo, 128); };
     const uint64_t dLhi = desc(Lhi, NT_LBO64), dLlo = desc(Llo, NT_LBO64);
     const uint64_t dN2hi = desc(N2hi, NT_LBO64), dN2lo = desc(N2lo, NT_LBO64);
     const uint64_t dNXhi = desc(NXhi, NT_LBO192), dNXlo = desc(NXlo, NT_LBO192);
@@ -301,8 +247,8 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
 
         // ---- h -> A (fp16 hi/lo);  D = h·Lᵀ -------------------------------------------------------------------
         uint32_t ahi[16], alo[16];
-        float sha = 1.0f, shb = 1.0f;
-        encode_rows([&](int j, f32x2& xa, f32x2& xb, bool) { rows_of(a.h, j, xa, xb); }, ahi, alo, sha, shb);
+        tc16::RowScales sh;
+        tc16::encode_rows<true>([&](int j, f32x2& xa, f32x2& xb, auto) { rows_of(a.h, j, xa, xb); }, ahi, alo, sh);
         float d[32];
         tc16::mma_f16x3_rA<NT_LBO64>(d, ahi, alo, dLhi, dLlo);
         float inv_deg_a = 0.f, inv_deg_b = 0.f;
@@ -313,7 +259,7 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
         // ---- φ_v(h) (FastEGNN.py:183: the OLD h) per row --------------------------------------------------------
         float phia = 0.f, phib = 0.f;
         {
-            const float iha = 1.0f / sha, ihb = 1.0f / shb;
+            const float iha = 1.0f / sh.a, ihb = 1.0f / sh.b;
 #pragma unroll
             for (int j = 0; j < 8; ++j)
 #pragma unroll
@@ -323,8 +269,8 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
                     phib = fmaf(silu(fmaf(d[4 * j + 2 + e], ihb, lbs[col])), lw3s[col], phib);
                 }
             const float lb3 = __ldg(a.lb3);
-            phia = lb3 + quad_sum(phia);
-            phib = lb3 + quad_sum(phib);
+            phia = lb3 + tc16::quad_sum(phia);
+            phib = lb3 + tc16::quad_sum(phib);
         }
 
         // ---- x' = x + agg_x/deg + trans_v + φ_v·v, entry q of the thread's rows (q = 3: x' has 0, Σ(x',1) counts 1) ------
@@ -366,31 +312,31 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
         // kernel's wgmma (C7518).
         tc16::mma_f16x3_rA<NT_LBO64>(d, ahi, alo, desc(N1hi, NT_LBO64), desc(N1lo, NT_LBO64));   // A still holds h
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
-        float s2a = sha, s2b = shb;                   // the scales the D rows currently carry
+        float s2a = sh.a, s2b = sh.b;                 // the scales the D rows currently carry
         auto l1_chunk = [&](const float* src, float rsa, float rsb, int c, bool zero_src) {
-            float sna = s2a, snb = s2b;
-            encode_rows(
-                [&](int j, f32x2& xa, f32x2& xb, bool) {
+            tc16::RowScales sn{s2a, s2b};
+            tc16::encode_rows<true>(
+                [&](int j, f32x2& xa, f32x2& xb, auto) {
                     rows_of(src, j, xa, xb);
                     xa = mul2(xa, bc2(rsa));
                     xb = mul2(xb, bc2(rsb));
                 },
-                ahi, alo, sna, snb);
+                ahi, alo, sn);
             if (zero_src)                             // after the last read of the rows
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     if (r.va) st_pair(const_cast<float*>(src) + r.na * H + 8 * j + 2 * q, 0ull);
                     if (r.vb) st_pair(const_cast<float*>(src) + r.nb * H + 8 * j + 2 * q, 0ull);
                 }
-            if (__any_sync(FULL, sna != s2a || snb != s2b)) {   // cold: bring the partial sums in D to the new row scales
-                const float fa = sna / s2a, fb = snb / s2b;
+            if (__any_sync(FULL, sn.a != s2a || sn.b != s2b)) {   // cold: bring the partial sums in D to the new row scales
+                const float fa = sn.a / s2a, fb = sn.b / s2b;
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     d[4 * j + 0] *= fa; d[4 * j + 1] *= fa;
                     d[4 * j + 2] *= fb; d[4 * j + 3] *= fb;
                 }
-                s2a = sna;
-                s2b = snb;
+                s2a = sn.a;
+                s2b = sn.b;
             }
             tc16::mma_f16x3_rA<NT_LBO64, true>(d, ahi, alo, desc(N1hi + c * NT_W, NT_LBO64), desc(N1lo + c * NT_W, NT_LBO64));
             tc16::mma_f16x3_rA_wait(d, ahi, alo);
@@ -405,11 +351,11 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
             attra[k] = (k < Na && r.va) ? __ldg(a.attr + r.na * Na + k) : 0.f;
             attrb[k] = (k < Na && r.vb) ? __ldg(a.attr + r.nb * Na + k) : 0.f;
         }
-        float ta = 1.0f, tb = 1.0f;
+        tc16::RowScales st;
         {
             const float i2a = 1.0f / s2a, i2b = 1.0f / s2b;
-            encode_rows(
-                [&](int j, f32x2& xa, f32x2& xb, bool) {
+            tc16::encode_rows<true>(
+                [&](int j, f32x2& xa, f32x2& xb, auto) {
                     float za[2], zb[2];
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -426,13 +372,13 @@ __global__ void __launch_bounds__(NT_THREADS, 1) node_layer_tc_kernel(const Node
                     xa = pk2(silu(za[0]), silu(za[1]));
                     xb = pk2(silu(zb[0]), silu(zb[1]));
                 },
-                ahi, alo, ta, tb);
+                ahi, alo, st);
         }
         tc16::mma_f16x3_rA<NT_LBO64>(d, ahi, alo, dN2hi, dN2lo);
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
         // ---- h' = h + D/s + b2 -> HBM and -> A;  P, Q, Hn = h'·[W1a';W1b';W1vh']ᵀ -----------------------------------
-        const float ita = ta == 1.0f ? 1.0f : 1.0f / ta, itb = tb == 1.0f ? 1.0f : 1.0f / tb;
+        const float ita = st.a == 1.0f ? 1.0f : 1.0f / st.a, itb = st.b == 1.0f ? 1.0f : 1.0f / st.b;
         store_h_project(
             [&](int j, f32x2& xa, f32x2& xb) {
                 const int col = 8 * j + 2 * q;
@@ -491,7 +437,7 @@ __global__ void __launch_bounds__(NT_THREADS, 1) embed_tc_kernel(const EmbedTcAr
     fence_proxy_async_smem();
     __syncthreads();
 
-    const uint64_t dNXhi = make_b_desc(smem_u32(NXhi), NT_LBO192, 128), dNXlo = make_b_desc(smem_u32(NXlo), NT_LBO192, 128);
+    const uint64_t dNXhi = make_desc(smem_u32(NXhi), NT_LBO192, 128), dNXlo = make_desc(smem_u32(NXlo), NT_LBO192, 128);
     XSum xs{a.vsum, a.K, accx_all + 4 * warp, accx_all + 16 * wg, 1u + (uint32_t)wg, t, lane, -1};
     const int ra = 16 * w + (lane >> 2), rb = ra + 8;
     // precondition of every per-graph reduction downstream: ids sorted and inside [0,B) (PyG batches are; the reference

@@ -6,7 +6,9 @@
 // in the canonical no-swizzle K-major layout for 16-bit types: core matrix = 8 rows x 8 halfs (128 B),
 // element (n,k) at (k/8)*LBO + (n/8)*128 B + (n%8)*16 B + (k%8)*2 B with LBO = (N/8)*128 B.
 // fp16 range: a row whose |max| exceeds 3e4 is re-encoded with a power-of-two scale s (cold path) and the
-// caller multiplies the accumulator row by 1/s — results stay range-safe like fp32.
+// caller multiplies the accumulator row by 1/s — results stay range-safe like fp32.  encode_rows is that rescue for the
+// forward kernels' register fragments, together with the batched SiLU's stage-level guard; phi_head_t is their
+// t-domain φ head.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -132,17 +134,139 @@ __device__ __forceinline__ void mma_f16x3_rA_wait(float (&d)[32], uint32_t (&a_h
 __device__ __forceinline__ bool row_overflow(__half2 mx) {
     return fmaxf(__low2float(mx), __high2float(mx)) > RANGE;
 }
-// power-of-two scale that brings |rowmax| below 2^15, and its inverse
-__device__ __forceinline__ void range_scale(float rowmax, float& s, float& inv_s) {
+// power-of-two scale that brings |rowmax| below 2^15 (1 for a smaller rowmax)
+__device__ __forceinline__ float range_scale(float rowmax) {
     const uint32_t eb = (__float_as_uint(rowmax) >> 23) & 0xffu;
     const uint32_t sb = eb > 141u ? 268u - eb : 127u;
-    s = __uint_as_float((sb < 1u ? 1u : sb) << 23);
-    inv_s = 1.0f / s;
+    return __uint_as_float((sb < 1u ? 1u : sb) << 23);
+}
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(FULL, v, 1));
+    return fmaxf(v, __shfl_xor_sync(FULL, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(FULL, v, 1);
+    return v + __shfl_xor_sync(FULL, v, 2);
+}
+
+// ---- A fragments of the register-operand GEMMs: the fp16 range rescue --------------------------------------------
+// The power-of-two scales of the calling thread's rows a and b (1: not scaled) and their inverses.
+struct RowScales {
+    float a = 1.0f, b = 1.0f, inv_a = 1.0f, inv_b = 1.0f;
+};
+// The passes of encode_rows, given to its producer as std::integral_constant<int, pass>.
+constexpr int FAST_PASS = 0, MAX_PASS = 1, ENCODE_PASS = 2;
+template <int P>
+using Pass = std::integral_constant<int, P>;
+struct NoGuard {
+    __device__ __forceinline__ bool operator()() const { return false; }
+};
+
+// Encode the thread's rows a and b, produced as column pairs by f(j, xa, xb, pass) (columns 8j + 2q, +1), into the fp16
+// hi/lo A fragments (register 2j + r holds pair j of row a / b for r = 0 / 1).  The fast pass splits the values as they
+// are and tests |hi| > RANGE.  When a row of the warp fails it, or guard() (evaluated once, after the fast pass) is true,
+// the warp takes the cold path: a pass that takes max |v| per row, then an encode pass with the row scaled by the
+// power-of-two s = range_scale(max); s.a, s.b become those scales (only smaller than 1 where a row would leave the fp16
+// range) and s.inv_a, s.inv_b their inverses.  f returns the same values on every pass, except that the fast pass may
+// return values the guard rejects (the batched SiLU, silu4p / silu4t); where it stores what it produces is its own
+// business (each pass is told apart).  Masking of invalid rows is the producer's too: a row it zeroes is 0 in the
+// fragments and leaves the row maximum at 0.
+//   SCALES_IN: the rows may already carry scales s.a, s.b != 1 (accumulation over several encodes into one D); then the
+//              warp goes straight to the cold path and a row keeps the smaller of its incoming and its own scale.  Without
+//              it s must come in as 1 and the call votes once less.
+//   ROLLED_MAX: the row-max pass is not unrolled (only for producers that read memory, not accumulator registers).
+// One range test for every producer, with the same decisions and scales as a test on the side that can overflow:
+//   - SiLU outputs are ≥ −0.279 and t-domain outputs (SILU_T_IN·SiLU) ≤ 0.41, so |hi| > RANGE and max |v| differ from
+//     the one-sided max hi / −min hi only where both are below 2^15;
+//   - __hmax2 ignores NaN with or without __habs2, as fmaxf does in the row maximum;
+//   - range_scale changes the scale only for a row maximum ≥ 2^15.
+template <bool SCALES_IN, bool ROLLED_MAX = false, class F, class Guard = NoGuard>
+__device__ __forceinline__ void encode_rows(F&& f, uint32_t (&hi)[16], uint32_t (&lo)[16], RowScales& s,
+                                            Guard&& guard = Guard{}) {
+    bool cold = SCALES_IN && __any_sync(FULL, s.a != 1.0f || s.b != 1.0f);
+    if (!cold) {
+        __half2 mx = __floats2half2_rn(0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            f32x2 xa, xb;
+            f(j, xa, xb, Pass<FAST_PASS>{});
+            split_pair(xa, hi[2 * j], lo[2 * j]);
+            split_pair(xb, hi[2 * j + 1], lo[2 * j + 1]);
+            mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[2 * j])));
+            mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[2 * j + 1])));
+        }
+        cold = __any_sync(FULL, row_overflow(mx) || guard());
+    }
+    if (!cold) return;
+    // cold, per warp: some row of the warp carries a scale already or leaves the fp16 range, or the guard fired
+    float fa = 0.f, fb = 0.f;
+    auto row_max = [&](int j) {
+        f32x2 xa, xb;
+        float v0, v1;
+        f(j, xa, xb, Pass<MAX_PASS>{});
+        upk2(xa, v0, v1);
+        fa = fmaxf(fa, fmaxf(fabsf(v0), fabsf(v1)));
+        upk2(xb, v0, v1);
+        fb = fmaxf(fb, fmaxf(fabsf(v0), fabsf(v1)));
+    };
+    if constexpr (ROLLED_MAX) {
+#pragma unroll 1
+        for (int j = 0; j < 8; ++j) row_max(j);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) row_max(j);
+    }
+    // row a's scale and inverse before row b's: with both divisions after both scales, ptxas spills in the edge kernel's
+    // FLAG_LAST instantiations
+    float ca = range_scale(quad_max(fa)), ia = 1.0f / ca;
+    float cb = range_scale(quad_max(fb)), ib = 1.0f / cb;
+    if constexpr (SCALES_IN) {
+        ca = fminf(ca, s.a);
+        cb = fminf(cb, s.b);
+        ia = 1.0f / ca;
+        ib = 1.0f / cb;
+    }
+    s = {ca, cb, ia, ib};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        f32x2 xa, xb;
+        f(j, xa, xb, Pass<ENCODE_PASS>{});
+        split_pair(mul2(xa, bc2(s.a)), hi[2 * j], lo[2 * j]);
+        split_pair(mul2(xb, bc2(s.b)), hi[2 * j + 1], lo[2 * j + 1]);
+    }
+}
+
+// The φ head of the t-domain kernels (common.cuh silu4t): φ = Σ_k w[k]·SiLU_t(D[row, k]·inv + b[k]) for the thread's rows
+// a and b, summed over the quad, with b = SILU_T_IN·bias and w = SILU_T_OUT·w3 in shared memory.  The batched SiLU's
+// guard redoes the warp with the per-element form; no range rescue (no fp16 operand follows).  Each pass forms the
+// pre-activations from D again.
+__device__ __forceinline__ void phi_head_t(const float (&d)[32], float inv_a, float inv_b, const float* b, const float* w,
+                                           int q, float& phia, float& phib) {
+    float qmax = 0.f;
+    f32x2 pha, phb;
+    auto pass = [&](auto safe) {
+        pha = phb = bc2(0.f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const f32x2 bb = *reinterpret_cast<const f32x2*>(b + 8 * j + 2 * q);
+            const f32x2 ww = *reinterpret_cast<const f32x2*>(w + 8 * j + 2 * q);
+            f32x2 sa = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv_a), bb);
+            f32x2 sb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv_b), bb);
+            silu4t<decltype(safe)::value>(sa, sb, qmax);
+            pha = fma2(sa, ww, pha);
+            phb = fma2(sb, ww, phb);
+        }
+    };
+    pass(std::false_type{});
+    if (__any_sync(FULL, silu_q_overflow(qmax))) pass(std::true_type{});
+    float p0, p1;
+    upk2(pha, p0, p1);
+    phia = quad_sum(p0 + p1);
+    upk2(phb, p0, p1);
+    phib = quad_sum(p0 + p1);
 }
 
 // ---- register-pair flavour (fp32 pairs, common.cuh) ------------------------------------------------------------
-constexpr std::false_type kFast{};   // silu4p flavour tags
-constexpr std::true_type kSafe{};
 template <bool SCALED>
 __device__ __forceinline__ void split16p(const f32x2 (&v)[8], float s, uint32_t (&hi)[8], uint32_t (&lo)[8],
                                          __half2& mx) {

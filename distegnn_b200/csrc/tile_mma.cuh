@@ -45,14 +45,10 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo, 
     return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
            ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
 }
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    return make_desc(smem_addr, lbo, sbo);
-}
 
-// make generic-proxy smem writes (st.shared) visible to the async proxy (wgmma operand reads / bulk copies)
+// make generic-proxy smem writes (st.shared) visible to the async proxy (wgmma operand reads / bulk copies); for
+// tile-memory stores, once the group barrier that follows has been passed
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// tile-memory stores of this thread -> visible to the tensor cores once the group barrier that follows has been passed
-__device__ __forceinline__ void tm_st_fence() { fence_proxy_async_smem(); }
 
 // ---- tile memory <-> registers, the own row, 4 / 8 / 16 consecutive columns (column offset a multiple of 4) --------------
 __device__ __forceinline__ void tm_st4(uint32_t taddr, const uint32_t (&r)[4]) {
@@ -70,10 +66,6 @@ __device__ __forceinline__ void tm_st8(uint32_t taddr, const uint32_t (&r)[8]) {
 __device__ __forceinline__ void tm_st16(uint32_t taddr, const uint32_t (&r)[16]) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) tm_st4(taddr + 4 * i, *reinterpret_cast<const uint32_t(*)[4]>(&r[4 * i]));
-}
-__device__ __forceinline__ void tm_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    tm_ld4(taddr, &r[0]);
-    tm_ld4(taddr + 4, &r[4]);
 }
 __device__ __forceinline__ void tm_ld16(uint32_t taddr, uint32_t (&r)[16]) {
 #pragma unroll

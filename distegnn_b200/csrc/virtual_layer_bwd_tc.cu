@@ -168,13 +168,13 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
     // publish the A operand at tile-memory column `acol` (col0: over D, col0 + 64: A2), wait for the weight slot, and run the
     // three split products over the whole tile (the group's warpgroup): D (+)= A·Wᵀ
     auto issue = [&](uint32_t acol, bool accumulate) {
-        tm_st_fence();
+        fence_proxy_async_smem();
         named_bar(bar_id, VT_GROUP);
         const int slot = (int)(q_use & 1);
         mbar_wait(wbar + slot, (uint32_t)((q_use >> 1) & 1));
         const __half* whi = myslots + slot * VT_IMG;
-        tc16::mma_f16x3<VT_LBO>(col0, acol, acol + 32u, make_b_desc(smem_u32(whi), VT_LBO, 128),
-                                make_b_desc(smem_u32(whi + 64 * 64), VT_LBO, 128), 1, accumulate, 0, 2);
+        tc16::mma_f16x3<VT_LBO>(col0, acol, acol + 32u, make_desc(smem_u32(whi), VT_LBO, 128),
+                                make_desc(smem_u32(whi + 64 * 64), VT_LBO, 128), 1, accumulate, 0, 2);
         ++q_use;
     };
     auto mma_done = [&]() {                                      // D visible; the slot it read is refilled two matrices ahead

@@ -10,7 +10,8 @@
 // it holds (tile_mma.cuh); thread (g = lane/4, q = lane%4) owns rows g and g+8 of the warp, columns 8j + 2q + {0,1}.
 // The A operands and the accumulators stay in registers; the weights, the G rows of the warpgroup's current graph and the
 // fp32 mv rows (for the pools) are in shared memory.  Per tile (numerics as in the edge kernel: fp16 2-term split,
-// per-row power-of-two range rescue, one reciprocal per four SiLUs with a stage-level guard, cold paths per warp):
+// per-row power-of-two range rescue, one reciprocal per four SiLUs with a stage-level guard, cold paths per warp; the
+// rescue and the guard are tc16.cuh encode_rows, both φ heads phi_head_t):
 //   stage 1  a1 = SiLU(Hn[node] + G[graph,c] + w_r·‖ΔX‖) -> fp16 hi/lo A fragments                 MMA 1: D = a1·W2vᵀ
 //   stage 2  mv = SiLU(D + b2v) -> fp32 staging rows + hi/lo A fragments (kept for both heads)        MMA 2: D = mv·Wxvᵀ
 //            while MMA 2 runs: agg_v[node] = mean_c mv, Σ_i mv per graph (lane <-> column pair)
@@ -66,8 +67,6 @@ __host__ __device__ constexpr int vw_smem_floats(int C) {
            + VW_WARPS * 4 * C;
 }
 __host__ __device__ constexpr int vw_smem_bytes(int C) { return vw_smem_floats(C) * 4; }
-using tc16::kFast;
-using tc16::kSafe;
 
 // DET (deterministic mode, det.cuh): a warpgroup takes whole chunks of 2^chunk_shift consecutive tiles, in tile order, and
 // the per-graph sums are walked node by node in row order by the thread that owns the element (accumulators in the
@@ -127,7 +126,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
 
     // descriptor of weight matrix k (W2v hi, lo, Wxv hi, lo, WX hi, lo): the matrices are 8 KB apart, and the start-address
     // field (bits 0..13, address >> 4) of the first one has room for all six
-    const uint64_t bW0 = make_b_desc(smem_u32(W2hi), VW_LBO, 128);
+    const uint64_t bW0 = make_desc(smem_u32(W2hi), VW_LBO, 128);
     auto bW = [&](int k) { return bW0 + (uint64_t)(k * (VW_W * 2 / 16)); };
     float* tile_s = stage_all + wg * VW_TILE * VW_ROW;            // the group's 64 mv rows (warp w: rows 16w ..)
     float* dXs = dX_all + wg * VW_TILE * 4;
@@ -259,52 +258,18 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         };
         // register i = 2j + r of a fragment array <-> row g + 8r, columns 8j + 2q + {0,1} (= accumulator pair d[2i], d[2i+1])
         uint32_t ahi[16], alo[16];
-        float inv1a = 1.0f, inv1b = 1.0f;  // 1 / the rows' range scales
-        {
-            __half2 mx = __floats2half2_rn(0.f, 0.f);
-            float qmax = 0.f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                f32x2 xa = pre(j, pa, ga, vra), xb = pre(j, pb, gb, vrb);
-                silu4p<false>(xa, xb, qmax);
+        float qmax = 0.f;
+        auto silu_guard = [&] { return silu_q_overflow(qmax); };
+        tc16::RowScales s1;
+        tc16::encode_rows<false, true>(
+            [&](int j, f32x2& xa, f32x2& xb, auto pass) {
+                xa = pre(j, pa, ga, vra);
+                xb = pre(j, pb, gb, vrb);
+                silu4p<decltype(pass)::value != tc16::FAST_PASS>(xa, xb, qmax);
                 if (!va) xa = 0ull;
                 if (!vb) xb = 0ull;
-                tc16::split_pair(xa, ahi[2 * j], alo[2 * j]);
-                tc16::split_pair(xb, ahi[2 * j + 1], alo[2 * j + 1]);
-                // SiLU outputs are bounded below (−0.28): only the positive side can leave the fp16 range
-                mx = __hmax2(mx, __hmax2(*reinterpret_cast<const __half2*>(&ahi[2 * j]),
-                                         *reinterpret_cast<const __half2*>(&ahi[2 * j + 1])));
-            }
-            if (__any_sync(FULL, tc16::row_overflow(mx) || silu_q_overflow(qmax))) {
-                // cold: some row leaves the fp16 range, or the SiLU batch guard fired — per-element SiLU, row scales
-                float fa = 0.f, fb = 0.f, sa, sb;
-#pragma unroll 1
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 xa = pre(j, pa, ga, vra), xb = pre(j, pb, gb, vrb);
-                    silu4p<true>(xa, xb, qmax);
-                    float v0, v1;
-                    upk2(xa, v0, v1);
-                    if (va) fa = fmaxf(fa, fmaxf(v0, v1));
-                    upk2(xb, v0, v1);
-                    if (vb) fb = fmaxf(fb, fmaxf(v0, v1));
-                }
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 1));
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 2));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 1));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 2));
-                tc16::range_scale(fa, sa, inv1a);
-                tc16::range_scale(fb, sb, inv1b);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 xa = pre(j, pa, ga, vra), xb = pre(j, pb, gb, vrb);
-                    silu4p<true>(xa, xb, qmax);
-                    if (!va) xa = 0ull;
-                    if (!vb) xb = 0ull;
-                    tc16::split_pair(mul2(xa, bc2(sa)), ahi[2 * j], alo[2 * j]);
-                    tc16::split_pair(mul2(xb, bc2(sb)), ahi[2 * j + 1], alo[2 * j + 1]);
-                }
-            }
-        }
+            },
+            ahi, alo, s1, silu_guard);
 
         // ---- MMA 1 ----------------------------------------------------------------------------------------------
         float d[32];
@@ -312,62 +277,23 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
         // ---- stage 2: mv = SiLU(D/s + b2v) -> fp32 staging rows (pools) and fp16 hi/lo A fragments ----------------------
-        float inv2a = 1.0f, inv2b = 1.0f, s2a = 1.0f, s2b = 1.0f;     // 1 / the rows' range scales, the scales
-        auto m_pair = [&](int j, f32x2& ma, f32x2& mb) {
-            const f32x2 bb = *reinterpret_cast<const f32x2*>(b2s + 8 * j + 2 * q);
-            ma = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv1a), bb);
-            mb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv1b), bb);
-        };
-        // (ma, mb) = SILU_T_IN·mv -> the staging rows: the pools undo the factor, and MMA 3 re-splits its A operand from them
-        auto store_m = [&](int j, f32x2 ma, f32x2 mb) {
-            *reinterpret_cast<f32x2*>(tile_s + ra * VW_ROW + 8 * j + 2 * q) = ma;
-            *reinterpret_cast<f32x2*>(tile_s + rb * VW_ROW + 8 * j + 2 * q) = mb;
-        };
-        {
-            __half2 mx = __floats2half2_rn(0.f, 0.f);
-            float qmax = 0.f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                f32x2 ma, mb;
-                m_pair(j, ma, mb);
-                silu4t<false>(ma, mb, qmax);
-                store_m(j, ma, mb);
-                tc16::split_pair(ma, ahi[2 * j], alo[2 * j]);
-                tc16::split_pair(mb, ahi[2 * j + 1], alo[2 * j + 1]);
-                // t-domain values: ≤ 0.41, unbounded below — track the minimum
-                mx = __hmin2(mx, __hmin2(*reinterpret_cast<const __half2*>(&ahi[2 * j]),
-                                         *reinterpret_cast<const __half2*>(&ahi[2 * j + 1])));
-            }
-            if (__any_sync(FULL, fminf(__low2float(mx), __high2float(mx)) < -tc16::RANGE || silu_q_overflow(qmax))) {
-                float fa = 0.f, fb = 0.f;      // cold (unrolled: d stays in registers)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 ma, mb;
-                    m_pair(j, ma, mb);
-                    silu4t<true>(ma, mb, qmax);
-                    store_m(j, ma, mb);    // also rewrites the mv rows of the batch-guard case
-                    float v0, v1;
-                    upk2(ma, v0, v1);
-                    fa = fmaxf(fa, -fminf(v0, v1));
-                    upk2(mb, v0, v1);
-                    fb = fmaxf(fb, -fminf(v0, v1));
+        // (ma, mb) = SILU_T_IN·mv -> the staging rows: the pools undo the factor, and MMA 3 re-splits its A operand from
+        // them.  The rows are stored by the pass whose values are final: the fast pass, and again by the row-max pass when
+        // the warp takes the cold path (batch guard included).
+        qmax = 0.f;
+        tc16::RowScales s2;
+        tc16::encode_rows<false>(
+            [&](int j, f32x2& ma, f32x2& mb, auto pass) {
+                const f32x2 bb = *reinterpret_cast<const f32x2*>(b2s + 8 * j + 2 * q);
+                ma = fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(s1.inv_a), bb);
+                mb = fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(s1.inv_b), bb);
+                silu4t<decltype(pass)::value != tc16::FAST_PASS>(ma, mb, qmax);
+                if (decltype(pass)::value != tc16::ENCODE_PASS) {
+                    *reinterpret_cast<f32x2*>(tile_s + ra * VW_ROW + 8 * j + 2 * q) = ma;
+                    *reinterpret_cast<f32x2*>(tile_s + rb * VW_ROW + 8 * j + 2 * q) = mb;
                 }
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 1));
-                fa = fmaxf(fa, __shfl_xor_sync(FULL, fa, 2));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 1));
-                fb = fmaxf(fb, __shfl_xor_sync(FULL, fb, 2));
-                tc16::range_scale(fa, s2a, inv2a);
-                tc16::range_scale(fb, s2b, inv2b);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f32x2 ma, mb;
-                    m_pair(j, ma, mb);
-                    silu4t<true>(ma, mb, qmax);
-                    tc16::split_pair(mul2(ma, bc2(s2a)), ahi[2 * j], alo[2 * j]);
-                    tc16::split_pair(mul2(mb, bc2(s2b)), ahi[2 * j + 1], alo[2 * j + 1]);
-                }
-            }
-        }
+            },
+            ahi, alo, s2, silu_guard);
 
         // the nodes whose per-node outputs (agg_v, trans_v) this warp writes: its own when nodes never straddle warps,
         // else every fourth node of the tile (the rows of the other warps are read behind a group barrier)
@@ -435,42 +361,9 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
         // ---- stage 3: φ = w3·SiLU(D/s + b) per row (quad shuffles) ----------------------------------------------------
-        auto head = [&](const float* bs, const float* ws, float& phia, float& phib) {
-            // the pre-activations t = D/s + b replace D in place: both passes read them, and D is not needed again
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const f32x2 bb = *reinterpret_cast<const f32x2*>(bs + 8 * j + 2 * q);
-                upk2(fma2(pk2(d[4 * j + 0], d[4 * j + 1]), bc2(inv2a), bb), d[4 * j + 0], d[4 * j + 1]);
-                upk2(fma2(pk2(d[4 * j + 2], d[4 * j + 3]), bc2(inv2b), bb), d[4 * j + 2], d[4 * j + 3]);
-            }
-            float qmax = 0.f;
-            f32x2 pha, phb;
-            auto pass = [&](auto safe) {
-                pha = phb = bc2(0.f);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const f32x2 ww = *reinterpret_cast<const f32x2*>(ws + 8 * j + 2 * q);
-                    f32x2 sa = pk2(d[4 * j + 0], d[4 * j + 1]), sb = pk2(d[4 * j + 2], d[4 * j + 3]);
-                    silu4t<decltype(safe)::value>(sa, sb, qmax);
-                    pha = fma2(sa, ww, pha);
-                    phb = fma2(sb, ww, phb);
-                }
-            };
-            pass(kFast);
-            if (__any_sync(FULL, silu_q_overflow(qmax))) pass(kSafe);      // cold (no scale)
-            float p0, p1;
-            upk2(pha, p0, p1);
-            phia = p0 + p1;
-            upk2(phb, p0, p1);
-            phib = p0 + p1;
-            phia += __shfl_xor_sync(FULL, phia, 1);
-            phia += __shfl_xor_sync(FULL, phia, 2);
-            phib += __shfl_xor_sync(FULL, phib, 1);
-            phib += __shfl_xor_sync(FULL, phib, 2);
-        };
         {
             float phia, phib;
-            head(bxvs, w3xvs, phia, phib);
+            tc16::phi_head_t(d, s2.inv_a, s2.inv_b, bxvs, w3xvs, q, phia, phib);
             if (q == 0) {
                 phis[ra] = phia;
                 phis[rb] = phib;
@@ -484,8 +377,8 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         for (int j = 0; j < 8; ++j) {
             const f32x2 ma = *reinterpret_cast<const f32x2*>(tile_s + ra * VW_ROW + 8 * j + 2 * q);
             const f32x2 mb = *reinterpret_cast<const f32x2*>(tile_s + rb * VW_ROW + 8 * j + 2 * q);
-            tc16::split_pair(mul2(ma, bc2(s2a)), ahi[2 * j], alo[2 * j]);
-            tc16::split_pair(mul2(mb, bc2(s2b)), ahi[2 * j + 1], alo[2 * j + 1]);
+            tc16::split_pair(mul2(ma, bc2(s2.a)), ahi[2 * j], alo[2 * j]);
+            tc16::split_pair(mul2(mb, bc2(s2.b)), ahi[2 * j + 1], alo[2 * j + 1]);
         }
         tc16::mma_f16x3_rA<VW_LBO>(d, ahi, alo, bW(4), bW(5));
         if (warp_local) __syncwarp();
@@ -501,7 +394,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         // ---- stage 3b: φ_X; Σ_i ΔX_ic·φ_X,ic over the warp's own rows, per graph [3][C] -------------------------------
         {
             float phia, phib;
-            head(bxs, w3xs, phia, phib);
+            tc16::phi_head_t(d, s2.inv_a, s2.inv_b, bxs, w3xs, q, phia, phib);
             if (q == 0) {
                 phis[VW_TILE + ra] = phia;
                 phis[VW_TILE + rb] = phib;
