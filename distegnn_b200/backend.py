@@ -311,6 +311,31 @@ class CudaBackend:
               "rollout_chamfer_workspace_bytes")
         return torch.empty(int(nbytes.value), dtype=torch.uint8, device=device)
 
+    def chamfer_distance(self, pred: Tensor, target: Tensor, batch: Optional[Tensor], out: Tensor, nearest: Tensor,
+                         ws: Tensor) -> None:
+        """out float64 [B,2] = per-graph Chamfer sums of pred against target, nearest int32 [2N] the minimiser of every
+        minimum (see distegnn_chamfer_distance; `ws` from rollout_chamfer_workspace)."""
+        N = int(pred.shape[0])
+        check(self.lib.distegnn_chamfer_distance(N, int(out.shape[0]), ptr(pred), ptr(target), ptr(batch), ptr(out),
+                                                 ptr(nearest), ptr(ws), ws.numel(), self._s(pred)), "chamfer_distance")
+        self.launches += 7 if N else 0                         # ours; the cub scan comes on top
+
+    def chamfer_distance_bwd(self, pred: Tensor, target: Tensor, batch: Optional[Tensor], nearest: Tensor, g: Tensor,
+                             g_pred: Optional[Tensor], g_target: Optional[Tensor], ws: Tensor) -> None:
+        """g_pred / g_target [N,3] (either may be None: not written) = the gradient of chamfer_distance's sums given the
+        upstream g float64 [B,2] (see distegnn_chamfer_distance_bwd; `ws` from chamfer_distance_bwd_workspace)."""
+        N = int(pred.shape[0])
+        check(self.lib.distegnn_chamfer_distance_bwd(N, int(g.shape[0]), ptr(pred), ptr(target), ptr(batch),
+                                                     ptr(nearest), ptr(g), ptr(g_pred), ptr(g_target), ptr(ws),
+                                                     ws.numel(), self._s(pred)), "chamfer_distance_bwd")
+        self.launches += 2 if N and (g_pred is not None or g_target is not None) else 0   # ours; the cub sort on top
+
+    def chamfer_distance_bwd_workspace(self, n_nodes: int, device) -> Tensor:
+        nbytes = C.c_int64(0)
+        check(self.lib.distegnn_chamfer_distance_bwd_workspace_bytes(n_nodes, C.byref(nbytes)),
+              "chamfer_distance_bwd_workspace_bytes")
+        return torch.empty(int(nbytes.value), dtype=torch.uint8, device=device)
+
     def allreduce_packed(self, comm: "Comm", buf: Tensor) -> None:
         """In-place SUM of `buf` over the partitions through the communicator's peer-mapped segments."""
         check(self.lib.distegnn_allreduce_packed(comm.handle, ptr(buf), buf.numel(), self._s(buf)), "allreduce_packed")

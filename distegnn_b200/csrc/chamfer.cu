@@ -26,6 +26,12 @@
 // for R >= 1.  So the search stops once best <= (c·R·(1 − 2^-10))² (R = 0: best = 0), or once the rings cover the grid:
 // no point left can beat best.  An axis with one cell (extent 0, or past FLT_MAX) never separates two points.  This is
 // the radius build's cell margin (kRadiusCellMargin, DESIGN §10) read the other way round.
+//
+// The differentiable Chamfer distance (DESIGN §21) lives here too: distegnn_chamfer_distance runs the same launches for
+// one frame, with the search also writing the nearest id of every point (chamfer_search_kernel<true>), and
+// distegnn_chamfer_distance_bwd turns those ids into gradients in a fixed order.
+#include <climits>
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "cell_grid.cuh"
@@ -56,6 +62,7 @@ struct ChamferArgs {
     double* minima;            // [2N] per-node minima: P -> Q at [0, N), Q -> P at [N, 2N)
     double* slots;             // [chunks, 2]
     unsigned* ticket;
+    int32_t* nearest;          // [2N] nearest ids (chamfer_search_kernel<true> only): P -> Q at [0, N), Q -> P at [N, 2N)
 };
 
 __device__ __forceinline__ const float* chf_frame(const ChamferArgs& a) {   // targets[t]; row 0 outside [0, steps)
@@ -159,7 +166,29 @@ __device__ __forceinline__ double chf_ring_bound(float cell, int R) {
     return r * r;
 }
 
-__global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a) {
+// Nearest id (DESIGN §21): (best, id) after candidate (d, k) of the query whose matched node is m.  A smaller d wins; on a
+// tie the matched node keeps its place, otherwise the smaller id wins.  id != m implies best < d(m), so the result does
+// not depend on the order the candidates come in.
+__device__ __forceinline__ void chf_take(double& best, int& id, int m, double d, int k) {
+    const bool take = d < best || (d == best && id != m && k < id);
+    id = take ? k : id;
+    best = take ? d : best;
+}
+
+// (d, k) <- the lexicographically smaller of (d, k) and (d2, k2): the outlier scan's lane partials
+__device__ __forceinline__ void chf_min_pair(double& d, int& k, double d2, int k2) {
+    if (d2 < d || (d2 == d && k2 < k)) {
+        d = d2;
+        k = k2;
+    }
+}
+
+// NEAREST: also the nearest id of every point, under chf_take's rule, to a.nearest (−1 in a non-finite graph).  The ring
+// stop rule is strict (every unscanned point has d > bound >= best), so when the matched node is not a minimiser every
+// minimiser has been scanned, and the id is the smallest among them.  The minimum of one block per SM lets ptxas keep
+// NEAREST's extra state in registers (54, no spill) rather than aim for the occupancy of 40 registers.
+template <bool NEAREST>
+__global__ void __launch_bounds__(256, NEAREST ? 1 : 0) chamfer_search_kernel(const ChamferArgs a) {
     const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
     const bool live = s < 2 * a.N;                             // every lane reaches the warp's outlier scans below
@@ -171,6 +200,7 @@ __global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a
     const ChamferGrid g = a.grid[b];
     const int* start = a.cell_start + (1 - c) * a.T + g.base;
     double best = INFINITY;
+    int id = (int)i;                                           // NEAREST: the minimiser so far
     auto dist = [&](const float4& v) {
         return target_sq_dist([&](int k) { return xyz(q, k); }, [&](int k) { return xyz(v, k); });
     };
@@ -184,7 +214,14 @@ __global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a
         const int reach = max(max(max(ix, g.nx - 1 - ix), max(iy, g.ny - 1 - iy)), max(iz, g.nz - 1 - iz));
         auto scan = [&](int k0, int k1) {                      // the points of cells k0 .. k1 − 1
             const int e = __ldg(start + k1);
-            for (int p = __ldg(start + k0); p < e; ++p) best = fmin(best, dist(a.sorted[p]));
+            for (int p = __ldg(start + k0); p < e; ++p) {
+                if constexpr (NEAREST) {
+                    const float4 v = a.sorted[p];
+                    chf_take(best, id, (int)i, dist(v), __float_as_int(v.w));
+                } else {
+                    best = fmin(best, dist(a.sorted[p]));
+                }
+            }
         };
         for (int R = 0;; ++R) {
             // rings 0 .. R − 1 are scanned: no point left is nearer than their bound (none scanned: 0)
@@ -214,16 +251,33 @@ __global__ void __launch_bounds__(256) chamfer_search_kernel(const ChamferArgs a
         const int lo = __shfl_sync(FULL, __ldg(st), L);
         const int hi = __shfl_sync(FULL, __ldg(st + g.ncell), L);
         double m = INFINITY;
+        if constexpr (NEAREST) {                               // (d, id) pairs: the lexicographic min over the lanes
+            int mk = INT_MAX;
 #pragma unroll 4
-        for (int p = lo + lane; p < hi; p += 32) {
-            const float4 v = a.sorted[p];
-            m = fmin(m, target_sq_dist([&](int k) { return xyz(o, k); }, [&](int k) { return xyz(v, k); }));
-        }
+            for (int p = lo + lane; p < hi; p += 32) {
+                const float4 v = a.sorted[p];
+                chf_min_pair(m, mk, target_sq_dist([&](int k) { return xyz(o, k); }, [&](int k) { return xyz(v, k); }),
+                             __float_as_int(v.w));
+            }
 #pragma unroll
-        for (int off = 16; off > 0; off >>= 1) m = fmin(m, __shfl_xor_sync(FULL, m, off));
-        if (lane == L) best = fmin(best, m);
+            for (int off = 16; off > 0; off >>= 1)
+                chf_min_pair(m, mk, __shfl_xor_sync(FULL, m, off), __shfl_xor_sync(FULL, mk, off));
+            if (lane == L) chf_take(best, id, (int)i, m, mk);
+        } else {
+#pragma unroll 4
+            for (int p = lo + lane; p < hi; p += 32) {
+                const float4 v = a.sorted[p];
+                m = fmin(m, target_sq_dist([&](int k) { return xyz(o, k); }, [&](int k) { return xyz(v, k); }));
+            }
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) m = fmin(m, __shfl_xor_sync(FULL, m, off));
+            if (lane == L) best = fmin(best, m);
+        }
     }
     if (live) a.minima[c * a.N + i] = search ? best : __longlong_as_double(0x7ff8000000000000ll);
+    if constexpr (NEAREST) {
+        if (live) a.nearest[c * a.N + i] = search ? id : -1;
+    }
 }
 
 // distegnn_rollout_sq_err's reduction on the per-node minima, both directions at once.  The workspace is not
@@ -236,6 +290,73 @@ __global__ void __launch_bounds__(DET_RED) chamfer_sum_kernel(const ChamferArgs 
                            s[0] += __ldg(a.minima + k);
                            s[1] += __ldg(a.minima + a.N + k);
                        });
+}
+
+// ---- backward of the Chamfer distance (DESIGN §21) --------------------------------------------------------------------
+// Output row r (predictions at [0, N), records at [N, 2N)) is its own term, then the term of every row whose nearest node
+// it is, in ascending row.  Row s of the nearest table points at output row N + nearest[s] (s < N: a prediction's nearest
+// record) or nearest[s] (s >= N: a record's nearest prediction); a stable radix sort of the 2N (output row, s) pairs by
+// output row puts each row's list in ascending s.  An id outside [0, N) (a non-finite graph) gets key 2N, past every row.
+// Every output row is one plain store: no floating-point atomics, so the gradient is bitwise reproducible.
+struct ChamferBwdArgs {
+    int64_t N;
+    int B;
+    const float* pred;         // [N,3]
+    const float* target;       // [N,3]
+    const int64_t* batch;      // [N] sorted, or null (one graph)
+    const int32_t* nearest;    // [2N] from distegnn_chamfer_distance
+    const double* g;           // [B,2] upstream gradient
+    float* g_pred;             // [N,3] or null
+    float* g_target;           // [N,3] or null
+    const unsigned* keys;      // [2N] output rows, sorted
+    const int* rows;           // [2N] the rows s of the nearest table, in key order
+};
+
+__global__ void __launch_bounds__(256) chamfer_bwd_keys_kernel(int64_t N, const int32_t* nearest, unsigned* keys,
+                                                               int* rows) {
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= 2 * N) return;
+    const int n = __ldg(nearest + s);
+    keys[s] = (unsigned)(n >= 0 && n < N ? (s < N ? N + n : n) : 2 * N);
+    rows[s] = (int)s;
+}
+
+// acc[k] (+)= g2 · fl32(x_k − y_k): the difference in fp32, the product and the sum in fp64, each rounded to nearest
+template <bool FIRST>
+__device__ __forceinline__ void chf_grad_term(double (&acc)[3], double g2, const float (&x)[3], const float* y) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const double t = __dmul_rn(g2, (double)__fsub_rn(x[k], __ldg(y + k)));
+        acc[k] = FIRST ? t : __dadd_rn(acc[k], t);
+    }
+}
+
+__global__ void __launch_bounds__(256) chamfer_bwd_kernel(const ChamferBwdArgs a) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= 2 * a.N) return;
+    const int c = r >= a.N;                                    // 0: a prediction's row, 1: a record's
+    float* out = c ? a.g_target : a.g_pred;
+    if (!out) return;
+    const int64_t i = r - c * a.N;
+    const float* other = c ? a.pred : a.target;
+    const int n = __ldg(a.nearest + r);
+    float* o = out + i * 3;
+    if (n < 0 || n >= a.N) {                                   // a non-finite graph
+        o[0] = o[1] = o[2] = __int_as_float(0x7fc00000);
+        return;
+    }
+    const float* p = (c ? a.target : a.pred) + i * 3;
+    const float x[3] = {__ldg(p), __ldg(p + 1), __ldg(p + 2)};
+    const int b = graph_id(a.batch, i, a.B);
+    const double g_own = __dmul_rn(2.0, __ldg(a.g + 2 * b + c)), g_in = __dmul_rn(2.0, __ldg(a.g + 2 * b + 1 - c));
+    double acc[3];
+    chf_grad_term<true>(acc, g_own, x, other + (int64_t)n * 3);
+    for (int64_t k = lower_bound_dev(a.keys, 2 * a.N, r); k < 2 * a.N && __ldg(a.keys + k) == (unsigned)r; ++k) {
+        const int64_t s = __ldg(a.rows + k);                   // a record (s >= N) for c = 0, a prediction for c = 1
+        chf_grad_term<false>(acc, g_in, x, other + (s - (1 - c) * a.N) * 3);
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) o[k] = __double2float_rn(acc[k]);
 }
 
 struct ChamferLayout {
@@ -264,7 +385,73 @@ static int chamfer_layout(int64_t N, int B, ChamferLayout& L) {
     return DISTEGNN_OK;
 }
 
+struct ChamferBwdLayout {
+    size_t keys[2], rows[2], tmp, tmp_bytes, total;
+    int end_bit;               // keys lie in [0, 2N]: the sort looks at bits [0, end_bit)
+};
+
+static int chamfer_bwd_layout(int64_t N, ChamferBwdLayout& L) {
+    L.end_bit = 1;
+    while (((int64_t)1 << L.end_bit) <= 2 * N) ++L.end_bit;
+    cub::DoubleBuffer<unsigned> k(nullptr, nullptr);
+    cub::DoubleBuffer<int> v(nullptr, nullptr);
+    size_t sort = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, sort, k, v, (int)(2 * N), 0, L.end_bit) != cudaSuccess)
+        return DISTEGNN_ECUDA;
+    WorkspaceCursor ws;
+    for (int d = 0; d < 2; ++d) L.keys[d] = ws.take((size_t)N * 2 * 4);
+    for (int d = 0; d < 2; ++d) L.rows[d] = ws.take((size_t)N * 2 * 4);
+    L.tmp_bytes = sort;
+    L.tmp = ws.take(sort);
+    L.total = ws.end;
+    return DISTEGNN_OK;
+}
+
 constexpr int64_t CHF_MAX_ROWS = (int64_t)1 << 29;   // N + n_graphs: the table's 2(N + B) + 1 keys stay in int32
+
+// The launches of distegnn_rollout_chamfer and distegnn_chamfer_distance (a.nearest set: the search also writes the
+// nearest ids); the arguments are checked and a.N > 0.  A null a.counter reads the scanned table's first entry (see
+// distegnn_chamfer_distance).
+static int chamfer_run(const char* who, ChamferArgs a, void* workspace, int64_t workspace_bytes, cudaStream_t stream) {
+    ChamferLayout L;
+    if (int rc = chamfer_layout(a.N, a.B, L)) {
+        set_error("%s: cub temp-size query failed", who);
+        return rc;
+    }
+    if (workspace_bytes < (int64_t)L.total) {
+        set_error("%s: workspace %lld < %lld bytes", who, (long long)workspace_bytes, (long long)L.total);
+        return DISTEGNN_EWORKSPACE;
+    }
+    char* ws = (char*)workspace;
+    a.T = a.N + a.B;
+    a.bounds = (int*)(ws + L.bounds); a.flags = (int*)(ws + L.flags); a.grid = (ChamferGrid*)(ws + L.grid);
+    a.keyrank = (int2*)(ws + L.keyrank); a.cell_start = (int*)(ws + L.cell_start); a.sorted = (float4*)(ws + L.sorted);
+    a.minima = (double*)(ws + L.minima); a.slots = (double*)(ws + L.slots); a.ticket = (unsigned*)(ws + L.ticket);
+    if (!a.counter) a.counter = a.cell_start;
+    size_t tmp_bytes = L.tmp_bytes;
+    const int64_t init = 2 * a.T + 1 > (int64_t)a.B * 6 ? 2 * a.T + 1 : (int64_t)a.B * 6;
+    const unsigned nb2 = (unsigned)((2 * a.N + 255) / 256);
+    const int64_t warps = (a.N + CHF_WARP_ROWS - 1) / CHF_WARP_ROWS;
+    chamfer_init_kernel<<<(unsigned)((init + 255) / 256), 256, 0, stream>>>(a);
+    chamfer_bounds_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(a);
+    chamfer_grid_kernel<<<(unsigned)((a.B + 127) / 128), 128, 0, stream>>>(a);
+    chamfer_keys_kernel<<<nb2, 256, 0, stream>>>(a);
+    DEGNN_CHECK_LAUNCH();
+    const cudaError_t e = cub::DeviceScan::ExclusiveSum(ws + L.tmp, tmp_bytes, (const int32_t*)a.cell_start,
+                                                        a.cell_start, (int)(2 * a.T + 1), stream);
+    if (e != cudaSuccess) {
+        set_error("%s: cub scan failed: %s", who, cudaGetErrorString(e));
+        return DISTEGNN_ECUDA;
+    }
+    chamfer_scatter_kernel<<<nb2, 256, 0, stream>>>(a);
+    if (a.nearest)
+        chamfer_search_kernel<true><<<nb2, 256, 0, stream>>>(a);
+    else
+        chamfer_search_kernel<false><<<nb2, 256, 0, stream>>>(a);
+    chamfer_sum_kernel<<<(unsigned)err_chunks(a.N), DET_RED, 0, stream>>>(a);
+    DEGNN_CHECK_LAUNCH();
+    return DISTEGNN_OK;
+}
 
 }  // namespace degnn
 
@@ -288,7 +475,6 @@ int distegnn_rollout_chamfer(int64_t n_nodes, int n_graphs, int steps, const flo
                              const int64_t* data_batch, const int32_t* counter, double* chamfer, void* workspace,
                              int64_t workspace_bytes, void* stream_) {
     using namespace degnn;
-    cudaStream_t stream = (cudaStream_t)stream_;
     DEGNN_CHECK_ARG(n_nodes >= 0 && n_graphs > 0 && steps >= 1, "bad size");
     DEGNN_CHECK_ARG(n_nodes + n_graphs <= CHF_MAX_ROWS, "n_nodes + n_graphs above 2^29");
     DEGNN_CHECK_ARG(n_graphs == 1 || data_batch, "data_batch needed for more than one graph");
@@ -296,42 +482,93 @@ int distegnn_rollout_chamfer(int64_t n_nodes, int n_graphs, int steps, const flo
     if (n_nodes == 0) return DISTEGNN_OK;
     DEGNN_CHECK_ARG(pred && targets && workspace, "null pointer");
     DEGNN_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "workspace not 16-byte aligned");
-    ChamferLayout L;
-    if (int rc = chamfer_layout(n_nodes, n_graphs, L)) {
+    ChamferArgs a{};
+    a.N = n_nodes; a.B = n_graphs; a.steps = steps;
+    a.pred = pred; a.targets = targets; a.batch = n_graphs > 1 ? data_batch : nullptr; a.counter = counter;
+    a.chamfer = chamfer;
+    return chamfer_run(__func__, a, workspace, workspace_bytes, (cudaStream_t)stream_);
+}
+
+int distegnn_chamfer_distance(int64_t n_nodes, int n_graphs, const float* pred, const float* target,
+                              const int64_t* data_batch, double* out, int32_t* nearest, void* workspace,
+                              int64_t workspace_bytes, void* stream_) {
+    using namespace degnn;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    DEGNN_CHECK_ARG(n_nodes >= 0 && n_graphs > 0, "bad size");
+    DEGNN_CHECK_ARG(n_nodes + n_graphs <= CHF_MAX_ROWS, "n_nodes + n_graphs above 2^29");
+    DEGNN_CHECK_ARG(out, "null pointer");
+    if (n_nodes == 0) {                                        // every graph is empty: 0
+        const cudaError_t e = cudaMemsetAsync(out, 0, (size_t)n_graphs * 2 * sizeof(double), stream);
+        if (e != cudaSuccess) {
+            set_error("%s: %s", __func__, cudaGetErrorString(e));
+            return DISTEGNN_ECUDA;
+        }
+        return DISTEGNN_OK;
+    }
+    DEGNN_CHECK_ARG(n_graphs == 1 || data_batch, "data_batch needed for more than one graph");
+    DEGNN_CHECK_ARG(pred && target && nearest && workspace, "null pointer");
+    DEGNN_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "workspace not 16-byte aligned");
+    // One step of the rollout's launches with steps = 1 and the search's nearest ids.  Every kernel before the sums reads
+    // frame 0 whatever the counter holds (steps = 1); the sums read the scanned table's first entry, which is 0.  So no
+    // device counter is needed.
+    ChamferArgs a{};
+    a.N = n_nodes; a.B = n_graphs; a.steps = 1;
+    a.pred = pred; a.targets = target; a.batch = n_graphs > 1 ? data_batch : nullptr; a.counter = nullptr;
+    a.chamfer = out; a.nearest = nearest;
+    return chamfer_run(__func__, a, workspace, workspace_bytes, stream);
+}
+
+int distegnn_chamfer_distance_bwd_workspace_bytes(int64_t n_nodes, int64_t* bytes_host) {
+    using namespace degnn;
+    DEGNN_CHECK_ARG(bytes_host, "null output pointer");
+    DEGNN_CHECK_ARG(n_nodes >= 0 && n_nodes < CHF_MAX_ROWS, "n_nodes outside [0, 2^29)");
+    ChamferBwdLayout L;
+    if (int rc = chamfer_bwd_layout(n_nodes, L)) {
         set_error("cub temp-size query failed");
         return rc;
     }
+    *bytes_host = (int64_t)L.total;
+    return DISTEGNN_OK;
+}
+
+int distegnn_chamfer_distance_bwd(int64_t n_nodes, int n_graphs, const float* pred, const float* target,
+                                  const int64_t* data_batch, const int32_t* nearest, const double* g, float* g_pred,
+                                  float* g_target, void* workspace, int64_t workspace_bytes, void* stream_) {
+    using namespace degnn;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    DEGNN_CHECK_ARG(n_nodes >= 0 && n_graphs > 0, "bad size");
+    DEGNN_CHECK_ARG(n_nodes + n_graphs <= CHF_MAX_ROWS, "n_nodes + n_graphs above 2^29");
+    if (n_nodes == 0 || (!g_pred && !g_target)) return DISTEGNN_OK;
+    DEGNN_CHECK_ARG(n_graphs == 1 || data_batch, "data_batch needed for more than one graph");
+    DEGNN_CHECK_ARG(pred && target && nearest && g && workspace, "null pointer");
+    DEGNN_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "workspace not 16-byte aligned");
+    ChamferBwdLayout L;
+    if (int rc = chamfer_bwd_layout(n_nodes, L)) {
+        set_error("%s: cub temp-size query failed", __func__);
+        return rc;
+    }
     if (workspace_bytes < (int64_t)L.total) {
-        set_error("distegnn_rollout_chamfer: workspace %lld < %lld bytes", (long long)workspace_bytes,
-                  (long long)L.total);
+        set_error("%s: workspace %lld < %lld bytes", __func__, (long long)workspace_bytes, (long long)L.total);
         return DISTEGNN_EWORKSPACE;
     }
     char* ws = (char*)workspace;
-    ChamferArgs a;
-    a.N = n_nodes; a.B = n_graphs; a.steps = steps; a.T = n_nodes + n_graphs;
-    a.pred = pred; a.targets = targets; a.batch = n_graphs > 1 ? data_batch : nullptr; a.counter = counter;
-    a.chamfer = chamfer;
-    a.bounds = (int*)(ws + L.bounds); a.flags = (int*)(ws + L.flags); a.grid = (ChamferGrid*)(ws + L.grid);
-    a.keyrank = (int2*)(ws + L.keyrank); a.cell_start = (int*)(ws + L.cell_start); a.sorted = (float4*)(ws + L.sorted);
-    a.minima = (double*)(ws + L.minima); a.slots = (double*)(ws + L.slots); a.ticket = (unsigned*)(ws + L.ticket);
-    size_t tmp_bytes = L.tmp_bytes;
-    const int64_t init = 2 * a.T + 1 > (int64_t)n_graphs * 6 ? 2 * a.T + 1 : (int64_t)n_graphs * 6;
+    cub::DoubleBuffer<unsigned> keys((unsigned*)(ws + L.keys[0]), (unsigned*)(ws + L.keys[1]));
+    cub::DoubleBuffer<int> rows((int*)(ws + L.rows[0]), (int*)(ws + L.rows[1]));
     const unsigned nb2 = (unsigned)((2 * n_nodes + 255) / 256);
-    const int64_t warps = (n_nodes + CHF_WARP_ROWS - 1) / CHF_WARP_ROWS;
-    chamfer_init_kernel<<<(unsigned)((init + 255) / 256), 256, 0, stream>>>(a);
-    chamfer_bounds_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(a);
-    chamfer_grid_kernel<<<(unsigned)((n_graphs + 127) / 128), 128, 0, stream>>>(a);
-    chamfer_keys_kernel<<<nb2, 256, 0, stream>>>(a);
+    chamfer_bwd_keys_kernel<<<nb2, 256, 0, stream>>>(n_nodes, nearest, keys.Current(), rows.Current());
     DEGNN_CHECK_LAUNCH();
-    const cudaError_t e = cub::DeviceScan::ExclusiveSum(ws + L.tmp, tmp_bytes, (const int32_t*)a.cell_start,
-                                                        a.cell_start, (int)(2 * a.T + 1), stream);
+    size_t tmp_bytes = L.tmp_bytes;
+    const cudaError_t e = cub::DeviceRadixSort::SortPairs(ws + L.tmp, tmp_bytes, keys, rows, (int)(2 * n_nodes), 0,
+                                                          L.end_bit, stream);
     if (e != cudaSuccess) {
-        set_error("distegnn_rollout_chamfer: cub scan failed: %s", cudaGetErrorString(e));
+        set_error("%s: cub sort failed: %s", __func__, cudaGetErrorString(e));
         return DISTEGNN_ECUDA;
     }
-    chamfer_scatter_kernel<<<nb2, 256, 0, stream>>>(a);
-    chamfer_search_kernel<<<nb2, 256, 0, stream>>>(a);
-    chamfer_sum_kernel<<<(unsigned)err_chunks(n_nodes), DET_RED, 0, stream>>>(a);
+    ChamferBwdArgs a;
+    a.N = n_nodes; a.B = n_graphs; a.pred = pred; a.target = target; a.batch = n_graphs > 1 ? data_batch : nullptr;
+    a.nearest = nearest; a.g = g; a.g_pred = g_pred; a.g_target = g_target;
+    a.keys = keys.Current(); a.rows = rows.Current();
+    chamfer_bwd_kernel<<<nb2, 256, 0, stream>>>(a);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

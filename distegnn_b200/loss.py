@@ -126,3 +126,79 @@ def train_loss(loc_pred: Tensor, loc_target: Tensor, virtual_node_loc: Tensor, b
     loss, out = _TrainLoss.apply(loc_pred.to(torch.float32), virtual_node_loc.to(torch.float32),
                                  loc_target.detach().to(torch.float32), gptr, samples, lm, cfg)
     return loss, {"logged": out[1], "mmd": out[2], "loc_mean_dev": out[3], "samples": samples}
+
+
+class _ChamferDistance(torch.autograd.Function):
+    """Forward: distegnn_chamfer_distance (the sums and each minimum's nearest id); backward: distegnn_chamfer_distance_bwd
+    on those ids.  See DESIGN §21."""
+
+    @staticmethod
+    def forward(ctx, pred, target, batch, B):
+        from .backend import cuda_backend
+        be = cuda_backend()
+        dev, N = pred.device, int(pred.shape[0])
+        p, t = pred.detach(), target.detach()
+        out = torch.empty(B, 2, dtype=torch.float64, device=dev)
+        nearest = torch.empty(2 * N, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            be.chamfer_distance(p, t, batch, out, nearest, be.rollout_chamfer_workspace(N, B, dev))
+        ctx.save_for_backward(p, t, nearest, batch)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        from .backend import cuda_backend
+        be = cuda_backend()
+        p, t, nearest, batch = ctx.saved_tensors
+        g_pred = torch.empty_like(p) if ctx.needs_input_grad[0] else None
+        g_target = torch.empty_like(t) if ctx.needs_input_grad[1] else None
+        if g_pred is not None or g_target is not None:
+            with torch.cuda.device(p.device):
+                be.chamfer_distance_bwd(p, t, batch, nearest, g.to(torch.float64).contiguous(), g_pred, g_target,
+                                        be.chamfer_distance_bwd_workspace(int(p.shape[0]), p.device))
+        return g_pred, g_target, None, None
+
+
+def chamfer_distance(pred: Tensor, target: Tensor, data_batch: Optional[Tensor] = None,
+                     n_graphs: Optional[int] = None) -> Tensor:
+    """Differentiable per-graph Chamfer distance of two clouds with the same rows (DESIGN §21) -> float64 [B, 2]:
+
+        out[b, 0] = Σ_{i in graph b} min_{j in graph b} d(pred_i, target_j)      (prediction -> record)
+        out[b, 1] = Σ_{j in graph b} min_{i in graph b} d(target_j, pred_i)      (record -> prediction)
+
+    with d the rollout's per-node squared error (fp32 differences, fp64 squares and sums), bit for bit one step of
+    `rollout(..., chamfer=True)`.  pred, target: contiguous float32 [N,3] CUDA tensors, row i of both node i;
+    data_batch: sorted int64 [N] (None: one graph).  A graph without nodes gives 0, a graph with a non-finite coordinate
+    NaN (and NaN gradient rows).  The gradient flows to whichever of pred and target requires it, in a fixed order with no
+    floating-point atomics, so it is bitwise reproducible.  n_graphs=None reads data_batch.max() + 1 once (a host sync);
+    with n_graphs given, neither the forward nor the backward synchronises.  With several ranks the value and the
+    gradients are this rank's partition-local ones.  Memory is O(N + B): nothing of N² size."""
+    for name, x in (("pred", pred), ("target", target)):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError(f"{name} must be a tensor")
+        if x.dtype != torch.float32:
+            raise ValueError(f"{name} must be float32 (got {x.dtype})")
+        if x.dim() != 2 or x.shape[1] != 3:
+            raise ValueError(f"{name} must be [N,3] (got {list(x.shape)})")
+        if not x.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+    if pred.shape[0] != target.shape[0]:
+        raise ValueError(f"pred and target must have the same rows (got {pred.shape[0]} and {target.shape[0]})")
+    N = int(pred.shape[0])
+    if data_batch is not None:
+        if not isinstance(data_batch, torch.Tensor) or data_batch.dtype != torch.int64 or data_batch.shape != (N,):
+            raise ValueError(f"data_batch must be an int64 [N={N}] tensor")
+        if not data_batch.is_contiguous():
+            raise ValueError("data_batch must be contiguous")
+    if n_graphs is not None and (isinstance(n_graphs, bool) or not isinstance(n_graphs, int) or n_graphs < 1):
+        raise ValueError(f"n_graphs must be an int >= 1 (got {n_graphs!r})")
+    if data_batch is None and n_graphs is not None and n_graphs > 1:
+        raise ValueError("n_graphs > 1 needs data_batch")
+    for name, x in (("pred", pred), ("target", target), ("data_batch", data_batch)):
+        if x is not None and x.device.type != "cuda":
+            raise ValueError(f"{name} must be a CUDA tensor (distegnn_b200 has no CPU path)")
+        if x is not None and x.device != pred.device:
+            raise ValueError(f"{name} is on {x.device}, pred on {pred.device}")
+    if n_graphs is None:
+        n_graphs = 1 if data_batch is None or N == 0 else int(data_batch.max()) + 1
+    return _ChamferDistance.apply(pred, target, data_batch, int(n_graphs))

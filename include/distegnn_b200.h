@@ -541,6 +541,30 @@ DISTEGNN_API int distegnn_rollout_chamfer_workspace_bytes(int64_t n_nodes, int n
 DISTEGNN_API int distegnn_rollout_chamfer(int64_t n_nodes, int n_graphs, int steps, const float *pred,
                                           const float *targets, const int64_t *data_batch, const int32_t *counter,
                                           double *chamfer, void *workspace, int64_t workspace_bytes, void *stream);
+/* distegnn_chamfer_distance: the differentiable Chamfer distance of one frame (DESIGN §21).  pred and target float32
+ * [N, 3], row i of both is node i; out float64 [n_graphs, 2] gets what distegnn_rollout_chamfer stores for one step (the
+ * same launches, bit for bit), and nearest int32 [2N] the minimiser of every minimum: nearest[i] = n0(i) (a prediction's
+ * nearest record) and nearest[N + j] = n1(j) (a record's nearest prediction).  Tie rule: the matched node when it attains
+ * the minimum, else the smallest node id among the minimisers; −1 in a graph with a non-finite coordinate.  Row-for-row
+ * the same graph: data_batch int64 [N] sorted (NULL for one graph); n_nodes + n_graphs <= 2^29.  The workspace is sized
+ * by distegnn_rollout_chamfer_workspace_bytes (the same layout; 16-byte aligned, needs no initialisation).  n_nodes 0:
+ * out is zeroed, nothing else happens.  No allocation, no host synchronisation; capturable. */
+DISTEGNN_API int distegnn_chamfer_distance(int64_t n_nodes, int n_graphs, const float *pred, const float *target,
+                                           const int64_t *data_batch, double *out, int32_t *nearest, void *workspace,
+                                           int64_t workspace_bytes, void *stream);
+/* distegnn_chamfer_distance_bwd: with g float64 [n_graphs, 2] the upstream gradient of out and nearest from
+ * distegnn_chamfer_distance on the same inputs, for a row i of graph b (each row one plain store, computed in fp64 with
+ * round-to-nearest and rounded once to fp32):
+ *   g_pred[i]   = 2·g[b,0]·fl32(pred_i − target_{n0(i)})  + Σ_{j: n1(j) = i, ascending} 2·g[b,1]·fl32(pred_i − target_j)
+ *   g_target[j] = 2·g[b,1]·fl32(target_j − pred_{n1(j)}) + Σ_{i: n0(i) = j, ascending} 2·g[b,0]·fl32(target_j − pred_i)
+ * NaN rows in a graph with a non-finite coordinate (nearest −1).  g_pred or g_target may be NULL (not written).  No
+ * floating-point atomics: the result is bitwise reproducible.  The workspace (distegnn_chamfer_distance_bwd_workspace_bytes,
+ * 16-byte aligned) needs no initialisation.  No allocation, no host synchronisation; capturable. */
+DISTEGNN_API int distegnn_chamfer_distance_bwd_workspace_bytes(int64_t n_nodes, int64_t *bytes_host);
+DISTEGNN_API int distegnn_chamfer_distance_bwd(int64_t n_nodes, int n_graphs, const float *pred, const float *target,
+                                               const int64_t *data_batch, const int32_t *nearest, const double *g,
+                                               float *g_pred, float *g_target, void *workspace,
+                                               int64_t workspace_bytes, void *stream);
 
 /* ---- frame assembly (csrc/frames.cu; distegnn_b200/frames.py: training batches from raw trajectories) ----------------
  * For a batch of n_samples samples, from the staged frames of each sample's WHOLE scene — frames float32 [3, n_frame_nodes,
