@@ -26,6 +26,7 @@ that `radius_graph_csr` builds on the device: `rollout.differentiable_rollout` b
 """
 from __future__ import annotations
 
+import contextlib
 from collections import OrderedDict
 from typing import Dict, List, Optional, Tuple
 
@@ -81,19 +82,13 @@ class E_GCL_vel(nn.Module):
 # --------------------------------------------------------------------------------------------------
 # packing of one layer's weights into the flat block the kernels read (include/distegnn_b200.h)
 # --------------------------------------------------------------------------------------------------
-def pack_layer_params(g: nn.Module, A: int, Cn: int, Na: int, device, offs: Dict[str, int],
-                      total: int, differentiable: bool = False) -> Tensor:
-    """Flat parameter block of one layer.  `differentiable=True` (training) builds it with torch.cat from the live
-    parameters, so that the gradient of the block flows back to the nn.Parameters through autograd."""
-    buf = None if differentiable else torch.zeros(total, dtype=torch.float32, device=device)
+def pack_layer_params(g: nn.Module, A: int, Cn: int, Na: int, device, offs: Dict[str, int], total: int) -> Tensor:
+    """Flat parameter block of one layer, built with torch.cat from the live parameters (zeros in the gaps of the
+    layout), so that the gradient of the block flows back to the nn.Parameters through autograd."""
     pieces: List[Tuple[int, Tensor]] = []
 
     def put(name: str, t: Tensor) -> None:
-        if differentiable:
-            pieces.append((offs[name], t.to(device=device, dtype=torch.float32).reshape(-1)))
-            return
-        t = t.detach().to(device=device, dtype=torch.float32).reshape(-1)
-        buf[offs[name]:offs[name] + t.numel()] = t
+        pieces.append((offs[name], t.to(device=device, dtype=torch.float32).reshape(-1)))
 
     W1, b1 = g.edge_mlp[0].weight, g.edge_mlp[0].bias            # [64, 2H+1+A]
     put("E_W1A", W1[:, 0:H].t()); put("E_W1B", W1[:, H:2 * H].t()); put("E_W1R", W1[:, 2 * H])
@@ -117,8 +112,6 @@ def pack_layer_params(g: nn.Module, A: int, Cn: int, Na: int, device, offs: Dict
     put("N_W2", g.node_mlp[2].weight.t()); put("N_B2", g.node_mlp[2].bias)
     put("M_W1", g.node_mlp_virtual[0].weight.t()); put("M_B1", g.node_mlp_virtual[0].bias)
     put("M_W2", g.node_mlp_virtual[2].weight.t()); put("M_B2", g.node_mlp_virtual[2].bias)
-    if not differentiable:
-        return buf
     parts, pos = [], 0
     for off, t in sorted(pieces, key=lambda p: p[0]):
         if off > pos:
@@ -255,19 +248,28 @@ class FastEGNN(nn.Module):
         from .backend import cuda_backend
         return cuda_backend()
 
-    def _packed_params(self, device: torch.device):
-        params = list(self.parameters())
-        key = (str(device),) + tuple((p.data_ptr(), p._version) for p in params)
-        if self._packed is not None and self._packed[0] == key:
-            return self._packed[1]
+    def _pack_params(self, device: torch.device) -> Dict:
+        """The weights as the kernels read them, {layers: [flat block per layer], emb_wt, emb_b, hv0 [C,64]}, packed from
+        the live parameters with torch ops, so that the gradients of the packed tensors flow back to the nn.Parameters."""
         A, Cn, Na = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf
         offs, total = _lib.param_layout(A, Cn, Na)
         layers = [pack_layer_params(getattr(self, "gcl_%d" % i), A, Cn, Na, device, offs, total)
                   for i in range(self.n_layers)]
-        emb_wt = self.embedding_in.weight.detach().t().contiguous().to(device=device, dtype=torch.float32)
-        emb_b = self.embedding_in.bias.detach().contiguous().to(device=device, dtype=torch.float32)
-        hv0 = self.virtual_node_feat.detach()[0].t().contiguous().to(device=device, dtype=torch.float32)  # [C,64]
-        packed = dict(layers=layers, emb_wt=emb_wt, emb_b=emb_b, hv0=hv0)
+        emb_wt = self.embedding_in.weight.t().contiguous().to(device=device, dtype=torch.float32)
+        emb_b = self.embedding_in.bias.to(device=device, dtype=torch.float32)
+        hv0 = self.virtual_node_feat[0].t().contiguous().to(device=device, dtype=torch.float32)
+        return dict(layers=layers, emb_wt=emb_wt, emb_b=emb_b, hv0=hv0)
+
+    def _packed_params(self, device: torch.device) -> Dict:
+        """`_pack_params` detached, cached while no parameter is replaced or changed in place."""
+        key = (str(device),) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        if self._packed is not None and self._packed[0] == key:
+            return self._packed[1]
+        with torch.no_grad():
+            pk = self._pack_params(device)
+        # detached: emb_b may be the bias Parameter itself (`.to` returns it when nothing changes)
+        packed = dict(layers=[t.detach() for t in pk["layers"]], emb_wt=pk["emb_wt"].detach(),
+                      emb_b=pk["emb_b"].detach(), hv0=pk["hv0"].detach())
         self._packed = (key, packed)
         return packed
 
@@ -321,13 +323,6 @@ class FastEGNN(nn.Module):
             import torch.distributed as dist
             dist.all_reduce(vsum, op=dist.ReduceOp.SUM, group=self.process_group)
 
-    def _mark(self, name: str):
-        if self._timing is None:
-            return None
-        ev = torch.cuda.Event(enable_timing=True)
-        ev.record()
-        return (name, ev)
-
     # ---- forward -------------------------------------------------------------------------------
     def forward(self, node_feat, node_loc, node_vel, loc_mean, edge_index, data_batch, edge_attr=None,
                 node_attr=None) -> Tuple[Tensor, Tensor]:
@@ -358,14 +353,14 @@ class FastEGNN(nn.Module):
         if loc_mean.shape != (B, 3):
             raise ValueError("loc_mean must be [B,3]")
         K = 4 + 3 * Cn + H * Cn
-        f32 = lambda t: t if (t.dtype == torch.float32 and t.is_contiguous() and not t.requires_grad) \
-            else t.detach().to(dtype=torch.float32).contiguous()
+        dims = (N, E, B, K)
         if pre_csr:
             edge_index.validate(dev)
-        import contextlib
-        guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
-        with guard:                                           # launches and smem opt-ins happen on the tensors' device
-            if training_path:
+        with device_guard(dev):                               # launches and smem opt-ins happen on the tensors' device
+            with torch.no_grad():
+                args = self._kernel_args(be, N, node_feat, node_loc, node_vel, loc_mean, edge_index, data_batch,
+                                         edge_attr, node_attr)
+            if training_path:      # per-layer activations kept (N-sized only), gradients through _FastEGNNFunction
                 for name, t in (("node_feat", node_feat), ("node_loc", node_loc), ("node_vel", node_vel),
                                 ("edge_attr", edge_attr), ("node_attr", node_attr)):
                     if t is not None and t.requires_grad and not self.input_grads:
@@ -374,15 +369,12 @@ class FastEGNN(nn.Module):
                                       "as constants (the reference trains weights only, utils/train.py:149-158): no "
                                       "gradient will flow to it; set `model.input_grads = True` to back-propagate into "
                                       "the inputs", RuntimeWarning, stacklevel=2)
-                return self._forward_autograd(be, dev, (N, E, B, K), f32, node_feat, node_loc, node_vel, loc_mean,
-                                              edge_index, data_batch, edge_attr, node_attr)
+                pk = self._pack_params(dev)
+                ins = inputs if self.input_grads else ()
+                return _FastEGNNFunction.apply(self, be, dims, args, pk["emb_wt"], pk["emb_b"], pk["hv0"], *pk["layers"],
+                                               *ins)
             with torch.no_grad():
                 pk = self._packed_params(dev)
-                rowptr, row, col, ea, nE = self._csr_inputs(be, edge_index, edge_attr, N, f32)
-                args = dict(node_feat=f32(node_feat), node_loc=f32(node_loc), node_vel=f32(node_vel),
-                            loc_mean=f32(loc_mean), attr=f32(node_attr) if Na > 0 else None,
-                            data_batch=data_batch.contiguous(), rowptr=rowptr, row=row, col=col, ea=ea, nE=nE)
-                dims = (N, E, B, K)
                 comm = self._get_comm(be, dev, B, K)
                 graph_ok = self.world_size == 1 or comm is not None      # NCCL calls are not captured
                 if self.cuda_graph and graph_ok and self._backend is None and dev.type == "cuda" \
@@ -390,9 +382,9 @@ class FastEGNN(nn.Module):
                     return self._forward_graphed(be, pk, dims, args, comm)
                 ws = self._workspace(dev, N, B, K)
                 # results go straight into fresh tensors (no copy launch); everything else lives in the workspace
-                return self._run(be, pk, dims, args, ws, comm,
-                                 out=torch.empty(N, 3, dtype=torch.float32, device=dev),
-                                 Xv=torch.empty(B, 3, Cn, dtype=torch.float32, device=dev))
+                out, Xv, _ = self._forward(be, pk, dims, args, ws, out=torch.empty(N, 3, dtype=torch.float32, device=dev),
+                                           Xv=torch.empty(B, 3, Cn, dtype=torch.float32, device=dev))
+                return out, Xv
 
     def _batch_checked(self, data_batch: Tensor, N: int, B: int) -> bool:
         v = self._validated_batch
@@ -418,111 +410,26 @@ class FastEGNN(nn.Module):
                              "per-graph reductions rely on it")
         self._validated_batch = (data_batch, data_batch._version, N, B)
 
-    def _csr_inputs(self, be, edge_index, edge_attr, N: int, f32):
-        """(rowptr, row, col, edge_attr in CSR order): from the cache / a radix sort for an int64 edge_index, or straight
-        from a pre-sorted CSRGraph (shards.py) — then nothing is sorted or permuted."""
+    def _kernel_args(self, be, N: int, node_feat, node_loc, node_vel, loc_mean, edge_index, data_batch, edge_attr,
+                     node_attr) -> Dict[str, Tensor]:
+        """The caller's tensors as the kernels read them (float32, contiguous, detached), and the graph as rowptr, row,
+        col, edge_attr in CSR order and the device edge count: from the cache / a radix sort for an int64 edge_index
+        (then `perm` maps CSR positions to the caller's edges), or straight from a pre-sorted CSRGraph (shards.py) — then
+        nothing is sorted or permuted."""
         from .shards import CSRGraph
-        A = self.edge_attr_nf
+        A, Na = self.edge_attr_nf, self.node_attr_nf
+        f32 = lambda t: t if (t.dtype == torch.float32 and t.is_contiguous() and not t.requires_grad) \
+            else t.detach().to(dtype=torch.float32).contiguous()
+        a = dict(node_feat=f32(node_feat), node_loc=f32(node_loc), node_vel=f32(node_vel), loc_mean=f32(loc_mean),
+                 attr=f32(node_attr) if Na > 0 else None, data_batch=data_batch.contiguous())
         if isinstance(edge_index, CSRGraph):
-            return (edge_index.rowptr.contiguous(), edge_index.rows().contiguous(), edge_index.col.contiguous(),
-                    f32(edge_attr) if A > 0 else None, edge_index.n_edges_dev)
+            a.update(rowptr=edge_index.rowptr.contiguous(), row=edge_index.rows().contiguous(),
+                     col=edge_index.col.contiguous(), ea=f32(edge_attr) if A > 0 else None, nE=edge_index.n_edges_dev)
+            return a
         rowptr, row, col, perm = self._graphs.get(be, edge_index, N, self.validate_inputs)
         ea = self._graphs.sorted_edge_attr(be, edge_index, edge_attr, perm) if A > 0 else None
-        return rowptr, row, col, ea, None
-
-    # ---- training path (SURVEY §8 f-1) -----------------------------------------------------------------
-    def _forward_autograd(self, be, dev, dims, f32, node_feat, node_loc, node_vel, loc_mean, edge_index, data_batch,
-                          edge_attr, node_attr) -> Tuple[Tensor, Tensor]:
-        """Forward with a backward: same kernels as the inference path, per-layer activations kept (N-sized only:
-        nothing of size [E,.] or [N,C,.] is ever stored), gradients through `_FastEGNNFunction`.  Inputs are treated
-        as constants (the reference trains weights only: utils/train.py:149-158) unless `self.input_grads` is set: then the
-        six raw input tensors are inputs of the autograd node as well."""
-        A, Cn, Na = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf
-        N, E, B, K = dims
-        emb_wt, emb_b, hv0, lps = self._differentiable_params(dev)
-        with torch.no_grad():
-            rowptr, row, col, ea, nE = self._csr_inputs(be, edge_index, edge_attr, N, f32)
-            args = dict(node_feat=f32(node_feat), node_loc=f32(node_loc), node_vel=f32(node_vel),
-                        loc_mean=f32(loc_mean), attr=f32(node_attr) if Na > 0 else None,
-                        data_batch=data_batch.contiguous(), rowptr=rowptr, row=row, col=col, ea=ea, nE=nE)
-            from .shards import CSRGraph
-            if self.input_grads and A > 0 and not isinstance(edge_index, CSRGraph):   # CSR position -> caller's edge
-                args["perm"] = self._graphs.get(be, edge_index, N, self.validate_inputs)[3]
-        if not self.input_grads:
-            return _FastEGNNFunction.apply(self, be, dims, args, emb_wt, emb_b, hv0, *lps)
-        return _FastEGNNFunction.apply(self, be, dims, args, emb_wt, emb_b, hv0, *lps,
-                                       node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr)
-
-    def _differentiable_params(self, dev):
-        """(emb_wt, emb_b, hv0, [layer blocks]) packed from the live parameters with torch ops, so that the gradients of
-        the packed tensors flow back to the nn.Parameters through autograd."""
-        A, Cn, Na = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf
-        offs, total = _lib.param_layout(A, Cn, Na)
-        lps = [pack_layer_params(getattr(self, "gcl_%d" % i), A, Cn, Na, dev, offs, total, differentiable=True)
-               for i in range(self.n_layers)]
-        emb_wt = self.embedding_in.weight.t().contiguous().to(device=dev, dtype=torch.float32)
-        emb_b = self.embedding_in.bias.to(device=dev, dtype=torch.float32)
-        hv0 = self.virtual_node_feat[0].t().contiguous().to(device=dev, dtype=torch.float32)          # [C,64]
-        return emb_wt, emb_b, hv0, lps
-
-    def _run_saving(self, be, dims, a: Dict[str, Tensor], emb_wt, emb_b, hv0, layers: List[Tensor],
-                    init_centroid: bool = False):
-        """`_run` with fresh buffers per layer; returns (out, Xv_L, saved state for the backward).  `init_centroid` as in
-        `_run` (the differentiable rollout's steps t >= 1): X_0 is the summed x̄ of node_loc, loc_mean is not read."""
-        A, Cn, Na, F = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf, self.node_feat_nf
-        N, E, B, K = dims
-        dev = a["node_loc"].device
-        new = lambda *s, dt=torch.float32: torch.empty(*s, dtype=dt, device=dev)
-        zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        L = self.n_layers
-        base = _lib.FLAG_NORMALIZE if self.normalize else 0
-        Xv = new(B, 3, Cn) if init_centroid else a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn).contiguous()
-        Hv = hv0.unsqueeze(0).expand(B, Cn, H).contiguous()
-        h, x4, batch32, P, Q, Hn = new(N, H), new(N, 4), new(N, dt=torch.int32), new(N, H), new(N, H), new(N, H)
-        vsum = zeros(B, K)
-        comm = self._get_comm(be, dev, B, K)
-        counter = None if self._batch_checked(a["data_batch"], N, B) else torch.zeros(1, dtype=torch.int32, device=dev)
-        det = self._det_workspace({}, dev, N, E) if self.deterministic and L else None
-        dk = {} if det is None else dict(det_ws=det)
-        be.embed((N, B, F, A, Cn, Na), a["node_feat"], a["node_loc"], a["data_batch"], emb_wt, emb_b,
-                 layers[0] if L else None, h, x4, batch32, P, Q, Hn, vsum, counter, **dk)
-        self._check_batch(counter, a["data_batch"], N, B)
-        st = dict(batch32=batch32, vsum_init=vsum, layers=[], comm=comm)
-        if L == 0:
-            return a["node_loc"].clone(), Xv, st
-        if comm is None:
-            self._sync_virtual(vsum)
-        G = new(B, Cn, H)
-        init = _lib.FLAG_INIT | (_lib.FLAG_INIT_CENTROID if init_centroid else 0)
-        be.virtual_update((B, A, Cn, Na), init, vsum, Xv, Hv, None, layers[0], G, comm=comm)
-        out = None
-        for i in range(L):
-            last = i == L - 1
-            flags = base | (_lib.FLAG_LAST if last else 0)
-            lp, lp_next = layers[i], (None if last else layers[i + 1])
-            agg_x, trans_v, vs = zeros(N, 4), new(N, 4), zeros(B, K)
-            agg_m = None if last else zeros(N, H)
-            agg_v = None if last else new(N, H)
-            be.edge_layer((N, E, A, Cn, Na), flags, a["row"], a["col"], a["ea"], x4, P, Q, lp, agg_m, agg_x, a["nE"],
-                          **dk)
-            be.virtual_layer((N, B, A, Cn, Na), flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vs, **dk)
-            x4n = new(N, 4)
-            hn, Pn, Qn, Hnn = (None,) * 4 if last else (new(N, H), new(N, H), new(N, H), new(N, H))
-            out = new(N, 3) if last else None
-            be.node_layer((N, B, A, Cn, Na), flags, a["rowptr"], batch32, h, x4, a["node_vel"], a["attr"], agg_m,
-                          agg_x, agg_v, trans_v, lp, lp_next, hn, x4n, Pn, Qn, Hnn, out, vs, **dk)
-            if comm is None:
-                self._sync_virtual(vs)
-            st["layers"].append(dict(h=h, x4=x4, P=P, Q=Q, Hn=Hn, Xv=Xv, Hv=Hv, G=G, agg_m=agg_m, agg_x=agg_x,
-                                     agg_v=agg_v, trans_v=trans_v, vsum=vs, flags=flags))
-            Xv, Hv = Xv.clone(), (Hv if last else Hv.clone())
-            Gn = None if last else new(B, Cn, H)
-            # with a communicator the update kernel all-reduces `vs` first and leaves the summed statistics in it
-            be.virtual_update((B, A, Cn, Na), flags & ~_lib.FLAG_NORMALIZE, vs, Xv, Hv, lp, lp_next, Gn, comm=comm)
-            h, x4, P, Q, Hn, G = hn, x4n, Pn, Qn, Hnn, Gn
-        if self._keep_state is not None:
-            self._keep_state.append(st)
-        return out, Xv, st
+        a.update(rowptr=rowptr, row=row, col=col, ea=ea, nE=None, perm=perm)
+        return a
 
     # ---- device work ---------------------------------------------------------------------------
     def _det_workspace(self, ws: Dict[str, Tensor], dev, N: int, E: int) -> Tensor:
@@ -554,76 +461,107 @@ class FastEGNN(nn.Module):
             self._workspaces[key] = ws
         return ws
 
-    def _run(self, be, pk, dims, a: Dict[str, Tensor], ws: Dict[str, Tensor], comm=None, out: Optional[Tensor] = None,
-             Xv: Optional[Tensor] = None, init_centroid: bool = False) -> Tuple[Tensor, Tensor]:
-        """Enqueue one forward on the current stream: 2 + 4L kernel launches (buffers in `ws`; nothing allocates,
-        nothing syncs unless a new data_batch tensor has to be validated).  Results are written to `out` / `Xv`
-        (default: the workspace's own buffers, which the next forward overwrites).  `init_centroid` (rollouts): the
-        initial virtual coordinates are the per-graph centroid of `node_loc` over all partitions, taken from the
-        statistics the first exchange already sums, instead of `loc_mean` (which is then not read)."""
+    def _forward(self, be, pk, dims, a: Dict[str, Tensor], ws: Optional[Dict[str, Tensor]] = None,
+                 out: Optional[Tensor] = None, Xv: Optional[Tensor] = None, init_centroid: bool = False):
+        """Enqueue one forward on the current stream: 2 + 4L kernel launches; nothing syncs unless a new data_batch tensor
+        has to be validated.  Returns (out, Xv, saved state or None).
+
+        With a workspace `ws` (inference) nothing allocates: every buffer is reused, and the consuming kernels clear the
+        accumulators for the next layer and the next call (FLAG_ZERO_AGG / FLAG_ZERO_VSUM).  Results are written to `out` /
+        `Xv` (default: the workspace's own buffers, which the next forward overwrites).  Without one (the training path and
+        the differentiable rollout's recompute) every layer writes fresh tensors, and the saved state keeps them for
+        `_backward_saved`.
+
+        `init_centroid` (rollouts): the initial virtual coordinates are the per-graph centroid of `node_loc` over all
+        partitions, taken from the statistics the first exchange already sums, instead of `loc_mean` (which is then not
+        read)."""
         A, Cn, Na, F = self.edge_attr_nf, self.virtual_channels, self.node_attr_nf, self.node_feat_nf
         N, E, B, K = dims
-        layers: List[Tensor] = pk["layers"]
-        h, P, Q, Hn, agg_m, agg_v = ws["h"], ws["P"], ws["Q"], ws["Hn"], ws["agg_m"], ws["agg_v"]
-        x4, agg_x, trans_v, batch32 = ws["x4"], ws["agg_x"], ws["trans_v"], ws["batch32"]
+        L, layers = self.n_layers, pk["layers"]
+        dev = a["node_loc"].device
+        save = ws is None
+        new = lambda *s, dt=torch.float32: torch.empty(*s, dtype=dt, device=dev)
+        zeros = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
+        if save:
+            ws = dict(h=new(N, H), P=new(N, H), Q=new(N, H), Hn=new(N, H), x4=new(N, 4), batch32=new(N, dt=torch.int32),
+                      vsum=zeros(B, K), G=new(B, Cn, H), Xv=new(B, 3, Cn), Hv=new(B, Cn, H), out=new(N, 3), dirty=False)
+        h, P, Q, Hn, x4, batch32 = ws["h"], ws["P"], ws["Q"], ws["Hn"], ws["x4"], ws["batch32"]
         vsum, G, Hv = ws["vsum"], ws["G"], ws["Hv"]
         out = ws["out"] if out is None else out
         Xv = ws["Xv"] if Xv is None else Xv
         if ws["dirty"]:
-            vsum.zero_(); agg_m.zero_(); agg_x.zero_()
+            vsum.zero_(); ws["agg_m"].zero_(); ws["agg_x"].zero_()
         ws["dirty"] = True
-        base = _lib.FLAG_NORMALIZE if self.normalize else 0
-        L = self.n_layers
         counter = None
         if not self._batch_checked(a["data_batch"], N, B):
-            counter = ws["counter"]
-            counter.zero_()
-        det = self._det_workspace(ws, a["node_loc"].device, N, E) if self.deterministic and L else None
+            counter = zeros(1, dt=torch.int32) if save else ws["counter"].zero_()
+        comm = self._get_comm(be, dev, B, K)
+        det = self._det_workspace(ws, dev, N, E) if self.deterministic and L else None
         dk = {} if det is None else dict(det_ws=det)
         be.embed((N, B, F, A, Cn, Na), a["node_feat"], a["node_loc"], a["data_batch"], pk["emb_wt"], pk["emb_b"],
                  layers[0] if L else None, h, x4, batch32, P, Q, Hn, vsum, counter, **dk)
         self._check_batch(counter, a["data_batch"], N, B)
+        st = dict(batch32=batch32, vsum_init=vsum, layers=[], comm=comm) if save else None
         if L == 0:
             vsum.zero_()
             out.copy_(a["node_loc"])
             Xv.copy_(a["loc_mean"].unsqueeze(-1).expand(B, 3, Cn))
             ws["dirty"] = False
-            return out, Xv
+            return out, Xv, st
         sync = comm is None and self.world_size > 1              # torch.distributed path (stand-in backend / no P2P)
         if sync:
             self._sync_virtual(vsum)
+        # the saved statistics and aggregates of every layer outlive it: only the inference path clears them
+        zero_vsum, zero_agg = (0, 0) if save else (_lib.FLAG_ZERO_VSUM, _lib.FLAG_ZERO_AGG)
         # FastEGNN.py:299-300 (initial Hv, Xv) are folded into the INIT update
-        init = _lib.FLAG_INIT | _lib.FLAG_ZERO_VSUM | (_lib.FLAG_INIT_CENTROID if init_centroid else 0)
+        init = _lib.FLAG_INIT | zero_vsum | (_lib.FLAG_INIT_CENTROID if init_centroid else 0)
         be.virtual_update((B, A, Cn, Na), init, vsum, Xv, Hv, None, layers[0], G,
                           None if init_centroid else a["loc_mean"], pk["hv0"], comm)
+        base = _lib.FLAG_NORMALIZE if self.normalize else 0
+        timed = not save and self._timing is not None
+        mark = _event if timed else (lambda: None)
         for i in range(L):
             last = i == L - 1
             flags = base | (_lib.FLAG_LAST if last else 0)
             lp, lp_next = layers[i], (None if last else layers[i + 1])
-            t0 = self._mark("edge")
-            be.edge_layer((N, E, A, Cn, Na), flags, a["row"], a["col"], a["ea"], x4, P, Q, lp,
-                          None if last else agg_m, agg_x, a["nE"], **dk)
-            t1 = self._mark("edge_end")
-            be.virtual_layer((N, B, A, Cn, Na), flags, batch32, x4, Hn, Xv, G, lp,
-                             None if last else agg_v, trans_v, vsum, **dk)
-            t2 = self._mark("virtual_end")
-            be.node_layer((N, B, A, Cn, Na), flags | _lib.FLAG_ZERO_AGG, a["rowptr"], batch32, h, x4, a["node_vel"],
-                          a["attr"], None if last else agg_m, agg_x, None if last else agg_v, trans_v, lp, lp_next,
-                          None if last else h, x4, None if last else P, None if last else Q,
-                          None if last else Hn, out if last else None, vsum, **dk)
-            t3 = self._mark("node_end")
+            if save:
+                agg_m, agg_v = (None, None) if last else (zeros(N, H), new(N, H))
+                agg_x, trans_v, vsum = zeros(N, 4), new(N, 4), zeros(B, K)
+                hn, Pn, Qn, Hnn = (None,) * 4 if last else (new(N, H), new(N, H), new(N, H), new(N, H))
+                x4n, Gn = new(N, 4), (None if last else new(B, Cn, H))
+            else:
+                agg_m, agg_v = (None, None) if last else (ws["agg_m"], ws["agg_v"])
+                agg_x, trans_v = ws["agg_x"], ws["trans_v"]
+                hn, Pn, Qn, Hnn = (None,) * 4 if last else (h, P, Q, Hn)
+                x4n, Gn = x4, G
+            t0 = mark()
+            be.edge_layer((N, E, A, Cn, Na), flags, a["row"], a["col"], a["ea"], x4, P, Q, lp, agg_m, agg_x, a["nE"], **dk)
+            t1 = mark()
+            be.virtual_layer((N, B, A, Cn, Na), flags, batch32, x4, Hn, Xv, G, lp, agg_v, trans_v, vsum, **dk)
+            t2 = mark()
+            be.node_layer((N, B, A, Cn, Na), flags | zero_agg, a["rowptr"], batch32, h, x4, a["node_vel"], a["attr"], agg_m,
+                          agg_x, agg_v, trans_v, lp, lp_next, hn, x4n, Pn, Qn, Hnn, out if last else None, vsum, **dk)
+            t3 = mark()
             if sync:
                 self._sync_virtual(vsum)
-            be.virtual_update((B, A, Cn, Na), (flags & ~_lib.FLAG_NORMALIZE) | _lib.FLAG_ZERO_VSUM, vsum, Xv, Hv, lp,
-                              lp_next, G, comm=comm)
-            t4 = self._mark("update_end")
-            if self._timing is not None:
-                self._timing.append((i, t0[1], t1[1], t2[1], t3[1], t4[1]))
+            if save:
+                st["layers"].append(dict(h=h, x4=x4, P=P, Q=Q, Hn=Hn, Xv=Xv, Hv=Hv, G=G, agg_m=agg_m, agg_x=agg_x,
+                                         agg_v=agg_v, trans_v=trans_v, vsum=vsum, flags=flags))
+                Xv, Hv = Xv.clone(), (Hv if last else Hv.clone())
+            # with a communicator the update kernel all-reduces `vsum` first and leaves the summed statistics in it
+            be.virtual_update((B, A, Cn, Na), (flags & ~_lib.FLAG_NORMALIZE) | zero_vsum, vsum, Xv, Hv, lp, lp_next, Gn,
+                              comm=comm)
+            t4 = mark()
+            if timed:
+                self._timing.append((i, t0, t1, t2, t3, t4))
+            h, x4, P, Q, Hn, G = hn, x4n, Pn, Qn, Hnn, Gn
         ws["dirty"] = False
-        return out, Xv
+        if save and self._keep_state is not None:
+            self._keep_state.append(st)
+        return out, Xv, st
 
     def _forward_graphed(self, be, pk, dims, a: Dict[str, Tensor], comm=None) -> Tuple[Tensor, Tensor]:
-        """CUDA-graph replay of `_run` (opt-in: `model.cuda_graph = True`).  Works for any world size when the
+        """CUDA-graph replay of `_forward` (opt-in: `model.cuda_graph = True`).  Works for any world size when the
         virtual-node sync is the library's own peer-memory exchange (it is part of the update kernels, so the graph holds
         the collectives too; every rank must replay — same call sequence as eager).  The graph is keyed by the addresses
         and shapes of every tensor it reads, so it is valid for as long as the caller keeps passing the same (possibly
@@ -635,19 +573,19 @@ class FastEGNN(nn.Module):
         if ent is None:
             ws = self._workspace(dev, dims[0], dims[2], dims[3])
             if len(self._graph_cache) >= self._graph_max_captures:
-                out, Xv = self._run(be, pk, dims, a, ws, comm)
+                out, Xv, _ = self._forward(be, pk, dims, a, ws)
                 return out.clone(), Xv.clone()
             # warm-up run + capture run: both are real forwards on every rank (the exchange inside stays matched)
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(side):            # warm-up outside capture: lazy inits (smem opt-ins)
-                self._run(be, pk, dims, a, ws, comm)
+                self._forward(be, pk, dims, a, ws)
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
             g = torch.cuda.CUDAGraph()
             n0 = be.launches
             with torch.cuda.graph(g):
-                self._run(be, pk, dims, a, ws, comm)
+                self._forward(be, pk, dims, a, ws)
             # keep the keyed tensors alive: their addresses are baked in.  So is the deterministic workspace, which `ws`
             # swaps for a larger one when a later call brings more edges: the entry keeps the one it captured
             ent = (g, ws, be.launches - n0, a, pk, ws.get("det"))
@@ -657,8 +595,19 @@ class FastEGNN(nn.Module):
         return ent[1]["out"].clone(), ent[1]["Xv"].clone()
 
 
+def _event():
+    ev = torch.cuda.Event(enable_timing=True)
+    ev.record()
+    return ev
+
+
+def device_guard(dev: torch.device):
+    """Make `dev` current for the launches and shared-memory opt-ins of a call (no-op for the CPU stand-ins' tensors)."""
+    return torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
+
+
 class _FastEGNNFunction(torch.autograd.Function):
-    """Autograd node of the fused path.  forward = the sm_90a kernels (FastEGNN._run_saving); backward = per layer, in
+    """Autograd node of the fused path.  forward = the sm_90a kernels (FastEGNN._forward, saving); backward = per layer, in
     reverse: virtual-node update, ONE packed all-reduce of the statistics' gradient (the reference's _AllReduce.backward,
     FastEGNN.py:19-21, issues one per aggregate), per-node stage, real<->virtual stage, per-edge stage, and finally the
     initial virtual state and the embedding prologue — every one a hand-written kernel behind the C ABI (csrc/*bwd*.cu,
@@ -673,11 +622,9 @@ class _FastEGNNFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, be, dims, a, emb_wt, emb_b, hv0, *rest):
         L = model.n_layers
-        layers = [lp.detach().contiguous() for lp in rest[:L]]
-        out, Xv, st = model._run_saving(be, dims, a, emb_wt.detach().contiguous(), emb_b.detach().contiguous(),
-                                        hv0.detach().contiguous(), layers)
+        ctx.pk = _detached(emb_wt, emb_b, hv0, rest[:L])
+        out, Xv, st = model._forward(be, ctx.pk, dims, a)
         ctx.model, ctx.be, ctx.dims, ctx.a, ctx.st = model, be, dims, a, st
-        ctx.params = (emb_wt.detach(), emb_b.detach(), hv0.detach(), layers)
         ctx.inputs = [None if t is None else (t.dtype, t.shape) for t in rest[L:]]
         return out, Xv
 
@@ -685,8 +632,8 @@ class _FastEGNNFunction(torch.autograd.Function):
     def backward(ctx, g_out, g_Xv_out):
         model = ctx.model
         N, E, B, K = ctx.dims
-        emb_wt, emb_b, hv0, layers = ctx.params
-        L = len(layers)
+        emb_wt, emb_b, hv0 = ctx.pk["emb_wt"], ctx.pk["emb_b"], ctx.pk["hv0"]
+        L = len(ctx.pk["layers"])
         n_in = len(ctx.inputs)
         want = ctx.needs_input_grad[7 + L:7 + L + n_in] if n_in else (False,) * 6
         if L == 0:                                           # out = node_loc, Xv = loc_mean broadcast
@@ -697,13 +644,13 @@ class _FastEGNNFunction(torch.autograd.Function):
             g_in = (None, g_x if want[1] else None, None, g_Xv.sum(-1) if want[3] else None, None, None)
             return (None, None, None, None, torch.zeros_like(emb_wt), torch.zeros_like(emb_b),
                     torch.zeros_like(hv0)) + _FastEGNNFunction._input_grads(ctx, g_in)
-        g_emb_wt, g_emb_b, g_hv0, g_lps, g_in = _backward_saved(model, ctx.be, ctx.dims, ctx.a, ctx.st, ctx.params, g_out,
+        g_emb_wt, g_emb_b, g_hv0, g_lps, g_in = _backward_saved(model, ctx.be, ctx.dims, ctx.a, ctx.st, ctx.pk, g_out,
                                                                       g_Xv_out, want)
         grads = (None, None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps)
         if not n_in:
             return grads
         g_ea = g_in[4]
-        if g_ea is not None and "perm" in ctx.a:             # CSR order -> the caller's edge order
+        if g_ea is not None and ctx.a.get("perm") is not None:             # CSR order -> the caller's edge order
             g_ea = ctx.be.gather_rows(g_ea, ctx.a["perm"], inverse=True)
         return grads + _FastEGNNFunction._input_grads(ctx, g_in[:4] + (g_ea,) + g_in[5:])
 
@@ -714,18 +661,24 @@ class _FastEGNNFunction(torch.autograd.Function):
         if not ctx.inputs:
             return ()
         out = []
-        for want, meta, g in zip(ctx.needs_input_grad[7 + len(ctx.params[3]):], ctx.inputs, g_in):
+        for want, meta, g in zip(ctx.needs_input_grad[7 + len(ctx.pk["layers"]):], ctx.inputs, g_in):
             if not want:
                 out.append(None)
                 continue
             dtype, shape = meta
-            dev = ctx.params[0].device
+            dev = ctx.pk["emb_wt"].device
             out.append(torch.zeros(shape, dtype=dtype, device=dev) if g is None else g.to(dtype).reshape(shape))
         return tuple(out)
 
 
-def _backward_saved(model: FastEGNN, be, dims, a, st, params, g_out, g_Xv_out, want, init_centroid: bool = False):
-    """The backward kernels of one forward kept by `FastEGNN._run_saving` (L >= 1), shared by `_FastEGNNFunction` and the
+def _detached(emb_wt, emb_b, hv0, layers) -> Dict:
+    """The packed parameters that an autograd node received, as `FastEGNN._forward` and `_backward_saved` read them."""
+    return dict(layers=[lp.detach().contiguous() for lp in layers], emb_wt=emb_wt.detach().contiguous(),
+                emb_b=emb_b.detach().contiguous(), hv0=hv0.detach().contiguous())
+
+
+def _backward_saved(model: FastEGNN, be, dims, a, st, pk, g_out, g_Xv_out, want, init_centroid: bool = False):
+    """The backward kernels of one forward whose activations `FastEGNN._forward` kept (L >= 1), shared by `_FastEGNNFunction` and the
     differentiable rollout.  `want` = which of (node_feat, node_loc, node_vel, loc_mean, edge_attr, node_attr) need a
     gradient.  Returns (g_emb_wt, g_emb_b, g_hv0, [g_layer_params], (g_feat, g_loc, g_vel, g_loc_mean, g_ea in CSR order,
     g_attr)), None for the inputs not wanted.
@@ -736,7 +689,7 @@ def _backward_saved(model: FastEGNN, be, dims, a, st, params, g_out, g_Xv_out, w
     and the embedding backward spreads it onto every node's g_loc.  No loc_mean gradient then."""
     N, E, B, K = dims
     A, Cn, Na = model.edge_attr_nf, model.virtual_channels, model.node_attr_nf
-    emb_wt, emb_b, hv0, layers = params
+    emb_wt, emb_b, hv0, layers = pk["emb_wt"], pk["emb_b"], pk["hv0"], pk["layers"]
     L = len(layers)
     dev = emb_wt.device
     offs, total = _lib.param_layout(A, Cn, Na)

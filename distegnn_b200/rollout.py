@@ -40,7 +40,7 @@ from typing import List, Optional
 import torch
 
 from . import _lib
-from .fast_egnn import FastEGNN
+from .fast_egnn import FastEGNN, _backward_saved, _detached, device_guard
 from .partition import _check_rate
 from .shards import CSRGraph
 
@@ -168,8 +168,8 @@ def _check_targets(targets, steps: int, node_loc: Tensor, chamfer: bool = False)
 class _Rollout:
     """State buffers at fixed addresses + the per-step enqueue (eager or CUDA-graph replay)."""
 
-    def __init__(self, m: FastEGNN, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius,
-                 graph, loop, tau, speed_col, return_trajectory, cutoff_rate=0.0, targets=None, chamfer=False):
+    def __init__(self, m: FastEGNN, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, *, steps,
+                 radius, graph, loop, tau, speed_col, cutoff_rate, return_trajectory=False, targets=None, chamfer=False):
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).clone().contiguous()
         self.m, self.be, self.dev = m, be, dev
         self.N, self.B = int(node_loc.shape[0]), int(loc_mean.shape[0])
@@ -200,24 +200,29 @@ class _Rollout:
         self.graphed = (m.cuda_graph and (m.world_size == 1 or self.comm is not None) and m._backend is None
                         and dev.type == "cuda" and m._timing is None)
         self.cuda_graph, self.graph_launches, self.replays = None, 0, 0
-        self.bufs, self.capacity = None, None
         self.keep = None                                       # differentiable_rollout: per-step state for the backward
         self.rate = float(cutoff_rate)
-        self.cut, self.cand = None, None                       # cutoff: kept-edge buffers, the candidate graph
-        if graph is not None:                                  # fixed graph: only edge_attr changes
+        # the step graph: radius mode rebuilds it into `bufs` (sized by set_capacity), a fixed graph only gets its edge
+        # lengths; with a cutoff either one is the candidate set `cand` and the model runs on the kept edges in `cut`
+        self.bufs = self.capacity = self.overflow = self.cand = self.cut = None
+        if graph is not None:
             graph.validate(dev)
-            self.rowptr, self.row, self.col = graph.rowptr.contiguous(), graph.rows().contiguous(), graph.col.contiguous()
-            self.E = graph.num_edges
-            self.nE = graph.n_edges_dev
-            self.edge_count = self.nE if self.nE is not None else \
-                torch.full((1,), self.E, dtype=torch.int32, device=dev)
-            self.overflow = None
-            self.ea = torch.empty(self.E, self.A, dtype=torch.float32, device=dev) if self.A > 0 and not self.rate else None
-            if self.rate > 0:                                  # the caller's graph is the candidate set
-                self.cand = graph
-                self._cut_buffers()
+            self._use_graph(graph, torch.empty(graph.num_edges, self.A, dtype=torch.float32, device=dev)
+                            if self.A > 0 and not self.rate else None)
 
-    # ---- graph buffers (radius mode) ----------------------------------------------------------------------------------
+    # ---- the step graph -----------------------------------------------------------------------------------------------
+    def _use_graph(self, g: CSRGraph, ea: Optional[Tensor]) -> None:
+        """Run the model on `g` with edge_attr `ea`, or with a cutoff on the kept edges of `g`, in buffers of as many
+        entries.  Sets the model's graph arguments, the edge capacity E and the edge count the advance records."""
+        if self.rate > 0:
+            self.cand, self.cut = g, self.be.graph_buffers(self.N, g.num_edges, self.A, self.dev)
+            g, ea = self.cut.graph, self.cut.edge_attr
+        self.graph, self.E = g, g.num_edges
+        self.graph_args = dict(rowptr=g.rowptr.contiguous(), row=g.rows().contiguous(), col=g.col.contiguous(), ea=ea,
+                               nE=g.n_edges_dev)
+        self.edge_count = g.n_edges_dev if g.n_edges_dev is not None else \
+            torch.full((1,), self.E, dtype=torch.int32, device=self.dev)
+
     def exact_capacity(self) -> int:
         """Count the edges of step 0's graph (one host read): the initial capacity is GROWTH x that."""
         probe = self.be.graph_buffers(self.N, 0, self.A, self.dev)
@@ -225,32 +230,36 @@ class _Rollout:
         return max(1, math.ceil(GROWTH * int(probe.info[0].item())))
 
     def set_capacity(self, cap: int) -> None:
+        """(Re)allocate the radius mode's graph buffers for `cap` edges."""
         self.capacity = int(cap)
         # with a cutoff the radius graph is only the candidate set: no edge_attr (the cutoff writes the kept lengths)
         self.bufs = self.be.graph_buffers(self.N, self.capacity, 0 if self.rate > 0 else self.A, self.dev)
-        g = self.bufs.graph
-        self.rowptr, self.row, self.col, self.ea = g.rowptr, g.row, g.col, self.bufs.edge_attr
-        self.E, self.nE = self.capacity, g.n_edges_dev
-        self.edge_count, self.overflow = self.bufs.info[0:1], self.bufs.info[1:2]
-        if self.rate > 0:
-            self.cand = g
-            self._cut_buffers()
+        self.overflow = self.bufs.info[1:2]
+        self._use_graph(self.bufs.graph, self.bufs.edge_attr)
         if self.m.deterministic:                               # sized here: the next step may be captured straight away
             self.m._det_workspace(self.ws, self.dev, self.N, self.E)
         self.cuda_graph = None                                 # captured addresses are stale
 
-    def _cut_buffers(self) -> None:
-        """Buffers of the kept edges (as many entries as the candidates): the model runs on them, and the advance records
-        their count."""
-        self.cut = self.be.graph_buffers(self.N, self.E, self.A, self.dev)
-        g = self.cut.graph
-        self.rowptr, self.row, self.col, self.ea, self.nE = g.rowptr, g.row, g.col, self.cut.edge_attr, g.n_edges_dev
-        self.edge_count = self.cut.info[0:1]
+    def graph_at(self, x: Tensor) -> None:
+        """Enqueue the step graph for positions x: the radius build, or the fixed graph's edge lengths; then the cutoff's
+        kept edges, with counter[6] the largest candidate count (regrowth)."""
+        a = self.graph_args
+        if self.bufs is not None:
+            self.be.radius_graph_into(self.bufs, x, self.radius, self._gbatch(), self.B, self.loop)
+        elif a["ea"] is not None and self.cut is None:
+            self.be.edge_lengths(a["row"], a["col"], x, a["nE"], a["ea"])
+        if self.cut is not None:
+            self.be.cutoff_into(self.cut, self.cand, x, self.rate, self._gbatch(), self.B)
+            torch.maximum(self.counter[6:7], self.cut.info[2:3], out=self.counter[6:7])
 
-    def cut_graph(self, x: Tensor) -> None:
-        """The kept edges of the candidates at positions x; counter[6] keeps the largest candidate count (regrowth)."""
-        self.be.cutoff_into(self.cut, self.cand, x, self.rate, self._gbatch(), self.B)
-        torch.maximum(self.counter[6:7], self.cut.info[2:3], out=self.counter[6:7])
+    def model_args(self, feat: Tensor, x: Tensor, vel: Tensor) -> dict:
+        """The model's kernel arguments for one step from state (feat, x, vel) on the step graph."""
+        return dict(node_feat=feat, node_loc=x, node_vel=vel, loc_mean=self.loc_mean0, attr=self.attr,
+                    data_batch=self.batch, **self.graph_args)
+
+    @property
+    def dims(self):
+        return self.N, self.E, self.B, self.K
 
     def _gbatch(self) -> Optional[Tensor]:
         return self.batch if self.B > 1 else None
@@ -271,15 +280,9 @@ class _Rollout:
             self.keep["vel"].index_copy_(0, idx, self.vel.unsqueeze(0))
             if self.keep["speed"] is not None:
                 self.keep["speed"].index_copy_(0, idx, self.feat[:, self.speed_col].unsqueeze(0))
-        if self.bufs is not None:
-            be.radius_graph_into(self.bufs, self.loc, self.radius, self._gbatch(), self.B, self.loop)
-        elif self.ea is not None and self.cut is None:
-            be.edge_lengths(self.row, self.col, self.loc, self.nE, self.ea)
-        if self.cut is not None:
-            self.cut_graph(self.loc)
-        args = dict(node_feat=self.feat, node_loc=self.loc, node_vel=self.vel, loc_mean=self.loc_mean0, attr=self.attr,
-                    data_batch=self.batch, rowptr=self.rowptr, row=self.row, col=self.col, ea=self.ea, nE=self.nE)
-        m._run(be, self.pk, (self.N, self.E, self.B, self.K), args, self.ws, self.comm, init_centroid=init_centroid)
+        self.graph_at(self.loc)
+        m._forward(be, self.pk, self.dims, self.model_args(self.feat, self.loc, self.vel), self.ws,
+                   init_centroid=init_centroid)
         if self.keep is not None:
             self.keep["Xv"].index_copy_(0, idx, self.ws["Xv"].unsqueeze(0))
         if self.targets is not None:                           # reads the step counter before the advance moves it
@@ -362,6 +365,17 @@ class _Rollout:
             out.update(chamfer=self.chamfer, chamfer_mse=self.chamfer.sum(1) / denom)
         return out
 
+    def run(self, capacity: Optional[int], check_every: Optional[int]) -> None:
+        """Every step with the overflow policy of the module docstring, then the final centroid."""
+        self.regrowths = _drive(self, capacity, check_every)
+        self.loc_mean = self.finish()
+
+    def result(self, **fields) -> RolloutResult:
+        return RolloutResult(node_loc=self.loc, node_vel=self.vel, node_feat=self.feat, loc_mean=self.loc_mean,
+                             virtual_loc=self.ws["Xv"].clone(), n_edges=self.n_edges, capacity=self.capacity,
+                             regrowths=self.regrowths, replays=self.replays, status=self.counter, graph=self.graph,
+                             edge_attr=self.graph_args["ea"], **fields)
+
 
 def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_mean: Tensor, data_batch: Tensor,
             node_attr: Optional[Tensor] = None, *, steps: int, radius: Optional[float] = None,
@@ -394,29 +408,24 @@ def rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel: Tensor, loc_me
     [steps,2] (normalised like `mse`, and never above it) hold it.  With several ranks each rank's partition-local sums
     are added in the end-of-rollout all-reduce: the result lies between the whole-cloud Chamfer sum and sq_err.  The
     trajectory, sq_err and mse do not change with it."""
-    m = _unwrap(model)
-    _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
-              capacity, check_every, cutoff_rate)
     _check_targets(targets, steps, node_loc, chamfer)
-    dev = node_loc.device
-    be = m._get_backend(dev)                                    # raises on a CPU tensor (no CPU path)
-    import contextlib
-    guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
-    with guard, torch.no_grad():
-        r = _Rollout(m, be, dev, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph,
-                     loop, tau, speed_col, return_trajectory, cutoff_rate, targets, chamfer)
-        grown = _drive(r, capacity, check_every)
-        loc_mean_out = r.finish()
-        return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=loc_mean_out,
-                             virtual_loc=r.ws["Xv"].clone(), trajectory=r.traj, n_edges=r.n_edges, capacity=r.capacity,
-                             regrowths=grown, replays=r.replays, status=r.counter,
-                             graph=_result_graph(r), edge_attr=r.ea, **r.errors())
+    opts = dict(steps=steps, radius=radius, graph=graph, loop=loop, tau=tau, speed_col=speed_col, cutoff_rate=cutoff_rate)
+    state = (node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr)
+    m, be = _setup(model, state, opts, capacity, check_every)
+    with device_guard(node_loc.device), torch.no_grad():
+        r = _Rollout(m, be, node_loc.device, *state, **opts, return_trajectory=return_trajectory, targets=targets,
+                     chamfer=chamfer)
+        r.run(capacity, check_every)
+        return r.result(trajectory=r.traj, **r.errors())
 
 
-def _result_graph(r: _Rollout) -> CSRGraph:
-    if r.cut is not None:
-        return r.cut.graph
-    return r.bufs.graph if r.bufs is not None else CSRGraph(r.rowptr, r.col, r.row)
+def _setup(model, state, opts, capacity, check_every):
+    """(the FastEGNN, its backend) of a rollout, after every argument check: nothing is enqueued before."""
+    m = _unwrap(model)
+    o = opts
+    _validate(m, *state, o["steps"], o["radius"], o["graph"], o["tau"], o["speed_col"], capacity, check_every,
+              o["cutoff_rate"])
+    return m, m._get_backend(state[1].device)                 # raises on a CPU tensor (no CPU path)
 
 
 def _drive(r: _Rollout, capacity: Optional[int], check_every: Optional[int]) -> List[int]:
@@ -478,57 +487,40 @@ def differentiable_rollout(model, node_feat: Tensor, node_loc: Tensor, node_vel:
     and then backward on its own partition.  The state gradients are exact on every rank (every cross-rank term goes
     through the model's packed exchanges).  The parameter gradients are this rank's contribution only — DDP's reducer does
     not see this call — so sum them over the ranks yourself, e.g. `dist.all_reduce(p.grad)` for every parameter."""
-    m = _unwrap(model)
-    _validate(m, node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr, steps, radius, graph, tau, speed_col,
-              capacity, check_every, cutoff_rate)
+    opts = dict(steps=steps, radius=radius, graph=graph, loop=loop, tau=tau, speed_col=speed_col, cutoff_rate=cutoff_rate)
+    state = (node_feat, node_loc, node_vel, loc_mean, data_batch, node_attr)
+    m, be = _setup(model, state, opts, capacity, check_every)
     dev = node_loc.device
-    be = m._get_backend(dev)
-    import contextlib
-    guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
-    with guard:
-        emb_wt, emb_b, hv0, lps = m._differentiable_params(dev)
-        out = {}
-        opts = dict(data_batch=data_batch, steps=steps, radius=radius, graph=graph, loop=loop, tau=tau,
-                    speed_col=speed_col, capacity=capacity, check_every=check_every, cutoff_rate=cutoff_rate)
-        traj, vlocs = _RolloutFunction.apply(out, m, be, opts, emb_wt, emb_b, hv0, *lps, node_feat, node_loc, node_vel,
-                                             loc_mean, node_attr)
-    r = out["r"]
-    return RolloutResult(node_loc=r.loc, node_vel=r.vel, node_feat=r.feat, loc_mean=out["loc_mean"],
-                         virtual_loc=r.ws["Xv"].clone(), trajectory=traj, n_edges=r.n_edges, capacity=r.capacity,
-                         regrowths=out["grown"], replays=r.replays, status=r.counter,
-                         graph=_result_graph(r), edge_attr=r.ea, virtual_locs=vlocs)
+    with device_guard(dev):
+        r = _Rollout(m, be, dev, *state, **opts, return_trajectory=True)
+        pk = m._pack_params(dev)
+        traj, vlocs = _RolloutFunction.apply(r, capacity, check_every, pk["emb_wt"], pk["emb_b"], pk["hv0"], *pk["layers"],
+                                             node_feat, node_loc, node_vel, loc_mean, node_attr)
+    return r.result(trajectory=traj, virtual_locs=vlocs)
 
 
 class _RolloutFunction(torch.autograd.Function):
-    """Autograd node of `differentiable_rollout`: inputs (packed parameters, then node_feat, node_loc, node_vel,
-    loc_mean, node_attr), outputs (trajectory, virtual_locs).  See DESIGN §15."""
+    """Autograd node of `differentiable_rollout`: inputs (the `_Rollout`, capacity, check_every, the packed parameters,
+    then node_feat, node_loc, node_vel, loc_mean, node_attr), outputs (trajectory, virtual_locs).  See DESIGN §15."""
 
     @staticmethod
-    def forward(ctx, out, m, be, opts, emb_wt, emb_b, hv0, *rest):
-        L = m.n_layers
-        node_feat, node_loc, node_vel, loc_mean, node_attr = rest[L:]
-        o = opts
-        r = _Rollout(m, be, node_loc.device, node_feat, node_loc, node_vel, loc_mean, o["data_batch"], node_attr,
-                     o["steps"], o["radius"], o["graph"], o["loop"], o["tau"], o["speed_col"], True, o["cutoff_rate"])
+    def forward(ctx, r, capacity, check_every, emb_wt, emb_b, hv0, *rest):
+        L = r.m.n_layers
         r.keep_steps()
-        out["grown"] = _drive(r, o["capacity"], o["check_every"])
-        out["loc_mean"], out["r"] = r.finish(), r
-        ctx.r = r
-        ctx.params = (emb_wt.detach().contiguous(), emb_b.detach().contiguous(), hv0.detach().contiguous(),
-                      [lp.detach().contiguous() for lp in rest[:L]])
+        r.run(capacity, check_every)
+        ctx.r, ctx.pk = r, _detached(emb_wt, emb_b, hv0, rest[:L])
         ctx.inputs = [None if t is None else t.dtype for t in rest[L:]]
         ctx.save_for_backward(r.traj)                          # an in-place change of the trajectory is caught
         return r.traj, r.keep["Xv"]
 
     @staticmethod
     def backward(ctx, g_traj, g_vlocs):
-        from .fast_egnn import _backward_saved
         r = ctx.r
         (traj,) = ctx.saved_tensors
         m, be, dev = r.m, r.be, r.dev
-        emb_wt, emb_b, hv0, layers = ctx.params
+        emb_wt, emb_b, hv0, layers = ctx.pk["emb_wt"], ctx.pk["emb_b"], ctx.pk["hv0"], ctx.pk["layers"]
         L, N, B, Cn, Na, A = len(layers), r.N, r.B, m.virtual_channels, m.node_attr_nf, r.A
-        w_feat, w_loc, w_vel, w_lm, w_attr = ctx.needs_input_grad[7 + L:7 + L + 5]
+        w_feat, w_loc, w_vel, w_lm, w_attr = ctx.needs_input_grad[6 + L:6 + L + 5]
         sc = r.speed_col
         zeros = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         g_traj = g_traj.contiguous().float() if g_traj is not None else zeros(r.steps, N, 3)
@@ -538,30 +530,22 @@ class _RolloutFunction(torch.autograd.Function):
         g_attr_sum = zeros(N, Na) if (w_attr and Na > 0) else None
         g_x_next = g_v_next = g_f_next = g_lm = None
         feat_t = r.keep["feat0"].clone()
-        import contextlib
-        guard = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
-        with guard, torch.no_grad():
+        with device_guard(dev), torch.no_grad():
             for t in reversed(range(r.steps)):
                 mark = _marker(t)
                 mark("rebuild")
                 x_t = r.keep["x0"] if t == 0 else traj[t - 1]
                 # 1. step t's graph from x_t: rebuilt (deterministic: the forward's graph) or the kept one's lengths
-                if r.bufs is not None:
-                    be.radius_graph_into(r.bufs, x_t, r.radius, r._gbatch(), r.B, r.loop)
-                elif r.ea is not None and r.cut is None:
-                    be.edge_lengths(r.row, r.col, x_t, r.nE, r.ea)
-                if r.cut is not None:                          # the kept edges, re-selected from x_t
-                    r.cut_graph(x_t)
+                #    (with a cutoff, the kept edges re-selected from x_t)
+                r.graph_at(x_t)
                 if r.bufs is not None or r.cut is not None:    # the edge count the model ran on, against the forward's
                     r.counter[5:6] += (r.edge_count != r.n_edges[t:t + 1]).to(torch.int32)
                 # 2. step t's forward again, with its activations
                 if sc is not None:
                     feat_t[:, sc] = r.keep["speed"][t]
-                a = dict(node_feat=feat_t, node_loc=x_t, node_vel=r.keep["vel"][t], loc_mean=r.loc_mean0, attr=r.attr,
-                         data_batch=r.batch, rowptr=r.rowptr, row=r.row, col=r.col, ea=r.ea, nE=r.nE)
-                dims = (N, r.E, B, r.K)
+                a = r.model_args(feat_t, x_t, r.keep["vel"][t])
                 mark("recompute")
-                _, _, st = m._run_saving(be, dims, a, emb_wt, emb_b, hv0, layers, init_centroid=t > 0)
+                _, _, st = m._forward(be, ctx.pk, r.dims, a, init_centroid=t > 0)
                 # 3. the advance: upstream of the prediction x_{t+1}, and its −g_v/tau share of g_x_t
                 mark("advance_bwd")
                 g_pred, g_x = torch.empty(N, 3, device=dev), torch.empty(N, 3, device=dev)
@@ -573,9 +557,9 @@ class _RolloutFunction(torch.autograd.Function):
                 first = t == 0
                 want = (w_feat or (not first and sc is not None), w_loc or not first, w_vel or not first,
                         first and w_lm, A > 0 and (w_loc or not first), w_attr)
-                ge, gb, gh, glps, g_in = _backward_saved(m, be, dims, a, st, ctx.params, g_pred, g_vlocs[t], want,
+                ge, gb, gh, glps, g_in = _backward_saved(m, be, r.dims, a, st, ctx.pk, g_pred, g_vlocs[t], want,
                                                          init_centroid=not first)
-                del st, a
+                del st
                 g_emb_wt += ge
                 g_emb_b += gb
                 g_hv0 += gh
@@ -589,8 +573,8 @@ class _RolloutFunction(torch.autograd.Function):
                     g_x += g_loc
                 mark("edge_lengths_bwd")
                 if g_ea is not None:
-                    be.edge_lengths_bwd(r.row, r.col, x_t, r.nE, g_ea, g_x)
-                del g_ea
+                    be.edge_lengths_bwd(a["row"], a["col"], x_t, a["nE"], g_ea, g_x)
+                del g_ea, a
                 mark("end")
                 if g_feat is not None and g_f_next is not None:
                     g_feat += g_f_next                         # columns other than speed_col pass straight through
@@ -606,7 +590,7 @@ class _RolloutFunction(torch.autograd.Function):
                 outs.append(None)
             else:
                 outs.append(torch.zeros(shape, dtype=dtype, device=dev) if g is None else g.to(dtype))
-        return (None, None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps, *outs)
+        return (None, None, None, g_emb_wt, g_emb_b, g_hv0, *g_lps, *outs)
 
 
 def _marker(step: int):

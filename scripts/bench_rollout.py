@@ -104,17 +104,16 @@ def main():
     be = model._get_backend(dev)
     with torch.no_grad():
         ro = _Rollout(model, be, dev, node["node_feat"], node["node_loc"], node["node_vel"], node["loc_mean"],
-                      node["data_batch"], node["node_attr"], K, r, None, False, 1.0, 0, False)
+                      node["data_batch"], node["node_attr"], steps=K, radius=r, graph=None, loop=False, tau=1.0,
+                      speed_col=0, cutoff_rate=0.0)
         ro.set_capacity(cap["c"])
         comp = {"graph_build": [], "forward": [], "advance": []}
         for s in range(K):
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
             ev[0].record()
-            be.radius_graph_into(ro.bufs, ro.loc, r, None, 1, False)
+            ro.graph_at(ro.loc)
             ev[1].record()
-            args_ = dict(node_feat=ro.feat, node_loc=ro.loc, node_vel=ro.vel, loc_mean=ro.loc_mean0, attr=ro.attr,
-                         data_batch=ro.batch, rowptr=ro.rowptr, row=ro.row, col=ro.col, ea=ro.ea, nE=ro.nE)
-            model._run(be, ro.pk, (ro.N, ro.E, ro.B, ro.K), args_, ro.ws, None, init_centroid=s > 0)
+            model._forward(be, ro.pk, ro.dims, ro.model_args(ro.feat, ro.loc, ro.vel), ro.ws, init_centroid=s > 0)
             ev[2].record()
             be.rollout_advance(0, 1.0, ro.ws["out"], ro.loc, ro.vel, ro.feat, None, ro.edge_count, ro.overflow,
                                ro.n_edges, ro.counter)

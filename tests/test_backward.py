@@ -1,6 +1,6 @@
 """Backward pass (SURVEY §8 f-1) on CPU: (1) the oracle's autograd is pinned to gradient fixtures produced by the
 unmodified reference under autograd (oracle/make_golden_grads.py); (2) the product's host-side backward orchestration
-(FastEGNN._forward_autograd / _FastEGNNFunction: per-layer chain, packed gradient all-reduce, dense stages, parameter
+(FastEGNN._forward / _FastEGNNFunction: per-layer chain, packed gradient all-reduce, dense stages, parameter
 unpacking) reproduces those gradients with the kernels replaced by the torch stand-in; (3) the same under gloo with
 world_size=2 against the reference's own 2-rank backward."""
 import os
