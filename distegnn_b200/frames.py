@@ -28,6 +28,17 @@ every graph (:103, `cutoff_edges_csr`).  `edge_attr` is the length in every colu
 Input layout.  N-body: the reference's own `loc_*.npy`, `vel_*.npy` [S,T,n,3] and `charges_*.npy` [S,n,1].  Water-3D and
 Fluid113K: one `.npz` per scene holding `position` [T,n,3], optionally `velocity` [T,n,3], and the static fields
 (`particle_type` [n], or `viscosity` and `mass` [n]).  Uncompressed `.npz` members (np.savez) are memory-mapped.
+
+Training noise (DESIGN §22).  `FrameLoader(..., noise=(σ_x, σ_v))` trains on a perturbed input state, so that the model
+sees inputs like the slightly wrong ones it feeds itself in a rollout (GNS's input noise):
+
+    train = FrameLoader(traj, samples, ..., shuffle=True, noise=(3e-4, 3e-4))            # clean valid loader: no noise
+
+Every node gets x + ε_x, v + ε_v (‖v‖ of the noisy v) and every target row + ε_x, so the displacement to learn stays the
+recorded one; loc_mean is the whole-scene mean of the noisy positions and the graph is built on them.  The split is the
+clean frame's.  ε is a pure function of (noise_seed, epoch, sample index, scene node), generated inside the assembly
+kernels: every rank, world size, batch size and order sees the same noise for the same node.  The epoch is the number of
+earlier `batches()` calls (every iteration draws one).
 """
 from __future__ import annotations
 
@@ -229,6 +240,21 @@ def check_samples(traj: Trajectories, samples: Sequence[Tuple[int, int]], delta_
                              f"(delta_t={delta_t}){more}")
 
 
+def _check_noise(noise) -> Optional[Tuple[float, float]]:
+    """FrameLoader's `noise` as (σ_x, σ_v) floats, or None for no noise (None or (0, 0)); ValueError otherwise."""
+    if noise is None:
+        return None
+    if isinstance(noise, (str, bytes)):
+        raise ValueError(f"noise must be (sigma_x, sigma_v) or None (got {noise!r})")
+    try:
+        sx, sv = (float(v) for v in noise)
+    except (TypeError, ValueError):
+        raise ValueError(f"noise must be (sigma_x, sigma_v) or None (got {noise!r})") from None
+    if not (np.isfinite(sx) and np.isfinite(sv) and sx >= 0 and sv >= 0):
+        raise ValueError(f"noise sigmas must be finite and >= 0 (got {noise!r})")
+    return None if sx == 0 and sv == 0 else (sx, sv)
+
+
 def complete_graph_edges(n: int) -> Tensor:
     """The reference's fully connected edge list (process_dataset.py:98): [[i, j] for i for j if i != j], int64 [2,E]."""
     i = torch.arange(n).repeat_interleave(max(n - 1, 0))
@@ -252,13 +278,17 @@ class FrameLoader:
     horizon         K >= 1 target frames per sample: extras["targets"] float32 [K,M,3] holds this rank's nodes at frames
                     f + tΔ, t = 1..K (targets[0] is extras["target"] itself), for `rollout(targets=...)` or a loss on a
                     differentiable rollout.  2 + K frames per sample are staged; K = 1 stages and launches as without it
+    noise           (σ_x, σ_v), finite and >= 0: training noise on positions (and every target row) and velocities (module
+                    docstring, DESIGN §22).  None or (0, 0): no noise, the same launches as without the argument
+    noise_seed      the noise's seed, an int in [0, 2^64) (default `seed`)
     """
 
     def __init__(self, traj: Trajectories, samples: Sequence[Tuple[int, int]], delta_t: int = 1,
                  radius: Optional[float] = None, batch_size: int = 1, shuffle: bool = False, seed: int = 0,
                  drop_last: bool = True, device=None, prefetch: int = 2, world_size: int = 1, rank: int = 0,
                  split_mode: str = "random", split_seed: Optional[int] = None, cutoff_rate: float = 0.0,
-                 capacity: Optional[int] = None, edge_attr_nf: int = 2, loop: bool = False, horizon: int = 1):
+                 capacity: Optional[int] = None, edge_attr_nf: int = 2, loop: bool = False, horizon: int = 1,
+                 noise: Optional[Tuple[float, float]] = None, noise_seed: Optional[int] = None):
         self.traj, self.samples, self.delta_t = traj, [(int(s), int(f)) for s, f in samples], int(delta_t)
         check_samples(traj, self.samples, self.delta_t, horizon)
         self.horizon = horizon
@@ -278,13 +308,24 @@ class FrameLoader:
         self._kmeans: Dict[int, Tuple[Tensor, List[int]]] = {}
         self._complete: Dict[Tuple[int, ...], CSRGraph] = {}
         self._overflow: Optional[Tensor] = None
+        self.noise = _check_noise(noise)
+        self.noise_seed = int(seed if noise_seed is None else noise_seed)
+        if self.noise is not None:
+            if not 0 <= self.noise_seed < 1 << 64:
+                raise ValueError(f"noise_seed must be an int in [0, 2^64) (got {self.noise_seed})")
+            if len(self.samples) >= 1 << 32:
+                raise ValueError(f"training noise numbers samples with 32 bits: {len(self.samples)} samples are too many")
+        self.epoch = 0
 
     def __len__(self) -> int:
         return n_batches(len(self.samples), self.batch_size, self.drop_last)
 
     def batches(self) -> List[List[int]]:
-        """The next epoch's batches of sample indices (advances the sampler's generator, as iterating does)."""
-        return sampler_batches(len(self.samples), self.batch_size, self.shuffle, self.generator, self.drop_last)
+        """The next epoch's batches of sample indices (advances the sampler's generator and `epoch`, as iterating
+        does)."""
+        out = sampler_batches(len(self.samples), self.batch_size, self.shuffle, self.generator, self.drop_last)
+        self.epoch += 1
+        return out
 
     # ---- partitions ----------------------------------------------------------------------------------------------
     def sample_generator(self, i: int) -> torch.Generator:
@@ -320,7 +361,7 @@ class FrameLoader:
                              f"leaves a rank without nodes ({counts}); every graph needs nodes on every rank")
 
     # ---- staging (host) ------------------------------------------------------------------------------------------
-    def _host_batch(self, idx: Sequence[int]) -> Dict[str, object]:
+    def _host_batch(self, idx: Sequence[int], epoch: int = 0) -> Dict[str, object]:
         rc = self.traj.recipe
         pin = self.device is not None and self.device.type == "cuda"
         scenes = [self.traj.scenes[self.samples[i][0]] for i in idx]
@@ -342,10 +383,13 @@ class FrameLoader:
             counts.append(cnt[self.rank])
             off += n
         B = len(idx)
-        meta = torch.empty(2 * B + 2, dtype=torch.int64, pin_memory=pin)
+        noisy = self.noise is not None
+        meta = torch.empty(2 * B + 2 + (B if noisy else 0), dtype=torch.int64, pin_memory=pin)
         meta[:B + 1] = torch.tensor([0] + list(np.cumsum(ns)), dtype=torch.int64)
-        meta[B + 1:] = torch.tensor([0] + list(np.cumsum(counts)), dtype=torch.int64)
-        host = dict(frames=frames, statics=statics, meta=meta, n_frame=N, node_counts=counts)
+        meta[B + 1:2 * B + 2] = torch.tensor([0] + list(np.cumsum(counts)), dtype=torch.int64)
+        if noisy:                                                # the samples' indices: the noise's sample numbers
+            meta[2 * B + 2:] = torch.tensor(list(idx), dtype=torch.int64)
+        host = dict(frames=frames, statics=statics, meta=meta, n_frame=N, node_counts=counts, epoch=epoch)
         if self.world_size > 1:
             index = torch.empty(sum(counts), dtype=torch.int32, pin_memory=pin)
             torch.cat(parts, out=index)
@@ -384,15 +428,23 @@ class FrameLoader:
         target = targets[0]
         batch = torch.empty(M, dtype=torch.int64, device=dev)
         loc_mean, scene_max = torch.empty(B, 3, **f32), torch.empty(B, **f32)
+        scene_ptr, out_ptr = meta[:B + 1], meta[B + 1:2 * B + 2]
         with torch.cuda.device(dev):
-            check(_lib.load().distegnn_frames_assemble(
-                rc.code, B, host["n_frame"], M, ptr(frames), ptr(statics), ptr(meta[:B + 1]), ptr(meta[B + 1:]),
-                ptr(index), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(target), ptr(batch), ptr(loc_mean),
-                ptr(scene_max), _lib.stream_ptr(dev)), "frames_assemble")
-            if K > 1:
-                check(_lib.load().distegnn_frames_targets(B, host["n_frame"], M, K, ptr(frames), ptr(meta[:B + 1]),
-                                                          ptr(meta[B + 1:]), ptr(index), ptr(targets),
-                                                          _lib.stream_ptr(dev)), "frames_targets")
+            if self.noise is not None:
+                check(_lib.load().distegnn_frames_assemble_noise(
+                    rc.code, B, host["n_frame"], M, K, ptr(frames), ptr(statics), ptr(scene_ptr), ptr(out_ptr),
+                    ptr(index), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(targets), ptr(batch), ptr(loc_mean),
+                    ptr(scene_max), ptr(meta[2 * B + 2:]), self.noise_seed, host["epoch"] % (1 << 32), self.noise[0],
+                    self.noise[1], _lib.stream_ptr(dev)), "frames_assemble_noise")
+            else:
+                check(_lib.load().distegnn_frames_assemble(
+                    rc.code, B, host["n_frame"], M, ptr(frames), ptr(statics), ptr(scene_ptr), ptr(out_ptr),
+                    ptr(index), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(target), ptr(batch), ptr(loc_mean),
+                    ptr(scene_max), _lib.stream_ptr(dev)), "frames_assemble")
+                if K > 1:
+                    check(_lib.load().distegnn_frames_targets(B, host["n_frame"], M, K, ptr(frames), ptr(scene_ptr),
+                                                              ptr(out_ptr), ptr(index), ptr(targets),
+                                                              _lib.stream_ptr(dev)), "frames_targets")
         graph, edge_attr = self._graph(loc, batch, tuple(counts))
         kwargs = dict(node_feat=feat, node_loc=loc, node_vel=vel, loc_mean=loc_mean, edge_index=graph,
                       data_batch=batch, edge_attr=edge_attr, node_attr=attr)
@@ -428,7 +480,9 @@ class FrameLoader:
     def __iter__(self):
         if self.device is None or self.device.type != "cuda":
             raise _lib.DistEGNNError("FrameLoader assembles batches on a CUDA device (no CPU path)")
-        yield from staged(self.batches(), self._host_batch, self._to_device, self.device, self.prefetch)
+        epoch = self.epoch                                       # this epoch's number, fixed before the order is drawn
+        yield from staged(self.batches(), lambda idx: self._host_batch(idx, epoch), self._to_device, self.device,
+                          self.prefetch)
 
     def check(self) -> None:
         """Capacity mode: raise if any batch's graph outgrew `capacity` since the last check (one host read)."""

@@ -599,6 +599,26 @@ DISTEGNN_API int distegnn_frames_assemble(int recipe, int n_samples, int64_t n_f
 DISTEGNN_API int distegnn_frames_targets(int n_samples, int64_t n_frame_nodes, int64_t n_out, int horizon,
                                          const float *frames, const int64_t *scene_ptr, const int64_t *out_ptr,
                                          const int32_t *index, float *targets, void *stream);
+/* distegnn_frames_assemble_noise: the assembly and its multi-step targets with training noise (DESIGN §22).  Arguments as
+ * for distegnn_frames_assemble and distegnn_frames_targets (frames float32 [2 + horizon, n_frame_nodes, 3]; targets
+ * float32 [horizon, n_out, 3], row 0 the target), and sample_ids int64 [n_samples] (device): each sample's index in the
+ * caller's sample list, the same on every rank.  For sample b = sample_ids[·], epoch e, seed s and scene node j, ε of
+ * stream q (0 position, 1 velocity) is σ_q·z with z the Box–Muller normal of Philox4x32-10(counter (j, q, b, e), key
+ * (lo32 s, hi32 s)) (csrc/frames_noise.cuh).  Then, each a single round-to-nearest fp32 add:
+ *   node_loc = x + ε_x,  node_vel = v + ε_v (v as without noise),  ‖v‖ of the noisy v,  targets[t] = recorded + ε_x
+ *   loc_mean = the fp64 fixed-order mean of x + ε_x over the WHOLE scene (every rank gets the same bits)
+ * node_attr, the static feature columns, scene_max and data_batch are as without noise.  A sample id outside [0, 2^32)
+ * gives NaN in every noisy value of that sample (the ids are device data; reading them here would synchronise).
+ * Rejects σ < 0 or not finite, a NULL sample_ids, horizon < 1 and the assembly's argument errors before any launch.
+ * Launches the scene, node and (horizon > 1) targets kernels; no workspace, no allocation, no host synchronisation;
+ * capturable. */
+DISTEGNN_API int distegnn_frames_assemble_noise(int recipe, int n_samples, int64_t n_frame_nodes, int64_t n_out,
+                                                int horizon, const float *frames, const float *statics,
+                                                const int64_t *scene_ptr, const int64_t *out_ptr, const int32_t *index,
+                                                float *node_feat, float *node_loc, float *node_vel, float *node_attr,
+                                                float *targets, int64_t *data_batch, float *loc_mean, float *scene_max,
+                                                const int64_t *sample_ids, uint64_t seed, uint32_t epoch,
+                                                float sigma_x, float sigma_v, void *stream);
 
 #ifdef __cplusplus
 }

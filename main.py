@@ -27,8 +27,9 @@ config's recipe (N-body, Water-3D, Fluid113K), radius / inner_radius, delta_t (N
 cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  With `--rollout_steps K`
 it then rolls the trained model out K steps from every validation batch and prints the per-step MSE against the recorded
 frames f + Δ .. f + KΔ (DESIGN §19; `--rollout_tau` sets the velocity's time step, Water-3D defaults to Δ);
-`--rollout_chamfer` adds both directions of the normalised Chamfer distance to every step's line (DESIGN §20).  Without the
-flag the synthetic path below runs unchanged.
+`--rollout_chamfer` adds both directions of the normalised Chamfer distance to every step's line (DESIGN §20).
+`--train_noise SX,SV` trains on noisy input states (FrameLoader's `noise`, DESIGN §22); the evaluation and the rollout stay
+noise-free.  Without the flag the synthetic path below runs unchanged.
 
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
 `batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
@@ -108,11 +109,37 @@ def parse():
     p.add_argument("--rollout_tau", type=float, default=None, help="(new) time step of a --trajectory rollout's "
                    "velocity v = (x' − x)/tau; default Δ for Water-3D (one-frame differences), required for N-body and "
                    "Fluid113K (physical velocities; the frame time is not in the files)")
+    p.add_argument("--train_noise", type=str, default=None, help="(new) with --trajectory: SX,SV, the standard deviations "
+                   "of the training noise on positions (and targets) and on velocities (FrameLoader's noise, DESIGN §22); "
+                   "the train loader only, the evaluation and the rollout stay noise-free")
     return p.parse_args()
+
+
+def train_noise_of(args):
+    """--train_noise SX,SV as (σ_x, σ_v), or None; exits with a message on a malformed or negative value."""
+    if args.train_noise is None:
+        return None
+    import math
+    msg = None
+    try:
+        sx, sv = (float(v) for v in args.train_noise.split(","))
+    except ValueError:
+        msg = "two comma-separated numbers SX,SV"
+    else:
+        if not (math.isfinite(sx) and math.isfinite(sv) and sx >= 0 and sv >= 0):
+            msg = "finite and >= 0"
+    if msg is None and not args.trajectory:
+        msg = "used with --trajectory"
+    if msg is not None:
+        if int(os.environ.get("LOCAL_RANK", "0")) == 0:
+            print(f"--train_noise {args.train_noise!r}: must be {msg}", flush=True)
+        sys.exit(2)
+    return sx, sv
 
 
 def main():
     args = parse()
+    noise = train_noise_of(args)
     with open(args.config_path) as f:
         cfg = yaml.safe_load(f)
     cfg.setdefault("data", {})
@@ -172,7 +199,7 @@ def main():
         model = DistributedDataParallel(model, device_ids=[local_rank], find_unused_parameters=True)
     model.eval()
     if args.trajectory:
-        trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate)
+        trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise)
         if distributed:
             dist.destroy_process_group()
         return
@@ -258,14 +285,15 @@ def recipe_of_config(cfg):
     return recipe, 0, int(d.get("delta_t", 1))
 
 
-def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("train", "valid")):
+def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("train", "valid"), noise=None):
     """FrameLoaders over the raw trajectories under `path` with the config's recipe (datasets/process_dataset.py):
     N-body (`dataset_name: nbody*`, the reference's loc_/vel_/charges_ .npy files, frame_0 / frame_T), Water-3D or
     Fluid113K (`path`/train/*.npz, `path`/valid/*.npz).  cutoff_edges mode: one graph per sample, radius = data.radius
     (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
     sample split over the ranks by split_mode (metis / spectral fall back to random), a radius graph per partition with
     inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
-    N-body frame_0 that cannot hold them exits with a message).  Returns (recipe name, {part: loader or None})."""
+    N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only.
+    Returns (recipe name, {part: loader or None})."""
     import glob
     from distegnn_b200.frames import FrameLoader, load_nbody, load_scenes, sample_list
     d = cfg["data"]
@@ -302,15 +330,16 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
         samples = sample_list(traj, seed=seed, max_samples=d.get("max_samples"), delta_t=delta, frame_0=frame_0, **kw)
         out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
                                 seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
-                                cutoff_rate=rate or 0.0, horizon=horizon)
+                                cutoff_rate=rate or 0.0, horizon=horizon, noise=noise if part == "train" else None)
     if "train" in parts and out["train"] is None:
         raise SystemExit(f"--trajectory {path}: no training data for recipe {recipe!r}")
     return recipe, out
 
 
-def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate):
+def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None):
     """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
-    reference's training step on batches from FrameLoader, then the mean MSE over the validation batches."""
+    reference's training step on batches from FrameLoader (with `noise` on its inputs), then the mean MSE over the
+    validation batches (noise-free)."""
     from distegnn_b200 import train_loss
     recipe, _, delta = recipe_of_config(cfg)
     K = args.rollout_steps
@@ -320,7 +349,8 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate):
             print(f"--rollout_steps with --trajectory on {recipe!r} needs --rollout_tau: its velocities are physical and "
                   "the frame time is not in the files (Water-3D defaults to delta_t)", flush=True)
         sys.exit(2)
-    recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, torch.device("cuda", local_rank), rate)
+    dev = torch.device("cuda", local_rank)
+    recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, noise=noise)
     tc = cfg.get("train", {}) or {}
     mmd = tc.get("mmd", {}) or {}
     lr = args.lr if args.lr is not None else float(tc.get("learning_rate", tc.get("lr", 5e-4)))
@@ -357,7 +387,10 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate):
     torch.cuda.synchronize()
     if local_rank == 0:
         print(f"[{recipe}] {steps} train steps on raw frames: {(time.perf_counter() - t0) / steps * 1e3:.2f} ms/step")
-    ev = loaders["valid"] or loaders["train"]
+    ev = loaders["valid"]
+    if not ev:                                                 # no valid split or no batch in it: the train split, clean
+        ev = loaders["train"] if noise is None else \
+            frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, parts=("train",))[1]["train"]
     model.eval()
     tot, n = 0.0, 0
     with torch.no_grad():

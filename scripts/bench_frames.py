@@ -15,6 +15,8 @@ Per size:
     node index list at 4 B per node of this rank) against a shard of the same sample (node arrays, CSR, edge_attr).
 (3) One training step (forward + fused loss + backward) fed by FrameLoader (prefetch 2) against one fed by ShardLoader
     (prefetch 2) over shards written from the loader's own batch: ms per step over `--steps` steps, after a warm-up epoch.
+(4) Training noise (DESIGN §22, σ = NOISE): the batch time in capacity mode with noise, and the noisy assembly
+    (distegnn_frames_assemble_noise, horizon 1) between CUDA events beside the assembly without noise.
 Reports the card name and power limit read in the same run.  Prints one JSON line; `--out` also writes it to a file.
 """
 from __future__ import annotations
@@ -43,6 +45,7 @@ from distegnn_b200.shards import write_shard  # noqa: E402
 from bench_rollout import power_limit_w  # noqa: E402
 
 T_FRAMES = 4
+NOISE = (3e-4, 3e-4)
 
 
 def stats(v):
@@ -146,6 +149,17 @@ def run_size(name, n, P, reps, steps, tmp, dev):
             ptr(batch), ptr(lm), ptr(smax), _lib.stream_ptr(dev)), "frames_assemble")
 
     t_asm = event_ms(assemble, reps)
+    noisy, _, _ = loader_batch_ms(lambda: FrameLoader(traj, one, capacity=cap, noise=NOISE, **kw_), reps)
+    ids = torch.zeros(1, dtype=torch.int64, device=dev)
+
+    def assemble_noise():
+        check(_lib.load().distegnn_frames_assemble_noise(
+            _lib.FRAMES_LARGEFLUID, 1, n, M, 1, ptr(host["frames"]), ptr(host["statics"]), ptr(host["meta"][:2]),
+            ptr(host["meta"][2:]), ptr(host.get("index")), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(target),
+            ptr(batch), ptr(lm), ptr(smax), ptr(ids), 0, 0, NOISE[0], NOISE[1], _lib.stream_ptr(dev)),
+            "frames_assemble_noise")
+
+    t_asm_noise = event_ms(assemble_noise, reps)
     t_graph = event_ms(lambda: radius_graph_csr(loc, w.radius, batch, capacity=cap, n_graphs=1), reps)
     staged = 3 * n * 3 * 4 + n * 2 * 4 + 4 * 8 + (4 * M if P > 1 else 0)
     arrays = shard_arrays(kw, ex)
@@ -159,7 +173,8 @@ def run_size(name, n, P, reps, steps, tmp, dev):
                                            rank=0, capacity=cap), steps)
     t_shard = train_ms(model, ShardLoader([spath] * steps, device=dev), steps)
     return dict(nodes_scene=n, world_size=P, nodes_rank=M, edges=E, capacity=cap,
-                batch_ms=dict(exact=exact, capacity=capm), assembly_kernel_ms=t_asm, radius_graph_ms=t_graph,
+                batch_ms=dict(exact=exact, capacity=capm, capacity_noise=noisy), assembly_kernel_ms=t_asm,
+                assembly_noise_kernel_ms=t_asm_noise, radius_graph_ms=t_graph,
                 pcie_bytes=dict(frames=staged, shard=shard_bytes, ratio=staged / shard_bytes),
                 train_step_ms=dict(frame_loader=t_frames, shard_loader=t_shard))
 
@@ -174,7 +189,8 @@ def main():
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     sizes = dict(fluid113k_p1=(113_140, 1), fluid113k_p2=(113_140, 2), config5=(1_000_000, 1))
-    res = dict(gpu=torch.cuda.get_device_name(dev), power_limit_w=power_limit_w(), reps=args.reps, steps=args.steps)
+    res = dict(gpu=torch.cuda.get_device_name(dev), power_limit_w=power_limit_w(), reps=args.reps, steps=args.steps,
+               noise=NOISE)
     tmp = tempfile.mkdtemp(prefix="bench_frames_")
     try:
         for name in args.sizes.split(","):
