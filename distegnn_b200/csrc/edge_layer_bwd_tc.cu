@@ -1,20 +1,21 @@
 // Backward of the real<->real edge stage on the tensor cores (wgmma) — production kernel behind
-// distegnn_edge_layer_bwd (the fp32-FMA kernel of edge_layer_bwd.cu is kept as distegnn_edge_layer_bwd_simt, its twin).
-// Same contract and math as edge_layer_bwd.cu (reference: autograd through models/FastEGNN.py:144-150, 169-177, 206,
-// 237-246, 322-337); what changes is where the six tile GEMMs of a 128-edge tile run:
+// distegnn_edge_layer_bwd.  Its twin, the fp32-FMA kernel of csrc/testing/edge_layer_bwd.cu behind
+// distegnn_edge_layer_bwd_simt, has the same contract and math (reference: autograd through models/FastEGNN.py:144-150,
+// 169-177, 206, 237-246, 322-337); what changes is where the six tile GEMMs of a 128-edge tile run:
 //   * the four ROW-WISE GEMMs (recompute z2 = a1·W2ᵀ, zc = m·Wcᵀ; data gradients g_m = g_zc·Wc, g_a1 = g_z2·W2) run as
 //     wgmma f16 with the fp16 2-term split of both operands (tc16.cuh), A written to tile memory by the thread that owns
 //     the row, B (W and Wᵀ, hi/lo) resident in shared memory, D read back row-per-thread;
 //   * the two WEIGHT-GRADIENT GEMMs (g_Wc += g_zcᵀ·m, g_W2 += g_z2ᵀ·a1; contraction over the 128 edges) stay on the CUDA
 //     cores for now: they need the operands edge-major ("MN-major"), which the K-major machinery of the forward kernels
 //     does not provide; they read the two fp32 row tiles the row threads leave in shared memory.
-// One CTA per SM, 128 threads = 1 tile group = 1 warpgroup; thread r owns edge r of the group's tile end to end and holds
-// a whole 64-wide row in registers.  Tile memory per group (tile_mma.cuh, 128 columns): A_hi 32 | A_lo 32 | z2 64, and
-// D overwrites the A operand it was computed from (every D row is read into registers before its thread writes the next
-// A).  z2 is parked in tile memory between the forward recompute and the SiLU' factors of the backward chain; z1 is
-// recomputed from P, Q and the edge geometry where it is needed again.
+// One CTA per SM, 128 threads = 1 warpgroup; thread r owns edge r of the tile end to end and holds a whole 64-wide row in
+// registers.  Tile memory (tile_mma.cuh, 128 columns): A_hi 32 | A_lo 32 | z2 64, and D overwrites the A operand it was
+// computed from (every D row is read into registers before its thread writes the next A).  z2 is parked in tile memory
+// between the forward recompute and the SiLU' factors of the backward chain; z1 is recomputed from P, Q and the edge
+// geometry where it is needed again.
 // Gradient rows span many orders of magnitude, so EVERY row is encoded with its own power-of-two scale (row maximum
 // taken from the registers), not only the rows that would overflow; D rows are multiplied by 1/scale on the way out.
+// The row rules (encoding, row-tile GEMM, φ-head backward, column sums, weight gradients) live in bwd_tc_common.cuh.
 #include "edge_layer_bwd_tc.cuh"
 
 namespace degnn {
@@ -51,8 +52,7 @@ static int edge_layer_bwd_launch(int64_t n_nodes, int64_t n_edges, int A, int C,
     a.g_wc = g_layer_params + L.off[DISTEGNN_P_E_WC];
     a.g_bc = g_layer_params + L.off[DISTEGNN_P_E_BC];
     a.g_w3 = g_layer_params + L.off[DISTEGNN_P_E_W3];
-    const int64_t tiles = (n_edges + TILE_M - 1) / TILE_M;
-    int64_t grid = (tiles + BT_GROUPS - 1) / BT_GROUPS;
+    int64_t grid = (n_edges + TILE_M - 1) / TILE_M;
     if (grid > sm_count()) grid = sm_count();
     if (g_edge_attr_sorted != nullptr && A > 0) {
         launch_edge_layer_bwd_tc_inputs(a, (unsigned)grid, (cudaStream_t)stream);

@@ -42,38 +42,25 @@ struct EdgeBwdTcArgs {
     float* g_ea;            // [E,A] CSR order, accumulated (kInputs only)
 };
 
-constexpr int BT_THREADS = 128, BT_GROUPS = 1, BT_GROUP = 128;
-constexpr int BT_TM_COLS = 128;                                // per tile group: A_hi 32 | A_lo 32 (= D 64) | z2 64
+constexpr int BT_THREADS = 128;
+constexpr int BT_TM_COLS = 128;                                // A_hi 32 | A_lo 32 (= D 64) | z2 64
 constexpr int BT_W = 64 * 64;                                   // halfs per staged weight matrix
-constexpr int BT_SMEM_BYTES = tmma::tm_bytes(BT_GROUPS * BT_TM_COLS)
+constexpr int BT_SMEM_BYTES = tmma::tm_bytes(BT_TM_COLS)
                               + 8 * BT_W * 2                    // W2, Wc, W2ᵀ, Wcᵀ (hi + lo each)
-                              + BT_GROUPS * 2 * TILE_M * LDA * 4    // gradient tile + activation tile per group
+                              + 2 * TILE_M * LDA * 4            // gradient tile + activation tile
                               + (4 * H + DISTEGNN_MAX_EDGE_ATTR * H) * 4     // b2, bc, w3, w1r, w1e
                               + (4 * H + DISTEGNN_MAX_EDGE_ATTR * H) * 4     // gradient accumulators of the same
-                              + BT_GROUPS * TILE_M * (DISTEGNN_MAX_EDGE_ATTR + 1) * 4   // per-row edge attrs + radial
-                              + BT_GROUPS * TILE_M * 2 * 4      // row, col per edge
-                              + BT_GROUPS * 4 * 4               // run-start masks
+                              + TILE_M * (DISTEGNN_MAX_EDGE_ATTR + 1) * 4    // per-row edge attrs + radial
+                              + TILE_M * 2 * 4                  // row, col per edge
+                              + 4 * 4                           // run-start masks
                               ;
-constexpr uint32_t BT_LBO = 1024;
-
-// B operand of D = A·Bᵀ holding Wᵀ: B[n'][k'] = src[n'*64 + k'] (src = the k-major array of W itself)
-__device__ __forceinline__ void stage_weight_t(__half* hi, __half* lo, const float* __restrict__ src, int tid, int nthreads) {
-    for (int i = tid; i < H * H; i += nthreads) {
-        const int n = i >> 6, k = i & 63;
-        const float w = __ldg(src + i);
-        const __half h = __float2half_rn(w);
-        const uint32_t o = (uint32_t)(k >> 3) * 512u + (uint32_t)(n >> 3) * 64u + (uint32_t)(n & 7) * 8u + (k & 7);
-        hi[o] = h;
-        lo[o] = __float2half_rn(w - __half2float(h));
-    }
-}
 
 // kInputs: also accumulate g_ea[e,k] += Σ_n g_z1[e,n]·W_e[k,n] (edge_attr in CSR order); the edge's row thread owns the
 // row, so plain read-modify-writes suffice.  The <false> instantiation is the weights-only kernel, unchanged.
 template <bool kInputs>
 __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const EdgeBwdTcArgs a) {
     using namespace tmma;
-    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(BT_GROUPS * BT_TM_COLS);
+    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(BT_TM_COLS);
     __half* W2hi = reinterpret_cast<__half*>(smem_raw);
     __half* W2lo = W2hi + BT_W;
     __half* Wchi = W2lo + BT_W;
@@ -82,8 +69,9 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
     __half* W2Tlo = W2Thi + BT_W;
     __half* WcThi = W2Tlo + BT_W;
     __half* WcTlo = WcThi + BT_W;
-    float* tiles = reinterpret_cast<float*>(WcTlo + BT_W);                 // [groups][G tile | Act tile]
-    float* b2s = tiles + BT_GROUPS * 2 * TILE_M * LDA;
+    float* Gt = reinterpret_cast<float*>(WcTlo + BT_W);                    // gradient tile
+    float* At = Gt + TILE_M * LDA;                                          // activation tile
+    float* b2s = At + TILE_M * LDA;
     float* bcs = b2s + H;
     float* w3s = bcs + H;
     float* w1rs = w3s + H;
@@ -93,64 +81,41 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
     float* gw3 = gbc + H;
     float* gw1r = gw3 + H;
     float* gw1e = gw1r + H;
-    float* rowsc_all = gw1e + DISTEGNN_MAX_EDGE_ATTR * H;                  // [groups][128][9]: edge attrs, radial
-    int* srow_all = reinterpret_cast<int*>(rowsc_all + BT_GROUPS * TILE_M * (DISTEGNN_MAX_EDGE_ATTR + 1));
-    int* scol_all = srow_all + BT_GROUPS * TILE_M;
-    uint32_t* rmask_all = reinterpret_cast<uint32_t*>(scol_all + BT_GROUPS * TILE_M);
+    float* rowsc = gw1e + DISTEGNN_MAX_EDGE_ATTR * H;                      // [128][9]: edge attrs, radial
+    int* srow = reinterpret_cast<int*>(rowsc + TILE_M * (DISTEGNN_MAX_EDGE_ATTR + 1));
+    int* scol = srow + TILE_M;
+    uint32_t* rmask = reinterpret_cast<uint32_t*>(scol + TILE_M);
 
-    const int tid = threadIdx.x;
-    const int grp = tid / BT_GROUP, t = tid % BT_GROUP, lane = tid & 31, wq = (tid >> 5) & 3;
+    const int t = threadIdx.x, lane = t & 31, wq = t >> 5;
     const int A = a.A;
     const bool normalize = a.flags & DISTEGNN_FLAG_NORMALIZE;
     const bool need_m = !(a.flags & DISTEGNN_FLAG_LAST) && a.g_aggm != nullptr;
 
     // ---- one-time setup -------------------------------------------------------------------------------------
-    tc16::stage_weight<BT_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid);
-    tc16::stage_weight<BT_THREADS>(Wchi, Wclo, a.wc, 0, 64, tid);
-    stage_weight_t(W2Thi, W2Tlo, a.w2, tid, BT_THREADS);
-    stage_weight_t(WcThi, WcTlo, a.wc, tid, BT_THREADS);
-    if (tid < H) {
-        b2s[tid] = a.b2[tid];
-        bcs[tid] = a.bc[tid];
-        w3s[tid] = a.w3[tid];
-        w1rs[tid] = a.w1r[tid];
+    tc16::stage_weight<BT_THREADS>(W2hi, W2lo, a.w2, 0, 64, t);
+    tc16::stage_weight<BT_THREADS>(Wchi, Wclo, a.wc, 0, 64, t);
+    tc16::stage_weight<BT_THREADS, true>(W2Thi, W2Tlo, a.w2, 0, 64, t);
+    tc16::stage_weight<BT_THREADS, true>(WcThi, WcTlo, a.wc, 0, 64, t);
+    if (t < H) {
+        b2s[t] = a.b2[t];
+        bcs[t] = a.bc[t];
+        w3s[t] = a.w3[t];
+        w1rs[t] = a.w1r[t];
     }
-    for (int i = tid; i < DISTEGNN_MAX_EDGE_ATTR * H; i += BT_THREADS) w1es[i] = i < A * H ? a.w1e[i] : 0.f;
-    for (int i = tid; i < 4 * H + DISTEGNN_MAX_EDGE_ATTR * H; i += BT_THREADS) gb2[i] = 0.f;
+    for (int i = t; i < DISTEGNN_MAX_EDGE_ATTR * H; i += BT_THREADS) w1es[i] = i < A * H ? a.w1e[i] : 0.f;
+    for (int i = t; i < 4 * H + DISTEGNN_MAX_EDGE_ATTR * H; i += BT_THREADS) gb2[i] = 0.f;
     fence_proxy_async_smem();
     __syncthreads();
 
-    const uint32_t col0 = (uint32_t)(grp * BT_TM_COLS);
     const uint32_t lane_off = ((uint32_t)(32 * wq)) << 16;
-    const uint32_t tA_hi = lane_off + col0, tA_lo = lane_off + col0 + 32, tD = lane_off + col0;
-    const uint32_t tZ2 = lane_off + col0 + 64;
-    float* Gt = tiles + grp * 2 * TILE_M * LDA;
-    float* At = Gt + TILE_M * LDA;
-    float* rowsc = rowsc_all + grp * TILE_M * (DISTEGNN_MAX_EDGE_ATTR + 1);
-    int* srow = srow_all + grp * TILE_M;
-    int* scol = scol_all + grp * TILE_M;
-    uint32_t* rmask = rmask_all + grp * 4;
-    const uint32_t bar_id = 1 + grp;
-    // after the group barrier that publishes the A operand: D = A·Wᵀ over the whole tile by the group's warpgroup, written
-    // over A; mma_done() publishes D to every row thread
-    auto issue = [&](const __half* whi, const __half* wlo) {
-        tc16::mma_f16x3<BT_LBO>(col0, col0, col0 + 32u, make_desc(smem_u32(whi), BT_LBO, 128),
-                                make_desc(smem_u32(wlo), BT_LBO, 128), 1, false, 0, 2);
-    };
-    auto mma_done = [&]() { named_bar(bar_id, BT_GROUP); };
+    const uint32_t tA_hi = lane_off, tA_lo = lane_off + 32, tD = lane_off, tZ2 = lane_off + 64;
+    // after the barrier that publishes the A operand: D = A·Wᵀ over the whole tile, written over A; mma_done() publishes
+    // D to every row thread
+    auto issue = [&](const __half* whi, const __half* wlo) { mma_f16x3_tile(0u, 0u, 32u, whi, wlo, false); };
+    auto mma_done = [&]() { __syncthreads(); };
     auto a_ready = [&]() {
         fence_proxy_async_smem();
-        named_bar(bar_id, BT_GROUP);
-    };
-    // column sums of the gradient tile into a shared accumulator: thread <-> (column, half of the rows)
-    auto colsum_G = [&](float* acc) {
-        const int c = t & 63, h = t >> 6;
-        float s0 = 0.f, s1 = 0.f;
-        for (int e = 64 * h; e < 64 * h + 64; e += 2) {
-            s0 += Gt[e * LDA + c];
-            s1 += Gt[(e + 1) * LDA + c];
-        }
-        atomicAdd(acc + c, s0 + s1);
+        __syncthreads();
     };
 
     float gW2[8][4], gWc[8][4];
@@ -161,7 +126,7 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
 
     const int64_t nE = a.E_dev ? min((int64_t)__ldg(a.E_dev), a.E) : a.E;
     const int64_t num_tiles = (nE + TILE_M - 1) / TILE_M;
-    for (int64_t tile = (int64_t)blockIdx.x * BT_GROUPS + grp; tile < num_tiles; tile += (int64_t)gridDim.x * BT_GROUPS) {
+    for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         // ---- the thread's edge: ids, attributes, geometry, upstream scalars ---------------------------------------
         const int64_t e = tile * TILE_M + t;
         const bool valid = e < nE;
@@ -207,10 +172,10 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
 #pragma unroll
             for (int j = 0; j < 64; ++j) v[j] = silu(v[j]);
         }
-        const float inv1 = encode_row_regs(v, tA_hi, tA_lo);
-        a_ready();                                  // also publishes srow/scol/rowsc of this tile to the group
+        const float inv1 = encode_row_own_scale(v, tA_hi, tA_lo);
+        a_ready();                                  // also publishes srow/scol/rowsc of this tile
         issue(W2hi, W2lo);
-        if (t < 128 && lane < 32) {                 // run starts (whole warps): bit i of rmask[q] = edge 32q+i starts a run
+        {                                           // run starts (whole warps): bit i of rmask[q] = edge 32q+i starts a run
             const int prev = t > 0 ? srow[t - 1] : -2;
             const uint32_t starts = __ballot_sync(FULL, prev != r);
             if (lane == 0) rmask[wq] = starts;
@@ -225,36 +190,21 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
 #pragma unroll
         for (int j = 0; j < 64; ++j) v[j] = silu(v[j]);
         smem_store_row(At + t * LDA, v);
-        const float inv2 = encode_row_regs(v, tA_hi, tA_lo);
+        const float inv2 = encode_row_own_scale(v, tA_hi, tA_lo);
         a_ready();
         issue(Wchi, Wclo);
         mma_done();
 
         // ---- stage 3: zc = D/s + bc; φ; g_w3; g_zc = gφ·w3 ⊙ SiLU'(zc) -> gradient tile + A ------------------------------
-        float phi = 0.f;
         tm_load_row(tD, v);
-        {
-            float u[64];                            // gφ·SiLU(zc): its column sums over the tile are g_w3
-#pragma unroll
-            for (int j = 0; j < 64; ++j) {
-                const float zc = fmaf(v[j], inv2, bcs[j]);
-                const float s = sigmoid_f(zc);
-                const float ac = zc * s, w3j = w3s[j];
-                phi = fmaf(ac, w3j, phi);
-                u[j] = gphi * ac;                   // gφ = 0 on rows beyond E
-                v[j] = gphi * w3j * (s * fmaf(zc, 1.0f - s, 1.0f));
-            }
-            warp_colsum64(u, lane);
-            atomicAdd(gw3 + 2 * lane, u[0]);
-            atomicAdd(gw3 + 2 * lane + 1, u[1]);
-        }
+        const float phi = phi_head_bwd(v, inv2, bcs, w3s, gphi, gw3, lane);   // gφ = 0 on rows beyond E
         smem_store_row(Gt + t * LDA, v);
-        const float inv3 = encode_row_regs(v, tA_hi, tA_lo);
+        const float inv3 = encode_row_own_scale(v, tA_hi, tA_lo);
         a_ready();                                  // gradient tile + activation tile visible, A complete, D fully read
         issue(WcThi, WcTlo);
         wgrad128(gWc, Gt, At, t);                   // g_Wc += g_zcᵀ·m
-        colsum_G(gbc);
-        named_bar(bar_id, BT_GROUP);                // both tiles fully read
+        tile_colsum(gbc, Gt, t);
+        __syncthreads();                            // both tiles fully read
         mma_done();
 
         // ---- stage 4: g_m = D/s + g_aggm[row]; g_z2 = g_m ⊙ SiLU'(z2) -> gradient tile + A; a1 -> activation tile ----------
@@ -273,7 +223,7 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
                 v[4 * j4 + 3] = fmaf(v[4 * j4 + 3], inv3, u.w) * dsilu(z2[4 * j4 + 3]);
             }
             smem_store_row(Gt + t * LDA, v);
-            const float inv4_ = encode_row_regs(v, tA_hi, tA_lo);
+            const float inv4_ = encode_row_own_scale(v, tA_hi, tA_lo);
             z1_row(z2);                             // reuse the buffer: z1 -> a1 row for the weight gradient
 #pragma unroll
             for (int j = 0; j < 64; ++j) z2[j] = silu(z2[j]);
@@ -281,8 +231,8 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
             a_ready();
             issue(W2Thi, W2Tlo);
             wgrad128(gW2, Gt, At, t);               // g_W2 += g_z2ᵀ·a1
-            colsum_G(gb2);
-            named_bar(bar_id, BT_GROUP);
+            tile_colsum(gb2, Gt, t);
+            __syncthreads();
             mma_done();
 
             // ---- stage 5: g_z1 = D/s ⊙ SiLU'(z1) -> gradient tile; g_r ---------------------------------------------------
@@ -318,7 +268,7 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
                 atomicAdd(a.g_x + (size_t)c * 4 + 2, -gdz);
             }
         }
-        named_bar(bar_id, BT_GROUP);                // g_z1 tile visible
+        __syncthreads();                            // g_z1 tile visible
 
         // ---- scatter of the g_z1 tile: g_P by runs of equal row, g_Q per edge, g_w_r / g_W_e column sums -----------------
         {   // g_P: warp <-> 32 edges, lane <-> column pair, one RED.v2 per run
@@ -363,20 +313,20 @@ __global__ void __launch_bounds__(BT_THREADS, 1) edge_layer_bwd_tc_kernel(const 
             for (int k = 0; k < DISTEGNN_MAX_EDGE_ATTR; ++k)
                 if (k < A) atomicAdd(gw1e + k * H + cc, se[k]);
         }
-        named_bar(bar_id, BT_GROUP);                // tiles and per-row arrays are rewritten by the next iteration
+        __syncthreads();                            // tiles and per-row arrays are rewritten by the next iteration
     }
 
     // ---- flush the CTA's parameter gradients ------------------------------------------------------------------------
     wgrad128_flush(a.g_w2, gW2, t);
     wgrad128_flush(a.g_wc, gWc, t);
     __syncthreads();
-    if (tid < H) {
-        atomicAdd(a.g_b2 + tid, gb2[tid]);
-        atomicAdd(a.g_bc + tid, gbc[tid]);
-        atomicAdd(a.g_w3 + tid, gw3[tid]);
-        atomicAdd(a.g_w1r + tid, gw1r[tid]);
+    if (t < H) {
+        atomicAdd(a.g_b2 + t, gb2[t]);
+        atomicAdd(a.g_bc + t, gbc[t]);
+        atomicAdd(a.g_w3 + t, gw3[t]);
+        atomicAdd(a.g_w1r + t, gw1r[t]);
     }
-    for (int i = tid; i < A * H; i += BT_THREADS) atomicAdd(a.g_w1e + i, gw1e[i]);
+    for (int i = t; i < A * H; i += BT_THREADS) atomicAdd(a.g_w1e + i, gw1e[i]);
 }
 
 }  // namespace degnn

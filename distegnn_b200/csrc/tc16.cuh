@@ -34,10 +34,13 @@ __device__ __forceinline__ void split_pair(f32x2 x, uint32_t& hi, uint32_t& lo) 
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
-// stage W[n][k] (given k-major: wt[k*64+n]) as rows n_off..n_off+63 of an N_total-row B operand, fp16 hi/lo
+// stage W[n][k] (given k-major: wt[k*64+n]) as rows n_off..n_off+63 of an N_total-row B operand, fp16 hi/lo;
+// TRANSPOSED: stage Wᵀ instead, B[n][k] = wt[n*64+k].  Every B operand and weight image is laid out here.
 // NTHREADS is a template parameter so that the H·H / NTHREADS loads of a thread are all issued before the first conversion
-// (a rolled load -> convert -> store loop pays one global round trip per element and thread).
-template <int NTHREADS>
+// (a rolled load -> convert -> store loop pays one global round trip per element and thread).  The element offset stays
+// written out in the loop: as a function of its own, the compiler simplifies it before inlining and the forward kernels'
+// address arithmetic and register allocation change.
+template <int NTHREADS, bool TRANSPOSED = false>
 __device__ __forceinline__ void stage_weight(__half* hi, __half* lo, const float* __restrict__ wt_kmajor, int n_off,
                                              int n_total, int tid, float scale = 1.0f) {
     static_assert((H * H) % NTHREADS == 0, "thread count must divide the matrix");
@@ -49,7 +52,7 @@ __device__ __forceinline__ void stage_weight(__half* hi, __half* lo, const float
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const int i = tid + r * NTHREADS;
-        const int k = i >> 6, n = (i & 63) + n_off;
+        const int k = TRANSPOSED ? i & 63 : i >> 6, n = (TRANSPOSED ? i >> 6 : i & 63) + n_off;
         const float ws = w[r] * scale;
         const __half h = __float2half_rn(ws);
         const uint32_t o = (uint32_t)(k >> 3) * lbo_h + (uint32_t)(n >> 3) * 64u + (uint32_t)(n & 7) * 8u + (k & 7);
@@ -58,44 +61,6 @@ __device__ __forceinline__ void stage_weight(__half* hi, __half* lo, const float
     }
 }
 __host__ __device__ constexpr uint32_t lbo_bytes(int n_total) { return (uint32_t)(n_total / 8) * 128u; }
-
-// D (+)= A_lo·B_hiᵀ + A_hi·B_loᵀ + A_hi·B_hiᵀ with K = 64 (12 wgmma of K = 16 per 64x64 block) for the 64-row blocks
-// mb0 .. mb0 + nmb − 1 of the tile and N = 64·nchunks columns: A_hi / A_lo = tile-memory columns a_hi / a_lo (32 each),
-// B rows n = 64·chunk .. of the staged weights, D = tile-memory columns d .. d + 64·nchunks − 1.  `accumulate` = add to
-// the D already in tile memory.  Issued by every thread of ONE warpgroup and synchronous: on return the D rows of the
-// warpgroup's blocks are in tile memory (threads of other warps read them after a barrier).
-template <uint32_t LBO>
-__device__ __forceinline__ void mma_f16x3(uint32_t d, uint32_t a_hi, uint32_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                          int nchunks, bool accumulate, int mb0, int nmb) {
-    constexpr uint64_t B_KSTEP = (2 * LBO) >> 4, A_KSTEP = (2 * tmma::TM_COLGROUP_BYTES) >> 4, B_NCHUNK = (8 * 128) >> 4;
-#pragma unroll 1
-    for (int mb = mb0; mb < mb0 + nmb; ++mb) {
-        const uint64_t ahi = tmma::make_desc(tmma::tm_addr_rc(64u * mb, a_hi), tmma::TM_COLGROUP_BYTES, 128);
-        const uint64_t alo = tmma::make_desc(tmma::tm_addr_rc(64u * mb, a_lo), tmma::TM_COLGROUP_BYTES, 128);
-#pragma unroll 1
-        for (int nc = 0; nc < nchunks; ++nc) {
-            float acc[32];
-            if (accumulate) {
-                tmma::frag_load(acc, d + 64u * nc, mb);
-            } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-            }
-            const uint64_t bh = b_hi + nc * B_NCHUNK, bl = b_lo + nc * B_NCHUNK;
-            tmma::wgmma_fence();
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks)
-                tmma::wgmma_f16_m64n64k16(acc, alo + ks * A_KSTEP, bh + ks * B_KSTEP, (accumulate || ks > 0) ? 1u : 0u);
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) tmma::wgmma_f16_m64n64k16(acc, ahi + ks * A_KSTEP, bl + ks * B_KSTEP, 1u);
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) tmma::wgmma_f16_m64n64k16(acc, ahi + ks * A_KSTEP, bh + ks * B_KSTEP, 1u);
-            tmma::wgmma_commit();
-            tmma::wgmma_wait_all();
-            tmma::frag_store(acc, d + 64u * nc, mb);
-        }
-    }
-}
 
 // Register-operand flavour for one 64-row block held by a warpgroup: D = A_lo·B_hiᵀ + A_hi·B_loᵀ + A_hi·B_hiᵀ, K = 64,
 // N = 64.  a_hi / a_lo are the A fragments of the four k-steps (tile_mma.cuh wgmma_f16_m64n64k16_rA: registers 4ks ..
@@ -264,17 +229,6 @@ __device__ __forceinline__ void phi_head_t(const float (&d)[32], float inv_a, fl
     phia = quad_sum(p0 + p1);
     upk2(phb, p0, p1);
     phib = quad_sum(p0 + p1);
-}
-
-// ---- register-pair flavour (fp32 pairs, common.cuh) ------------------------------------------------------------
-template <bool SCALED>
-__device__ __forceinline__ void split16p(const f32x2 (&v)[8], float s, uint32_t (&hi)[8], uint32_t (&lo)[8],
-                                         __half2& mx) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        split_pair(SCALED ? mul2(v[j], bc2(s)) : v[j], hi[j], lo[j]);
-        mx = __hmax2(mx, __habs2(*reinterpret_cast<const __half2*>(&hi[j])));
-    }
 }
 
 }  // namespace tc16

@@ -1,20 +1,21 @@
 // Backward of the real<->virtual stage on the tensor cores (wgmma) — production kernel behind
-// distegnn_virtual_layer_bwd (the fp32-FMA kernel of virtual_layer_bwd.cu is kept as distegnn_virtual_layer_bwd_simt).
-// Same contract and math as virtual_layer_bwd.cu (reference: autograd through models/FastEGNN.py:154-163, 180, 191-193,
-// 207, 220-223, 252-253).  Per 128-row tile (rows = (node, channel)) the SIX row-wise tile GEMMs — recompute z2 = a1·W2vᵀ,
-// zxv = mv·Wxvᵀ, zx = mv·Wxᵀ; data gradients g_mv = g_zxv·Wxv + g_zx·Wx (two MMAs into ONE accumulator, both rows encoded
+// distegnn_virtual_layer_bwd.  Its twin, the fp32-FMA kernel of csrc/testing/virtual_layer_bwd.cu behind
+// distegnn_virtual_layer_bwd_simt, has the same contract and math (reference: autograd through models/FastEGNN.py:154-163,
+// 180, 191-193, 207, 220-223, 252-253).  Per 128-row tile (rows = (node, channel)) the SIX row-wise tile GEMMs —
+// recompute z2 = a1·W2vᵀ, zxv = mv·Wxvᵀ, zx = mv·Wxᵀ; data gradients g_mv = g_zxv·Wxv + g_zx·Wx (two MMAs into ONE accumulator, both rows encoded
 // with a common scale), g_a1 = g_z2·W2v — run as wgmma f16 with the fp16 2-term split (tc16.cuh), A written to tile memory
 // by the thread that owns the row; the three weight-gradient GEMMs stay on the CUDA cores (see edge_layer_bwd_tc.cu).
 //
 // Shared memory: six 64x64 B operands (hi + lo = 16 KB each) do not fit next to the two fp32 row tiles and the tile memory,
 // so the weights are NOT resident: distegnn_virtual_bwd_prepare writes them once per call as fp16 hi/lo IMAGES already in
-// the shared-memory operand layout, and every tile group streams them through two 16 KB slots with one TMA bulk copy per
+// the shared-memory operand layout, and the CTA streams them through two 16 KB slots with one TMA bulk copy per
 // matrix, two matrices ahead of their use (mbarrier per slot; the order W2v, Wxv, Wx, Wxvᵀ, Wxᵀ, W2vᵀ repeats every tile).
-// One CTA per SM, 128 threads = 1 tile group = 1 warpgroup; thread r owns row r and holds whole 64-wide rows in registers.
-// Tile memory per group (tile_mma.cuh, 192 columns): D 64 | A2_hi 32 | A2_lo 32 | z2 64, where the first 64 columns also
+// One CTA per SM, 128 threads = 1 warpgroup; thread r owns row r and holds whole 64-wide rows in registers.
+// Tile memory (tile_mma.cuh, 192 columns): D 64 | A2_hi 32 | A2_lo 32 | z2 64, where the first 64 columns also
 // hold the A operand (A_hi 32 | A_lo 32) that a GEMM writing D consumes: every D row is read into registers before its
 // thread writes the next A there.  A2 holds mv for the two GEMMs that read it, then g_zx while D = g_zxv·Wxv is added to;
-// z1 is recomputed from Hn, G and ‖ΔX‖ where it is needed again.  Every row is encoded with its own power-of-two scale (gradient rows span many orders of magnitude).
+// z1 is recomputed from Hn, G and ‖ΔX‖ where it is needed again.  Every row is encoded with its own power-of-two scale
+// (gradient rows span many orders of magnitude).  The row rules live in bwd_tc_common.cuh.
 #include <cuda_fp16.h>
 
 #include "bwd_common.cuh"
@@ -48,47 +49,41 @@ struct VirtBwdTcArgs {
     float* g_wx; float* g_bx; float* g_w3x;
 };
 
-constexpr int VT_THREADS = 128, VT_GROUPS = 1, VT_GROUP = 128;
-constexpr int VT_TM_COLS = 192;                                     // per tile group: A / D 64 | A2 64 | z2 64
+constexpr int VT_THREADS = 128;
+constexpr int VT_TM_COLS = 192;                                     // A / D 64 | A2 64 | z2 64
 constexpr int VT_MAXC = DISTEGNN_MAX_CHANNELS;
 constexpr int VT_IMG = 2 * 64 * 64;                                 // halfs per matrix image (hi + lo)
-constexpr int VT_SMEM_BYTES = tmma::tm_bytes(VT_GROUPS * VT_TM_COLS)
-                              + VT_GROUPS * 2 * VT_IMG * 2          // two weight slots per group
-                              + VT_GROUPS * 2 * TILE_M * LDA * 4    // gradient tile + activation tile per group
+constexpr int VT_SMEM_BYTES = tmma::tm_bytes(VT_TM_COLS)
+                              + 2 * VT_IMG * 2                      // two weight slots
+                              + 2 * TILE_M * LDA * 4                // gradient tile + activation tile
                               + 6 * H * 4 + 6 * H * 4               // w1r, b2, bxv, w3xv, bx, w3x + gradient accumulators
-                              + VT_GROUPS * VT_MAXC * H * 4         // Σ_i g_z1 per channel (-> g_G)
-                              + VT_GROUPS * 4 * VT_MAXC * 4         // Σ_i gΔX per channel (-> g_Xv)
-                              + VT_GROUPS * TILE_M * 4 * 4          // gΔX per row
-                              + VT_GROUPS * TILE_M * 4              // ‖ΔX‖ per row
-                              + VT_GROUPS * TILE_M * 4              // graph id per local node
+                              + VT_MAXC * H * 4                     // Σ_i g_z1 per channel (-> g_G)
+                              + 4 * VT_MAXC * 4                     // Σ_i gΔX per channel (-> g_Xv)
+                              + TILE_M * 4 * 4                      // gΔX per row
+                              + TILE_M * 4                          // ‖ΔX‖ per row
+                              + TILE_M * 4                          // graph id per local node
                               + 256;                                // mbarriers
-constexpr uint32_t VT_LBO = 1024;
 
-// fp16 hi/lo images of the six B operands in the shared-memory layout (K-major, no swizzle): element (n,k) of an image at
-// (k/8)*512 + (n/8)*64 + (n%8)*8 + k%8 halfs; forward matrices B[n][k] = W[n][k] = w_kmajor[k*64+n], transposed ones
-// B[n][k] = W[k][n] = w_kmajor[n*64+k].
+// fp16 hi/lo images of the six B operands in the shared-memory layout of tc16::stage_weight: forward matrices
+// B[n][k] = W[n][k] = w_kmajor[k*64+n], transposed ones B[n][k] = W[k][n] = w_kmajor[n*64+k].
+constexpr int VT_IMG_THREADS = 256;
 __global__ void virtual_bwd_images_kernel(const float* w2, const float* wxv, const float* wx, __half* img) {
     const int m = blockIdx.x;                    // 0..5
     const float* src = (m == 0 || m == 5) ? w2 : ((m == 1 || m == 3) ? wxv : wx);
-    const bool transposed = m >= 3;
     __half* hi = img + (size_t)m * VT_IMG;
-    __half* lo = hi + 64 * 64;
-    for (int i = threadIdx.x; i < 64 * 64; i += blockDim.x) {
-        const int n = i >> 6, k = i & 63;
-        const float w = transposed ? src[n * 64 + k] : src[k * 64 + n];
-        const __half h = __float2half_rn(w);
-        const uint32_t o = (uint32_t)(k >> 3) * 512u + (uint32_t)(n >> 3) * 64u + (uint32_t)(n & 7) * 8u + (k & 7);
-        hi[o] = h;
-        lo[o] = __float2half_rn(w - __half2float(h));
-    }
+    if (m >= 3)
+        tc16::stage_weight<VT_IMG_THREADS, true>(hi, hi + 64 * 64, src, 0, 64, threadIdx.x);
+    else
+        tc16::stage_weight<VT_IMG_THREADS>(hi, hi + 64 * 64, src, 0, 64, threadIdx.x);
 }
 
 __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(const VirtBwdTcArgs a) {
     using namespace tmma;
-    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(VT_GROUPS * VT_TM_COLS);
-    __half* slots = reinterpret_cast<__half*>(smem_raw);                     // [groups][2 slots][VT_IMG]
-    float* tiles = reinterpret_cast<float*>(slots + VT_GROUPS * 2 * VT_IMG); // [groups][G tile | Act tile]
-    float* w1rs = tiles + VT_GROUPS * 2 * TILE_M * LDA;
+    uint8_t* const smem_raw = degnn_dyn_smem + tm_bytes(VT_TM_COLS);
+    __half* slots = reinterpret_cast<__half*>(smem_raw);                     // [2 slots][VT_IMG]
+    float* Gt = reinterpret_cast<float*>(slots + 2 * VT_IMG);                // gradient tile
+    float* At = Gt + TILE_M * LDA;                                           // activation tile
+    float* w1rs = At + TILE_M * LDA;
     float* b2s = w1rs + H;
     float* bxvs = b2s + H;
     float* w3xvs = bxvs + H;
@@ -100,63 +95,49 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
     float* gw3xv = gbxv + H;
     float* gbx = gw3xv + H;
     float* gw3x = gbx + H;
-    float* accG_all = gw3x + H;                                              // [groups][C][64]
-    float* accX_all = accG_all + VT_GROUPS * VT_MAXC * H;                    // [groups][3][VT_MAXC] (pitch VT_MAXC, 4 rows)
-    float* gdX_all = accX_all + VT_GROUPS * 4 * VT_MAXC;                     // [groups][128][4]
-    float* vrs_all = gdX_all + VT_GROUPS * TILE_M * 4;                       // [groups][128]
-    int* sgraph_all = reinterpret_cast<int*>(vrs_all + VT_GROUPS * TILE_M);  // [groups][128]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sgraph_all + VT_GROUPS * TILE_M);   // [groups][slot0, slot1]
+    float* accG = gw3x + H;                                                  // [C][64]
+    float* accX = accG + VT_MAXC * H;                                        // [3][VT_MAXC] (pitch VT_MAXC, 4 rows)
+    float* gdX = accX + 4 * VT_MAXC;                                         // [128][4]
+    float* vrs = gdX + TILE_M * 4;                                           // [128]
+    int* sgraph = reinterpret_cast<int*>(vrs + TILE_M);                      // [128]
+    uint64_t* wbar = reinterpret_cast<uint64_t*>(sgraph + TILE_M);           // [2]: weight slot filled
 
-    const int tid = threadIdx.x;
-    const int grp = tid / VT_GROUP, t = tid % VT_GROUP, lane = tid & 31, wq = (tid >> 5) & 3;
+    const int t = threadIdx.x, lane = t & 31, wq = t >> 5;
     const int C = a.C;
     const int K = 4 + 3 * C + H * C;
     const int TN = TILE_M / C;
     const float invC = 1.0f / (float)C;
     const bool need_feat = !(a.flags & DISTEGNN_FLAG_LAST) && a.g_aggv != nullptr;
 
-    if (tid < H) {
-        w1rs[tid] = a.w1r[tid];
-        b2s[tid] = a.b2[tid];
-        bxvs[tid] = a.bxv[tid];
-        w3xvs[tid] = a.w3xv[tid];
-        bxs[tid] = a.bx[tid];
-        w3xs[tid] = a.w3x[tid];
+    if (t < H) {
+        w1rs[t] = a.w1r[t];
+        b2s[t] = a.b2[t];
+        bxvs[t] = a.bxv[t];
+        w3xvs[t] = a.w3xv[t];
+        bxs[t] = a.bx[t];
+        w3xs[t] = a.w3x[t];
     }
-    for (int i = tid; i < 6 * H + VT_GROUPS * (VT_MAXC * H + 4 * VT_MAXC); i += VT_THREADS) gw1r[i] = 0.f;
-    if (tid == 0) {
-        for (int i = 0; i < 2 * VT_GROUPS; ++i) mbar_init(&bars[i], 1);
+    for (int i = t; i < 6 * H + VT_MAXC * H + 4 * VT_MAXC; i += VT_THREADS) gw1r[i] = 0.f;
+    if (t == 0) {
+        for (int i = 0; i < 2; ++i) mbar_init(&wbar[i], 1);
         fence_mbar_init();
     }
     fence_proxy_async_smem();
     __syncthreads();
 
-    const uint32_t col0 = (uint32_t)(grp * VT_TM_COLS);
     const uint32_t lane_off = ((uint32_t)(32 * wq)) << 16;
-    const uint32_t tA_hi = lane_off + col0, tA_lo = lane_off + col0 + 32, tD = lane_off + col0;
-    const uint32_t tA2_hi = lane_off + col0 + 64, tA2_lo = lane_off + col0 + 96, tZ2 = lane_off + col0 + 128;
-    __half* myslots = slots + grp * 2 * VT_IMG;
-    float* Gt = tiles + grp * 2 * TILE_M * LDA;
-    float* At = Gt + TILE_M * LDA;
-    float* accG = accG_all + grp * VT_MAXC * H;
-    float* accX = accX_all + grp * 4 * VT_MAXC;
-    float* gdX = gdX_all + grp * TILE_M * 4;
-    float* vrs = vrs_all + grp * TILE_M;
-    int* sgraph = sgraph_all + grp * TILE_M;
-    uint64_t* wbar = bars + 2 * grp;                             // [2]: weight slot filled
-    const uint32_t bar_id = 1 + grp;
+    const uint32_t tA_hi = lane_off, tA_lo = lane_off + 32, tD = lane_off;
+    const uint32_t tA2_hi = lane_off + 64, tA2_lo = lane_off + 96, tZ2 = lane_off + 128;
 
     const int64_t num_tiles = (a.N + TN - 1) / TN;
-    const int64_t tstride = (int64_t)gridDim.x * VT_GROUPS;
-    const int64_t tile0 = (int64_t)blockIdx.x * VT_GROUPS + grp;
-    const int64_t my_tiles = tile0 < num_tiles ? (num_tiles - tile0 + tstride - 1) / tstride : 0;
-    const int64_t total_q = 6 * my_tiles;                        // matrices this group will consume, in order
-    int64_t q_next = 0;                                          // next matrix to be requested (thread 0 of the group)
+    const int64_t my_tiles = blockIdx.x < num_tiles ? (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+    const int64_t total_q = 6 * my_tiles;                        // matrices this CTA will consume, in order
+    int64_t q_next = 0;                                          // next matrix to be requested (thread 0)
     auto request = [&]() {                                       // thread 0: stream matrix q_next into slot q_next & 1
         if (q_next < total_q) {
             const int slot = (int)(q_next & 1), m = (int)(q_next % 6);
             mbar_expect_tx(wbar + slot, VT_IMG * 2);
-            bulk_g2s(myslots + slot * VT_IMG, a.wimg + (size_t)m * VT_IMG, VT_IMG * 2, wbar + slot);
+            bulk_g2s(slots + slot * VT_IMG, a.wimg + (size_t)m * VT_IMG, VT_IMG * 2, wbar + slot);
             ++q_next;
         }
     };
@@ -165,35 +146,25 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
         request();
     }
     int64_t q_use = 0;                                           // next matrix to be used (same on all threads)
-    // publish the A operand at tile-memory column `acol` (col0: over D, col0 + 64: A2), wait for the weight slot, and run the
-    // three split products over the whole tile (the group's warpgroup): D (+)= A·Wᵀ
+    // publish the A operand at tile-memory column `acol` (0: over D, 64: A2), wait for the weight slot, and run the
+    // three split products over the whole tile: D (+)= A·Wᵀ
     auto issue = [&](uint32_t acol, bool accumulate) {
         fence_proxy_async_smem();
-        named_bar(bar_id, VT_GROUP);
+        __syncthreads();
         const int slot = (int)(q_use & 1);
         mbar_wait(wbar + slot, (uint32_t)((q_use >> 1) & 1));
-        const __half* whi = myslots + slot * VT_IMG;
-        tc16::mma_f16x3<VT_LBO>(col0, acol, acol + 32u, make_desc(smem_u32(whi), VT_LBO, 128),
-                                make_desc(smem_u32(whi + 64 * 64), VT_LBO, 128), 1, accumulate, 0, 2);
+        const __half* whi = slots + slot * VT_IMG;
+        mma_f16x3_tile(0u, acol, acol + 32u, whi, whi + 64 * 64, accumulate);
         ++q_use;
     };
     auto mma_done = [&]() {                                      // D visible; the slot it read is refilled two matrices ahead
-        named_bar(bar_id, VT_GROUP);
+        __syncthreads();
         if (t == 0) request();
     };
-    auto colsum_G = [&](float* acc) {
-        const int c = t & 63, h = t >> 6;
-        float s0 = 0.f, s1 = 0.f;
-        for (int e = 64 * h; e < 64 * h + 64; e += 2) {
-            s0 += Gt[e * LDA + c];
-            s1 += Gt[(e + 1) * LDA + c];
-        }
-        atomicAdd(acc + c, s0 + s1);
-    };
     int cur_graph = -1;
-    auto flush = [&](int g) {                                    // all threads of the group; caller synchronises
+    auto flush = [&](int g) {                                    // all threads; caller synchronises
         if (g >= 0) {
-            for (int i = t; i < C * H; i += VT_GROUP) {
+            for (int i = t; i < C * H; i += VT_THREADS) {
                 atomicAdd(a.g_G + (size_t)g * C * H + i, accG[i]);
                 accG[i] = 0.f;
             }
@@ -211,18 +182,18 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
 #pragma unroll
         for (int j = 0; j < 4; ++j) gW2[i][j] = gWxv[i][j] = gWx[i][j] = 0.f;
 
-    for (int64_t tile = tile0; tile < num_tiles; tile += tstride) {
+    for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int64_t n0 = tile * TN;
         const int nvalid = (int)min((int64_t)TN, a.N - n0);
         const int rows = nvalid * C;
         if (t < TN) sgraph[t] = (t < nvalid) ? __ldg(a.batch + n0 + t) : -1;
-        named_bar(bar_id, VT_GROUP);
+        __syncthreads();
         const int g_first = sgraph[0];
         const bool single = (g_first == sgraph[nvalid - 1]);
         if (single && g_first != cur_graph) {
             flush(cur_graph);
             cur_graph = g_first;
-            named_bar(bar_id, VT_GROUP);
+            __syncthreads();
         }
 
         // ---- the thread's row: node, channel, geometry, upstream scalars -----------------------------------------------
@@ -267,8 +238,8 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
 #pragma unroll
             for (int j = 0; j < 64; ++j) v[j] = rvalid ? silu(v[j]) : 0.f;
         }
-        const float inv1 = encode_row_regs(v, tA_hi, tA_lo);
-        issue(col0, false);                           // W2v
+        const float inv1 = encode_row_own_scale(v, tA_hi, tA_lo);
+        issue(0u, false);                             // W2v
         mma_done();
 
         // ---- stage 2: z2 = D/s + b2v -> tile memory; mv = SiLU(z2) -> activation tile + A;  MMA: zxv = mv·Wxvᵀ --------------
@@ -279,54 +250,25 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
 #pragma unroll
         for (int j = 0; j < 64; ++j) v[j] = silu(v[j]);
         smem_store_row(At + t * LDA, v);
-        const float inv2 = encode_row_regs(v, tA2_hi, tA2_lo);
-        issue(col0 + 64u, false);                     // Wxv
+        const float inv2 = encode_row_own_scale(v, tA2_hi, tA2_lo);
+        issue(64u, false);                            // Wxv
         mma_done();
 
         // ---- head xv: φ_xv, g_w3xv, g_zxv -> gradient tile; mv -> A again;  MMA: zx = mv·Wxᵀ -----------------------------------
-        float phixv = 0.f, phix = 0.f;
         tm_load_row(tD, v);
-        {
-            float u[64];
-#pragma unroll
-            for (int j = 0; j < 64; ++j) {
-                const float zc = fmaf(v[j], inv2, bxvs[j]);
-                const float s = sigmoid_f(zc);
-                const float ac = zc * s, w3j = w3xvs[j];
-                phixv = fmaf(ac, w3j, phixv);
-                u[j] = gpxv * ac;
-                v[j] = gpxv * w3j * (s * fmaf(zc, 1.0f - s, 1.0f));
-            }
-            warp_colsum64(u, lane);
-            atomicAdd(gw3xv + 2 * lane, u[0]);
-            atomicAdd(gw3xv + 2 * lane + 1, u[1]);
-        }
+        const float phixv = phi_head_bwd(v, inv2, bxvs, w3xvs, gpxv, gw3xv, lane);
         smem_store_row(Gt + t * LDA, v);
         float fm = row_absmax(v);                     // the two heads' gradient rows share one scale (one accumulator)
-        issue(col0 + 64u, false);                     // Wx (A2 unchanged: still mv); the barrier inside publishes both tiles
+        issue(64u, false);                            // Wx (A2 unchanged: still mv); the barrier inside publishes both tiles
         wgrad128(gWxv, Gt, At, t);                    // g_Wxv += g_zxvᵀ·mv
-        colsum_G(gbxv);
-        named_bar(bar_id, VT_GROUP);                  // gradient tile fully read
+        tile_colsum(gbxv, Gt, t);
+        __syncthreads();                              // gradient tile fully read
         mma_done();
 
         // ---- head x: φ_X, g_w3x, g_zx;  MMAs: g_mv = g_zxv·Wxv + g_zx·Wx -----------------------------------------------------
         float gzx[64];
         tm_load_row(tD, gzx);
-        {
-            float u[64];
-#pragma unroll
-            for (int j = 0; j < 64; ++j) {
-                const float zc = fmaf(gzx[j], inv2, bxs[j]);
-                const float s = sigmoid_f(zc);
-                const float ac = zc * s, w3j = w3xs[j];
-                phix = fmaf(ac, w3j, phix);
-                u[j] = gpx * ac;
-                gzx[j] = gpx * w3j * (s * fmaf(zc, 1.0f - s, 1.0f));
-            }
-            warp_colsum64(u, lane);
-            atomicAdd(gw3x + 2 * lane, u[0]);
-            atomicAdd(gw3x + 2 * lane + 1, u[1]);
-        }
+        const float phix = phi_head_bwd(gzx, inv2, bxs, w3xs, gpx, gw3x, lane);
         fm = row_absmax(gzx, fm);
         float sc, inv3;
         row_scale(fm, sc, inv3);
@@ -335,15 +277,15 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
             const float4 q4 = *reinterpret_cast<const float4*>(Gt + t * LDA + 4 * j4);   // registers during the head)
             v[4 * j4] = q4.x; v[4 * j4 + 1] = q4.y; v[4 * j4 + 2] = q4.z; v[4 * j4 + 3] = q4.w;
         }
-        encode_row_scaled(v, sc, tA_hi, tA_lo);       // A = g_zxv
-        issue(col0, false);                           // Wxvᵀ
+        encode_row(v, sc, tA_hi, tA_lo);              // A = g_zxv
+        issue(0u, false);                             // Wxvᵀ
         smem_store_row(Gt + t * LDA, gzx);            // the gradient tile now holds g_zx (its readers passed the barrier above)
         mma_done();
-        encode_row_scaled(gzx, sc, tA2_hi, tA2_lo);   // A2 = g_zx
-        issue(col0 + 64u, true);                      // Wxᵀ, accumulating; the barrier inside publishes the g_zx tile
+        encode_row(gzx, sc, tA2_hi, tA2_lo);          // A2 = g_zx
+        issue(64u, true);                             // Wxᵀ, accumulating; the barrier inside publishes the g_zx tile
         wgrad128(gWx, Gt, At, t);                     // g_Wx += g_zxᵀ·mv
-        colsum_G(gbx);
-        named_bar(bar_id, VT_GROUP);                  // both tiles fully read
+        tile_colsum(gbx, Gt, t);
+        __syncthreads();                              // both tiles fully read
         mma_done();
 
         // ---- g_z2 = (g_mv + upstream) ⊙ SiLU'(z2) -> gradient tile + A; a1 -> activation tile;  MMA: g_a1 = g_z2·W2v ------------
@@ -361,16 +303,16 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
                 v[j] = gm * dsilu(gzx[j]);
             }
             smem_store_row(Gt + t * LDA, v);
-            inv4 = encode_row_regs(v, tA_hi, tA_lo);
+            inv4 = encode_row_own_scale(v, tA_hi, tA_lo);
             z1_row(gzx);                            // z1 -> a1 row for the weight gradient
 #pragma unroll
             for (int j = 0; j < 64; ++j) gzx[j] = rvalid ? silu(gzx[j]) : 0.f;
             smem_store_row(At + t * LDA, gzx);
         }
-        issue(col0, false);                           // W2vᵀ
+        issue(0u, false);                             // W2vᵀ
         wgrad128(gW2, Gt, At, t);                     // g_W2v += g_z2ᵀ·a1
-        colsum_G(gb2);
-        named_bar(bar_id, VT_GROUP);
+        tile_colsum(gb2, Gt, t);
+        __syncthreads();
         mma_done();
 
         // ---- g_z1 = D/s ⊙ SiLU'(z1) -> gradient tile; g_vr; geometry gradient ---------------------------------------------------
@@ -391,7 +333,7 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
                                          fmaf(gt.z, s1, fmaf(gv2, phix, s3 * dz)), 0.f);
             *reinterpret_cast<float4*>(gdX + 4 * t) = gd;
         }
-        named_bar(bar_id, VT_GROUP);                  // g_z1 tile and gΔX visible
+        __syncthreads();                              // g_z1 tile and gΔX visible
 
         // ---- reductions of the g_z1 tile and of gΔX ------------------------------------------------------------------------------
         {
@@ -434,7 +376,7 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
                 for (int n = 0; n < nvalid; ++n) atomicAdd(a.g_Xv + (size_t)sgraph[n] * 3 * C + k, gdX[4 * (n * C + c) + d]);
             }
         }
-        named_bar(bar_id, VT_GROUP);                  // tiles and per-row arrays are rewritten by the next iteration
+        __syncthreads();                              // tiles and per-row arrays are rewritten by the next iteration
     }
     flush(cur_graph);
 
@@ -442,13 +384,13 @@ __global__ void __launch_bounds__(VT_THREADS, 1) virtual_layer_bwd_tc_kernel(con
     wgrad128_flush(a.g_wxv, gWxv, t);
     wgrad128_flush(a.g_wx, gWx, t);
     __syncthreads();
-    if (tid < H) {
-        atomicAdd(a.g_w1r + tid, gw1r[tid]);
-        atomicAdd(a.g_b2 + tid, gb2[tid]);
-        atomicAdd(a.g_bxv + tid, gbxv[tid]);
-        atomicAdd(a.g_w3xv + tid, gw3xv[tid]);
-        atomicAdd(a.g_bx + tid, gbx[tid]);
-        atomicAdd(a.g_w3x + tid, gw3x[tid]);
+    if (t < H) {
+        atomicAdd(a.g_w1r + t, gw1r[t]);
+        atomicAdd(a.g_b2 + t, gb2[t]);
+        atomicAdd(a.g_bxv + t, gbxv[t]);
+        atomicAdd(a.g_w3xv + t, gw3xv[t]);
+        atomicAdd(a.g_bx + t, gbx[t]);
+        atomicAdd(a.g_w3x + t, gw3x[t]);
     }
 }
 
@@ -460,10 +402,10 @@ extern "C" int distegnn_virtual_bwd_prepare(int A, int C, int Na, const float* l
     if (int rc = check_dims(A, C, Na)) return rc;
     DEGNN_CHECK_ARG(layer_params && weight_images, "null pointer");
     Layout L = make_layout(A, C, Na);
-    virtual_bwd_images_kernel<<<6, 256, 0, (cudaStream_t)stream>>>(layer_params + L.off[DISTEGNN_P_V_W2],
-                                                                   layer_params + L.off[DISTEGNN_P_V_WXV],
-                                                                   layer_params + L.off[DISTEGNN_P_V_WX],
-                                                                   reinterpret_cast<__half*>(weight_images));
+    virtual_bwd_images_kernel<<<6, VT_IMG_THREADS, 0, (cudaStream_t)stream>>>(layer_params + L.off[DISTEGNN_P_V_W2],
+                                                                              layer_params + L.off[DISTEGNN_P_V_WXV],
+                                                                              layer_params + L.off[DISTEGNN_P_V_WX],
+                                                                              reinterpret_cast<__half*>(weight_images));
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }
@@ -505,8 +447,7 @@ extern "C" int distegnn_virtual_layer_bwd(int64_t n_nodes, int n_graphs, int A, 
     a.g_w3x = g_layer_params + L.off[DISTEGNN_P_V_W3X];
     ensure_dynamic_smem((const void*)virtual_layer_bwd_tc_kernel, (int)VT_SMEM_BYTES);
     const int TN = TILE_M / C;
-    const int64_t tiles = (n_nodes + TN - 1) / TN;
-    int64_t grid = (tiles + VT_GROUPS - 1) / VT_GROUPS;
+    int64_t grid = (n_nodes + TN - 1) / TN;
     if (grid > sm_count()) grid = sm_count();
     virtual_layer_bwd_tc_kernel<<<(unsigned)grid, VT_THREADS, VT_SMEM_BYTES, (cudaStream_t)stream>>>(a);
     DEGNN_CHECK_LAUNCH();
