@@ -78,6 +78,8 @@ SIGNATURES = {
     "distegnn_frames_targets": [_i32, _i64, _i64, _i32] + [_vp] * 6,
     "distegnn_frames_assemble_noise": [_i32, _i32, _i64, _i64, _i32] + [_vp] * 14 + [C.c_uint64, _u32, C.c_float,
                                                                                   C.c_float, _vp],
+    "distegnn_frames_assemble_transform": [_i32, _i32, _i64, _i64, _i32] + [_vp] * 14 + [C.c_uint64, _i32,
+                                                                                      C.c_float, _vp],
     "distegnn_rollout_sq_err_workspace_bytes": [_i64, C.POINTER(_i64)],
     "distegnn_rollout_sq_err": [_i64, _i32, _i32] + [_vp] * 6 + [_i64, _vp],
     "distegnn_rollout_chamfer_workspace_bytes": [_i64, _i32, C.POINTER(_i64)],

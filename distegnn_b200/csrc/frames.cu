@@ -11,8 +11,12 @@
 //   distegnn_frames_assemble_noise   the same launches with training noise (frames_noise.cuh, DESIGN §22): ε_x is added
 //                              to x (also inside the whole-scene sum of loc_mean) and to every target row, ε_v to v
 //                              before ‖v‖; the kernels regenerate a node's ε wherever they need it
+//   distegnn_frames_assemble_transform   the same launches with a rigid transform per sample (frames_transform.cuh,
+//                              DESIGN §23): every staged position becomes R·x + t and every staged velocity R·v as it
+//                              is gathered, before any of the recipe's arithmetic
 #include "common.cuh"
 #include "frames_noise.cuh"
+#include "frames_transform.cuh"
 
 namespace degnn {
 
@@ -34,17 +38,22 @@ struct FramesArgs {
 };
 
 // One block per scene: Σx in fp64 by a fixed per-thread stride and a fixed tree, so the result does not depend on
-// scheduling; the max of static column 0 (order-independent).  NOISE: Σ(x + ε_x) over every node of the scene.
-template <bool NOISE>
-__global__ void __launch_bounds__(RED_THREADS) frames_scene_kernel(const FramesArgs a, const FramesNoise nz) {
+// scheduling; the max of static column 0 (order-independent).  NOISE: Σ(x + ε_x) over every node of the scene.  XFORM:
+// Σ(R·x + t) over every node of the scene.
+template <bool NOISE, bool XFORM>
+__global__ void __launch_bounds__(RED_THREADS) frames_scene_kernel(const FramesArgs a, const FramesNoise nz,
+                                                                    const FramesTransform xf) {
     __shared__ double ssum[3][RED_THREADS];
     __shared__ float smax[RED_THREADS];
     const int b = blockIdx.x, t = threadIdx.x;
     const int64_t lo = a.scene_ptr[b], hi = a.scene_ptr[b + 1];
     double s0 = 0.0, s1 = 0.0, s2 = 0.0;
     float m = -INFINITY;
+    Rigid T;
+    if (XFORM) frames_rigid(xf, b, T);
     for (int64_t i = lo + t; i < hi; i += RED_THREADS) {
         float x[3] = {__ldg(a.x0 + i * 3), __ldg(a.x0 + i * 3 + 1), __ldg(a.x0 + i * 3 + 2)};
+        if (XFORM) rigid_apply(T, x, true);
         if (NOISE) {
             float e[3];
             frames_noise(nz, b, i - lo, NOISE_POS, e);
@@ -90,9 +99,11 @@ __device__ __forceinline__ float speed_of(const float v[3]) {
 
 // One thread per output node.  Gathers are copies; v, ‖v‖ and the division are round-to-nearest fp32 operations in the
 // reference's order (no contraction).  NOISE: x, v and the target get one fp32 add of ε_x, ε_v, ε_x (v first computed as
-// without noise), and ‖v‖ is taken of the noisy v.
-template <bool NOISE>
-__global__ void __launch_bounds__(256) frames_node_kernel(const FramesArgs a, const FramesNoise nz) {
+// without noise), and ‖v‖ is taken of the noisy v.  XFORM: x, the target and pos[f+1] (Water-3D) become R·x + t and
+// vel[f] becomes R·v as they are gathered; v, ‖v‖ and the rest follow from those as without the transform.
+template <bool NOISE, bool XFORM>
+__global__ void __launch_bounds__(256) frames_node_kernel(const FramesArgs a, const FramesNoise nz,
+                                                          const FramesTransform xf) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.n_out; k += (int64_t)gridDim.x * blockDim.x) {
         const int b = sample_of(a.out_ptr, a.B, k);
         const int64_t base = __ldg(a.scene_ptr + b), n = __ldg(a.scene_ptr + b + 1) - base;
@@ -106,7 +117,19 @@ __global__ void __launch_bounds__(256) frames_node_kernel(const FramesArgs a, co
             x[d] = ok ? __ldg(a.x0 + g * 3 + d) : nan;
             y[d] = ok ? __ldg(a.xt + g * 3 + d) : nan;
             const float w = ok ? __ldg(a.x1 + g * 3 + d) : nan;
-            v[d] = a.recipe == DISTEGNN_FRAMES_WATER3D ? __fsub_rn(w, x[d]) : w;
+            v[d] = (XFORM || a.recipe != DISTEGNN_FRAMES_WATER3D) ? w : __fsub_rn(w, x[d]);
+        }
+        if (XFORM) {
+            Rigid T;
+            frames_rigid(xf, b, T);
+            const bool w3d = a.recipe == DISTEGNN_FRAMES_WATER3D;      // v holds pos[f+1] (a position) or vel[f]
+            rigid_apply(T, x, true);
+            rigid_apply(T, y, true);
+            rigid_apply(T, v, w3d);
+            if (w3d) {
+#pragma unroll
+                for (int d = 0; d < 3; ++d) v[d] = __fsub_rn(v[d], x[d]);
+            }
         }
         if (NOISE) {
             float ex[3], ev[3];
@@ -141,12 +164,14 @@ __global__ void __launch_bounds__(256) frames_node_kernel(const FramesArgs a, co
 }
 
 // One thread per (horizon step t >= 1, output node): targets[t] = frame 2 + t of the staged block (pos[f + (t+1)Δ]),
-// by the node kernel's scene offsets and index.  Copies only; NOISE: every row plus the node's ε_x (one fp32 add).
-template <bool NOISE>
+// by the node kernel's scene offsets and index.  Copies only; NOISE: every row plus the node's ε_x (one fp32 add);
+// XFORM: every row R·x + t.
+template <bool NOISE, bool XFORM>
 __global__ void __launch_bounds__(256) frames_targets_kernel(int B, int64_t n_frame, int64_t n_out, int K,
                                                              const float* frames, const int64_t* scene_ptr,
                                                              const int64_t* out_ptr, const int32_t* index,
-                                                             float* targets, const FramesNoise nz) {
+                                                             float* targets, const FramesNoise nz,
+                                                             const FramesTransform xf) {
     const int64_t total = (int64_t)(K - 1) * n_out;
     for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
         const int64_t t = q / n_out + 1, k = q - (t - 1) * n_out;
@@ -162,6 +187,13 @@ __global__ void __launch_bounds__(256) frames_targets_kernel(int B, int64_t n_fr
             frames_noise(nz, b, li, NOISE_POS, e);
 #pragma unroll
             for (int d = 0; d < 3; ++d) dst[d] = __fadd_rn(ok ? __ldg(src + d) : nan, e[d]);
+        } else if (XFORM) {
+            Rigid T;
+            frames_rigid(xf, b, T);
+            float x[3] = {ok ? __ldg(src) : nan, ok ? __ldg(src + 1) : nan, ok ? __ldg(src + 2) : nan};
+            rigid_apply(T, x, true);
+#pragma unroll
+            for (int d = 0; d < 3; ++d) dst[d] = x[d];
         } else {
 #pragma unroll
             for (int d = 0; d < 3; ++d) dst[d] = ok ? __ldg(src + d) : nan;
@@ -217,10 +249,10 @@ extern "C" int distegnn_frames_assemble(int recipe, int n_samples, int64_t n_fra
                                a);
     if (rc != DISTEGNN_OK) return rc;
     const FramesNoise none{};
-    frames_scene_kernel<false><<<n_samples, RED_THREADS, 0, (cudaStream_t)stream>>>(a, none);
+    frames_scene_kernel<false, false><<<n_samples, RED_THREADS, 0, (cudaStream_t)stream>>>(a, none, FramesTransform{});
     DEGNN_CHECK_LAUNCH();
     if (n_out > 0) {
-        frames_node_kernel<false><<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a, none);
+        frames_node_kernel<false, false><<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a, none, FramesTransform{});
         DEGNN_CHECK_LAUNCH();
     }
     return DISTEGNN_OK;
@@ -234,8 +266,9 @@ extern "C" int distegnn_frames_targets(int n_samples, int64_t n_frame_nodes, int
     DEGNN_CHECK_ARG(index || n_out == n_frame_nodes, "without an index list every node is gathered (n_out == n_frame_nodes)");
     if (horizon == 1 || n_out == 0) return DISTEGNN_OK;
     DEGNN_CHECK_ARG(frames && scene_ptr && out_ptr && targets, "null pointer");
-    frames_targets_kernel<false><<<node_grid((int64_t)(horizon - 1) * n_out), 256, 0, (cudaStream_t)stream>>>(
-        n_samples, n_frame_nodes, n_out, horizon, frames, scene_ptr, out_ptr, index, targets, FramesNoise{});
+    frames_targets_kernel<false, false><<<node_grid((int64_t)(horizon - 1) * n_out), 256, 0, (cudaStream_t)stream>>>(
+        n_samples, n_frame_nodes, n_out, horizon, frames, scene_ptr, out_ptr, index, targets, FramesNoise{},
+        FramesTransform{});
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }
@@ -258,14 +291,51 @@ extern "C" int distegnn_frames_assemble_noise(int recipe, int n_samples, int64_t
                                a);
     if (rc != DISTEGNN_OK) return rc;
     const FramesNoise nz{sample_ids, seed, epoch, sigma_x, sigma_v};
-    frames_scene_kernel<true><<<n_samples, RED_THREADS, 0, (cudaStream_t)stream>>>(a, nz);
+    const FramesTransform none{};
+    frames_scene_kernel<true, false><<<n_samples, RED_THREADS, 0, (cudaStream_t)stream>>>(a, nz, none);
     DEGNN_CHECK_LAUNCH();
     if (n_out > 0) {
-        frames_node_kernel<true><<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a, nz);
+        frames_node_kernel<true, false><<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a, nz, none);
         DEGNN_CHECK_LAUNCH();
         if (horizon > 1) {
-            frames_targets_kernel<true><<<node_grid((int64_t)(horizon - 1) * n_out), 256, 0, (cudaStream_t)stream>>>(
-                n_samples, n_frame_nodes, n_out, horizon, frames, scene_ptr, out_ptr, index, targets, nz);
+            frames_targets_kernel<true, false><<<node_grid((int64_t)(horizon - 1) * n_out), 256, 0,
+                                                 (cudaStream_t)stream>>>(
+                n_samples, n_frame_nodes, n_out, horizon, frames, scene_ptr, out_ptr, index, targets, nz, none);
+            DEGNN_CHECK_LAUNCH();
+        }
+    }
+    return DISTEGNN_OK;
+}
+
+extern "C" int distegnn_frames_assemble_transform(int recipe, int n_samples, int64_t n_frame_nodes, int64_t n_out,
+                                                  int horizon, const float* frames, const float* statics,
+                                                  const int64_t* scene_ptr, const int64_t* out_ptr,
+                                                  const int32_t* index, float* node_feat, float* node_loc,
+                                                  float* node_vel, float* node_attr, float* targets,
+                                                  int64_t* data_batch, float* loc_mean, float* scene_max,
+                                                  const int64_t* sample_ids, uint64_t seed, int rotate,
+                                                  float translate, void* stream) {
+    using namespace degnn;
+    DEGNN_CHECK_ARG(horizon >= 1, "horizon must be >= 1");
+    DEGNN_CHECK_ARG(rotate == 0 || rotate == 1, "rotate must be 0 or 1");
+    DEGNN_CHECK_ARG(isfinite(translate) && translate >= 0.f, "translate must be finite and >= 0");
+    DEGNN_CHECK_ARG(sample_ids, "null sample_ids");
+    FramesArgs a;
+    const int rc = frames_args(__func__, recipe, n_samples, n_frame_nodes, n_out, frames, statics, scene_ptr, out_ptr,
+                               index, node_feat, node_loc, node_vel, node_attr, targets, data_batch, loc_mean, scene_max,
+                               a);
+    if (rc != DISTEGNN_OK) return rc;
+    const FramesNoise none{};
+    const FramesTransform xf{sample_ids, seed, translate, rotate};
+    frames_scene_kernel<false, true><<<n_samples, RED_THREADS, 0, (cudaStream_t)stream>>>(a, none, xf);
+    DEGNN_CHECK_LAUNCH();
+    if (n_out > 0) {
+        frames_node_kernel<false, true><<<node_grid(n_out), 256, 0, (cudaStream_t)stream>>>(a, none, xf);
+        DEGNN_CHECK_LAUNCH();
+        if (horizon > 1) {
+            frames_targets_kernel<false, true><<<node_grid((int64_t)(horizon - 1) * n_out), 256, 0,
+                                                 (cudaStream_t)stream>>>(
+                n_samples, n_frame_nodes, n_out, horizon, frames, scene_ptr, out_ptr, index, targets, none, xf);
             DEGNN_CHECK_LAUNCH();
         }
     }

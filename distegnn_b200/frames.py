@@ -39,6 +39,16 @@ recorded one; loc_mean is the whole-scene mean of the noisy positions and the gr
 clean frame's.  ε is a pure function of (noise_seed, epoch, sample index, scene node), generated inside the assembly
 kernels: every rank, world size, batch size and order sees the same noise for the same node.  The epoch is the number of
 earlier `batches()` calls (every iteration draws one).
+
+Rotated and translated evaluation splits (DESIGN §23).  `FrameLoader(..., rotate=True, translate=S)` gives every sample a
+rigid transform, R Haar-uniform on SO(3) and t ~ N(0, S²·I), applied to every staged position (R·x + t) and velocity
+(R·v) before the recipe's arithmetic, for measuring that test error does not depend on the frame (the reference's
+`test_rot` / `test_trans`):
+
+    valid = FrameLoader(traj, samples, ..., rotate=True, translate=1.0)                 # a fixed copy of the split
+
+(R, t) is a pure function of (transform_seed, sample index), independent of the epoch, generated inside the assembly
+kernels; the split is the untransformed frame's and the graph is built on the transformed positions.
 """
 from __future__ import annotations
 
@@ -255,6 +265,22 @@ def _check_noise(noise) -> Optional[Tuple[float, float]]:
     return None if sx == 0 and sv == 0 else (sx, sv)
 
 
+def _check_transform(rotate, translate) -> Optional[Tuple[bool, float]]:
+    """FrameLoader's `rotate`, `translate` as (rotate, translate), or None for no transform (False, 0); ValueError
+    otherwise."""
+    if not isinstance(rotate, (bool, np.bool_)):
+        raise ValueError(f"rotate must be True or False (got {rotate!r})")
+    if isinstance(translate, (str, bytes, bool)):
+        raise ValueError(f"translate must be a finite number >= 0 (got {translate!r})")
+    try:
+        t = float(translate)
+    except (TypeError, ValueError):
+        raise ValueError(f"translate must be a finite number >= 0 (got {translate!r})") from None
+    if not (np.isfinite(t) and t >= 0):
+        raise ValueError(f"translate must be a finite number >= 0 (got {translate!r})")
+    return None if not rotate and t == 0 else (bool(rotate), t)
+
+
 def complete_graph_edges(n: int) -> Tensor:
     """The reference's fully connected edge list (process_dataset.py:98): [[i, j] for i for j if i != j], int64 [2,E]."""
     i = torch.arange(n).repeat_interleave(max(n - 1, 0))
@@ -281,6 +307,11 @@ class FrameLoader:
     noise           (σ_x, σ_v), finite and >= 0: training noise on positions (and every target row) and velocities (module
                     docstring, DESIGN §22).  None or (0, 0): no noise, the same launches as without the argument
     noise_seed      the noise's seed, an int in [0, 2^64) (default `seed`)
+    rotate, translate   an evaluation split in another frame (module docstring, DESIGN §23): every sample gets a
+                    rotation (Haar-uniform; rotate=True) and a translation translate·N(0, I) (translate finite and >= 0),
+                    a function of (transform_seed, sample index) only.  False, 0: the same launches as without them.
+                    Not combined with `noise` (ValueError)
+    transform_seed  the transform's seed, an int in [0, 2^64) (default `seed`)
     """
 
     def __init__(self, traj: Trajectories, samples: Sequence[Tuple[int, int]], delta_t: int = 1,
@@ -288,7 +319,8 @@ class FrameLoader:
                  drop_last: bool = True, device=None, prefetch: int = 2, world_size: int = 1, rank: int = 0,
                  split_mode: str = "random", split_seed: Optional[int] = None, cutoff_rate: float = 0.0,
                  capacity: Optional[int] = None, edge_attr_nf: int = 2, loop: bool = False, horizon: int = 1,
-                 noise: Optional[Tuple[float, float]] = None, noise_seed: Optional[int] = None):
+                 noise: Optional[Tuple[float, float]] = None, noise_seed: Optional[int] = None,
+                 rotate: bool = False, translate: float = 0.0, transform_seed: Optional[int] = None):
         self.traj, self.samples, self.delta_t = traj, [(int(s), int(f)) for s, f in samples], int(delta_t)
         check_samples(traj, self.samples, self.delta_t, horizon)
         self.horizon = horizon
@@ -315,6 +347,17 @@ class FrameLoader:
                 raise ValueError(f"noise_seed must be an int in [0, 2^64) (got {self.noise_seed})")
             if len(self.samples) >= 1 << 32:
                 raise ValueError(f"training noise numbers samples with 32 bits: {len(self.samples)} samples are too many")
+        self.transform = _check_transform(rotate, translate)
+        self.transform_seed = int(seed if transform_seed is None else transform_seed)
+        if self.transform is not None:
+            if self.noise is not None:
+                raise ValueError("noise and a rigid transform (rotate / translate) cannot be combined: the noise is for "
+                                 "training, the transform for evaluation splits")
+            if not 0 <= self.transform_seed < 1 << 64:
+                raise ValueError(f"transform_seed must be an int in [0, 2^64) (got {self.transform_seed})")
+            if len(self.samples) >= 1 << 32:
+                raise ValueError(f"the rigid transform numbers samples with 32 bits: {len(self.samples)} samples are "
+                                 "too many")
         self.epoch = 0
 
     def __len__(self) -> int:
@@ -383,11 +426,11 @@ class FrameLoader:
             counts.append(cnt[self.rank])
             off += n
         B = len(idx)
-        noisy = self.noise is not None
+        noisy = self.noise is not None or self.transform is not None
         meta = torch.empty(2 * B + 2 + (B if noisy else 0), dtype=torch.int64, pin_memory=pin)
         meta[:B + 1] = torch.tensor([0] + list(np.cumsum(ns)), dtype=torch.int64)
         meta[B + 1:2 * B + 2] = torch.tensor([0] + list(np.cumsum(counts)), dtype=torch.int64)
-        if noisy:                                                # the samples' indices: the noise's sample numbers
+        if noisy:                                                # the samples' indices: the noise's / transform's
             meta[2 * B + 2:] = torch.tensor(list(idx), dtype=torch.int64)
         host = dict(frames=frames, statics=statics, meta=meta, n_frame=N, node_counts=counts, epoch=epoch)
         if self.world_size > 1:
@@ -436,6 +479,12 @@ class FrameLoader:
                     ptr(index), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(targets), ptr(batch), ptr(loc_mean),
                     ptr(scene_max), ptr(meta[2 * B + 2:]), self.noise_seed, host["epoch"] % (1 << 32), self.noise[0],
                     self.noise[1], _lib.stream_ptr(dev)), "frames_assemble_noise")
+            elif self.transform is not None:
+                check(_lib.load().distegnn_frames_assemble_transform(
+                    rc.code, B, host["n_frame"], M, K, ptr(frames), ptr(statics), ptr(scene_ptr), ptr(out_ptr),
+                    ptr(index), ptr(feat), ptr(loc), ptr(vel), ptr(attr), ptr(targets), ptr(batch), ptr(loc_mean),
+                    ptr(scene_max), ptr(meta[2 * B + 2:]), self.transform_seed, int(self.transform[0]),
+                    self.transform[1], _lib.stream_ptr(dev)), "frames_assemble_transform")
             else:
                 check(_lib.load().distegnn_frames_assemble(
                     rc.code, B, host["n_frame"], M, ptr(frames), ptr(statics), ptr(scene_ptr), ptr(out_ptr),

@@ -619,6 +619,26 @@ DISTEGNN_API int distegnn_frames_assemble_noise(int recipe, int n_samples, int64
                                                 float *targets, int64_t *data_batch, float *loc_mean, float *scene_max,
                                                 const int64_t *sample_ids, uint64_t seed, uint32_t epoch,
                                                 float sigma_x, float sigma_v, void *stream);
+/* distegnn_frames_assemble_transform: the assembly and its multi-step targets with a rigid transform per sample (DESIGN
+ * §23), for rotated and translated evaluation splits.  Arguments as for distegnn_frames_assemble_noise, with rotate
+ * (0 or 1) and translate (>= 0) in place of epoch and the σs.  For sample b = sample_ids[·] and seed s, R is the matrix
+ * of the unit quaternion of the four Box–Muller normals of Philox4x32-10(counter (0, 2, b, 0), key (lo32 s, hi32 s))
+ * (Haar-uniform on SO(3); R = I for rotate = 0) and t = translate·(z0, z1, z2) of counter (0, 3, b, 0)
+ * (csrc/frames_transform.cuh).  Every staged position (pos[f], Water-3D's pos[f+1], every pos[f + tΔ]) becomes
+ * ((R_a0·x0 + R_a1·x1) + R_a2·x2) + t_a and every staged velocity the same without t, round-to-nearest fp32, as it is
+ * gathered; v, ‖v‖, loc_mean (over the WHOLE transformed scene), the targets and the other fields follow from them as
+ * without the transform.  A sample id outside [0, 2^32) gives NaN in every transformed value of that sample.  Rejects
+ * rotate other than 0 / 1, translate < 0 or not finite, a NULL sample_ids, horizon < 1 and the assembly's argument
+ * errors before any launch.  Launches the scene, node and (horizon > 1) targets kernels; no workspace, no allocation, no
+ * host synchronisation; capturable. */
+DISTEGNN_API int distegnn_frames_assemble_transform(int recipe, int n_samples, int64_t n_frame_nodes, int64_t n_out,
+                                                    int horizon, const float *frames, const float *statics,
+                                                    const int64_t *scene_ptr, const int64_t *out_ptr,
+                                                    const int32_t *index, float *node_feat, float *node_loc,
+                                                    float *node_vel, float *node_attr, float *targets,
+                                                    int64_t *data_batch, float *loc_mean, float *scene_max,
+                                                    const int64_t *sample_ids, uint64_t seed, int rotate,
+                                                    float translate, void *stream);
 
 #ifdef __cplusplus
 }

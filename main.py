@@ -29,7 +29,10 @@ it then rolls the trained model out K steps from every validation batch and prin
 frames f + Δ .. f + KΔ (DESIGN §19; `--rollout_tau` sets the velocity's time step, Water-3D defaults to Δ);
 `--rollout_chamfer` adds both directions of the normalised Chamfer distance to every step's line (DESIGN §20).
 `--train_noise SX,SV` trains on noisy input states (FrameLoader's `noise`, DESIGN §22); the evaluation and the rollout stay
-noise-free.  Without the flag the synthetic path below runs unchanged.
+noise-free.  `--eval_rotate` and / or `--eval_translate S` evaluate (and roll out) the validation split twice, as recorded
+and with every sample rotated and translated (FrameLoader's `rotate` / `translate`, DESIGN §23), and print the relative
+difference of the two mean MSEs: an equivariant model's error does not depend on the frame.  Without the flags the
+synthetic path below runs unchanged.
 
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
 `batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
@@ -112,6 +115,11 @@ def parse():
     p.add_argument("--train_noise", type=str, default=None, help="(new) with --trajectory: SX,SV, the standard deviations "
                    "of the training noise on positions (and targets) and on velocities (FrameLoader's noise, DESIGN §22); "
                    "the train loader only, the evaluation and the rollout stay noise-free")
+    p.add_argument("--eval_rotate", action="store_true", help="(new) with --trajectory: evaluate (and roll out) the "
+                   "validation split a second time with every sample rotated, Haar-uniform (FrameLoader's rotate, "
+                   "DESIGN §23), and print the relative difference of the mean MSEs")
+    p.add_argument("--eval_translate", type=str, default=None, help="(new) with --trajectory: S >= 0, the scale of the "
+                   "second evaluation's per-sample translation S·N(0, I) (FrameLoader's translate, DESIGN §23)")
     return p.parse_args()
 
 
@@ -137,9 +145,35 @@ def train_noise_of(args):
     return sx, sv
 
 
+def eval_transform_of(args):
+    """--eval_rotate / --eval_translate S as (rotate, translate), or None; exits with a message on a malformed or
+    negative scale."""
+    if not args.eval_rotate and args.eval_translate is None:
+        return None
+    import math
+    msg, t = None, 0.0
+    if args.eval_translate is not None:
+        try:
+            t = float(args.eval_translate)
+        except ValueError:
+            msg = "a number"
+        else:
+            if not (math.isfinite(t) and t >= 0):
+                msg = "finite and >= 0"
+    if msg is None and not args.trajectory:
+        msg = "used with --trajectory"
+    if msg is not None:
+        if int(os.environ.get("LOCAL_RANK", "0")) == 0:
+            what = f"--eval_translate {args.eval_translate!r}" if args.eval_translate is not None else "--eval_rotate"
+            print(f"{what}: must be {msg}", flush=True)
+        sys.exit(2)
+    return bool(args.eval_rotate), t
+
+
 def main():
     args = parse()
     noise = train_noise_of(args)
+    transform = eval_transform_of(args)
     with open(args.config_path) as f:
         cfg = yaml.safe_load(f)
     cfg.setdefault("data", {})
@@ -199,7 +233,7 @@ def main():
         model = DistributedDataParallel(model, device_ids=[local_rank], find_unused_parameters=True)
     model.eval()
     if args.trajectory:
-        trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise)
+        trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform)
         if distributed:
             dist.destroy_process_group()
         return
@@ -285,15 +319,17 @@ def recipe_of_config(cfg):
     return recipe, 0, int(d.get("delta_t", 1))
 
 
-def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("train", "valid"), noise=None):
+def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("train", "valid"), noise=None,
+                  transform=None):
     """FrameLoaders over the raw trajectories under `path` with the config's recipe (datasets/process_dataset.py):
     N-body (`dataset_name: nbody*`, the reference's loc_/vel_/charges_ .npy files, frame_0 / frame_T), Water-3D or
     Fluid113K (`path`/train/*.npz, `path`/valid/*.npz).  cutoff_edges mode: one graph per sample, radius = data.radius
     (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
     sample split over the ranks by split_mode (metis / spectral fall back to random), a radius graph per partition with
     inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
-    N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only.
-    Returns (recipe name, {part: loader or None})."""
+    N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only;
+    `transform` (rotate, translate) to every loader built (the same samples as without it: a rotated and translated
+    copy of the split).  Returns (recipe name, {part: loader or None})."""
     import glob
     from distegnn_b200.frames import FrameLoader, load_nbody, load_scenes, sample_list
     d = cfg["data"]
@@ -307,6 +343,7 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     if split not in ("random", "kmeans"):
         split = "random"
     seed, bs = int(cfg.get("seed", 0)), int(d.get("batch_size", 1))
+    xf = {} if transform is None else dict(rotate=transform[0], translate=transform[1])
     out = {}
     for part in parts:
         if recipe == "nbody":
@@ -330,16 +367,18 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
         samples = sample_list(traj, seed=seed, max_samples=d.get("max_samples"), delta_t=delta, frame_0=frame_0, **kw)
         out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
                                 seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
-                                cutoff_rate=rate or 0.0, horizon=horizon, noise=noise if part == "train" else None)
+                                cutoff_rate=rate or 0.0, horizon=horizon, noise=noise if part == "train" else None,
+                                **xf)
     if "train" in parts and out["train"] is None:
         raise SystemExit(f"--trajectory {path}: no training data for recipe {recipe!r}")
     return recipe, out
 
 
-def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None):
+def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None):
     """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
     reference's training step on batches from FrameLoader (with `noise` on its inputs), then the mean MSE over the
-    validation batches (noise-free)."""
+    validation batches (noise-free); with `transform` (rotate, translate) also over the same batches rigidly
+    transformed, and the relative difference of the two."""
     from distegnn_b200 import train_loss
     recipe, _, delta = recipe_of_config(cfg)
     K = args.rollout_steps
@@ -392,36 +431,59 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, 
         ev = loaders["train"] if noise is None else \
             frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, parts=("train",))[1]["train"]
     model.eval()
-    tot, n = 0.0, 0
-    with torch.no_grad():
-        for kw, ex in ev:
-            _, info = loss_of(kw, ex)
-            tot, n = tot + float(info["logged"]), n + 1
+    part = "valid" if loaders["valid"] else "train"
+
+    def mean_mse(ld):
+        tot, n = 0.0, 0
+        with torch.no_grad():
+            for kw, ex in ld:
+                _, info = loss_of(kw, ex)
+                tot, n = tot + float(info["logged"]), n + 1
+        return tot / max(n, 1), n
+
+    plain, n = mean_mse(ev)
     if local_rank == 0:
-        print(f"[{recipe}] evaluation over {n} batches ({'valid' if loaders['valid'] else 'train'}): mean MSE "
-              f"{tot / max(n, 1):.6e}")
+        print(f"[{recipe}] evaluation over {n} batches ({part}): mean MSE {plain:.6e}")
+    if transform is not None:                                  # the same samples, batches and split, transformed
+        moved, n = mean_mse(frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, parts=(part,),
+                                          transform=transform)[1][part])
+        if local_rank == 0:
+            rel = (moved - plain) / plain if plain != 0 else float("nan")
+            print(f"[{recipe}] evaluation over {n} batches ({part}, {transform_label(transform)}): mean MSE "
+                  f"{moved:.6e}, relative difference {rel:+.3e}", flush=True)
     if K > 0:
         rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau)
+        if transform is not None:
+            rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau, transform)
+
+
+def transform_label(transform):
+    rotate, translate = transform
+    return " and ".join((["rotated"] if rotate else []) + ([f"translated by {translate:g}"] if translate else [])) \
+        or "untransformed"
 
 
 # the |v| column of each recipe's node features (distegnn_b200/frames.py): N-body, Water-3D [‖v‖, ·], Fluid113K [·, ·, ‖v‖]
 SPEED_COL = {"nbody": 0, "water3d": 0, "largefluid": 2}
 
 
-def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau):
+def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau, transform=None):
     """--trajectory with --rollout_steps K: a K-step `rollout(targets=...)` from every batch of the valid split (the
     train split without one), through a FrameLoader with horizon K and the config's radius and cutoff rate; prints the
     per-step MSE averaged over the batches, each weighted by its graph count (utils/train.py:112-114, 166).  With
-    --rollout_chamfer each line also carries the two directions of `chamfer_mse`, averaged the same way."""
+    --rollout_chamfer each line also carries the two directions of `chamfer_mse`, averaged the same way.  `transform`
+    (rotate, translate): the split rigidly transformed (its targets too), lines marked with the transform."""
     from distegnn_b200 import rollout
     K = args.rollout_steps
     dev = torch.device("cuda", local_rank)
     part = "valid"
     try:
-        _, lds = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=K, parts=(part,))
+        _, lds = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=K, parts=(part,),
+                               transform=transform)
         if lds[part] is None:
             part = "train"
-            _, lds = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=K, parts=(part,))
+            _, lds = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=K, parts=(part,),
+                                   transform=transform)
     except ValueError as e:                                    # a sample that cannot hold K steps
         if local_rank == 0:
             print(f"--rollout_steps {K}: {e}", flush=True)
@@ -447,11 +509,13 @@ def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau):
     ch = (ch_tot / max(graphs, 1)).tolist()
     dt = time.perf_counter() - t0
     if local_rank == 0:
-        print(f"[{recipe}] rollout evaluation over {n} batches ({part}), {K} steps, tau={tau:g}: "
+        which = part if transform is None else f"{part}, {transform_label(transform)}"
+        print(f"[{recipe}] rollout evaluation over {n} batches ({which}), {K} steps, tau={tau:g}: "
               f"{dt / max(n * K, 1) * 1e3:.2f} ms/step", flush=True)
+        tag = "" if transform is None else f" ({transform_label(transform)})"
         for t, v in enumerate(mse):
             extra = f", Chamfer pred->rec {ch[t][0]:.6e}, rec->pred {ch[t][1]:.6e}" if args.rollout_chamfer else ""
-            print(f"[{recipe}] rollout step {t + 1}: MSE {v:.6e}{extra}", flush=True)
+            print(f"[{recipe}] rollout step {t + 1}{tag}: MSE {v:.6e}{extra}", flush=True)
 
 
 def cutoff_inputs(w, batch_size, seed, rate, device):
