@@ -31,6 +31,7 @@ SIGNATURES = {
     "distegnn_param_layout": [_i32, _i32, _i32, C.POINTER(_i64), C.POINTER(_i64)],
     "distegnn_csr_workspace_bytes": [_i64, _i64, C.POINTER(_i64)],
     "distegnn_build_csr": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp],
+    "distegnn_build_csr_cells": [_vp, _i64, _i64, _vp, _vp, _i32] + [_vp] * 5 + [_i64, _vp, _vp],
     "distegnn_gather_rows": [_vp, _vp, _i64, _i32, _vp, _vp],
     "distegnn_scatter_rows": [_vp, _vp, _i64, _i32, _vp, _vp],
     "distegnn_embed_fwd": [_i64, _i32, _i32, _i32, _i32, _i32] + [_vp] * 15,

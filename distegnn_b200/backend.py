@@ -35,10 +35,20 @@ class CudaBackend:
     # ---- graph preprocessing -------------------------------------------------------------------
     def build_csr(self, edge_index: Tensor, n_nodes: int, validate: bool = True
                   ) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
-        """int64 COO -> int32 CSR by destination.  `validate`: read back the out-of-range counter (one host sync per
-        build; builds are cached per edge_index) and raise ValueError like the reference's index assert would;
-        validate="defer" hands the device counter back as a fifth value instead (the caller reads it together with the
-        data_batch counter after the embed kernel: one pipeline drain for both checks; ids are clamped meanwhile)."""
+        """int64 COO -> int32 CSR by destination, rows in id order.  `validate`: read back the out-of-range counter (one
+        host sync per build; builds are cached per edge_index) and raise ValueError like the reference's index assert
+        would; validate="defer" hands the device counter back as a fifth value instead (the caller reads it together with
+        the data_batch counter after the embed kernel: one pipeline drain for both checks; ids are clamped meanwhile)."""
+        return self._build_csr(edge_index, n_nodes, validate, None, None, 1)
+
+    def build_csr_cells(self, edge_index: Tensor, n_nodes: int, pos: Tensor, batch: Optional[Tensor], n_graphs: int,
+                        validate: bool = True):
+        """`build_csr` with the rows in (graph, cell of `pos`, id) order (DESIGN §3): the same rowptr, the edges of every
+        row contiguous, the rows of nearby destinations next to each other.  `pos` float32 [N,3] contiguous, `batch`
+        int64 sorted or None for one graph."""
+        return self._build_csr(edge_index, n_nodes, validate, pos, batch, n_graphs)
+
+    def _build_csr(self, edge_index, n_nodes, validate, pos, batch, n_graphs):
         E = int(edge_index.shape[1])
         dev = edge_index.device
         stream = self._s(edge_index)
@@ -50,9 +60,14 @@ class CudaBackend:
         check(self.lib.distegnn_csr_workspace_bytes(n_nodes, E, C.byref(nbytes)), "csr_workspace_bytes")
         ws = torch.empty(max(int(nbytes.value), 1), dtype=torch.uint8, device=dev)
         bad = torch.empty(1, dtype=torch.int32, device=dev) if validate else None
-        check(self.lib.distegnn_build_csr(ptr(edge_index), n_nodes, E, ptr(rowptr), ptr(row), ptr(col),
-                                          ptr(perm), ptr(ws), ws.numel(), ptr(bad), stream), "build_csr")
-        self.launches += (5 if E else 1) + (1 if validate else 0)
+        if pos is None:
+            check(self.lib.distegnn_build_csr(ptr(edge_index), n_nodes, E, ptr(rowptr), ptr(row), ptr(col),
+                                              ptr(perm), ptr(ws), ws.numel(), ptr(bad), stream), "build_csr")
+        else:
+            check(self.lib.distegnn_build_csr_cells(ptr(edge_index), n_nodes, E, ptr(pos), ptr(batch), n_graphs,
+                                                    ptr(rowptr), ptr(row), ptr(col), ptr(perm), ptr(ws), ws.numel(),
+                                                    ptr(bad), stream), "build_csr_cells")
+        self.launches += (6 + (7 if pos is not None else 0) if E else 1) + (1 if validate else 0)
         if validate == "defer":
             return rowptr, row, col, perm, (bad if E else None)
         if validate and E and int(bad.item()) != 0:

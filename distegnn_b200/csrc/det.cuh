@@ -4,7 +4,8 @@
 //   edge stage   the edges are cut into slices of 16 (warp w of tile t owns edges 16(4t + w) .. +15, whatever the grid);
 //                a slice sums its runs of equal destination row in edge order and stores each partial.  A row's first
 //                slice writes it to the row, every later slice of the row to its slot; distegnn_edge_combine_det adds
-//                the slots in slice order.
+//                the slots in slice order.  The rows need only have contiguous edges, in any row order: a row's
+//                slices are consecutive, and its first slice is the one whose edge before it has another row.
 //   vsum         the real<->virtual kernel's tiles are grouped into chunks of 2^det_chunk_shift(N, C) consecutive tiles
 //                (16 or more, a power of two: at most DET_MAX_CHUNKS chunks); a chunk is summed in tile order by one
 //                pipeline.  A graph's first chunk writes its partial to vsum, every later chunk of the graph to the

@@ -16,6 +16,8 @@
 // Gradient rows span many orders of magnitude, so EVERY row is encoded with its own power-of-two scale (row maximum
 // taken from the registers), not only the rows that would overflow; D rows are multiplied by 1/scale on the way out.
 // The row rules (encoding, row-tile GEMM, φ-head backward, column sums, weight gradients) live in bwd_tc_common.cuh.
+// Edge order: g_P is summed over runs of equal destination row, so the edges of a row must be contiguous; the rows may
+// come in any order (the cached graph's spatial order, DESIGN §3).
 #include "edge_layer_bwd_tc.cuh"
 
 namespace degnn {

@@ -21,9 +21,12 @@
 //                                     per buffer)
 //   x[row], x[col] of tile i+1        cp.async at the start of tile i, read at its end
 //   (row, col, edge_attr) of tile i+2 cp.async at the start of tile i, moved to registers at its end
-//   P[row] of tile i+1                prefetched towards L1 at the start of tile i (rows are sorted: a tile has few)
+//   P[row] of tile i+1                prefetched towards L1 at the start of tile i (rows are contiguous: a tile has few)
 // Stages 2 and 3 run in the "t domain" (common.cuh silu4t): −log2(e) is folded into W2 and the biases, −ln 2 into w3 and
 // the segment-sum flush, so the SiLU never forms its exponent argument explicitly.
+// Edge order: the one thing the kernel needs is that the edges of a destination row are contiguous (the run masks compare
+// neighbouring rows; the deterministic slots compare row[e0 - 1] with the slice's first row).  The rows themselves may come
+// in any order: the cached graph stores them in a spatial order (DESIGN §3), graphs from shards in id order.
 #include <cuda_fp16.h>
 #include <string.h>
 
@@ -271,7 +274,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         // ---- MMA 1; the run-start mask of the warp's edges while it runs --------------------------------------------
         float d[32];
         tc16::mma_f16x3_rA<CS_LBO>(d, ahi, alo, bW2hi, bW2lo);
-        // bit e = edge e of the warp starts a new run of equal destination rows (rows are sorted; warp-uniform)
+        // bit e = edge e of the warp starts a new run of equal destination rows (rows are contiguous; warp-uniform)
         const int row_prev = __shfl_up_sync(FULL, row_c, 1);
         const uint32_t M = __ballot_sync(FULL, lane == 0 || row_prev != row_c) & 0xffffu;
         tc16::mma_f16x3_rA_wait(d, ahi, alo);

@@ -124,24 +124,34 @@ def pack_layer_params(g: nn.Module, A: int, Cn: int, Na: int, device, offs: Dict
 
 
 class _GraphCache:
-    """CSR (sorted-by-destination) form of recent edge_index tensors.  Entries hold a strong reference
-    to the tensor they were built from, so its storage cannot be recycled under the same pointer; a hit
-    additionally requires an unchanged in-place version counter."""
+    """CSR form of recent edge_index tensors.  Entries hold a strong reference to the tensor they were built from, so its
+    storage cannot be recycled under the same pointer; a hit additionally requires an unchanged in-place version counter.
+
+    With `pos`, the rows are stored in the spatial order of those positions, the ones of the call that builds the entry
+    (DESIGN §3); later calls reuse that order whatever their positions, since outside the deterministic mode the order
+    only decides which neighbour rows the edge kernels find in L2.  Without `pos` they are in id order, which depends on
+    edge_index alone: the deterministic mode's bits depend on where each row starts in the edge list (§17), so it asks
+    for id order.  The two orders are cached as separate entries.  The torch stand-in of the CPU tests has no
+    `build_csr_cells`; it restates the kernels with order-independent sums, and gets id order."""
 
     def __init__(self, capacity: int = 4):
         self.capacity = capacity
-        self.entries: "OrderedDict[int, tuple]" = OrderedDict()
+        self.entries: "OrderedDict[Tuple[int, bool], tuple]" = OrderedDict()
         self.builds = 0
         self.pending = None                # device counter of the last build's out-of-range edge ids (read after embed)
 
-    def get(self, backend, edge_index: Tensor, n_nodes: int, validate: bool = True):
-        key = id(edge_index)
+    def get(self, backend, edge_index: Tensor, n_nodes: int, validate: bool = True, pos: Optional[Tensor] = None,
+            batch: Optional[Tensor] = None, n_graphs: int = 1):
+        spatial = pos is not None and hasattr(backend, "build_csr_cells")
+        key = (id(edge_index), spatial)
         hit = self.entries.get(key)
         if hit is not None and hit[0] is edge_index and hit[1] == edge_index._version and hit[2] == n_nodes:   # noqa: E501
             self.entries.move_to_end(key)
             return hit[3]
         ei = edge_index if edge_index.is_contiguous() else edge_index.contiguous()
-        built = backend.build_csr(ei, n_nodes, "defer" if validate else False)
+        mode = "defer" if validate else False
+        built = (backend.build_csr_cells(ei, n_nodes, pos, batch, n_graphs, mode) if spatial
+                 else backend.build_csr(ei, n_nodes, mode))
         csr, self.pending = tuple(built[:4]), (built[4] if validate else None)     # counter of out-of-range ids, not yet read
         self.builds += 1
         self.entries[key] = (edge_index, edge_index._version, n_nodes, csr)
@@ -150,15 +160,16 @@ class _GraphCache:
         return csr
 
     def sorted_edge_attr(self, backend, edge_index: Tensor, edge_attr: Tensor, perm: Tensor) -> Tensor:
-        """edge_attr permuted into CSR order, cached next to the CSR of `edge_index` while the SAME edge_attr
-        tensor (identity + in-place version) keeps being passed — the steady state of inference / rollouts."""
-        ent = self.entries.get(id(edge_index))
+        """edge_attr permuted into CSR order, cached next to the CSR of `edge_index` that `perm` belongs to while the SAME
+        edge_attr tensor (identity + in-place version) keeps being passed — the steady state of inference / rollouts."""
+        key = next((k for k, e in self.entries.items() if e[3][3] is perm), None)
+        ent = self.entries.get(key)
         if ent is not None and ent[0] is edge_index and len(ent) == 6 and ent[4][0] is edge_attr \
                 and ent[4][1] == edge_attr._version:
             return ent[5]
         ea = backend.gather_rows(edge_attr.detach().to(torch.float32).contiguous(), perm)
         if ent is not None and ent[0] is edge_index:
-            self.entries[id(edge_index)] = ent[:4] + ((edge_attr, edge_attr._version), ea)
+            self.entries[key] = ent[:4] + ((edge_attr, edge_attr._version), ea)
         return ea
 
 
@@ -426,7 +437,10 @@ class FastEGNN(nn.Module):
             a.update(rowptr=edge_index.rowptr.contiguous(), row=edge_index.rows().contiguous(),
                      col=edge_index.col.contiguous(), ea=f32(edge_attr) if A > 0 else None, nE=edge_index.n_edges_dev)
             return a
-        rowptr, row, col, perm = self._graphs.get(be, edge_index, N, self.validate_inputs)
+        B = int(loc_mean.shape[0])
+        pos = None if self.deterministic else a["node_loc"]         # the deterministic mode's bits need id order (§17)
+        rowptr, row, col, perm = self._graphs.get(be, edge_index, N, self.validate_inputs, pos,
+                                                  None if B == 1 else a["data_batch"], B)
         ea = self._graphs.sorted_edge_attr(be, edge_index, edge_attr, perm) if A > 0 else None
         a.update(rowptr=rowptr, row=row, col=col, ea=ea, nE=None, perm=perm)
         return a

@@ -142,6 +142,14 @@ DISTEGNN_API int distegnn_build_csr(const int64_t *edge_index, int64_t n_nodes, 
                        int32_t *rowptr /*[N+1]*/, int32_t *row /*[E]*/, int32_t *col /*[E]*/,
                        int32_t *perm /*[E]*/, void *workspace, int64_t workspace_bytes,
                        int32_t *n_invalid /*[1], device, may be NULL*/, void *stream);
+/* distegnn_build_csr with the rows in a spatial order: the same rowptr, and the edges of every row contiguous and in the
+ * same relative order, but the rows sorted by (graph, cell of the destination in pos [N,3], destination) instead of by
+ * id.  Graphs stay contiguous and in order (data_batch sorted; NULL for n_graphs == 1).  The order changes what the edge
+ * kernels read from L2, not what they compute (DESIGN §3).  Same workspace as distegnn_build_csr. */
+DISTEGNN_API int distegnn_build_csr_cells(const int64_t *edge_index, int64_t n_nodes, int64_t n_edges, const float *pos,
+                       const int64_t *data_batch, int n_graphs, int32_t *rowptr /*[N+1]*/, int32_t *row /*[E]*/,
+                       int32_t *col /*[E]*/, int32_t *perm /*[E]*/, void *workspace, int64_t workspace_bytes,
+                       int32_t *n_invalid /*[1], device, may be NULL*/, void *stream);
 
 /* dst[i,:] = src[perm[i],:] for i < n_rows, rows of `width` floats (edge_attr into CSR order). */
 DISTEGNN_API int distegnn_gather_rows(const float *src, const int32_t *perm, int64_t n_rows, int width, float *dst,
