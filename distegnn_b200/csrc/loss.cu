@@ -5,7 +5,15 @@
 // logged loss :109) and an all_gather consistency check of `loc_mean` (:52-61) per step, then a Python loop over the
 // graphs of the batch with `randperm` sampling, two `cdist` kernels (:11-14) per graph and ~20 small ATen launches each.
 //
-// Here (fp32; sums of at most a few thousand positive terms):
+// Here (fp32).  Every sum is a chain per thread, a tree over the block (block_sum: 5 shuffle levels in a warp, 3 over
+// the 8 warps) and one atomicAdd per block into a global accumulator, in no fixed order:
+//   SSE         ⌈6144/256⌉ = 24 fmaf per thread of a node block, the tree, one atomicAdd per block of 2048 nodes
+//   l_vv, l_rv  ⌈C²/256⌉ and ⌈S·C/256⌉ terms per thread, the tree, one atomicAdd per graph
+//   ∂/∂Xv       the C + S pair terms of an entry, added by shared-memory atomicAdd
+// so a sum Σ of positive terms is within γ_n·Σ, γ_n = n·u/(1 − n·u), u = 2⁻²⁴: n ≈ 2 + 24 + 8 + node_blocks + 2 for
+// the SSE (489 node blocks at 1M nodes), n ≈ ⌈S·C/256⌉ + 8 + B for l_vv and l_rv, and an entry of ∂/∂Xv is within
+// γ_{C+S−1}·Σ|term| plus each term's own roundings (tests/test_loss_kernel.py derives its bounds from this).
+// n_r is converted to float, which is exact up to 2^24 nodes per rank.
 //   distegnn_loss_partials   one launch: Σ(pred−target)² over the rank's nodes folded straight into the packed vector
 //                            [n_r, n_r·MSE_r, loc_mean of this rank in its slot], and per graph l_vv = Σ k(V_c,V_c'),
 //                            l_rv = Σ k(R_s,V_c), k(x,y) = exp(−‖x−y‖/(2σ²)) (distance NOT squared, :12-13), together with
