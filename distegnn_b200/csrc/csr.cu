@@ -121,11 +121,14 @@ static int key_bits(int64_t n) {
     return b;
 }
 
-// cells per graph of the row order; n_graphs · budget < 2^30, so every (graph, cell) key is a non-negative int32
+// cells per graph of the row order, at least one: n_graphs · budget <= max(2^30, n_graphs) <= INT32_MAX, so every
+// (graph, cell) key is a non-negative int32 and key_bits(n_graphs · budget) <= 31 covers them all.  The floor matters for
+// n_graphs > 2^30, where the cap is 0: a budget of 0 would sort the nodes on one key bit and leave the graphs unordered.
 static int64_t cell_budget(int64_t n_nodes, int n_graphs) {
     const int64_t per = n_nodes / ((int64_t)n_graphs * kCsrNodesPerCell) + 1;
     const int64_t cap = ((int64_t)1 << 30) / n_graphs;
-    return per < cap ? per : cap;
+    const int64_t budget = per < cap ? per : cap;
+    return budget > 1 ? budget : 1;
 }
 
 struct CsrLayout {

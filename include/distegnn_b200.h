@@ -21,7 +21,7 @@
  *   - hidden width H is fixed at 64 (every shipped config: config/ *.yaml `hidden_nf: 64`);
  *   - preconditions the kernels rely on and the host mirror validates (fast_egnn.py): data_batch is
  *     non-decreasing with ids in [0, n_graphs) (FastEGNN.py:298 takes B from data_batch[-1]+1 and PyG batches are
- *     sorted); edge ids lie in [0, n_nodes) (distegnn_build_csr returns DISTEGNN_EINVAL otherwise);
+ *     sorted); edge ids lie in [0, n_nodes) (distegnn_build_csr counts the others into *n_invalid and clamps them);
  *   - cross-check twins of these entry points (fp32 FMA on the CUDA cores) live in
  *     distegnn_b200_testing.h / libdistegnn_b200_testing.so and are not part of the product.
  *
