@@ -48,6 +48,11 @@ SIGNATURES = {
     "distegnn_cutoff_csr_workspace_bytes": [_i64, _i32, _i64, C.POINTER(_i64)],
     "distegnn_cutoff_csr": [_i64, _i32, _vp, _vp, C.c_double, _i32, _vp, _vp, _vp, _vp, _i64] + [_vp] * 7 + [_i64, _vp],
     "distegnn_kmeans_lloyd": [_i64, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp],
+    "distegnn_kmeans_lloyd_d": [_i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp, _vp],
+    "distegnn_spectral_workspace_bytes": [_i64, _i32, _i32, C.POINTER(_i64)],
+    "distegnn_spectral_apply": [_i64, _i32, _vp, C.c_float, _vp, _vp, _vp, _vp, _i64, _vp],
+    "distegnn_spectral_gram": [_i64, _i32, _i32, _vp, _vp, _vp, _vp, _i64, _vp],
+    "distegnn_spectral_combine": [_i64, _i32, _i32, _vp, _vp, _vp, _i32, _vp],
     "distegnn_virtual_layer_bwd": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 16,
     "distegnn_virtual_bwd_prepare": [_i32, _i32, _i32, _vp, _vp, _vp],
     "distegnn_virtual_layer_fwd": [_i64, _i32, _i32, _i32, _i32, _u32] + [_vp] * 10,

@@ -296,8 +296,8 @@ class FrameLoader:
     delta_t         target frame offset (N-body: frame_T − frame_0)
     radius          radius of the graph (per partition: the reference's inner_radius); None or < 0 = fully connected
     world_size, rank, split_mode   this rank's share of every sample: "random" (a randperm chunk from a generator seeded
-                    per sample, `sample_generator(i)`, identical on every rank) or "kmeans" (labels computed on first use
-                    and cached); every rank needs nodes of every sample, else ValueError
+                    per sample, `sample_generator(i)`, identical on every rank), "kmeans" or "spectral" (labels computed
+                    on first use and cached; spectral: world_size <= 16); every rank needs nodes of every sample, else ValueError
     cutoff_rate     > 0: keep the int(E_b·(1 − rate)) shortest edges of every graph
     capacity        None: exact graph allocation (the edge counts are read back every batch).  K: edge buffers of K
                     entries and no host synchronisation at all; `check()` raises if a batch overflowed them
@@ -326,8 +326,10 @@ class FrameLoader:
         self.horizon = horizon
         if world_size < 1 or not 0 <= rank < world_size:
             raise ValueError(f"rank {rank} outside world_size {world_size}")
-        if world_size > 1 and split_mode not in ("random", "kmeans"):
-            raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans)")
+        if world_size > 1 and split_mode not in ("random", "kmeans", "spectral"):
+            raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral)")
+        if world_size > 1 and split_mode == "spectral" and world_size > 16:
+            raise ValueError(f"split_mode='spectral' splits into at most 16 parts (world_size {world_size})")
         self.radius = None if radius is None or radius < 0 else float(radius)
         self.batch_size, self.shuffle, self.drop_last = int(batch_size), shuffle, drop_last
         self.device = torch.device(device) if device is not None else None
@@ -382,12 +384,12 @@ class FrameLoader:
         n = self.traj.scenes[s].n_nodes
         if self.world_size == 1:
             return None, [n]
-        if self.split_mode == "kmeans":
+        if self.split_mode in ("kmeans", "spectral"):
             if i not in self._kmeans:
                 if self.device is None or self.device.type != "cuda":
-                    raise _lib.DistEGNNError("split_mode='kmeans' runs on a CUDA device")
+                    raise _lib.DistEGNNError(f"split_mode={self.split_mode!r} runs on a CUDA device")
                 pos = torch.from_numpy(np.array(self.traj.scenes[s].position[f], dtype=np.float32))
-                chunks = node_chunks(n, self.world_size, "kmeans", pos=pos.to(self.device))
+                chunks = node_chunks(n, self.world_size, self.split_mode, pos=pos.to(self.device))
                 counts = [int(c.numel()) for c in chunks]
                 self._check_counts(i, counts)
                 self._kmeans[i] = (chunks[self.rank].to("cpu", torch.int32), counts)

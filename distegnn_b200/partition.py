@@ -4,7 +4,8 @@
     edge_index, edge_attr = radius_graph(pos, r, batch=None)         # the same graph as PyG's int64 edge_index
     graph, edge_attr = cutoff_edges_csr(graph, pos, 0.5, batch)      # FastEGNN's cutoff: the shortest half of each graph
     labels = kmeans_labels(pos, world_size)                          # == sklearn KMeans(random_state=0).fit_predict
-    parts = split_large_graph(pos, x, target, vel, attr, r, P, split_mode="random" | "kmeans")
+    labels = spectral_labels(pos, world_size)                        # the reference's SpectralClustering (spectral.py)
+    parts = split_large_graph(pos, x, target, vel, attr, r, P, split_mode="random" | "kmeans" | "spectral")
 
 `radius_graph_csr` is one C-ABI call (csrc/radius_csr.cu): bounding box, grid sizing, cell keys, sort, counts, prefix sums
 and the fill all run on the device, so it never synchronises when the caller passes a `capacity` (rollouts: reuse the
@@ -26,6 +27,7 @@ import torch
 from . import _lib
 from ._lib import check, ptr
 from .shards import CSRGraph
+from .spectral import spectral_labels
 
 Tensor = torch.Tensor
 _TABLE_CELLS = 1 << 22          # dense cell table (graphs x cells), int32: 16 MiB of workspace
@@ -305,27 +307,28 @@ def node_chunks(n_nodes: int, world_size: int, split_mode: str = "random", pos: 
                 generator=None) -> List[Tensor]:
     """The node sets of the reference's partitioners, one int64 index tensor per rank: "random" = a host `randperm(n)` cut
     into P−1 chunks of ⌊n/P⌋ plus the remainder, in permutation order (distribute_graphs.py:26-30; host tensors);
-    "kmeans" = `nonzero(kmeans_labels(pos) == i)`, nodes in index order (:188-198; on `pos.device`, needs `pos`)."""
+    "kmeans" = `nonzero(kmeans_labels(pos) == i)`, nodes in index order (:188-198; on `pos.device`, needs `pos`);
+    "spectral" = the same with `spectral_labels(pos)` (:201-223; world_size <= 16)."""
     n = int(n_nodes)
     if split_mode == "random":
         idx = torch.randperm(n, generator=generator)             # on the host, as the reference (device == 'cpu')
         sizes = [n // world_size] * (world_size - 1)
         sizes.append(n - sum(sizes))
         return list(torch.split(idx, sizes))
-    if split_mode == "kmeans":
+    if split_mode in ("kmeans", "spectral"):
         if pos is None:
-            raise ValueError("split_mode='kmeans' needs the positions")
-        labels = kmeans_labels(pos, world_size)
+            raise ValueError(f"split_mode={split_mode!r} needs the positions")
+        labels = kmeans_labels(pos, world_size) if split_mode == "kmeans" else spectral_labels(pos, world_size)
         return [torch.nonzero(labels == i, as_tuple=False).flatten() for i in range(world_size)]
-    raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans)")
+    raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral)")
 
 
 def split_large_graph(pos: Tensor, x: Tensor, target: Tensor, vel: Tensor, attr: Optional[Tensor], radius: float,
                       world_size: int, split_mode: str = "random", special_nodes: Optional[Tensor] = None, generator=None,
                       edge_attr_nf: int = 2) -> List[Dict[str, Tensor]]:
-    """Device-side form of the reference's partitioners (datasets/distribute_graphs.py:17-51 random, :118-143 k-means):
-    node chunks by a host `randperm` (P−1 chunks of ⌊N/P⌋ + remainder) or by k-means cluster (`pos[cluster == i]`, nodes in
-    index order), every chunk with its own radius graph built on the device as CSR, `edge_attr` = the edge length in
+    """Device-side form of the reference's partitioners (datasets/distribute_graphs.py:17-51 random, :118-143 k-means,
+    :90-115 spectral): node chunks by a host `randperm` (P−1 chunks of ⌊N/P⌋ + remainder) or by k-means or spectral
+    cluster (`pos[cluster == i]`, nodes in index order), every chunk with its own radius graph built on the device as CSR, `edge_attr` = the edge length in
     `edge_attr_nf` columns (:44) and the GLOBAL `loc_mean` (:32).  Returns dicts with the reference's `Data` field names,
     `edge_index` being a `CSRGraph` (what `FastEGNN.forward` consumes directly)."""
     n = int(pos.shape[0])

@@ -8,8 +8,9 @@ synthetic restatement of what the reference's data pipeline hands to ``FastEGNN.
   ``datasets/distribute_graphs.py:43`` (all ordered pairs with ‖Δx‖ < r, both directions),
 * ``edge_attr`` = the edge length duplicated into two columns (``distribute_graphs.py:44``),
 * ``loc_mean`` = centroid of the *whole* graph, shared by all partitions (``distribute_graphs.py:32``),
-* ``split_mode=random`` (``distribute_graphs.py:26-30``) and ``split_mode=kmeans``
-  (``distribute_graphs.py:118-143,188-198``) node partitioning with per-partition radius graphs
+* ``split_mode=random`` (``distribute_graphs.py:26-30``), ``split_mode=kmeans``
+  (``distribute_graphs.py:118-143,188-198``) and ``split_mode=spectral`` (``:90-115,201-223``)
+  node partitioning with per-partition radius graphs
   (cross-partition edges are dropped, as in the reference).
 
 CPU/numpy only — this is input preparation, not part of the measured path.
@@ -130,13 +131,34 @@ def kmeans_partition(pos: np.ndarray, world_size: int) -> List[np.ndarray]:
     return [np.nonzero(labels == i)[0] for i in range(world_size)]
 
 
+def spectral_partition(pos: np.ndarray, world_size: int) -> List[np.ndarray]:
+    """distribute_graphs.py:201-223 — sklearn SpectralClustering(n_clusters=P, affinity='rbf', gamma=1/(2σ²),
+    assign_labels='kmeans', random_state=0, eigen_solver='arpack') on float32 positions, σ the median nonzero distance
+    among min(N, 2000) nodes drawn by RandomState(0), plus 1e-12; partition i = nodes with label i, in index order.
+    Forms the dense N×N affinity (51 GB at 113,140 nodes): a host restatement for tests and small
+    benchmarks; ``make_partitions(..., device=...)`` uses the device partitioner instead."""
+    from sklearn.cluster import SpectralClustering
+    X = pos.astype(np.float32)
+    n = X.shape[0]
+    idx = np.random.RandomState(0).choice(n, size=min(n, 2000), replace=False)
+    D = np.linalg.norm(X[idx, None, :] - X[None, idx, :], axis=2)
+    sigma = np.median(D[D > 0]) + 1e-12
+    sc = SpectralClustering(n_clusters=world_size, affinity="rbf", gamma=1.0 / (2.0 * (sigma ** 2)),
+                            assign_labels="kmeans", random_state=0, eigen_solver="arpack")
+    labels = sc.fit_predict(X)
+    return [np.nonzero(labels == i)[0] for i in range(world_size)]
+
+
 def make_partitions(w: Workload, world_size: int = 1, split_mode: str = "random", seed: int = 0,
-                    n_nodes: Optional[int] = None, only_rank: Optional[int] = None
+                    n_nodes: Optional[int] = None, only_rank: Optional[int] = None, device=None
                     ) -> List[Optional[Dict[str, torch.Tensor]]]:
     """One input dict per partition (= per rank), each with the forward() argument names.
 
     ``only_rank`` builds the (expensive) radius graph for that rank only and leaves ``None``
     elsewhere — every rank of a torchrun job calls this with its own rank and the same seed.
+    ``device`` (a CUDA device) takes the spectral split's labels from the device partitioner
+    (``distegnn_b200.spectral_labels``, O(N) memory) instead of the dense host restatement,
+    which only suits small clouds; the other modes ignore it.
     """
     pts = make_points(w, seed, n_nodes)
     n = pts["pos"].shape[0]
@@ -147,8 +169,14 @@ def make_partitions(w: Workload, world_size: int = 1, split_mode: str = "random"
         chunks = random_partition(n, world_size, seed)
     elif split_mode == "kmeans":
         chunks = kmeans_partition(pts["pos"], world_size)
+    elif split_mode == "spectral" and device is not None:
+        from .partition import node_chunks
+        pos = torch.from_numpy(pts["pos"]).to(device)
+        chunks = [c.cpu().numpy() for c in node_chunks(n, world_size, "spectral", pos=pos)]
+    elif split_mode == "spectral":
+        chunks = spectral_partition(pts["pos"], world_size)
     else:
-        raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans)")
+        raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral)")
     out: List[Optional[Dict[str, torch.Tensor]]] = []
     for r, idx in enumerate(chunks):
         if only_rank is not None and r != only_rank:

@@ -67,6 +67,8 @@ enum {
 #define DISTEGNN_MAX_EDGE_ATTR 8   /* edge_attr_nf A                */
 #define DISTEGNN_MAX_NODE_ATTR 8   /* node_attr_nf Na               */
 #define DISTEGNN_MAX_NODE_FEAT 16  /* node_feat_nf F                */
+#define DISTEGNN_SPECTRAL_MAX_K 16 /* vectors per spectral product   */
+#define DISTEGNN_KMEANS_MAX_DIM 16 /* k-means point dimension D      */
 
 /* flags */
 #define DISTEGNN_FLAG_NORMALIZE 1u  /* E_GCL_vel(normalize=True), FastEGNN.py:242-244                  */
@@ -308,8 +310,39 @@ DISTEGNN_API int distegnn_cutoff_csr(int64_t n_nodes, int n_graphs, const float 
                                      float *edge_attr_out, int32_t *info, void *workspace, int64_t workspace_bytes,
                                      void *stream);
 
+/* ---- k-means partitioner (csrc/kmeans.cu; distribute_graphs.py:188-198 and the label step of :201-223) ----------------
+ * `iters` Lloyd iterations from `centers` with sklearn's stopping rules evaluated on the device (state [4], zero on the
+ * first call: [0] 0 running / 1 final assignment pending / 2 done, [1] iterations done, [2] labels changed in the last
+ * pass).  labels int32 [N] (−1 initially), sums fp64 [K, D+1] zeroed before the first call.  distegnn_kmeans_lloyd is
+ * the D = 3 case.  distegnn_kmeans_lloyd_d takes D in [1, 16] (pos [N,D], centers [K,D]) and, when `inertia` is not
+ * NULL, writes Σ_i ‖pos_i − centers[labels_i]‖² (fp32 terms, fp64 sum in a fixed order) to inertia[0] once state[0]
+ * is 2.  A caller that stops after its iteration cap without convergence sets state[0] = 1 and calls once more with
+ * iters = 1: that pass assigns every point to the final centres without moving them (sklearn's closing E-step), ends
+ * in state 2 and writes the inertia.  n_clusters in [1, 64]. */
 DISTEGNN_API int distegnn_kmeans_lloyd(int64_t n_nodes, int n_clusters, const float *pos, float *centers,
                                        int32_t *labels, double *sums, int32_t *state, float tol, int iters, void *stream);
+DISTEGNN_API int distegnn_kmeans_lloyd_d(int64_t n_nodes, int n_clusters, int dim, const float *pos, float *centers,
+                                         int32_t *labels, double *sums, int32_t *state, float tol, int iters,
+                                         double *inertia, void *stream);
+
+/* ---- spectral partitioner (csrc/spectral.cu; distribute_graphs.py:90-115, 201-223) -------------------------------------
+ * distegnn_spectral_apply: y = s ⊙ (A_off · (s ⊙ x)) for k <= 16 fp64 vectors without forming A:
+ *   A_ij = 2^(−gamma_log2e · ‖pos_i − pos_j‖²) for j != i (fp32 ex2 of an fp32 squared distance), A_ii = 0.
+ * pos float32 [N,3] (centre it first: the distances are fp32), x fp64 [N,k] row-major (NULL: all ones, k = 1),
+ * scale fp64 [N] (NULL: 1), y fp64 [N,k].  s = d^−½ gives S·x with S = D^−½ (A − I) D^−½; x = NULL and scale = NULL
+ * give the degrees d.  fp32 partial sums of at most 128 terms, added in fp64 in a fixed order: bitwise deterministic.
+ * distegnn_spectral_gram: g [a,b] = u·vᵀ for u fp64 [a,N], v fp64 [b,N] (vectors stored one after the other), b <= 16.
+ * distegnn_spectral_combine: y [b,N] = u[a,N]ᵀ-combination Σ_p c[p][q] u[p] (subtract = 1: y −= it), c fp64 [a,b]
+ * row-major, b <= 16.  Both with a fixed summation order.  Workspace (apply and gram): distegnn_spectral_workspace_bytes
+ * with the largest k (b) and a the caller uses. */
+DISTEGNN_API int distegnn_spectral_workspace_bytes(int64_t n_nodes, int k, int a, int64_t *bytes_host);
+DISTEGNN_API int distegnn_spectral_apply(int64_t n_nodes, int k, const float *pos, float gamma_log2e,
+                                         const double *scale, const double *x, double *y, void *workspace,
+                                         int64_t workspace_bytes, void *stream);
+DISTEGNN_API int distegnn_spectral_gram(int64_t n_nodes, int a, int b, const double *u, const double *v, double *g,
+                                        void *workspace, int64_t workspace_bytes, void *stream);
+DISTEGNN_API int distegnn_spectral_combine(int64_t n_nodes, int a, int b, const double *u, const double *c, double *y,
+                                           int subtract, void *stream);
 
 /* ---- real↔virtual stage --------------------------------------------------------------------------
  * Virtual geometry + edge_mode_virtual + the virtual parts of coord_model_vel, coord_model_virtual,

@@ -253,9 +253,9 @@ def main():
                        base.degree, m["node_feat_nf"], m["node_attr_nf"], m["edge_attr_nf"], m["virtual_channels"],
                        m["normalize"])
     split = d.get("split_mode", "random")
-    if world_size > 1 and split not in ("random", "kmeans"):
+    if world_size > 1 and split not in ("random", "kmeans", "spectral"):
         if local_rank == 0:
-            print(f"split_mode={split!r} needs METIS/spectral partitioners of the reference's data pipeline; "
+            print(f"split_mode={split!r} needs the METIS partitioner of the reference's data pipeline; "
                   "using 'random' for the synthetic graph")
         split = "random"
     cut = None
@@ -264,7 +264,7 @@ def main():
         n_r, e_r = inp["node_loc"].shape[0], cut["kept"]
     else:
         part = synth.make_partitions(w, world_size=world_size, split_mode=split, seed=cfg.get("seed", 0),
-                                     only_rank=local_rank)[local_rank]
+                                     only_rank=local_rank, device=torch.device("cuda", local_rank))[local_rank]
         inp = {k: (v.to(local_rank) if v is not None else None) for k, v in part.items()}
         n_r, e_r = inp["node_loc"].shape[0], inp["edge_index"].shape[1]
 
@@ -325,7 +325,7 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     N-body (`dataset_name: nbody*`, the reference's loc_/vel_/charges_ .npy files, frame_0 / frame_T), Water-3D or
     Fluid113K (`path`/train/*.npz, `path`/valid/*.npz).  cutoff_edges mode: one graph per sample, radius = data.radius
     (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
-    sample split over the ranks by split_mode (metis / spectral fall back to random), a radius graph per partition with
+    sample split over the ranks by split_mode (metis falls back to random, with a message), a radius graph per partition with
     inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
     N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only;
     `transform` (rotate, translate) to every loader built (the same samples as without it: a rotated and translated
@@ -340,7 +340,10 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     else:
         radius = d.get("inner_radius")
     split = str(d.get("split_mode", "random"))
-    if split not in ("random", "kmeans"):
+    if split not in ("random", "kmeans", "spectral"):
+        if world_size > 1 and rank == 0:
+            print(f"split_mode={split!r} needs the METIS partitioner of the reference's data pipeline; "
+                  "using 'random' for the trajectories")
         split = "random"
     seed, bs = int(cfg.get("seed", 0)), int(d.get("batch_size", 1))
     xf = {} if transform is None else dict(rotate=transform[0], translate=transform[1])
