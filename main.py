@@ -19,8 +19,8 @@ same node/edge statistics, `radius`/`split_mode` semantics of datasets/distribut
 target (constant-velocity step).  It evaluates `--eval_steps` forward passes (graph-steps/s, edges/s) and, with
 `--train_steps K`, runs K optimisation steps of the reference's training step (utils/train.py:98-158: node-count
 weighted MSE x world_size, MMD regulariser on the virtual coordinates, gradient clipping 0.3, Adam) through the
-fused forward AND backward kernels under DDP — the epoch loop, loaders, checkpoints and wandb logging of
-utils/train.py stay with the reference (out of scope).
+fused forward AND backward kernels under DDP.  The synthetic path has no splits, so its epoch loop is `--trajectory`'s
+(below); wandb logging stays with the reference (out of scope).
 
 `--trajectory PATH` trains and evaluates on real frames instead (distegnn_b200.frames.FrameLoader, DESIGN §18): the
 config's recipe (N-body, Water-3D, Fluid113K), radius / inner_radius, delta_t (N-body: frame_0, frame_T), split_mode and
@@ -34,6 +34,13 @@ and with every sample rotated and translated (FrameLoader's `rotate` / `translat
 difference of the two mean MSEs: an equivariant model's error does not depend on the frame.  Without the flags the
 synthetic path below runs unchanged.
 
+`--trajectory PATH --epochs E` trains to convergence instead (`fit`, DESIGN §24): the reference's epoch loop
+(utils/train.py:17-289) over the train, valid and test splits, with `train.accumulation_steps`, `train.scheduler: cosine`,
+`train.early_stop` (`--early_stop` overrides it) and `log.test_interval`; `best_model.pth`, `last_model.pth` and
+`log.json` under `log.log_dir`/exp_name.  `--checkpoint` of such a file resumes the run after its epoch (optimiser,
+scheduler and the train loader's order included).  After the loop the best checkpoint's weights are restored and
+`--eval_rotate` / `--eval_translate` / `--rollout_steps` run on them.
+
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
 `batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
 graph, then `data.cutoff_rate` (`--cutoff_rate` overrides it, reference main.py:133-134) drops the longest edges of
@@ -45,6 +52,7 @@ the reference ignores it there.
 from __future__ import annotations
 
 import argparse
+import json
 import os
 import re
 import sys
@@ -120,7 +128,43 @@ def parse():
                    "DESIGN §23), and print the relative difference of the mean MSEs")
     p.add_argument("--eval_translate", type=str, default=None, help="(new) with --trajectory: S >= 0, the scale of the "
                    "second evaluation's per-sample translation S·N(0, I) (FrameLoader's translate, DESIGN §23)")
+    p.add_argument("--epochs", type=int, default=None, help="(new) with --trajectory: E >= 1 epochs of the reference's "
+                   "epoch loop (utils/train.py) over train/valid/test, with best/last checkpoints, early stopping and "
+                   "resume from --checkpoint (DESIGN §24)")
     return p.parse_args()
+
+
+def split_files(path, recipe, part):
+    """The files of split `part` under `path`: N-body's loc_`part`_... .npy, or `path`/`part`/*.npz; [] if missing."""
+    import glob
+    if recipe == "nbody":
+        f = os.path.join(path, f"loc_{part}_charged100_0_0_1.npy")
+        return [f] if os.path.exists(f) else []
+    return sorted(glob.glob(os.path.join(path, part, "*.npz")))
+
+
+def epochs_of(args, cfg):
+    """--epochs E, or None; exits with a message when it cannot run: no --trajectory, --train_steps given, E < 1, or
+    the trajectory has no valid or no test split."""
+    if args.epochs is None:
+        return None
+    msg = None
+    if not args.trajectory:
+        msg = "used with --trajectory"
+    elif args.train_steps:
+        msg = "used without --train_steps (the epochs set the number of steps)"
+    elif args.epochs < 1:
+        msg = ">= 1"
+    else:
+        recipe = recipe_of_config(cfg)[0]
+        missing = [part for part in ("valid", "test") if not split_files(args.trajectory, recipe, part)]
+        if missing:
+            msg = f"used with a trajectory that has valid and test splits ({args.trajectory} has no {' or '.join(missing)})"
+    if msg is not None:
+        if int(os.environ.get("LOCAL_RANK", "0")) == 0:
+            print(f"--epochs {args.epochs}: must be {msg}", flush=True)
+        sys.exit(2)
+    return args.epochs
 
 
 def train_noise_of(args):
@@ -191,6 +235,7 @@ def main():
         cfg["data"]["inner_radius"] = args.inner_radius
     if args.virtual_channels is not None:
         cfg["model"]["virtual_channels"] = args.virtual_channels
+    epochs = epochs_of(args, cfg)
 
     # FastEGNN's cutoff_edges mode (reference README.md:30-33): the cutoff rate applies; in distribute mode it does not
     cutoff_mode = str(cfg["data"].get("accelerate_mode", "distribute")) == "cutoff_edges"
@@ -203,7 +248,7 @@ def main():
                       "without torchrun or with one process (use accelerate_mode=distribute for several GPUs)", flush=True)
             sys.exit(2)
     # options of the reference CLI that belong to its data pipeline / epoch loop (out of scope here): say so, loudly
-    ignored = [n for n, v in (("--wandb", args.wandb), ("--early_stop", args.early_stop),
+    ignored = [n for n, v in (("--wandb", args.wandb), ("--early_stop", None if epochs else args.early_stop),
                               ("--cutoff_rate", None if cutoff_mode else args.cutoff_rate),
                               ("--outer_radius", args.outer_radius)) if v]
     if ignored and int(os.environ.get("LOCAL_RANK", "0")) == 0:
@@ -223,7 +268,7 @@ def main():
     torch.manual_seed(cfg.get("seed", 0))
 
     model = get_model(cfg, world_size).to(local_rank)
-    ck = cfg["model"].get("checkpoint")
+    ck, state = cfg["model"].get("checkpoint"), None
     if ck:
         state = torch.load(ck, map_location=f"cuda:{local_rank}")
         sd = state.get("model_state_dict", state)
@@ -233,7 +278,10 @@ def main():
         model = DistributedDataParallel(model, device_ids=[local_rank], find_unused_parameters=True)
     model.eval()
     if args.trajectory:
-        trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform)
+        if epochs:
+            trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform, state)
+        else:
+            trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform)
         if distributed:
             dist.destroy_process_group()
         return
@@ -323,14 +371,14 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
                   transform=None):
     """FrameLoaders over the raw trajectories under `path` with the config's recipe (datasets/process_dataset.py):
     N-body (`dataset_name: nbody*`, the reference's loc_/vel_/charges_ .npy files, frame_0 / frame_T), Water-3D or
-    Fluid113K (`path`/train/*.npz, `path`/valid/*.npz).  cutoff_edges mode: one graph per sample, radius = data.radius
+    Fluid113K (`path`/train/*.npz, `path`/valid/*.npz, `path`/test/*.npz).  Only the train loader shuffles (the
+    reference's same-seed sampler); a split without files gives None.  cutoff_edges mode: one graph per sample, radius = data.radius
     (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
     sample split over the ranks by split_mode (metis falls back to random, with a message), a radius graph per partition with
     inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
     N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only;
     `transform` (rotate, translate) to every loader built (the same samples as without it: a rotated and translated
     copy of the split).  Returns (recipe name, {part: loader or None})."""
-    import glob
     from distegnn_b200.frames import FrameLoader, load_nbody, load_scenes, sample_list
     d = cfg["data"]
     recipe, frame_0, delta = recipe_of_config(cfg)
@@ -349,17 +397,11 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     xf = {} if transform is None else dict(rotate=transform[0], translate=transform[1])
     out = {}
     for part in parts:
-        if recipe == "nbody":
-            if not os.path.exists(os.path.join(path, f"loc_{part}_charged100_0_0_1.npy")):
-                out[part] = None
-                continue
-            traj = load_nbody(path, part)
-        else:
-            files = sorted(glob.glob(os.path.join(path, part, "*.npz")))
-            if not files:
-                out[part] = None
-                continue
-            traj = load_scenes(files, recipe)
+        files = split_files(path, recipe, part)
+        if not files:
+            out[part] = None
+            continue
+        traj = load_nbody(path, part) if recipe == "nbody" else load_scenes(files, recipe)
         kw = {}
         if recipe != "nbody":
             shortest = min(sc.n_frames for sc in traj.scenes)
@@ -377,39 +419,48 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     return recipe, out
 
 
-def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None):
-    """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
-    reference's training step on batches from FrameLoader (with `noise` on its inputs), then the mean MSE over the
-    validation batches (noise-free); with `transform` (rotate, translate) also over the same batches rigidly
-    transformed, and the relative difference of the two."""
-    from distegnn_b200 import train_loss
+def rollout_args(args, cfg, local_rank):
+    """(recipe, K, tau) of `--rollout_steps K` on the trajectory; exits with a message before any training when the
+    rollout could not run (no `--rollout_tau` for a recipe with physical velocities)."""
     recipe, _, delta = recipe_of_config(cfg)
     K = args.rollout_steps
     tau = args.rollout_tau if args.rollout_tau is not None else (float(delta) if recipe == "water3d" else None)
-    if K > 0 and tau is None:                                  # before any training: the rollout could not run
+    if K > 0 and tau is None:
         if local_rank == 0:
             print(f"--rollout_steps with --trajectory on {recipe!r} needs --rollout_tau: its velocities are physical and "
                   "the frame time is not in the files (Water-3D defaults to delta_t)", flush=True)
         sys.exit(2)
-    dev = torch.device("cuda", local_rank)
-    recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, noise=noise)
-    tc = cfg.get("train", {}) or {}
-    mmd = tc.get("mmd", {}) or {}
-    lr = args.lr if args.lr is not None else float(tc.get("learning_rate", tc.get("lr", 5e-4)))
-    opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=float(tc.get("weight_decay", 1e-12)))
+    return recipe, K, tau
+
+
+def trajectory_loss(cfg, model, world_size, distributed):
+    """loss_of(kw, ex, accumulation_steps=1) -> (loss, info) of one FrameLoader batch: the model's positional call
+    (utils/train.py:63-71) and the fused `train_loss` with the config's MMD settings (utils/train.py:98-150)."""
+    from distegnn_b200 import train_loss
+    mmd = (cfg.get("train", {}) or {}).get("mmd", {}) or {}
     inner = model.module if distributed else model
     use_attr = cfg["model"]["node_attr_nf"] > 0
 
-    def forward(kw):                                           # positional call as in utils/train.py:63-71
-        return model(kw["node_feat"], kw["node_loc"], kw["node_vel"], kw["loc_mean"], kw["edge_index"],
-                     kw["data_batch"], kw["edge_attr"], kw["node_attr"] if use_attr else None)
-
-    def loss_of(kw, ex):
-        pred, X = forward(kw)
+    def loss_of(kw, ex, accumulation_steps=1):
+        pred, X = model(kw["node_feat"], kw["node_loc"], kw["node_vel"], kw["loc_mean"], kw["edge_index"],
+                        kw["data_batch"], kw["edge_attr"], kw["node_attr"] if use_attr else None)
         return train_loss(pred, ex["target"], X, kw["data_batch"], world_size=world_size,
                           mmd_samples=int(mmd.get("samples", 50)), mmd_sigma=float(mmd.get("sigma", 3)),
-                          mmd_weight=float(mmd.get("weight", 0.01)), loc_mean=kw["loc_mean"],
-                          node_counts=ex["node_counts"], model=inner)
+                          mmd_weight=float(mmd.get("weight", 0.01)), accumulation_steps=accumulation_steps,
+                          loc_mean=kw["loc_mean"], node_counts=ex["node_counts"], model=inner)
+    return loss_of
+
+
+def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None):
+    """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
+    reference's training step on batches from FrameLoader (with `noise` on its inputs), then `trajectory_eval`."""
+    recipe, K, tau = rollout_args(args, cfg, local_rank)
+    dev = torch.device("cuda", local_rank)
+    recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, noise=noise)
+    tc = cfg.get("train", {}) or {}
+    lr = args.lr if args.lr is not None else float(tc.get("learning_rate", tc.get("lr", 5e-4)))
+    opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=float(tc.get("weight_decay", 1e-12)))
+    loss_of = trajectory_loss(cfg, model, world_size, distributed)
 
     steps = args.train_steps or len(loaders["train"])
     model.train()
@@ -429,6 +480,15 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, 
     torch.cuda.synchronize()
     if local_rank == 0:
         print(f"[{recipe}] {steps} train steps on raw frames: {(time.perf_counter() - t0) / steps * 1e3:.2f} ms/step")
+    trajectory_eval(args, cfg, model, world_size, local_rank, rate, loaders, loss_of, noise, transform)
+
+
+def trajectory_eval(args, cfg, model, world_size, local_rank, rate, loaders, loss_of, noise=None, transform=None):
+    """The mean MSE over the validation batches (noise-free; the train split without a valid batch); with `transform`
+    (rotate, translate) also over the same batches rigidly transformed, and the relative difference of the two; with
+    `--rollout_steps K` the rollout evaluation (`rollout_eval`), plain and transformed."""
+    recipe, K, tau = rollout_args(args, cfg, local_rank)
+    dev = torch.device("cuda", local_rank)
     ev = loaders["valid"]
     if not ev:                                                 # no valid split or no batch in it: the train split, clean
         ev = loaders["train"] if noise is None else \
@@ -458,6 +518,184 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, 
         rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau)
         if transform is not None:
             rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau, transform)
+
+
+def reference_clips(cfg, world_size):
+    """The reference's clip condition (utils/train.py:153): FastEGNN with several ranks, or the dataset named exactly
+    `LargeFluid` (the shipped Fluid113K config is not, so one GPU does not clip it)."""
+    return (world_size > 1 or cfg["data"].get("dataset_name") == "LargeFluid") and \
+        cfg["model"].get("model_name") == "FastEGNN"
+
+
+def exp_name_of(cfg, world_size, rate=None):
+    """The reference's experiment name (main.py:147-157, the FastEGNN branches) with a local-time suffix."""
+    d, m = cfg["data"], cfg["model"]
+    suffix = time.strftime("%Y-%m-%d_%H-%M-%S", time.localtime(time.time()))
+    if rate is None:                                           # accelerate_mode: distribute
+        return (f"{d.get('dataset_name')}_{d.get('split_mode')}_{m['model_name']}_{d.get('outer_radius')}_"
+                f"{d.get('inner_radius')}_{world_size}_{m['virtual_channels']}_{suffix}")
+    return f"{d.get('dataset_name')}_{m['model_name']}_{d.get('radius')}_{rate:.3f}_{m['virtual_channels']}_{world_size}_{suffix}"
+
+
+def fit(model, opt, scheduler, loaders, loss_of, cfg, epochs, start_epoch=0, world_size=1, rank=0, out_dir="."):
+    """The reference's epoch loop (utils/train.py:17-289, DESIGN §24): epochs start_epoch + 1 .. `epochs`, each a train
+    pass, and every `log.test_interval` epochs a valid and a test pass; `best_model.pth` (strictly lower valid loss),
+    `last_model.pth` (every evaluation epoch) and `log/log.json` under `out_dir`, written by rank 0 only.
+
+    loaders     {"train", "valid", "test"}: iterables of (forward kwargs, extras with "n_graphs") with len(); the train
+                loader as constructed (its epoch 0): a resumed run calls its `batches()` `start_epoch` times first, so
+                its order (and FrameLoader's noise, keyed by the loader's epoch) continues as without the interruption
+    loss_of     (kw, ex, accumulation_steps) -> (loss, info), info["logged"] a 0-dim tensor: the batch's logged MSE
+    cfg         the run's config (a plain dict, stored in every checkpoint and in log.json): train.accumulation_steps
+                (1), train.early_stop (None: never), log.test_interval (1), and the clip condition `reference_clips`
+    Returns (best_log_dict, log_dict) on rank 0, (None, None) on the others."""
+    tc, lc = cfg.get("train") or {}, cfg.get("log") or {}
+    A, interval = int(tc.get("accumulation_steps", 1)), int(lc.get("test_interval", 1))
+    early_stop = tc.get("early_stop")
+    clip = reference_clips(cfg, world_size)
+    dev = next(model.parameters()).device
+    for _ in range(start_epoch):
+        loaders["train"].batches()
+    if rank == 0:
+        log_dict = {"epochs": [], "loss": [], "loss_train": []}
+        best = {"epoch_index": 0, "loss_valid": 1e8, "loss_test": 1e8, "loss_train": 1e8}
+        log_dir, sd_dir = os.path.join(out_dir, "log"), os.path.join(out_dir, "state_dict")
+        os.makedirs(log_dir, exist_ok=True)
+        os.makedirs(sd_dir, exist_ok=True)
+        print(f"logs and checkpoints: {out_dir}", flush=True)
+        t0 = time.perf_counter()
+    stop = torch.zeros((), dtype=torch.int64, device=dev)
+
+    def one_pass(tag, epoch):                                  # train.py:17-168
+        train = tag == "train"
+        if train:
+            model.train()
+            opt.zero_grad()
+        else:
+            model.eval()
+        tot, graphs = torch.zeros((), dtype=torch.float64, device=dev), 0
+        with torch.set_grad_enabled(train):
+            for step, (kw, ex) in enumerate(loaders[tag]):
+                loss, info = loss_of(kw, ex, A if train else 1)
+                tot += info["logged"].double() * ex["n_graphs"]
+                graphs += ex["n_graphs"]
+                if train:
+                    loss.backward()
+                    if (step + 1) % A == 0:
+                        if clip:
+                            torch.nn.utils.clip_grad_norm_(model.parameters(), max_norm=0.3)
+                        opt.step()
+                        if scheduler is not None:
+                            scheduler.step()
+                        opt.zero_grad()
+        value = float(tot) / graphs if graphs else float("nan")    # the one host read of the pass
+        if rank == 0:
+            print(f"{'' if train else '==> '}{tag} epoch: {epoch}, avg loss: {value:.5f}", flush=True)
+        return value
+
+    for epoch in range(start_epoch + 1, epochs + 1):
+        loss_train = one_pass("train", epoch)
+        if rank == 0:
+            log_dict["loss_train"].append(loss_train)
+        if epoch % interval == 0:
+            loss_valid, loss_test = one_pass("valid", epoch), one_pass("test", epoch)
+            if rank == 0:
+                log_dict["epochs"].append(epoch)
+                log_dict["loss"].append(loss_test)
+                state = {"epoch": epoch, "model_state_dict": model.state_dict(),
+                         "optimizer_state_dict": opt.state_dict(),
+                         "scheduler_state_dict": None if scheduler is None else scheduler.state_dict(),
+                         "loss_train": loss_train, "loss_valid": loss_valid, "loss_test": loss_test, "config": cfg}
+                if loss_valid < best["loss_valid"]:
+                    best = {"epoch_index": epoch, "loss_valid": loss_valid, "loss_test": loss_test,
+                            "loss_train": loss_train}
+                    torch.save(state, os.path.join(sd_dir, "best_model.pth"))
+                print(best_line(best), flush=True)
+                torch.save(state, os.path.join(sd_dir, "last_model.pth"))
+                if early_stop is not None and epoch - best["epoch_index"] >= early_stop:
+                    best["early_stop"] = epoch
+                    print(f"Early stopped! Epoch: {epoch}", flush=True)
+                    stop.fill_(1)
+            if world_size > 1:                                 # every rank leaves at rank 0's epoch
+                import torch.distributed as dist
+                dist.all_reduce(stop, op=dist.ReduceOp.MAX)
+        if rank == 0:
+            best["time_cost"] = time.perf_counter() - t0
+            with open(os.path.join(log_dir, "log.json"), "w") as f:
+                f.write(json.dumps([best, log_dict, cfg], indent=4))
+        if epoch % interval == 0 and int(stop):
+            break
+    return (best, log_dict) if rank == 0 else (None, None)
+
+
+def best_line(best):
+    return (f"*** Best Valid Loss: {best['loss_valid']:.5f} | Best Test Loss: {best['loss_test']:.5f} | "
+            f"Best Epoch Index: {best['epoch_index']}")
+
+
+def optimizer_of(model, cfg, epochs, n_batches):
+    """The reference's Adam (train.learning_rate, train.weight_decay) and, for train.scheduler: cosine, its
+    CosineAnnealingLR over the run's optimiser steps, T_max = epochs·n_batches // accumulation_steps, eta_min 1e-8
+    (main.py:197-202); any other scheduler value: None."""
+    tc = cfg.get("train") or {}
+    lr = float(tc.get("learning_rate", tc.get("lr", 5e-4)))
+    opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=float(tc.get("weight_decay", 1e-12)))
+    if tc.get("scheduler") != "cosine":
+        return opt, None
+    t_max = epochs * n_batches // int(tc.get("accumulation_steps", 1))
+    return opt, torch.optim.lr_scheduler.CosineAnnealingLR(opt, T_max=t_max, eta_min=1e-8)
+
+
+def trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None, state=None):
+    """--trajectory with --epochs E: `fit` on FrameLoader's train (with `noise`), valid and test splits, the reference's
+    Adam and optional cosine schedule (main.py:197-202); `state`, a checkpoint with an `epoch` key, resumes after that
+    epoch (main.py:208-220).  Then the best checkpoint's weights, and `trajectory_eval` on them."""
+    recipe, _, _ = rollout_args(args, cfg, local_rank)
+    dev = torch.device("cuda", local_rank)
+    _, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, parts=("train", "valid", "test"),
+                               noise=noise)
+    for part, ld in loaders.items():
+        if not ld:
+            if local_rank == 0:
+                print(f"--epochs: the {part} split of {args.trajectory} has fewer samples than batch_size "
+                      f"{ld.batch_size}: no batch", flush=True)
+            sys.exit(2)
+    cfg = json.loads(json.dumps(cfg))                          # a plain dict: the checkpoints' and log.json's config
+    tc = cfg["train"] = dict(cfg.get("train") or {})
+    if args.lr is not None:
+        tc["learning_rate"] = args.lr
+    if args.early_stop is not None:
+        tc["early_stop"] = args.early_stop
+    tc["epochs"] = args.epochs
+    cfg["data"]["world_size"] = world_size
+    opt, scheduler = optimizer_of(model, cfg, args.epochs, len(loaders["train"]))
+    start = 0
+    if state is not None and "epoch" in state:
+        start = int(state["epoch"])
+        opt.load_state_dict(state["optimizer_state_dict"])
+        if scheduler is not None:
+            scheduler.load_state_dict(state["scheduler_state_dict"])
+        if local_rank == 0:
+            print(f"resuming after epoch {start} of {args.checkpoint}", flush=True)
+    name = [exp_name_of(cfg, world_size, rate)]
+    if distributed:                                            # one directory: rank 0's clock
+        dist.broadcast_object_list(name, src=0)
+    cfg["log"] = dict(cfg.get("log") or {}, exp_name=name[0])
+    out_dir = os.path.join(cfg["log"].get("log_dir", "./logs"), name[0])
+    loss_of = trajectory_loss(cfg, model, world_size, distributed)
+    best, _ = fit(model, opt, scheduler, loaders, loss_of, cfg, args.epochs, start, world_size, local_rank, out_dir)
+    if distributed:
+        dist.barrier()
+    path = os.path.join(out_dir, "state_dict", "best_model.pth")
+    if not os.path.exists(path):
+        if local_rank == 0:
+            print(f"[{recipe}] no evaluation epoch in {start + 1} .. {args.epochs}: no best model", flush=True)
+        return
+    model.load_state_dict(torch.load(path, map_location=dev)["model_state_dict"])
+    if local_rank == 0:
+        print(f"[{recipe}] best model restored: {best_line(best)}", flush=True)
+    if transform is not None or args.rollout_steps > 0:
+        trajectory_eval(args, cfg, model, world_size, local_rank, rate, loaders, loss_of, noise, transform)
 
 
 def transform_label(transform):
