@@ -3,9 +3,9 @@
     python -m distegnn_b200.build [--force] [--verbose]
 
   libdistegnn_b200.so          the product: every entry point of include/distegnn_b200.h (csrc/*.cu)
-  libdistegnn_b200_testing.so  cross-check twins of include/distegnn_b200_testing.h (csrc/testing/*.cu), and the
-                               deterministic mode's entry points with a grid cap; loaded only by tests, never by the
-                               package
+  libdistegnn_b200_testing.so  cross-check twins of include/distegnn_b200_testing.h (csrc/testing/*.cu), the
+                               deterministic mode's entry points with a grid cap, and W ranks of the virtual-node
+                               exchange in one launch; loaded only by tests, never by the package
 
 The shared libraries and objects are build products (git-ignored); `build()` rebuilds them whenever a source, header or
 this file is newer.
@@ -33,6 +33,8 @@ CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler",
 COMMON = ["api.cu"]
 # the deterministic mode's kernels, also behind the testing library's grid-capped twins (testing/det_capped.cu)
 DET_SHARED = ["edge_layer_cs.cu", "virtual_layer_tc16.cu", "deterministic.cu"]
+# the virtual-node exchange, also behind the testing library's W-rank twins (testing/comm_ranks.cu)
+COMM_SHARED = ["comm.cu", "virtual_update.cu"]
 
 
 def sources():
@@ -85,7 +87,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs) + len(tsrcs))) as ex:
         objs = dict(zip(srcs + tsrcs, ex.map(lambda s: _compile(s, verbose), srcs + tsrcs)))
     _link(LIB, [objs[s] for s in srcs])
-    _link(LIB_TESTING, [objs[s] for s in COMMON + DET_SHARED] + [objs[s] for s in tsrcs])
+    _link(LIB_TESTING, [objs[s] for s in COMMON + DET_SHARED + COMM_SHARED] + [objs[s] for s in tsrcs])
     return LIB
 
 

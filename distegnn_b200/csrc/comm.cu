@@ -18,21 +18,6 @@ namespace degnn {
         }                                                                                          \
     } while (0)
 
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-struct SegLayout {
-    size_t flags_off, epoch_off, status_off, data_off, total;
-};
-static SegLayout seg_layout(int world, int max_slots, int stride) {
-    SegLayout s;
-    s.flags_off = 0;
-    s.epoch_off = align_up(s.flags_off + sizeof(unsigned) * 2 * (size_t)world * max_slots, 256);
-    s.status_off = align_up(s.epoch_off + sizeof(unsigned) * (size_t)max_slots, 256);
-    s.data_off = align_up(s.status_off + 64, 256);
-    s.total = align_up(s.data_off + sizeof(float) * 2 * (size_t)world * max_slots * stride, 256);
-    return s;
-}
-
 __global__ void __launch_bounds__(256) allreduce_packed_kernel(const CommDev cd, float* buf, int64_t count) {
     const int slot = blockIdx.x;
     const int64_t o = (int64_t)slot * cd.stride;

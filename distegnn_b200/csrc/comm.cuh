@@ -49,9 +49,18 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     return t;
 }
 
+// The default pause of comm_slot_allreduce: none.
+struct NoPause {
+    __device__ __forceinline__ void operator()() const {}
+};
+
 // All-reduce (SUM) of slot `slot`: `vals[0:n]` (global or shared memory of this CTA, n <= stride) in place.  Must be called
-// by ALL threads of the CTA; returns after a __syncthreads(), with vals holding the sum over the ranks.
-__device__ __forceinline__ void comm_slot_allreduce(const CommDev& cd, int slot, float* vals, int n) {
+// by ALL threads of the CTA; returns after a __syncthreads(), with vals holding the sum over the ranks.  `pause()` is called
+// by every thread between the wait and the reduce: the window in which a faster peer may already push the next call (the
+// parity double buffer keeps it out of the data being reduced).  Tests use it to make the ranks drift; the product passes
+// none.
+template <class Pause = NoPause>
+__device__ __forceinline__ void comm_slot_allreduce(const CommDev& cd, int slot, float* vals, int n, Pause pause = {}) {
     __shared__ unsigned s_epoch;
     const int tid = threadIdx.x, nt = blockDim.x;
     if (tid == 0) s_epoch = cd.epoch[slot] + 1u;
@@ -84,6 +93,7 @@ __device__ __forceinline__ void comm_slot_allreduce(const CommDev& cd, int slot,
         }
     }
     __syncthreads();
+    pause();
     // 4. reduce in rank order
     const float* base = cd.data[cd.rank] + par * cd.world * per_rank + (size_t)slot * cd.stride;
     for (int i = tid; i < n; i += nt) {
@@ -93,6 +103,21 @@ __device__ __forceinline__ void comm_slot_allreduce(const CommDev& cd, int slot,
     }
     if (tid == 0) cd.epoch[slot] = e;
     __syncthreads();
+}
+
+// Layout of one rank's segment: flags [2][world][max_slots], epoch [max_slots], status, data [2][world][max_slots][stride].
+struct SegLayout {
+    size_t flags_off, epoch_off, status_off, data_off, total;
+};
+inline size_t seg_align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+inline SegLayout seg_layout(int world, int max_slots, int stride) {
+    SegLayout s;
+    s.flags_off = 0;
+    s.epoch_off = seg_align_up(s.flags_off + sizeof(unsigned) * 2 * (size_t)world * max_slots, 256);
+    s.status_off = seg_align_up(s.epoch_off + sizeof(unsigned) * (size_t)max_slots, 256);
+    s.data_off = seg_align_up(s.status_off + 64, 256);
+    s.total = seg_align_up(s.data_off + sizeof(float) * 2 * (size_t)world * max_slots * stride, 256);
+    return s;
 }
 
 // host handle behind the opaque `void* comm` of the C ABI

@@ -8,110 +8,15 @@
 //   x̄ = vsum[b,0:3]/n;  m_X = (Xv−x̄)ᵀ(Xv−x̄);  G_next = W1v_V·Hv + W1v_M·m_X + b1v (next layer's)
 // and leaves vsum either holding the summed statistics (training path keeps them) or zeroed for the next layer's
 // accumulation (FLAG_ZERO_VSUM: no memset launch between layers).
-#include "comm.cuh"
-#include "common.cuh"
+#include "virtual_update.cuh"
 
 namespace degnn {
 
-struct VUpdArgs {
-    int B, C, K;
-    unsigned flags;
-    float* vsum;
-    float* Xv;   // [B,3,C]
-    float* Hv;   // [B,C,64]
-    const float* m1; const float* mb1; const float* m2; const float* mb2;   // node_mlp_virtual
-    const float* nv1v; const float* nv1m; const float* nvb1;                 // next layer's W1v_V, W1v_M, b1v
-    float* G;    // [B,C,64]
-    const float* init_loc_mean;   // [B,3]   (FLAG_INIT: Xv := loc_mean broadcast over channels, FastEGNN.py:300)
-    const float* init_hv0;        // [C,64]  (FLAG_INIT: Hv := virtual_node_feat, FastEGNN.py:299)
-};
-
-constexpr int VU_KMAX = 4 + 3 * DISTEGNN_MAX_CHANNELS + H * DISTEGNN_MAX_CHANNELS;
-constexpr int VU_THREADS = 512;          // one (channel, column) output per thread at C = 8: the kernel is pure latency
-
 template <bool SYNC>
 __global__ void __launch_bounds__(VU_THREADS) virtual_update_kernel(const VUpdArgs a, const CommDev cd) {
-    constexpr int MC = DISTEGNN_MAX_CHANNELS;
-    __shared__ float sV[VU_KMAX];       // vsum[b,:] (summed over the partitions)
-    __shared__ float sX[3 * MC];        // new Xv [3][C]
-    __shared__ float sZ[3 * MC];        // Xv − x̄
-    __shared__ float sM[MC * MC];       // m_X
-    __shared__ float sHv[MC * H];       // Hv (old, then new) [C][64]
-    __shared__ float sAg[MC * H];       // mean mv [C][64]
-    __shared__ float sT[MC * H];        // hidden of node_mlp_virtual
-    const int b = blockIdx.x, tid = threadIdx.x, C = a.C;
-    float* vg = a.vsum + (size_t)b * a.K;
-    const bool init = a.flags & DISTEGNN_FLAG_INIT;
-    const bool last = a.flags & DISTEGNN_FLAG_LAST;
-    const bool zero = a.flags & DISTEGNN_FLAG_ZERO_VSUM;
-    for (int i = tid; i < a.K; i += VU_THREADS) sV[i] = vg[i];
-    __syncthreads();
-    if (SYNC) comm_slot_allreduce(cd, b, sV, a.K);
-    if (zero) {
-        for (int i = tid; i < a.K; i += VU_THREADS) vg[i] = 0.f;
-    } else if (SYNC) {
-        for (int i = tid; i < a.K; i += VU_THREADS) vg[i] = sV[i];
-    }
-    const float* vs = sV;
-    const float inv = 1.0f / fmaxf(vs[3], 1.0f);
-
-    if (tid < 3 * C) {
-        float x;
-        if (init && (a.flags & DISTEGNN_FLAG_INIT_CENTROID)) x = vs[tid / C] * inv;   // X_0 = x̄ of these positions
-        else x = (init && a.init_loc_mean) ? a.init_loc_mean[(size_t)b * 3 + tid / C] : a.Xv[(size_t)b * 3 * C + tid];
-        if (!init) x += vs[4 + tid] * inv;
-        sX[tid] = x;
-        a.Xv[(size_t)b * 3 * C + tid] = x;
-        sZ[tid] = x - vs[tid / C] * inv;   // tid / C = spatial dim
-    }
-    if (last) return;
-    for (int i = tid; i < C * H; i += VU_THREADS) {
-        const float hv = (init && a.init_hv0) ? a.init_hv0[i] : a.Hv[(size_t)b * C * H + i];
-        sHv[i] = hv;
-        if (init && a.init_hv0) a.Hv[(size_t)b * C * H + i] = hv;
-        sAg[i] = init ? 0.f : vs[4 + 3 * C + i] * inv;
-    }
-    __syncthreads();
-    if (tid < C * C) {
-        const int i = tid / C, j = tid - i * C;
-        sM[tid] = sZ[i] * sZ[j] + sZ[C + i] * sZ[C + j] + sZ[2 * C + i] * sZ[2 * C + j];
-    }
-    if (!init) {
-        // Hv' = Hv + W2·SiLU(W1·[Hv; agg] + b1) + b2   (per channel; thread per (c, n))
-        for (int i = tid; i < C * H; i += VU_THREADS) {
-            const int c = i / H, n = i - c * H;
-            float s = __ldg(a.mb1 + n);
-            // weights come straight from L2 (each is used by C rows only); the 64-step loops are fully unrolled by the
-            // compiler, i.e. all loads of a row are in flight together
-            for (int k = 0; k < H; ++k) s = fmaf(sHv[c * H + k], __ldg(a.m1 + k * H + n), s);
-            for (int k = 0; k < H; ++k) s = fmaf(sAg[c * H + k], __ldg(a.m1 + (H + k) * H + n), s);
-            sT[i] = silu(s);
-        }
-        __syncthreads();
-        float upd[(MC * H + VU_THREADS - 1) / VU_THREADS];
-        int u = 0;
-        for (int i = tid; i < C * H; i += VU_THREADS, ++u) {
-            const int c = i / H, n = i - c * H;
-            float s = __ldg(a.mb2 + n);
-            for (int k = 0; k < H; ++k) s = fmaf(sT[c * H + k], __ldg(a.m2 + k * H + n), s);
-            upd[u] = sHv[i] + s;
-        }
-        __syncthreads();
-        u = 0;
-        for (int i = tid; i < C * H; i += VU_THREADS, ++u) {
-            sHv[i] = upd[u];
-            a.Hv[(size_t)b * C * H + i] = upd[u];
-        }
-    }
-    __syncthreads();
-    // G[c][n] = Σ_k W1v_V[k][n]·Hv'[c][k] + Σ_j W1v_M[j][n]·m_X[j][c] + b1v[n]
-    for (int i = tid; i < C * H; i += VU_THREADS) {
-        const int c = i / H, n = i - c * H;
-        float s = __ldg(a.nvb1 + n);
-        for (int k = 0; k < H; ++k) s = fmaf(sHv[c * H + k], __ldg(a.nv1v + k * H + n), s);
-        for (int j = 0; j < C; ++j) s = fmaf(sM[j * C + c], __ldg(a.nv1m + j * H + n), s);
-        a.G[(size_t)b * C * H + i] = s;
-    }
+    const int b = blockIdx.x;
+    const NoPause pause;
+#include "virtual_update_graph.cuh"
 }
 
 }  // namespace degnn
@@ -123,28 +28,10 @@ extern "C" int distegnn_virtual_update_fwd(int n_graphs, int A, int C, int Na, u
     using namespace degnn;
     if (int rc = check_dims(A, C, Na)) return rc;
     if (n_graphs == 0) return DISTEGNN_OK;
-    const bool last = flags & DISTEGNN_FLAG_LAST, init = flags & DISTEGNN_FLAG_INIT;
-    DEGNN_CHECK_ARG(n_graphs > 0, "bad size");
-    DEGNN_CHECK_ARG(vsum && Xv, "null pointer");
-    DEGNN_CHECK_ARG(last || (Hv && next_layer_params && G), "null pointer (non-last)");
-    DEGNN_CHECK_ARG(last || init || layer_params, "null layer_params");
-    DEGNN_CHECK_ARG(init || (!init_loc_mean && !init_hv0), "init_loc_mean / init_hv0 need FLAG_INIT");
-    DEGNN_CHECK_ARG(!(flags & DISTEGNN_FLAG_INIT_CENTROID) || (init && !init_loc_mean),
-                    "FLAG_INIT_CENTROID needs FLAG_INIT and no init_loc_mean");
-    Layout L = make_layout(A, C, Na);
     VUpdArgs a;
-    a.B = n_graphs; a.C = C; a.K = 4 + 3 * C + H * C; a.flags = flags;
-    a.vsum = vsum; a.Xv = Xv; a.Hv = Hv;
-    const float* lp = layer_params ? layer_params : next_layer_params;
-    a.m1 = lp ? lp + L.off[DISTEGNN_P_M_W1] : nullptr;
-    a.mb1 = lp ? lp + L.off[DISTEGNN_P_M_B1] : nullptr;
-    a.m2 = lp ? lp + L.off[DISTEGNN_P_M_W2] : nullptr;
-    a.mb2 = lp ? lp + L.off[DISTEGNN_P_M_B2] : nullptr;
-    a.nv1v = next_layer_params ? next_layer_params + L.off[DISTEGNN_P_V_W1V] : nullptr;
-    a.nv1m = next_layer_params ? next_layer_params + L.off[DISTEGNN_P_V_W1M] : nullptr;
-    a.nvb1 = next_layer_params ? next_layer_params + L.off[DISTEGNN_P_V_B1] : nullptr;
-    a.G = G;
-    a.init_loc_mean = init_loc_mean; a.init_hv0 = init_hv0;
+    if (int rc = virtual_update_args(__func__, n_graphs, A, C, Na, flags, vsum, Xv, Hv, layer_params, next_layer_params,
+                                     G, init_loc_mean, init_hv0, &a))
+        return rc;
     if (comm) {
         const CommHost* c = (const CommHost*)comm;
         DEGNN_CHECK_ARG(c->connected, "comm not connected (distegnn_comm_connect)");
