@@ -74,6 +74,9 @@ SIGNATURES = {
     "distegnn_loss_packed_floats": [_i32, _i32],
     "distegnn_loss_partials": [_i64, _i32, _i32, _i32, _i32, _i32, C.c_float] + [_vp] * 10,
     "distegnn_loss_finalize": [_i64, _i32, _i32, _i32, _i32, _i32, C.c_float, C.c_float, _i32] + [_vp] * 10,
+    "distegnn_loss_packed_floats_steps": [_i32, _i32, _i32],
+    "distegnn_loss_partials_steps": [_i32, _i64, _i32, _i32, _i32, _i32, _i32, C.c_float] + [_vp] * 10,
+    "distegnn_loss_finalize_steps": [_i32, _i64, _i32, _i32, _i32, _i32, _i32, C.c_float, C.c_float, _i32] + [_vp] * 11,
     "distegnn_deterministic_workspace_bytes": [_i64, _i64, _i32, C.POINTER(_i64)],
     "distegnn_edge_layer_fwd_det": [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 11 + [_i64, _vp],
     "distegnn_edge_combine_det": [_i64, _i64, _i32] + [_vp] * 5 + [_i64, _vp],

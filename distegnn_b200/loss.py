@@ -17,6 +17,8 @@ each and three collectives; the forward already produces the gradients w.r.t. `l
 backward only scales them by the incoming gradient.  Sampling follows the reference exactly — one
 `torch.randperm(num_node)[:S]` per graph on the global CPU generator, in graph order — unless `samples` is passed in.
 CUDA only (no CPU path); `info` holds device scalars (`logged`, `mmd`, `loc_mean_dev`) — reading them synchronises.
+Given [K,N,3] positions and [K,B,3,C] virtual coordinates (a rollout's `trajectory` and `virtual_locs`), it is the mean
+of the K one-step losses in the same two launches and one collective (DESIGN §26).
 """
 from __future__ import annotations
 
@@ -50,19 +52,22 @@ class _TrainLoss(torch.autograd.Function):
     def forward(ctx, pred, Xv, target, gptr, samples, loc_mean, cfg):
         lib = _lib.load()
         dev = pred.device
-        N, (B, _, Cn) = int(pred.shape[0]), Xv.shape
-        S, world, rank = int(samples.shape[1]), cfg["world"], cfg["rank"]
+        K = cfg["steps"]                                     # None: the one-step [N,3] call
+        N, (B, _, Cn) = int(pred.shape[-2]), Xv.shape[-3:]
+        S, world, rank = int(samples.shape[-1]), cfg["world"], cfg["rank"]
         stream = _lib.stream_ptr(dev)
-        npk = lib.distegnn_loss_packed_floats(B, world)
-        scratch = torch.zeros(3 + npk, dtype=torch.float32, device=dev)          # acc[3] | packed[npk]
-        acc, packed = scratch[:3], scratch[3:]
-        gV_raw = torch.empty(B, 3, Cn, dtype=torch.float32, device=dev)
+        npk = lib.distegnn_loss_packed_floats(B, world) if K is None else lib.distegnn_loss_packed_floats_steps(K, B, world)
+        na = 3 * (K or 1)
+        scratch = torch.zeros(na + npk, dtype=torch.float32, device=dev)         # acc[3K] | packed[npk]
+        acc, packed = scratch[:na], scratch[na:]
+        gV_raw = torch.empty(Xv.shape, dtype=torch.float32, device=dev)
         p, t, xv = pred.detach().contiguous(), target.contiguous(), Xv.detach().contiguous()
         with torch.cuda.device(dev):
-            check(lib.distegnn_loss_partials(N, B, Cn, S, world, rank, cfg["sigma"], ptr(p), ptr(t), ptr(xv), ptr(loc_mean),
-                                             ptr(gptr), ptr(samples), ptr(acc), ptr(packed), ptr(gV_raw), stream),
+            args = (N, B, Cn, S, world, rank, cfg["sigma"], ptr(p), ptr(t), ptr(xv), ptr(loc_mean), ptr(gptr),
+                    ptr(samples), ptr(acc), ptr(packed), ptr(gV_raw), stream)
+            check(lib.distegnn_loss_partials(*args) if K is None else lib.distegnn_loss_partials_steps(K, *args),
                   "loss_partials")
-            if world > 1:                                    # the ONE collective of the step
+            if world > 1:                                    # the ONE collective of the call (all K steps)
                 comm, be = cfg.get("comm"), cfg.get("backend")
                 if comm is not None and be is not None and npk <= comm.max_slots * comm.slot_floats:
                     be.allreduce_packed(comm, packed)
@@ -71,10 +76,11 @@ class _TrainLoss(torch.autograd.Function):
                     dist.all_reduce(packed, op=dist.ReduceOp.SUM, group=cfg.get("group"))
             g_pred = torch.empty_like(p)
             g_Xv = torch.empty_like(xv)
-            out = torch.empty(4, dtype=torch.float32, device=dev)
-            check(lib.distegnn_loss_finalize(N, B, Cn, S, world, rank, cfg["sigma"], cfg["weight"], cfg["accum"], ptr(p),
-                                             ptr(t), ptr(loc_mean), ptr(acc), ptr(packed), ptr(gV_raw), ptr(g_pred),
-                                             ptr(g_Xv), ptr(out), stream), "loss_finalize")
+            out = torch.empty(4 + 2 * (K or 0), dtype=torch.float32, device=dev)
+            args = (N, B, Cn, S, world, rank, cfg["sigma"], cfg["weight"], cfg["accum"], ptr(p), ptr(t), ptr(loc_mean),
+                    ptr(acc), ptr(packed), ptr(gV_raw), ptr(g_pred), ptr(g_Xv), ptr(out))
+            check(lib.distegnn_loss_finalize(*args, stream) if K is None else
+                  lib.distegnn_loss_finalize_steps(K, *args, ptr(out[4:]), stream), "loss_finalize")
         ctx.save_for_backward(g_pred, g_Xv)
         ctx.mark_non_differentiable(out)
         return out[0].clone(), out
@@ -93,15 +99,33 @@ def train_loss(loc_pred: Tensor, loc_target: Tensor, virtual_node_loc: Tensor, b
     """See the module docstring.  `node_counts` (host ints per graph, e.g. from the loader's `ptr`) avoids the one host
     sync needed to size the reference's `randperm` draws; `samples` (int32 [B,S], graph-local, −1 padded) overrides the
     draw; `model` (a distegnn_b200.FastEGNN of a multi-partition job) lends its peer-memory communicator to the
-    collective."""
+    collective.
+
+    Stepped (K steps of a rollout, DESIGN §26): loc_pred, loc_target [K,N,3], virtual_node_loc [K,B,3,C], samples
+    [K,B,S].  The loss is (1/K)·Σ_t ℓ_t, ℓ_t the one-step loss of step t (its MSE, and the MMD of virtual_node_loc[t]
+    against samples of loc_target[t]), in one partials launch, one packed all-reduce and one finalize launch; the
+    gradients are [K,N,3] and [K,B,3,C].  info["logged"] and info["mmd"] are the means over the steps,
+    info["logged_steps"] and info["mmd_steps"] float32 [K] the values of every step.  The default samples are
+    `draw_samples` once per step, in step order, so K = 1 draws what the one-step call draws and gives its bits.  With
+    several ranks the packed vector has 1 + K + world·3B floats; when it is larger than the model's communicator holds
+    (max_slots·slot_floats), the exchange goes through torch.distributed as without a communicator."""
     if loc_pred.device.type != "cuda":
         raise _lib.DistEGNNError("distegnn_b200.train_loss runs only on CUDA tensors (no CPU path)")
-    if loc_pred.shape != loc_target.shape or loc_pred.dim() != 2 or loc_pred.shape[1] != 3:
-        raise ValueError("loc_pred / loc_target must both be [N,3]")
-    if virtual_node_loc.dim() != 3 or virtual_node_loc.shape[1] != 3:
-        raise ValueError("virtual_node_loc must be [B,3,C]")
+    stepped = loc_pred.dim() == 3
+    if stepped:
+        if loc_pred.shape != loc_target.shape or loc_pred.shape[2] != 3 or loc_pred.shape[0] < 1:
+            raise ValueError("stepped loc_pred / loc_target must both be [K,N,3], K >= 1")
+        if virtual_node_loc.dim() != 4 or virtual_node_loc.shape[2] != 3 or \
+                virtual_node_loc.shape[0] != loc_pred.shape[0]:
+            raise ValueError(f"stepped virtual_node_loc must be [K={loc_pred.shape[0]},B,3,C]")
+    else:
+        if loc_pred.shape != loc_target.shape or loc_pred.dim() != 2 or loc_pred.shape[1] != 3:
+            raise ValueError("loc_pred / loc_target must both be [N,3]")
+        if virtual_node_loc.dim() != 3 or virtual_node_loc.shape[1] != 3:
+            raise ValueError("virtual_node_loc must be [B,3,C]")
     dev = loc_pred.device
-    B, _, Cn = virtual_node_loc.shape
+    K = int(loc_pred.shape[0]) if stepped else None
+    B, _, Cn = virtual_node_loc.shape[-3:]
     if Cn > _lib.MAX_CHANNELS:
         raise ValueError(f"virtual_channels={Cn} exceeds the compiled limit {_lib.MAX_CHANNELS}")
     S = int(mmd_samples) * Cn                                      # train.py:122
@@ -109,23 +133,28 @@ def train_loss(loc_pred: Tensor, loc_target: Tensor, virtual_node_loc: Tensor, b
     if samples is None:
         if node_counts is None:
             node_counts = (gptr[1:] - gptr[:-1]).tolist()          # one host sync (the reference has B of them)
-        samples = draw_samples(node_counts, S)
+        samples = draw_samples(node_counts, S) if not stepped else \
+            torch.stack([draw_samples(node_counts, S) for _ in range(K)])
     samples = samples.to(device=dev, dtype=torch.int32).contiguous()
-    if samples.shape != (B, S):
-        raise ValueError(f"samples must be [B={B}, S={S}]")
+    want = (B, S) if not stepped else (K, B, S)
+    if samples.shape != want:
+        raise ValueError(f"samples must be [{'K=%d, ' % K if stepped else ''}B={B}, S={S}]")
     rank = 0
     if world_size > 1:
         import torch.distributed as dist
         rank = dist.get_rank(process_group)
     cfg = dict(world=int(world_size), rank=rank, sigma=float(mmd_sigma), weight=float(mmd_weight),
-               accum=int(accumulation_steps), group=process_group)
+               accum=int(accumulation_steps), group=process_group, steps=K)
     if model is not None and getattr(model, "_comm", None):
         from .backend import cuda_backend
         cfg["comm"], cfg["backend"] = model._comm, cuda_backend()
     lm = None if loc_mean is None else loc_mean.detach().to(torch.float32).contiguous()
     loss, out = _TrainLoss.apply(loc_pred.to(torch.float32), virtual_node_loc.to(torch.float32),
                                  loc_target.detach().to(torch.float32), gptr, samples, lm, cfg)
-    return loss, {"logged": out[1], "mmd": out[2], "loc_mean_dev": out[3], "samples": samples}
+    info = {"logged": out[1], "mmd": out[2], "loc_mean_dev": out[3], "samples": samples}
+    if stepped:
+        info["logged_steps"], info["mmd_steps"] = out[4:4 + K], out[4 + K:]
+    return loss, info
 
 
 class _ChamferDistance(torch.autograd.Function):

@@ -507,6 +507,22 @@ DISTEGNN_API int distegnn_loss_finalize(int64_t n_nodes, int n_graphs, int C, in
                                         float weight, int accumulation_steps, const float *pred, const float *target,
                                         const float *loc_mean, const float *acc, const float *packed, const float *gV_raw,
                                         float *g_pred, float *g_Xv, float *out, void *stream);
+/* The same loss over K steps of a rollout in one partials launch, one all-reduce and one finalize launch: pred, target
+ * [K,N,3], Xv [K,B,3,C], samples [K,B,S], acc [3K], gV_raw [K,B,3,C]; loc_mean [B,3] as above (checked once).
+ *   packed [1 + K + world·3B]  [0] n_r, [1 + t] n_r·MSE_r of step t, [1 + K + r·3B ...] rank r's loc_mean
+ * out[0] = (1/K)·Σ_t ℓ_t with ℓ_t the one-step out[0] of step t, out[1] and out[2] the means over the steps of the logged
+ * loss and MMD_r, out[3] as above; out_steps [2K] (may be NULL) the per-step logged loss [0, K) and MMD_r [K, 2K);
+ * g_pred [K,N,3], g_Xv [K,B,3,C] the gradients of out[0].  K = 1 has the one-step layout and gives its bits. */
+DISTEGNN_API int distegnn_loss_packed_floats_steps(int steps, int n_graphs, int world);
+DISTEGNN_API int distegnn_loss_partials_steps(int steps, int64_t n_nodes, int n_graphs, int C, int S, int world, int rank,
+                                              float sigma, const float *pred, const float *target, const float *Xv,
+                                              const float *loc_mean, const int64_t *graph_ptr, const int32_t *samples,
+                                              float *acc, float *packed, float *gV_raw, void *stream);
+DISTEGNN_API int distegnn_loss_finalize_steps(int steps, int64_t n_nodes, int n_graphs, int C, int S, int world, int rank,
+                                              float sigma, float weight, int accumulation_steps, const float *pred,
+                                              const float *target, const float *loc_mean, const float *acc,
+                                              const float *packed, const float *gV_raw, float *g_pred, float *g_Xv,
+                                              float *out, float *out_steps, void *stream);
 
 /* ---- deterministic mode (csrc/deterministic.cu, csrc/det.cuh; DESIGN §17) ----------------------------------------------
  * Bitwise-reproducible forward: every floating-point sum is taken in an order fixed by the sizes, never by the grid, the

@@ -41,6 +41,11 @@ synthetic path below runs unchanged.
 scheduler and the train loader's order included).  After the loop the best checkpoint's weights are restored and
 `--eval_rotate` / `--eval_translate` / `--rollout_steps` run on them.
 
+`--train_rollout K` (with --trajectory, in both loops) trains on K-step rollouts instead (DESIGN §26): a train loader of
+horizon K, `differentiable_rollout` from every batch and the stepped `train_loss`, the mean of the K one-step losses;
+with several ranks `rollout_grad_sum` adds the parameter gradients up before the clip.  Valid, test and the evaluations
+stay one-step.
+
 `data.accelerate_mode: cutoff_edges` (FastEGNN, e.g. config/nbody_fastegnn.yaml) is the reference's single-device mode:
 `batch_size` synthetic graphs in one batch, the candidate graph fully connected for `radius: -1` (N-body) or a radius
 graph, then `data.cutoff_rate` (`--cutoff_rate` overrides it, reference main.py:133-134) drops the longest edges of
@@ -132,6 +137,9 @@ def parse():
     p.add_argument("--epochs", type=int, default=None, help="(new) with --trajectory: E >= 1 epochs of the reference's "
                    "epoch loop (utils/train.py) over train/valid/test, with best/last checkpoints, early stopping and "
                    "resume from --checkpoint (DESIGN §24)")
+    p.add_argument("--train_rollout", type=int, default=None, help="(new) with --trajectory: train on K-step rollouts "
+                   "(differentiable_rollout and the stepped train_loss, the mean of the K one-step losses against the "
+                   "recorded frames, DESIGN §26); valid, test and the evaluations stay one-step")
     return p.parse_args()
 
 
@@ -215,6 +223,56 @@ def eval_transform_of(args):
     return bool(args.eval_rotate), t
 
 
+def split_samples(path, cfg, part, horizon=1):
+    """(trajectories, (scene, frame) samples) of split `part` under `path` with the config's recipe, or None without
+    files.  Water-3D / Fluid113K: the frame draw is capped so that every sample holds `horizon` steps of delta_t frames;
+    SystemExit with a message when the shortest scene cannot hold them."""
+    from distegnn_b200.frames import load_nbody, load_scenes, sample_list
+    d = cfg["data"]
+    recipe, frame_0, delta = recipe_of_config(cfg)
+    files = split_files(path, recipe, part)
+    if not files:
+        return None
+    traj = load_nbody(path, part) if recipe == "nbody" else load_scenes(files, recipe)
+    kw = {}
+    if recipe != "nbody":
+        shortest = min(sc.n_frames for sc in traj.scenes)
+        kw["max_frame"] = min(traj.recipe.max_frame, shortest - 1 - max(horizon * delta, 1))
+        if horizon > 1 and kw["max_frame"] < 0:
+            raise SystemExit(f"--trajectory {path}/{part}: the shortest scene has {shortest} frames; it cannot hold "
+                             f"{horizon} step(s) of delta_t={delta} frames after any frame")
+    return traj, sample_list(traj, seed=int(cfg.get("seed", 0)), max_samples=d.get("max_samples"), delta_t=delta,
+                             frame_0=frame_0, **kw)
+
+
+def train_rollout_of(args, cfg):
+    """--train_rollout K, or None; exits with code 2 and a message, before any CUDA work, when it cannot run: K < 1, no
+    --trajectory, a train split whose samples cannot hold K steps (frame_loaders' horizon check), or no rollout time
+    step (rollout_args' rule)."""
+    K = args.train_rollout
+    if K is None:
+        return None
+    msg = None
+    if K < 1:
+        msg = ">= 1"
+    elif not args.trajectory:
+        msg = "used with --trajectory (the synthetic path has no recorded frames to train against)"
+    else:
+        from distegnn_b200.frames import check_samples
+        try:
+            found = split_samples(args.trajectory, cfg, "train", horizon=K)
+            if found is not None:
+                check_samples(found[0], found[1], recipe_of_config(cfg)[2], K)
+        except (SystemExit, ValueError) as e:
+            msg = f"used with a train split whose samples hold {K} step(s): {e}"
+    if msg is not None:
+        if int(os.environ.get("LOCAL_RANK", "0")) == 0:
+            print(f"--train_rollout {K}: must be {msg}", flush=True)
+        sys.exit(2)
+    rollout_args(args, cfg, int(os.environ.get("LOCAL_RANK", "0")), K, "--train_rollout")
+    return K
+
+
 def main():
     args = parse()
     noise = train_noise_of(args)
@@ -237,6 +295,7 @@ def main():
     if args.virtual_channels is not None:
         cfg["model"]["virtual_channels"] = args.virtual_channels
     epochs = epochs_of(args, cfg)
+    train_rollout = train_rollout_of(args, cfg)
 
     # FastEGNN's cutoff_edges mode (reference README.md:30-33): the cutoff rate applies; in distribute mode it does not
     cutoff_mode = str(cfg["data"].get("accelerate_mode", "distribute")) == "cutoff_edges"
@@ -280,9 +339,10 @@ def main():
     model.eval()
     if args.trajectory:
         if epochs:
-            trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform, state)
+            trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform, state,
+                           train_rollout)
         else:
-            trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform)
+            trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise, transform, train_rollout)
         if distributed:
             dist.destroy_process_group()
         return
@@ -380,9 +440,9 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only;
     `transform` (rotate, translate) to every loader built (the same samples as without it: a rotated and translated
     copy of the split).  Returns (recipe name, {part: loader or None})."""
-    from distegnn_b200.frames import FrameLoader, load_nbody, load_scenes, sample_list
+    from distegnn_b200.frames import FrameLoader
     d = cfg["data"]
-    recipe, frame_0, delta = recipe_of_config(cfg)
+    recipe, _, delta = recipe_of_config(cfg)
     cutoff_mode = rate is not None
     if cutoff_mode:
         radius = 0.035 if recipe == "water3d" else d.get("radius", -1)
@@ -398,19 +458,11 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     xf = {} if transform is None else dict(rotate=transform[0], translate=transform[1])
     out = {}
     for part in parts:
-        files = split_files(path, recipe, part)
-        if not files:
+        found = split_samples(path, cfg, part, horizon)
+        if found is None:
             out[part] = None
             continue
-        traj = load_nbody(path, part) if recipe == "nbody" else load_scenes(files, recipe)
-        kw = {}
-        if recipe != "nbody":
-            shortest = min(sc.n_frames for sc in traj.scenes)
-            kw["max_frame"] = min(traj.recipe.max_frame, shortest - 1 - max(horizon * delta, 1))
-            if horizon > 1 and kw["max_frame"] < 0:
-                raise SystemExit(f"--trajectory {path}/{part}: the shortest scene has {shortest} frames; it cannot hold "
-                                 f"{horizon} step(s) of delta_t={delta} frames after any frame")
-        samples = sample_list(traj, seed=seed, max_samples=d.get("max_samples"), delta_t=delta, frame_0=frame_0, **kw)
+        traj, samples = found
         out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
                                 seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
                                 cutoff_rate=rate or 0.0, horizon=horizon, noise=noise if part == "train" else None,
@@ -420,18 +472,18 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     return recipe, out
 
 
-def rollout_args(args, cfg, local_rank):
-    """(recipe, K, tau) of `--rollout_steps K` on the trajectory; exits with a message before any training when the
-    rollout could not run (no `--rollout_tau` for a recipe with physical velocities)."""
+def rollout_args(args, cfg, local_rank, K=None, flag="--rollout_steps"):
+    """(recipe, K, tau) of `--rollout_steps K` (or of `flag` with K steps) on the trajectory; exits with a message before
+    any training when the rollout could not run (no `--rollout_tau` for a recipe with physical velocities)."""
     recipe, _, delta = recipe_of_config(cfg)
-    K = args.rollout_steps
+    K = args.rollout_steps if K is None else K
     tau = args.rollout_tau if args.rollout_tau is not None else (float(delta) if recipe == "water3d" else None)
     if tau is None and recipe == "nbody" and args.trajectory:   # files written by distegnn_b200.nbody record their dt
         from distegnn_b200.nbody import meta_rollout_tau
         tau = meta_rollout_tau(args.trajectory, delta)
     if K > 0 and tau is None:
         if local_rank == 0:
-            print(f"--rollout_steps with --trajectory on {recipe!r} needs --rollout_tau: its velocities are physical and "
+            print(f"{flag} with --trajectory on {recipe!r} needs --rollout_tau: its velocities are physical and "
                   "the frame time is not in the files (Water-3D defaults to delta_t; N-body files written by "
                   "distegnn_b200.nbody default to delta_t·sample_freq·dt from their meta file)", flush=True)
         sys.exit(2)
@@ -456,9 +508,64 @@ def trajectory_loss(cfg, model, world_size, distributed):
     return loss_of
 
 
-def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None):
+def trajectory_rollout_loss(cfg, model, world_size, distributed, train_loader, recipe, tau, steps):
+    """loss_of(kw, ex, accumulation_steps=1) -> (loss, info) of `--train_rollout K` (DESIGN §26).  With gradients
+    enabled: a K-step `differentiable_rollout` from the batch's state, with `rollout_eval`'s graph arguments (the train
+    loader's radius, or its complete graph and cutoff rate) and `tau`, then the stepped `train_loss` of the trajectory
+    and the virtual coordinates against ex["targets"] [K,M,3]: the mean over the steps of the one-step loss.  Under
+    no_grad (fit's valid and test passes, the evaluations): `trajectory_loss`'s one-step loss, so that those losses mean
+    what they mean without the flag.  With several ranks the parameter gradients are this rank's only: `rollout_grad_sum`
+    adds them up once per optimiser step."""
+    from distegnn_b200 import differentiable_rollout, train_loss
+    one_step = trajectory_loss(cfg, model, world_size, distributed)
+    mmd = (cfg.get("train", {}) or {}).get("mmd", {}) or {}
+    inner = model.module if distributed else model
+    use_attr = cfg["model"]["node_attr_nf"] > 0
+    ld = train_loader
+
+    def loss_of(kw, ex, accumulation_steps=1):
+        if not torch.is_grad_enabled():
+            return one_step(kw, ex, accumulation_steps)
+        if ld.radius is not None:
+            g = dict(radius=ld.radius)
+        else:                                                  # fully connected: the candidates, cut again every step
+            g = dict(graph=ld.complete_graph(tuple(ex["node_counts"])) if ld.cutoff_rate > 0 else kw["edge_index"])
+        res = differentiable_rollout(model, kw["node_feat"], kw["node_loc"], kw["node_vel"], kw["loc_mean"],
+                                     kw["data_batch"], kw["node_attr"] if use_attr else None, steps=steps, tau=tau,
+                                     speed_col=SPEED_COL[recipe], cutoff_rate=ld.cutoff_rate, **g)
+        return train_loss(res.trajectory, ex["targets"], res.virtual_locs, kw["data_batch"], world_size=world_size,
+                          mmd_samples=int(mmd.get("samples", 50)), mmd_sigma=float(mmd.get("sigma", 3)),
+                          mmd_weight=float(mmd.get("weight", 0.01)), accumulation_steps=accumulation_steps,
+                          loc_mean=kw["loc_mean"], node_counts=ex["node_counts"], model=inner)
+    return loss_of
+
+
+def rollout_grad_sum(model, world_size):
+    """A callable that sums the parameter gradients over the ranks in one all-reduce, each divided by world_size first:
+    what DDP's reducer does for the one-step path, which it cannot do for a differentiable rollout (it never sees that
+    call).  Run once per optimiser step, after the last accumulated backward and before clipping; with the train
+    loss's world·n_r/Σn weighting, K = 1 then gives the one-step path's gradients."""
+    params = list(model.parameters())
+
+    def grad_sum():
+        have = [p for p in params if p.grad is not None]       # the same set on every rank: the same model and steps
+        if not have:
+            return
+        flat = torch.cat([p.grad.reshape(-1) for p in have]).div_(world_size)
+        dist.all_reduce(flat, op=dist.ReduceOp.SUM)
+        off = 0
+        for p in have:
+            p.grad.copy_(flat[off:off + p.numel()].view_as(p.grad))
+            off += p.numel()
+    return grad_sum
+
+
+def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None,
+                   train_rollout=None):
     """--trajectory: `--train_steps` optimisation steps (at least one epoch's worth if 0 is given: one pass) of the
-    reference's training step on batches from FrameLoader (with `noise` on its inputs), then `trajectory_eval`."""
+    reference's training step on batches from FrameLoader (with `noise` on its inputs), then `trajectory_eval`.  With
+    `train_rollout` K every step trains on a K-step rollout (`trajectory_rollout_loss`) from a train loader of horizon K;
+    the evaluation stays one-step."""
     recipe, K, tau = rollout_args(args, cfg, local_rank)
     dev = torch.device("cuda", local_rank)
     recipe, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, noise=noise)
@@ -466,20 +573,30 @@ def trajectory_run(args, cfg, model, world_size, local_rank, distributed, rate, 
     lr = args.lr if args.lr is not None else float(tc.get("learning_rate", tc.get("lr", 5e-4)))
     opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=float(tc.get("weight_decay", 1e-12)))
     loss_of = trajectory_loss(cfg, model, world_size, distributed)
+    train_ld, train_of, grad_sum, what = loaders["train"], loss_of, None, "MSE"
+    if train_rollout is not None:                              # the one-step train loader stays for the evaluation
+        _, _, r_tau = rollout_args(args, cfg, local_rank, train_rollout, "--train_rollout")
+        train_ld = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=train_rollout,
+                                 parts=("train",), noise=noise)[1]["train"]
+        train_of = trajectory_rollout_loss(cfg, model, world_size, distributed, train_ld, recipe, r_tau, train_rollout)
+        grad_sum = rollout_grad_sum(model, world_size) if distributed else None
+        what = f"{train_rollout}-step rollout mean MSE"
 
-    steps = args.train_steps or len(loaders["train"])
+    steps = args.train_steps or len(train_ld)
     model.train()
     done, t0 = 0, time.perf_counter()
     while done < steps:
-        for kw, ex in loaders["train"]:
+        for kw, ex in train_ld:
             opt.zero_grad()
-            loss, info = loss_of(kw, ex)
+            loss, info = train_of(kw, ex)
             loss.backward()
+            if grad_sum is not None:
+                grad_sum()
             torch.nn.utils.clip_grad_norm_(model.parameters(), max_norm=0.3)
             opt.step()
             done += 1
             if local_rank == 0 and (done % 10 == 0 or done == steps):
-                print(f"[{recipe}] train step {done}: MSE {info['logged'].item():.6e}", flush=True)
+                print(f"[{recipe}] train step {done}: {what} {info['logged'].item():.6e}", flush=True)
             if done == steps:
                 break
     torch.cuda.synchronize()
@@ -542,7 +659,8 @@ def exp_name_of(cfg, world_size, rate=None):
     return f"{d.get('dataset_name')}_{m['model_name']}_{d.get('radius')}_{rate:.3f}_{m['virtual_channels']}_{world_size}_{suffix}"
 
 
-def fit(model, opt, scheduler, loaders, loss_of, cfg, epochs, start_epoch=0, world_size=1, rank=0, out_dir="."):
+def fit(model, opt, scheduler, loaders, loss_of, cfg, epochs, start_epoch=0, world_size=1, rank=0, out_dir=".",
+        before_step=None, train_note=""):
     """The reference's epoch loop (utils/train.py:17-289, DESIGN §24): epochs start_epoch + 1 .. `epochs`, each a train
     pass, and every `log.test_interval` epochs a valid and a test pass; `best_model.pth` (strictly lower valid loss),
     `last_model.pth` (every evaluation epoch) and `log/log.json` under `out_dir`, written by rank 0 only.
@@ -553,6 +671,9 @@ def fit(model, opt, scheduler, loaders, loss_of, cfg, epochs, start_epoch=0, wor
     loss_of     (kw, ex, accumulation_steps) -> (loss, info), info["logged"] a 0-dim tensor: the batch's logged MSE
     cfg         the run's config (a plain dict, stored in every checkpoint and in log.json): train.accumulation_steps
                 (1), train.early_stop (None: never), log.test_interval (1), and the clip condition `reference_clips`
+    before_step None, or a callable run once per optimiser step after the last accumulated backward and before the
+                clip and the step (`rollout_grad_sum`: the rank sum of a differentiable rollout's gradients)
+    train_note  appended to every train pass's loss line (what the train loss is, when it is not the one-step MSE)
     Returns (best_log_dict, log_dict) on rank 0, (None, None) on the others."""
     tc, lc = cfg.get("train") or {}, cfg.get("log") or {}
     A, interval = int(tc.get("accumulation_steps", 1)), int(lc.get("test_interval", 1))
@@ -587,6 +708,8 @@ def fit(model, opt, scheduler, loaders, loss_of, cfg, epochs, start_epoch=0, wor
                 if train:
                     loss.backward()
                     if (step + 1) % A == 0:
+                        if before_step is not None:
+                            before_step()
                         if clip:
                             torch.nn.utils.clip_grad_norm_(model.parameters(), max_norm=0.3)
                         opt.step()
@@ -595,7 +718,8 @@ def fit(model, opt, scheduler, loaders, loss_of, cfg, epochs, start_epoch=0, wor
                         opt.zero_grad()
         value = float(tot) / graphs if graphs else float("nan")    # the one host read of the pass
         if rank == 0:
-            print(f"{'' if train else '==> '}{tag} epoch: {epoch}, avg loss: {value:.5f}", flush=True)
+            print(f"{'' if train else '==> '}{tag} epoch: {epoch}, avg loss: {value:.5f}{train_note if train else ''}",
+                  flush=True)
         return value
 
     for epoch in range(start_epoch + 1, epochs + 1):
@@ -651,14 +775,21 @@ def optimizer_of(model, cfg, epochs, n_batches):
     return opt, torch.optim.lr_scheduler.CosineAnnealingLR(opt, T_max=t_max, eta_min=1e-8)
 
 
-def trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None, state=None):
+def trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, noise=None, transform=None, state=None,
+                   train_rollout=None):
     """--trajectory with --epochs E: `fit` on FrameLoader's train (with `noise`), valid and test splits, the reference's
     Adam and optional cosine schedule (main.py:197-202); `state`, a checkpoint with an `epoch` key, resumes after that
-    epoch (main.py:208-220).  Then the best checkpoint's weights, and `trajectory_eval` on them."""
+    epoch (main.py:208-220).  Then the best checkpoint's weights, and `trajectory_eval` on them.  With `train_rollout` K
+    the train passes run on K-step rollouts from a train loader of horizon K (`trajectory_rollout_loss`, the ranks'
+    gradients summed by `rollout_grad_sum`); valid and test stay one-step, and K goes into the config as
+    train.train_rollout."""
     recipe, _, _ = rollout_args(args, cfg, local_rank)
     dev = torch.device("cuda", local_rank)
     _, loaders = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, parts=("train", "valid", "test"),
                                noise=noise)
+    if train_rollout is not None:
+        loaders["train"] = frame_loaders(args.trajectory, cfg, world_size, local_rank, dev, rate, horizon=train_rollout,
+                                         parts=("train",), noise=noise)[1]["train"]
     for part, ld in loaders.items():
         if not ld:
             if local_rank == 0:
@@ -672,6 +803,8 @@ def trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, 
     if args.early_stop is not None:
         tc["early_stop"] = args.early_stop
     tc["epochs"] = args.epochs
+    if train_rollout is not None:
+        tc["train_rollout"] = train_rollout
     cfg["data"]["world_size"] = world_size
     opt, scheduler = optimizer_of(model, cfg, args.epochs, len(loaders["train"]))
     start = 0
@@ -688,7 +821,17 @@ def trajectory_fit(args, cfg, model, world_size, local_rank, distributed, rate, 
     cfg["log"] = dict(cfg.get("log") or {}, exp_name=name[0])
     out_dir = os.path.join(cfg["log"].get("log_dir", "./logs"), name[0])
     loss_of = trajectory_loss(cfg, model, world_size, distributed)
-    best, _ = fit(model, opt, scheduler, loaders, loss_of, cfg, args.epochs, start, world_size, local_rank, out_dir)
+    extra = {}
+    if train_rollout is not None:
+        _, _, r_tau = rollout_args(args, cfg, local_rank, train_rollout, "--train_rollout")
+        extra = dict(train_note=f" (mean over {train_rollout} rollout steps)",
+                     before_step=rollout_grad_sum(model, world_size) if distributed else None)
+        train_of = trajectory_rollout_loss(cfg, model, world_size, distributed, loaders["train"], recipe, r_tau,
+                                           train_rollout)
+    else:
+        train_of = loss_of
+    best, _ = fit(model, opt, scheduler, loaders, train_of, cfg, args.epochs, start, world_size, local_rank, out_dir,
+                  **extra)
     if distributed:
         dist.barrier()
     path = os.path.join(out_dir, "state_dict", "best_model.pth")
