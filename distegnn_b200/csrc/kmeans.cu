@@ -7,7 +7,10 @@
 // (`_kmeans_single_lloyd`): stop when no label changed (strict convergence) or when the squared centre shift falls to
 // `tol` — then one more assignment pass so that labels match the final centres; iterations enqueued after convergence
 // are no-ops.  state[0]: 0 running, 1 final assignment pending, 2 done; state[1]: iterations done; state[2]: labels
-// changed in the last pass.  Cluster sums are accumulated in float64 (order-independent to ~1e-16).
+// changed in the last pass.  Cluster sums are accumulated in float64 (order-independent to ~1e-16).  The update step
+// is sklearn's M-step (`_k_means_common.pyx`): empty clusters are relocated to the points farthest from their centres,
+// then every centre is fp32(sum)·fp32(1/count) — so on data whose sums are exact the centres are sklearn's bit for bit.
+// No extra device memory and no host synchronisation: the relocation runs inside the update launch when a count is 0.
 //
 // Points have D coordinates: D = 3 for node positions (distegnn_kmeans_lloyd, the k-means partitioner) and D = P <= 16
 // for the spectral partitioner's embedding (distegnn_kmeans_lloyd_d, which also returns the inertia sklearn compares
@@ -19,6 +22,7 @@ namespace degnn {
 constexpr int KM_MAXK = 64;
 constexpr int KM_MAXD = DISTEGNN_KMEANS_MAX_DIM;
 constexpr int KM_THREADS = 256;
+constexpr int KM_UPDATE_THREADS = 1024;
 constexpr int KM_INERTIA_THREADS = 1024;
 
 struct KmArgs {
@@ -105,33 +109,126 @@ __global__ void __launch_bounds__(KM_THREADS) kmeans_assign_kernel(const KmArgs 
     if (tid == 0 && schanged) atomicAdd(a.state + 2, schanged);
 }
 
-__global__ void kmeans_update_kernel(const KmArgs a) {
-    __shared__ float shift[KM_MAXK];
-    const int st = a.state[0];
-    if (st == 2) return;
-    const int k = threadIdx.x, D = a.D, W = D + 1;
-    if (st == 1) {                                        // the final assignment has run
-        if (k == 0) a.state[0] = 2;
-        return;
-    }
-    float s = 0.f;
-    if (k < a.K) {
-        const double n = a.sums[W * k + D];
-        if (n > 0.0) {                                    // an empty cluster keeps its centre
-            for (int c = 0; c < D; ++c) {
-                const float cc = (float)(a.sums[W * k + c] / n);
-                const float dc = cc - a.centers[D * k + c];
-                s += dc * dc;
-                a.centers[D * k + c] = cc;
+// (d, i) comes before (d', i') in the relocation order: larger distance first, then lower index
+__device__ __forceinline__ bool km_before(float d, int64_t i, float d2, int64_t i2) {
+    return d > d2 || (d == d2 && i < i2);
+}
+
+// sklearn's `_relocate_empty_clusters_dense`, between the assignment and the averaging: with distances
+// d_i = ‖x_i − c_old[label_i]‖² to the centres the assignment used, the e-th empty cluster (ascending id) takes the e-th
+// point in the order (d descending, index ascending): its sums become that point and count 1, and the point's own
+// cluster loses it.  Labels are not changed.  Nothing moves when every d_i is 0.  One CTA, one pass over the points per
+// empty cluster, each pass finding the next point after the previous one in that order — empty clusters are rare, and
+// the launch costs only the count check otherwise.
+template <int DT>
+__device__ void km_relocate(const KmArgs& a, const float* sc, const int* empty, int n_empty) {
+    __shared__ float rd[KM_UPDATE_THREADS / 32];
+    __shared__ long long ri[KM_UPDATE_THREADS / 32];
+    __shared__ float pick_d;
+    __shared__ long long pick_i;
+    const int tid = threadIdx.x, D = DT == 3 ? 3 : a.D, W = D + 1;
+    float pd = INFINITY;
+    int64_t pi = -1;
+    for (int e = 0; e < n_empty; ++e) {
+        float bd = -1.f;
+        int64_t bi = -1;
+        for (int64_t i = tid; i < a.N; i += KM_UPDATE_THREADS) {
+            float x[KM_MAXD];
+            km_load<DT>(a.pos, i, D, x);
+            const float d = km_dist<DT>(x, sc, a.labels[i], D);
+            if (km_before(pd, pi, d, i) && (bi < 0 || km_before(d, i, bd, bi))) { bd = d; bi = i; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float od = __shfl_xor_sync(FULL, bd, o);
+            const long long oi = __shfl_xor_sync(FULL, (long long)bi, o);
+            if (oi >= 0 && (bi < 0 || km_before(od, oi, bd, bi))) { bd = od; bi = oi; }
+        }
+        if ((tid & 31) == 0) { rd[tid >> 5] = bd; ri[tid >> 5] = bi; }
+        __syncthreads();
+        if (tid == 0) {
+            for (int w = 1; w < KM_UPDATE_THREADS / 32; ++w)
+                if (ri[w] >= 0 && (bi < 0 || km_before(rd[w], ri[w], bd, bi))) { bd = rd[w]; bi = ri[w]; }
+            pick_d = bd; pick_i = bi;
+            if (bi >= 0 && !(e == 0 && bd == 0.f)) {       // the farthest point sits on its centre: nothing moves
+                const int knew = empty[e], kold = a.labels[bi];
+                float x[KM_MAXD];
+                km_load<DT>(a.pos, bi, D, x);
+                for (int c = 0; c < D; ++c) {
+                    a.sums[W * kold + c] -= (double)x[c];
+                    a.sums[W * knew + c] = (double)x[c];
+                }
+                a.sums[W * kold + D] -= 1.0;
+                a.sums[W * knew + D] = 1.0;
             }
         }
-        for (int c = 0; c < W; ++c) a.sums[W * k + c] = 0.0;
+        __syncthreads();
+        pd = pick_d; pi = pick_i;
+        if (pi < 0 || (e == 0 && pd == 0.f)) return;      // fewer points than empty clusters: the rest stay empty
     }
-    if (k < KM_MAXK) shift[k] = s;
+}
+
+// sklearn's `_average_centers` and `_center_shift`: centre = fp32(sum) · fp32(1/count), the product rounded once (the
+// fp64 sums hold the fp32 sums exactly wherever those are exact); a cluster still empty after the relocation (every
+// point on its centre, or a relocated point that was alone in its cluster) takes the centre of the first largest
+// cluster m — as sklearn fills its buffer in cluster order, that is m's mean when m < k and m's plain sum otherwise.
+template <int DT>
+__global__ void __launch_bounds__(KM_UPDATE_THREADS) kmeans_update_kernel(const KmArgs a) {
+    __shared__ float sc[KM_MAXK * KM_MAXD];
+    __shared__ float shift[KM_MAXK];
+    __shared__ int empty[KM_MAXK];
+    __shared__ int n_empty, amax;
+    const int st = a.state[0];
+    if (st == 2) return;
+    const int tid = threadIdx.x, K = a.K, D = a.D, W = D + 1;
+    if (st == 1) {                                        // the final assignment has run
+        if (tid == 0) a.state[0] = 2;
+        return;
+    }
+    for (int i = tid; i < K * D; i += KM_UPDATE_THREADS) sc[i] = a.centers[i];
+    if (tid == 0) {
+        int n = 0;
+        for (int k = 0; k < K; ++k)
+            if (a.sums[W * k + D] == 0.0) empty[n++] = k;
+        n_empty = n;
+    }
     __syncthreads();
-    if (k == 0) {
+    if (n_empty) km_relocate<DT>(a, sc, empty, n_empty);
+    if (tid == 0) {
+        int m = 0;
+        for (int k = 1; k < K; ++k)
+            if (a.sums[W * k + D] > a.sums[W * m + D]) m = k;
+        amax = m;
+    }
+    __syncthreads();
+    float cc[KM_MAXD];
+    if (tid < K) {
+        const int k = tid, m = amax;
+        const double n = a.sums[W * k + D];
+        const int src = n > 0.0 ? k : m;
+        const bool mean = n > 0.0 || m < k;
+        const double alpha = (double)(float)(1.0 / a.sums[W * src + D]);
+#pragma unroll
+        for (int c = 0; c < KM_MAXD; ++c)
+            if (c < D) cc[c] = mean ? (float)(a.sums[W * src + c] * alpha) : (float)a.sums[W * src + c];
+    }
+    __syncthreads();                                      // every thread has read the sums it needs
+    if (tid < K) {
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < KM_MAXD; ++c)
+            if (c < D) {
+                const float dc = cc[c] - sc[D * tid + c];
+                s += dc * dc;
+                a.centers[D * tid + c] = cc[c];
+            }
+        for (int c = 0; c < W; ++c) a.sums[W * tid + c] = 0.0;
+        shift[tid] = s;
+    }
+    __syncthreads();
+    if (tid == 0) {
         float tot = 0.f;
-        for (int i = 0; i < a.K; ++i) tot += shift[i];
+        for (int i = 0; i < K; ++i) tot += shift[i];
         a.state[1] += 1;
         if (a.state[2] == 0) a.state[0] = 2;              // strict convergence: labels already match the centres
         else if (tot <= a.tol) a.state[0] = 1;            // converged by tolerance: one more assignment pass
@@ -166,9 +263,13 @@ static int kmeans_run(const KmArgs& a, int iters, cudaStream_t st) {
     int64_t blocks = (a.N + KM_THREADS * 4 - 1) / (KM_THREADS * 4);
     if (blocks > 8 * sm_count()) blocks = 8 * sm_count();
     for (int it = 0; it < iters; ++it) {
-        if (a.D == 3) kmeans_assign_kernel<3><<<(unsigned)blocks, KM_THREADS, 0, st>>>(a);
-        else kmeans_assign_kernel<0><<<(unsigned)blocks, KM_THREADS, 0, st>>>(a);
-        kmeans_update_kernel<<<1, KM_MAXK, 0, st>>>(a);
+        if (a.D == 3) {
+            kmeans_assign_kernel<3><<<(unsigned)blocks, KM_THREADS, 0, st>>>(a);
+            kmeans_update_kernel<3><<<1, KM_UPDATE_THREADS, 0, st>>>(a);
+        } else {
+            kmeans_assign_kernel<0><<<(unsigned)blocks, KM_THREADS, 0, st>>>(a);
+            kmeans_update_kernel<0><<<1, KM_UPDATE_THREADS, 0, st>>>(a);
+        }
     }
     if (a.inertia) kmeans_inertia_kernel<<<1, KM_INERTIA_THREADS, 0, st>>>(a);
     return DISTEGNN_OK;

@@ -272,34 +272,39 @@ def kmeans_labels(pos: Tensor, n_clusters: int, random_state: int = 0, max_iter:
                   chunk: int = 16) -> Tensor:
     """`sklearn.cluster.KMeans(n_clusters, random_state=random_state, n_init="auto").fit_predict(pos)` with the Lloyd
     iterations on the device: int64 labels [N] on `pos.device` (distribute_graphs.py:188-198).  The seeding is sklearn's
-    own k-means++ on the host (on the mean-centred float32 positions, exactly as `KMeans.fit` does); iterations are
-    enqueued `chunk` at a time and the device-side convergence state is read once per chunk."""
+    own k-means++ on the host; the seeding and the iterations both run on the mean-centred float32 positions, exactly as
+    `KMeans.fit` does (fp32 distances and centres far from the origin would lose their digits to the offset).  Iterations
+    are enqueued `chunk` at a time and the device-side convergence state is read once per chunk; a run that reaches
+    `max_iter` ends with sklearn's closing assignment (the header's state[0] = 1 call)."""
     import numpy as np
     from sklearn.cluster import kmeans_plusplus
     if pos.device.type != "cuda":
         raise _lib.DistEGNNError("distegnn_b200.kmeans_labels runs only on CUDA tensors (no CPU path)")
     lib = _lib.load()
     dev = pos.device
-    p = pos.detach().to(torch.float32).contiguous()
-    N = int(p.shape[0])
-    X = p.cpu().numpy()
-    mean = X.mean(axis=0)
-    Xc = X - mean                                                # KMeans.fit centres the data first
+    X = pos.detach().to(torch.float32).cpu().numpy()
+    N = int(X.shape[0])
+    Xc = X - X.mean(axis=0)                                      # KMeans.fit centres the data first
     c0, _ = kmeans_plusplus(Xc, n_clusters, random_state=np.random.RandomState(random_state))
     tol_abs = float(tol * np.mean(np.var(Xc, axis=0)))           # sklearn's _tolerance
-    centers = torch.from_numpy((c0 + mean).astype(np.float32)).to(dev).contiguous()
+    p = torch.from_numpy(np.ascontiguousarray(Xc)).to(dev)
+    centers = torch.from_numpy(np.ascontiguousarray(c0, dtype=np.float32)).to(dev)
     labels = torch.full((N,), -1, dtype=torch.int32, device=dev)
     sums = torch.zeros(n_clusters, 4, dtype=torch.float64, device=dev)
     state = torch.zeros(4, dtype=torch.int32, device=dev)
+
+    def lloyd(n):
+        check(lib.distegnn_kmeans_lloyd(N, n_clusters, ptr(p), ptr(centers), ptr(labels), ptr(sums), ptr(state),
+                                        tol_abs, n, _lib.stream_ptr(dev)), "kmeans_lloyd")
     done = 0
     with torch.cuda.device(dev):
-        while done < max_iter + 1:
-            n = min(chunk, max_iter + 1 - done)
-            check(lib.distegnn_kmeans_lloyd(N, n_clusters, ptr(p), ptr(centers), ptr(labels), ptr(sums), ptr(state),
-                                            tol_abs, n, _lib.stream_ptr(dev)), "kmeans_lloyd")
+        while done < max_iter and int(state[0].item()) != 2:
+            n = min(chunk, max_iter - done)
+            lloyd(n)
             done += n
-            if int(state[0].item()) == 2:
-                break
+        if int(state[0].item()) != 2:
+            state[0] = 1                                         # max_iter passes: sklearn's closing E-step
+            lloyd(1)
     return labels.to(torch.int64)
 
 

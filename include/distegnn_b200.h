@@ -318,7 +318,11 @@ DISTEGNN_API int distegnn_cutoff_csr(int64_t n_nodes, int n_graphs, const float 
  * NULL, writes Σ_i ‖pos_i − centers[labels_i]‖² (fp32 terms, fp64 sum in a fixed order) to inertia[0] once state[0]
  * is 2.  A caller that stops after its iteration cap without convergence sets state[0] = 1 and calls once more with
  * iters = 1: that pass assigns every point to the final centres without moving them (sklearn's closing E-step), ends
- * in state 2 and writes the inertia.  n_clusters in [1, 64]. */
+ * in state 2 and writes the inertia.  Each update is sklearn's M-step: an empty cluster takes the point farthest from
+ * the centre it was assigned to (the e-th empty cluster the e-th farthest, ties to the lower index; none moves when
+ * every such distance is 0), then centre = fp32(sum)·fp32(1/count), and a cluster still empty takes the first largest
+ * cluster's centre (its plain sum when that cluster's id is higher, as sklearn's `_average_centers` does).  state[3] is
+ * unused.  n_clusters in [1, 64]. */
 DISTEGNN_API int distegnn_kmeans_lloyd(int64_t n_nodes, int n_clusters, const float *pos, float *centers,
                                        int32_t *labels, double *sums, int32_t *state, float tol, int iters, void *stream);
 DISTEGNN_API int distegnn_kmeans_lloyd_d(int64_t n_nodes, int n_clusters, int dim, const float *pos, float *centers,
