@@ -97,6 +97,9 @@ SIGNATURES = {
     "distegnn_chamfer_distance_bwd_workspace_bytes": [_i64, C.POINTER(_i64)],
     "distegnn_chamfer_distance_bwd": [_i64, _i32] + [_vp] * 8 + [_i64, _vp],
     "distegnn_nbody_simulate": [_i32, _i32, _i64, _i64, _i32, C.c_double, C.c_double] + [_vp] * 7,
+    "distegnn_nbody_objects_workspace_bytes": [_i32, _i32, C.POINTER(_i64)],
+    "distegnn_nbody_simulate_objects": [_i32, _i32, _i32, _i32, _i64, _i64, _i32, C.c_double, C.c_double] + [_vp] * 12
+                                       + [_i64, _vp],
 }
 FRAMES_NBODY, FRAMES_WATER3D, FRAMES_LARGEFLUID = 0, 1, 2
 ABI_VERSION = 3

@@ -716,6 +716,28 @@ DISTEGNN_API int distegnn_nbody_simulate(int n_systems, int n_bodies, int64_t fi
                                          int sample_freq, double dt, double max_f, double *x, double *v,
                                          const double *q, double *frames_x, double *frames_v, int64_t *status,
                                          void *stream);
+/* distegnn_nbody_simulate_objects: as distegnn_nbody_simulate, for systems with n_sticks sticks and n_hinges hinges
+ * (the reference's Stick / Hinge, physical_objects.py; DESIGN §25).  sticks int32 [n_systems, n_sticks, 2] and hinges
+ * int32 [n_systems, n_hinges, 3] name each object's bodies (a hinge's joint first); stick_state double [n_systems,
+ * n_sticks, 9] (xc, vc, wc) and hinge_state double [n_systems, n_hinges, 6] (w1, w2) are read and written in place, so
+ * that calls over consecutive step ranges give one call's bits.  Per step the force and clamp are
+ * distegnn_nbody_simulate's, then bodies no object names take v ← v + F·dt, x ← x + v·dt and each object its
+ * reference update restated in a fixed order (sin / cos by a Cody–Waite reduction and fixed polynomials, the hinge's
+ * 3×3 solve by the adjugate).  Table entries out of [0, n_bodies), or naming a body another entry names, are added to
+ * *invalid (int64, device; the caller zeroes it) once per call, and their system is not advanced (its frames repeat
+ * the state).  n_bodies <= 1024: one launch per recorded step, no workspace; otherwise, per call a memset and two table
+ * launches, per step two launches, in a workspace of distegnn_nbody_objects_workspace_bytes (0 for n_bodies <= 1024).
+ * Rejects n_sticks = n_hinges = 0 (distegnn_nbody_simulate covers it), negative counts, n_bodies < 2·n_sticks +
+ * 3·n_hinges and distegnn_nbody_simulate's argument errors; DISTEGNN_EWORKSPACE for a short workspace.  No allocation,
+ * no host synchronisation; capturable. */
+DISTEGNN_API int distegnn_nbody_objects_workspace_bytes(int n_systems, int n_bodies, int64_t *bytes);
+DISTEGNN_API int distegnn_nbody_simulate_objects(int n_systems, int n_bodies, int n_sticks, int n_hinges,
+                                                 int64_t first_step, int64_t n_steps, int sample_freq, double dt,
+                                                 double max_f, double *x, double *v, const double *q,
+                                                 const int32_t *sticks, const int32_t *hinges, double *stick_state,
+                                                 double *hinge_state, double *frames_x, double *frames_v,
+                                                 int64_t *status, int64_t *invalid, void *workspace,
+                                                 int64_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }

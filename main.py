@@ -143,11 +143,17 @@ def parse():
     return p.parse_args()
 
 
-def split_files(path, recipe, part):
-    """The files of split `part` under `path`: N-body's loc_`part`_... .npy, or `path`/`part`/*.npz; [] if missing."""
+def nbody_tag(cfg):
+    """The N-body file tag, without its leading underscore: the config's `data.nbody_tag` (e.g. charged0_5_0_1 for
+    files written by `nbody.generate_dataset(n_isolated=0, n_stick=5)`), by default charged100_0_0_1."""
+    return str((cfg.get("data") or {}).get("nbody_tag", "charged100_0_0_1"))
+
+
+def split_files(path, recipe, part, tag="charged100_0_0_1"):
+    """The files of split `part` under `path`: N-body's loc_`part`_`tag`.npy, or `path`/`part`/*.npz; [] if missing."""
     import glob
     if recipe == "nbody":
-        f = os.path.join(path, f"loc_{part}_charged100_0_0_1.npy")
+        f = os.path.join(path, f"loc_{part}_{tag}.npy")
         return [f] if os.path.exists(f) else []
     return sorted(glob.glob(os.path.join(path, part, "*.npz")))
 
@@ -166,7 +172,7 @@ def epochs_of(args, cfg):
         msg = ">= 1"
     else:
         recipe = recipe_of_config(cfg)[0]
-        missing = [part for part in ("valid", "test") if not split_files(args.trajectory, recipe, part)]
+        missing = [part for part in ("valid", "test") if not split_files(args.trajectory, recipe, part, nbody_tag(cfg))]
         if missing:
             msg = f"used with a trajectory that has valid and test splits ({args.trajectory} has no {' or '.join(missing)})"
     if msg is not None:
@@ -230,10 +236,10 @@ def split_samples(path, cfg, part, horizon=1):
     from distegnn_b200.frames import load_nbody, load_scenes, sample_list
     d = cfg["data"]
     recipe, frame_0, delta = recipe_of_config(cfg)
-    files = split_files(path, recipe, part)
+    files = split_files(path, recipe, part, nbody_tag(cfg))
     if not files:
         return None
-    traj = load_nbody(path, part) if recipe == "nbody" else load_scenes(files, recipe)
+    traj = load_nbody(path, part, nbody_tag(cfg)) if recipe == "nbody" else load_scenes(files, recipe)
     kw = {}
     if recipe != "nbody":
         shortest = min(sc.n_frames for sc in traj.scenes)
@@ -480,7 +486,7 @@ def rollout_args(args, cfg, local_rank, K=None, flag="--rollout_steps"):
     tau = args.rollout_tau if args.rollout_tau is not None else (float(delta) if recipe == "water3d" else None)
     if tau is None and recipe == "nbody" and args.trajectory:   # files written by distegnn_b200.nbody record their dt
         from distegnn_b200.nbody import meta_rollout_tau
-        tau = meta_rollout_tau(args.trajectory, delta)
+        tau = meta_rollout_tau(args.trajectory, delta, "_" + nbody_tag(cfg))
     if K > 0 and tau is None:
         if local_rank == 0:
             print(f"{flag} with --trajectory on {recipe!r} needs --rollout_tau: its velocities are physical and "
