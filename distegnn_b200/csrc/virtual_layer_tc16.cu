@@ -33,7 +33,7 @@ namespace degnn {
 
 struct VirtT16Args {
     int64_t N;
-    int B, C;
+    int B;
     unsigned flags;
     const int32_t* batch;
     const float* x4;
@@ -73,10 +73,11 @@ __host__ __device__ constexpr int vw_smem_bytes(int C) { return vw_smem_floats(C
 // group's accH / accX, which DET does not use per warp); a graph's partial of the chunk is stored to vsum when the graph
 // starts in the chunk, else to the chunk's slot.
 static_assert(VW_TILE == DET_VTILE, "det.cuh sizes the slots from the tile");
-template <bool DET>
+// C (the virtual channels) is a template parameter: every row <-> (node, channel) index, the pools' and sums' trip counts
+// and the tile -> node mapping are compile-time constants, so no runtime division is left on the hot path.
+template <int C, bool DET>
 __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const VirtT16Args a) {
     using namespace tmma;
-    const int C = a.C;
     __half* W2hi = reinterpret_cast<__half*>(degnn_dyn_smem);
     __half* W2lo = W2hi + VW_W;
     __half* Wxvhi = W2lo + VW_W;
@@ -103,10 +104,10 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
     const int w = warp & 3;                // warp inside the warpgroup: rows 16w .. 16w+15 of its tile
     const int t = tid & 127;               // thread inside the warpgroup
     const int g = lane >> 2, q = lane & 3; // fragment rows g, g+8 of the warp; columns 8j + 2q
-    const int K = 4 + 3 * C + H * C;
+    constexpr int K = 4 + 3 * C + H * C;
     const bool need_feat = !(a.flags & DISTEGNN_FLAG_LAST);
-    const int TN = VW_TILE / C;
-    const bool warp_local = (16 % C) == 0;   // nodes never straddle warps: the pools need no warpgroup barrier
+    constexpr int TN = VW_TILE / C;
+    constexpr bool warp_local = (16 % C) == 0;   // nodes never straddle warps: the pools need no warpgroup barrier
 
     // ---- one-time setup -------------------------------------------------------------------------
     tc16::stage_weight<VW_THREADS>(W2hi, W2lo, a.w2, 0, 64, tid, SILU_T_IN);   // t2 = SILU_T_IN·(a1·W2vᵀ + b2v); mv' = SILU_T_IN·mv
@@ -167,9 +168,9 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
     const int num_tiles = (int)((a.N + TN - 1) / TN);            // < 2^31 (the launch checks)
     const int stride = (int)gridDim.x * VW_WG;
     // DET: pipeline p takes the chunks p, p + stride, ...; inside a chunk the tiles follow each other
-    const int CH = 1 << a.chunk_shift;                 // DET: tiles per chunk
+    const int CH = 1 << a.chunk_shift;                 // DET: tiles per chunk (a power of two: tile % CH = tile & (CH − 1))
     auto next_tile = [&](int tl) {
-        if constexpr (DET) return (tl + 1) % CH != 0 ? tl + 1 : tl + 1 + (stride - 1) * CH;
+        if constexpr (DET) return ((tl + 1) & (CH - 1)) != 0 ? tl + 1 : tl + 1 + (stride - 1) * CH;
         else return tl + stride;
     };
     float* accG = accH_all + 4 * wg * C * H;          // DET: the group's sums [C][64] and [3][C], thread-owned elements
@@ -200,7 +201,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
     for (int tile = DET ? ((int)blockIdx.x * VW_WG + wg) * CH : (int)blockIdx.x * VW_WG + wg; tile < num_tiles;
          tile = next_tile(tile)) {
         const int64_t n0 = (int64_t)tile * TN;
-        if (DET && tile % CH == 0)
+        if (DET && (tile & (CH - 1)) == 0)
             cont = (n0 > 0 && __ldg(a.batch + n0 - 1) == __ldg(a.batch + n0)) ? __ldg(a.batch + n0) : -1;
         const int nvalid = (int)min((int64_t)TN, a.N - n0);
         const int rows = nvalid * C;
@@ -234,22 +235,35 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         const float* ga;
         const float* gb;
         float vra, vrb;
-        {
-            auto row_geo = [&](int r, bool v, const float*& hrow, const float*& grow) {
-                const int nl = v ? r / C : 0, ch = v ? r - nl * C : 0;
-                const size_t node = (size_t)(n0 + nl);
-                const int gr = single ? g_first : __ldg(a.batch + node);
-                const float4 xi = ldg4(a.x4 + node * 4);
-                const float* Xg = a.Xv + (size_t)gr * 3 * C;
-                const float dx = __ldg(Xg + ch) - xi.x, dy = __ldg(Xg + C + ch) - xi.y, dz = __ldg(Xg + 2 * C + ch) - xi.z;
+        {   // a row's geometry comes from its node (x4, graph id) and its channel (Xv[graph, :, c]).  The thread's second row
+            // reuses the first one's loads where the two share them: the node when C = 16 (rows g, g + 8 of one node), the
+            // channel when C divides 8 (and so the Xv values, when the graph is the same).  Invalid rows read node 0 of
+            // the tile: their values are never used.
+            const int nla = va ? ra / C : 0, nlb = vb ? rb / C : 0;
+            const int cha = va ? ra - nla * C : 0;
+            const int chb = 8 % C == 0 ? cha : (vb ? rb - nlb * C : 0);
+            const size_t nda = (size_t)(n0 + nla), ndb = C == 16 ? nda : (size_t)(n0 + nlb);
+            const int gra = single ? g_first : __ldg(a.batch + nda);
+            const int grb = (C == 16 || single) ? gra : __ldg(a.batch + ndb);
+            const float4 xia = ldg4(a.x4 + nda * 4);
+            const float4 xib = C == 16 ? xia : ldg4(a.x4 + ndb * 4);
+            auto xv = [&](int gr, int ch) {
+                const float* Xg = a.Xv + (size_t)gr * 3 * C + ch;
+                return make_float3(__ldg(Xg), __ldg(Xg + C), __ldg(Xg + 2 * C));
+            };
+            const float3 xva = xv(gra, cha);
+            const float3 xvb = (8 % C == 0 && grb == gra) ? xva : xv(grb, chb);
+            auto row_geo = [&](int r, size_t node, int gr, int ch, float4 xi, float3 xg, const float*& hrow,
+                               const float*& grow) {
+                const float dx = xg.x - xi.x, dy = xg.y - xi.y, dz = xg.z - xi.z;
                 if (q == 0) *reinterpret_cast<float4*>(dXs + 4 * r) = make_float4(dx, dy, dz, 0.f);
                 hrow = a.Hn + node * H + 2 * q;
                 // rows of the cached graph read shared memory, the others (tiles that straddle graphs) global memory
                 grow = (gr == cur_graph ? (const float*)(gs + ch * VW_ROW) : a.G + ((size_t)gr * C + ch) * H) + 2 * q;
                 return sqrtf(dx * dx + dy * dy + dz * dz);
             };
-            vra = row_geo(ra, va, pa, ga);
-            vrb = row_geo(rb, vb, pb, gb);
+            vra = row_geo(ra, nda, gra, cha, xia, xva, pa, ga);
+            vrb = row_geo(rb, ndb, grb, chb, xib, xvb, pb, gb);
         }
         auto pre = [&](int j, const float* hrow, const float* grow, float vr) {
             const f32x2 hh = __ldg(reinterpret_cast<const f32x2*>(hrow + 8 * j));
@@ -312,14 +326,13 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
 #pragma unroll 1
             for (int n = nb; n < ne; n += ns) {                  // mean over channels per node
                 const float* base = colp + (n * C) * VW_ROW;
-                f32x2 s0 = 0ull, s1 = 0ull;
-                int c = 0;
-#pragma unroll 1
-                for (; c + 1 < C; c += 2) {
+                f32x2 s0 = 0ull, s1 = 0ull;                      // even channels in s0, odd in s1
+#pragma unroll
+                for (int c = 0; c + 1 < C; c += 2) {
                     s0 = add2(s0, ld2(base + c * VW_ROW));
                     s1 = add2(s1, ld2(base + (c + 1) * VW_ROW));
                 }
-                if (c < C) s0 = add2(s0, ld2(base + c * VW_ROW));
+                if constexpr (C % 2 == 1) s0 = add2(s0, ld2(base + (C - 1) * VW_ROW));
                 *reinterpret_cast<f32x2*>(a.agg_v + (size_t)(n0 + n) * H + 2 * lane) = mul2(add2(s0, s1), invC2);
             }
             if constexpr (DET) {                                 // every row of the tile, in row order
@@ -329,20 +342,21 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
                         det_flush_m(tile);
                         curM = gr;
                     }
+#pragma unroll
                     for (int c = t >> 5; c < C; c += 4) {
                         f32x2* acc = reinterpret_cast<f32x2*>(accG + c * H + 2 * (t & 31));
                         *acc = add2(*acc, ld2(tile_s + (n * C + c) * VW_ROW + 2 * (t & 31)));
                     }
                 }
             } else if (single) {                                 // sum of the warp's own rows per channel
-                const int cn = min(C, 16);
 #pragma unroll 1
-                for (int i = 0; i < cn; ++i) {
+                for (int i = 0; i < C; ++i) {                    // C <= 16: one first row per channel
                     const int r = 16 * w + i;
                     if (r >= r_end) break;
                     f32x2 s = ld2(colp + r * VW_ROW);
-#pragma unroll 1
-                    for (int r2 = r + C; r2 < r_end; r2 += C) s = add2(s, ld2(colp + r2 * VW_ROW));
+#pragma unroll
+                    for (int k = 1; k < (16 - i + C - 1) / C; ++k)   // rows r + C, r + 2C, ... inside the warp's 16
+                        if (r + k * C < r_end) s = add2(s, ld2(colp + (r + k * C) * VW_ROW));
                     f32x2* acc = reinterpret_cast<f32x2*>(accH + (r % C) * H + 2 * lane);
                     *acc = add2(*acc, s);
                 }
@@ -386,6 +400,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         for (int i = lane; i < (ne - nb + ns - 1) / ns * 3; i += 32) {
             const int n = nb + (i / 3) * ns, dd = i - 3 * (i / 3);
             float s = 0.f;
+#pragma unroll 8   // not all 16 of C = 16: the loads in flight would spill under MMA 3
             for (int c = 0; c < C; ++c) s = fmaf(-dXs[4 * (n * C + c) + dd], phis[n * C + c], s);
             a.trans_v[(size_t)(n0 + n) * 4 + dd] = s / (float)C;
         }
@@ -416,12 +431,13 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
                 }
             }
         } else if (single) {
-            const int cn = min(C, 16);
-            for (int it = lane; it < 3 * cn; it += 32) {      // lane <-> (component, first row of a channel)
-                const int dd = it / cn, r = 16 * w + (it - dd * cn);
+            for (int it = lane; it < 3 * C; it += 32) {       // lane <-> (component, first row of a channel); C <= 16
+                const int dd = it / C, i = it - dd * C, r = 16 * w + i;
                 if (r < r_end) {
                     float s = 0.f;
-                    for (int r2 = r; r2 < r_end; r2 += C) s = fmaf(dXs[4 * r2 + dd], phx[r2], s);
+#pragma unroll
+                    for (int k = 0; k < (16 + C - 1) / C; ++k)       // rows r, r + C, ... inside the warp's 16
+                        if (r + k * C < r_end) s = fmaf(dXs[4 * (r + k * C) + dd], phx[r + k * C], s);
                     accX[dd * C + r % C] += s;
                 }
             }
@@ -438,7 +454,7 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
         // read other warps' rows)
         if (warp_local && !DET) __syncwarp();
         else named_bar(bar_id, 128);
-        if (DET && ((tile + 1) % CH == 0 || tile + 1 >= num_tiles)) {     // end of the chunk
+        if (DET && (((tile + 1) & (CH - 1)) == 0 || tile + 1 >= num_tiles)) {     // end of the chunk
             if (need_feat) det_flush_m(tile);
             det_flush_x(tile);
             curM = curX = -1;
@@ -453,6 +469,17 @@ __global__ void __launch_bounds__(VW_THREADS, 1) virtual_layer_t16_kernel(const 
 }  // namespace degnn
 
 namespace degnn {
+
+// launches the instantiation for channel count c (check_dims has kept it in [1, DISTEGNN_MAX_CHANNELS])
+template <bool DET, int C = 1>
+static void launch_virtual(int c, unsigned grid, const VirtT16Args& a, cudaStream_t stream) {
+    if constexpr (C <= DISTEGNN_MAX_CHANNELS) {
+        if (c != C) return launch_virtual<DET, C + 1>(c, grid, a, stream);
+        static_assert(vw_smem_bytes(C) <= 232448, "the shared memory of every C must fit");
+        ensure_dynamic_smem((const void*)virtual_layer_t16_kernel<C, DET>, vw_smem_bytes(C));
+        virtual_layer_t16_kernel<C, DET><<<grid, VW_THREADS, vw_smem_bytes(C), stream>>>(a);
+    }
+}
 
 template <bool DET>
 static int virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na, unsigned flags, const int32_t* batch32,
@@ -469,7 +496,7 @@ static int virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na
             return rc;
     Layout L = make_layout(A, C, Na);
     VirtT16Args a;
-    a.N = n_nodes; a.B = n_graphs; a.C = C; a.flags = flags;
+    a.N = n_nodes; a.B = n_graphs; a.flags = flags;
     a.batch = batch32; a.x4 = x4; a.Hn = Hn; a.Xv = Xv; a.G = G;
     a.w1r = layer_params + L.off[DISTEGNN_P_V_W1R];
     a.w2 = layer_params + L.off[DISTEGNN_P_V_W2];
@@ -483,8 +510,6 @@ static int virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na
     a.agg_v = agg_v; a.trans_v = trans_v; a.vsum = vsum;
     a.slots = DET ? det_vsum_slots(workspace) : nullptr;
     a.chunk_shift = DET ? det_chunk_shift(n_nodes, C) : 0;
-    static_assert(vw_smem_bytes(DISTEGNN_MAX_CHANNELS) <= 232448, "the widest C must fit");
-    ensure_dynamic_smem((const void*)virtual_layer_t16_kernel<DET>, vw_smem_bytes(DISTEGNN_MAX_CHANNELS));
     const int TN = VW_TILE / C;
     const int64_t tiles = (n_nodes + TN - 1) / TN;
     const int64_t units = DET ? det_chunks(n_nodes, C) : tiles;       // what the pipelines grid-stride over
@@ -493,7 +518,7 @@ static int virtual_layer_fwd(int64_t n_nodes, int n_graphs, int A, int C, int Na
     int64_t grid = (units + VW_WG - 1) / VW_WG;
     if (grid > sm_count()) grid = sm_count();
     if (DET) grid = det_grid(grid, max_ctas);
-    virtual_layer_t16_kernel<DET><<<(unsigned)grid, VW_THREADS, vw_smem_bytes(C), (cudaStream_t)stream>>>(a);
+    launch_virtual<DET>(C, (unsigned)grid, a, (cudaStream_t)stream);
     DEGNN_CHECK_LAUNCH();
     return DISTEGNN_OK;
 }

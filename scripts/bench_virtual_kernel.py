@@ -116,8 +116,8 @@ def main():
         for i, p in enumerate(libs):
             ms = [s.elapsed_time(e) for s, e in times[i]]
             mean = statistics.fmean(ms)
-            entry[p] = {"mean_ms": mean, "median_ms": statistics.median(ms), "min_ms": min(ms), "max_ms": max(ms),
-                        "TFLOPs": flops / (mean * 1e-3) / 1e12}
+            entry[p] = {"mean_ms": mean, "median_ms": statistics.median(ms), "stdev_ms": statistics.stdev(ms),
+                        "min_ms": min(ms), "max_ms": max(ms), "TFLOPs": flops / (mean * 1e-3) / 1e12}
         if len(fns) == 2:
             diff = {}
             for k, nm in enumerate(("agg_v", "trans_v", "vsum")):
