@@ -16,12 +16,13 @@
 //   stage 3  φ = w3·SiLU(D + bc) per row (quad shuffles); Δx·φ summed over runs of equal row, RED.ADD
 // The range rescue needs one scale per row: the four lanes of a quad share a row, so its maximum is two shuffles away and
 // the cold path is taken per warp (__any_sync); every path reconverges before the warpgroup-collective wgmma.
-// Everything a tile needs from memory is requested one tile ahead, per warp:
-//   Q[col] rows of tile i+1           one TMA bulk copy per edge at the start of tile i (staging double buffered, mbarrier
-//                                     per buffer)
-//   x[row], x[col] of tile i+1        cp.async at the start of tile i, read at its end
-//   (row, col, edge_attr) of tile i+2 cp.async at the start of tile i, moved to registers at its end
+// Everything a tile needs from memory is requested one tile ahead, per warp, as one cp.async commit group issued at the
+// start of tile i and waited for at its end (a __syncwarp then publishes every lane's copies to the warp):
+//   Q[col] rows of tile i+1           16-byte cp.async by all 32 lanes, two rows per pass (staging double buffered)
+//   x[row], x[col] of tile i+1        read at the end of tile i
+//   (row, col, edge_attr) of tile i+2 moved to registers at the end of tile i
 //   P[row] of tile i+1                prefetched towards L1 at the start of tile i (rows are contiguous: a tile has few)
+// Tile numbers and edge ids are int32: the host entry bounds the edge count (edge_layer_fwd).
 // Stages 2 and 3 run in the "t domain" (common.cuh silu4t): −log2(e) is folded into W2 and the biases, −ln 2 into w3 and
 // the segment-sum flush, so the SiLU never forms its exponent argument explicitly.
 // Edge order: the one thing the kernel needs is that the edges of a destination row are contiguous (the run masks compare
@@ -38,7 +39,8 @@
 namespace degnn {
 
 struct EdgeCsArgs {
-    int64_t N, E;
+    int64_t N;
+    int E;                  // < 2^31 - 64 (edge_layer_fwd)
     const int32_t* E_dev;   // optional: the edge count on the device (graphs built without a host round trip); E = capacity
     int A;
     unsigned flags;
@@ -71,7 +73,6 @@ constexpr int CS_WBUF = 16 * CS_QROW;                     // one staging buffer 
 constexpr int CS_IDX = 64;                                // staged ints per warp: row 16 | col 16 | edge_attr 16x2
 constexpr int CS_W = 64 * 64;                             // fp16 elements per weight matrix (8 KB)
 constexpr int CS_SMEM_BYTES = 4 * CS_W * 2                // W2 hi/lo, Wc hi/lo
-                              + CS_WARPS * 2 * 8          // mbarriers: one per staging buffer
                               + (4 * H + DISTEGNN_MAX_EDGE_ATTR * H) * 4   // b2, bc, w3, w1r, w1e
                               + CS_WARPS * 2 * CS_WBUF * 4                // Q rows / m, double buffered
                               + CS_WARPS * CS_IDX * 4                     // indices of the tile after next
@@ -91,8 +92,7 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
     __half* W2lo = W2hi + CS_W;
     __half* Wchi = W2lo + CS_W;
     __half* Wclo = Wchi + CS_W;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(Wclo + CS_W);                 // [warps][2]
-    float* b2s = reinterpret_cast<float*>(bars + CS_WARPS * 2);
+    float* b2s = reinterpret_cast<float*>(Wclo + CS_W);
     float* bcs = b2s + H;
     float* w3s = bcs + H;
     float* w1rs = w3s + H;
@@ -123,35 +123,43 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
     // staging rows of edges past the end are never loaded: keep them finite
     for (int i = tid; i < CS_WARPS * 2 * CS_WBUF / 4; i += CS_THREADS)
         reinterpret_cast<float4*>(qbufs)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (tid == 0) {
-        for (int i = 0; i < CS_WARPS * 2; ++i) mbar_init(&bars[i], 1);
-        fence_mbar_init();
-    }
     fence_proxy_async_smem();
     __syncthreads();
 
     float* qb = qbufs + warp * 2 * CS_WBUF;
     int* nidx = idx_all + warp * CS_IDX;
     float* xs = xs_all + warp * 16 * 8 + 8 * (lane & 15);     // (x_row, x_col) of edge `lane` of the next tile
-    uint64_t* qbar = bars + 2 * warp;
+    // per-thread bases of the row gathers, opaque to ptxas: a row address is then one IMAD.WIDE.U32 (row id x row bytes +
+    // base) instead of a 64-bit re-derivation of array + column offset each time
+    const float* Pq = a.P + 2 * q;                             // the thread's columns of P rows
+    asm("" : "+l"(Pq));
     const uint64_t bW2hi = make_desc(smem_u32(W2hi), CS_LBO, 128), bW2lo = make_desc(smem_u32(W2lo), CS_LBO, 128);
     const uint64_t bWchi = make_desc(smem_u32(Wchi), CS_LBO, 128), bWclo = make_desc(smem_u32(Wclo), CS_LBO, 128);
 
-    const int64_t nE = a.E_dev ? min((int64_t)__ldg(a.E_dev), a.E) : a.E;     // valid edges (<= the host-side bound)
-    const int64_t num_tiles = (nE + CS_TILE - 1) / CS_TILE;
-    const int64_t stride = (int64_t)gridDim.x * CS_WG;
-    int64_t tile = (int64_t)blockIdx.x * CS_WG + wg;
+    const int nE = a.E_dev ? min(__ldg(a.E_dev), a.E) : a.E;     // valid edges (<= the host-side bound)
+    const int num_tiles = (nE + CS_TILE - 1) / CS_TILE;
+    const int stride = gridDim.x * CS_WG;
+    int tile = blockIdx.x * CS_WG + wg;
 
     // lanes 0..15 carry the per-edge state of the warp's 16 edges; lanes 16..31 carry row -1
-    auto edge_of = [&](int64_t tl) { return tl * CS_TILE + 16 * w + lane; };
-    auto has_edge = [&](int64_t tl) { return lane < 16 && tl < num_tiles && edge_of(tl) < nE; };
-    // Q rows of tile tl into staging buffer b (tl < num_tiles: warp-uniform)
-    auto fetch_q = [&](int64_t tl, int b, int col_e, bool v) {
-        if (lane == 0) {
-            const int64_t nv = min((int64_t)16, max((int64_t)0, nE - (tl * CS_TILE + 16 * w)));
-            mbar_expect_tx(qbar + b, (uint32_t)nv * (H * 4));
+    auto edge_of = [&](int tl) { return tl * CS_TILE + 16 * w + lane; };
+    auto has_edge = [&](int tl) { return lane < 16 && tl < num_tiles && edge_of(tl) < nE; };
+    // Q rows of the warp's 16 edges into staging buffer b (cp.async, the caller commits): pass k copies edges 2k and 2k + 1,
+    // lane L its 16-byte chunk L & 15 of edge 2k + (L >> 4).  col_e = the edge's col on lanes 0..15, -1 for no edge.
+    // Rows of edges past the end are not copied: they keep what the buffer held (zeros, or m of an earlier tile), finite;
+    // the deterministic mode masks them in stage 1 (oka / okb).  Zero-filling them instead would change which rows take
+    // the default mode's warp-wide cold paths, and with it the bits of its valid rows.
+    auto fetch_q = [&](int b, int col_e) {
+        // lanes 16 + j hold the col of edge j + 1, so that one 16-lane shuffle per pass serves both halves of the warp
+        const int cols = __shfl_sync(FULL, col_e, (lane & 15) + (lane >> 4));
+        const uint32_t dst = smem_u32(qb + b * CS_WBUF + (lane >> 4) * CS_QROW + 4 * (lane & 15));
+        const char* src = reinterpret_cast<const char*>(a.Q + 4 * (lane & 15));
+        asm("" : "+l"(src));                   // opaque, as Pq
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int c = __shfl_sync(FULL, cols, 2 * k, 16);
+            if (c >= 0) cp_async16(dst + 2 * k * CS_QROW * 4, src + (size_t)(uint32_t)c * (H * 4));
         }
-        if (v) bulk_g2s(qb + b * CS_WBUF + lane * CS_QROW, a.Q + (size_t)col_e * H, H * 4, qbar + b);
     };
 
     int row_c = -1;
@@ -173,38 +181,41 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
     if (tile < num_tiles) {
         int col_c = 0;
         if (has_edge(tile)) {
-            const int64_t e = edge_of(tile);
+            const int e = edge_of(tile);
             row_c = __ldg(a.row + e);
             col_c = __ldg(a.col + e);
 #pragma unroll
-            for (int k = 0; k < AR; ++k) ea_c[k] = __ldg(a.ea + e * AR + k);
+            for (int k = 0; k < AR; ++k) ea_c[k] = __ldg(a.ea + (size_t)e * AR + k);
         }
-        fetch_q(tile, 0, col_c, row_c >= 0);
+        fetch_q(0, row_c >= 0 ? col_c : -1);
+        cp_async_commit();
         set_geometry(ldg4(a.x4 + (size_t)max(row_c, 0) * 4), ldg4(a.x4 + (size_t)col_c * 4));
         if (has_edge(tile + stride)) {
-            const int64_t e = edge_of(tile + stride);
+            const int e = edge_of(tile + stride);
             n_row = __ldg(a.row + e);
             n_col = __ldg(a.col + e);
 #pragma unroll
-            for (int k = 0; k < AR; ++k) n_ea[k] = __ldg(a.ea + e * AR + k);
+            for (int k = 0; k < AR; ++k) n_ea[k] = __ldg(a.ea + (size_t)e * AR + k);
         }
+        cp_async_wait_all();
+        __syncwarp();                          // every lane's Q rows of the first tile have landed
     }
 
     for (int it = 0; tile < num_tiles; ++it, tile += stride) {
-        const int64_t ntile = tile + stride, nntile = ntile + stride;
+        const int nntile = tile + 2 * stride;
         const int b = it & 1;
         float* qcur = qb + b * CS_WBUF;
 
         int cont_row = -1;                     // DET: the row this slice continues from the slice before, if any
         if constexpr (DET) {
-            const int64_t e0 = tile * CS_TILE + 16 * w;
+            const int e0 = tile * CS_TILE + 16 * w;
             const int r0 = __shfl_sync(FULL, row_c, 0);
             if (r0 >= 0 && e0 > 0 && __ldg(a.row + e0 - 1) == r0) cont_row = r0;
         }
         float* const slot = DET ? a.slots + (size_t)(tile * 4 + w) * DET_EDGE_SLOT : nullptr;
 
         // ---- requests for the next tile (its staging buffer was released at the end of the previous tile) -------------
-        if (ntile < num_tiles) fetch_q(ntile, b ^ 1, n_col, n_row >= 0);
+        fetch_q(b ^ 1, n_row >= 0 ? n_col : -1);
         if (n_row >= 0) {
             cp_async16(xs, a.x4 + (size_t)n_row * 4);
             cp_async16(xs + 4, a.x4 + (size_t)n_col * 4);
@@ -212,11 +223,11 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             prefetch_l1(a.P + (size_t)n_row * H + 32);
         }
         if (has_edge(nntile)) {
-            const int64_t e = edge_of(nntile);
+            const int e = edge_of(nntile);
             cp_async4(nidx + lane, a.row + e);
             cp_async4(nidx + 16 + lane, a.col + e);
             if (AT == 1) cp_async4(nidx + 32 + 2 * lane, a.ea + e);
-            if (AT == 2) cp_async8(nidx + 32 + 2 * lane, a.ea + e * 2);
+            if (AT == 2) cp_async8(nidx + 32 + 2 * lane, a.ea + (size_t)e * 2);
         }
         cp_async_commit();
 
@@ -230,15 +241,15 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 eaa[k] = __shfl_sync(FULL, ea_c[k < AR ? k : 0], g);
                 eab[k] = __shfl_sync(FULL, ea_c[k < AR ? k : 0], g + 8);
             } else if (AT < 0) {   // generic count: read in place; zero beyond A (zero weight rows there too)
-                const int64_t e = tile * CS_TILE + 16 * w + g;
-                eaa[k] = (k < A && ra >= 0) ? __ldg(a.ea + e * A + k) : 0.f;
-                eab[k] = (k < A && rb >= 0) ? __ldg(a.ea + (e + 8) * A + k) : 0.f;
+                const int e = tile * CS_TILE + 16 * w + g;
+                eaa[k] = (k < A && ra >= 0) ? __ldg(a.ea + (size_t)e * A + k) : 0.f;
+                eab[k] = (k < A && rb >= 0) ? __ldg(a.ea + (size_t)(e + 8) * A + k) : 0.f;
             } else {
                 eaa[k] = eab[k] = 0.f;
             }
         }
-        const float* pa = a.P + (size_t)max(ra, 0) * H + 2 * q;
-        const float* pb = a.P + (size_t)max(rb, 0) * H + 2 * q;
+        const float* pa = Pq + (size_t)(uint32_t)max(ra, 0) * H;
+        const float* pb = Pq + (size_t)(uint32_t)max(rb, 0) * H;
         const float* qa = qcur + g * CS_QROW + 2 * q;
         const float* qbr = qa + 8 * CS_QROW;
         // DET: rows past the edge count are zero — their staging rows and attributes are left over from earlier tiles, and
@@ -262,7 +273,6 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         float qmax = 0.f;
         auto silu_guard = [&] { return silu_q_overflow(qmax); };
         tc16::RowScales s1;
-        mbar_wait(qbar + b, (uint32_t)((it >> 1) & 1));
         tc16::encode_rows<false, true>(
             [&](int j, f32x2& va, f32x2& vb, auto pass) {
                 va = pre(j, pa, qa, rada, eaa, oka);
@@ -303,16 +313,18 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
             __syncwarp();                      // the warp's m rows, written in the fragment pattern, are complete
             // lane <-> columns 2·lane, 2·lane+1: per edge one LDS.64 and one pair add; one RED.v2 per run and lane
             const float* colp = qcur + 2 * lane;
+            float* mrow = a.agg_m + 2 * lane;  // opaque, as Pq
+            asm("" : "+l"(mrow));
             auto flush = [&](f32x2 acc, int e_last) {
                 const int rr = __shfl_sync(FULL, row_c, e_last);
                 if (rr >= 0) {
                     float v0, v1;
                     upk2(mul2(acc, bc2(SILU_T_OUT)), v0, v1);
                     if constexpr (DET)
-                        *reinterpret_cast<float2*>(rr == cont_row ? slot + 2 * lane : a.agg_m + (size_t)rr * H + 2 * lane) =
+                        *reinterpret_cast<float2*>(rr == cont_row ? slot + 2 * lane : mrow + (size_t)(uint32_t)rr * H) =
                             make_float2(v0, v1);
                     else
-                        red_add_v2(a.agg_m + (size_t)rr * H + 2 * lane, v0, v1);
+                        red_add_v2(mrow + (size_t)(uint32_t)rr * H, v0, v1);
                 }
             };
             f32x2 s0 = *reinterpret_cast<const f32x2*>(colp);
@@ -338,9 +350,6 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
                 flush(s0, 15);
             }
         }
-        // this staging buffer is refilled by bulk copies (async proxy) at the start of the next tile
-        fence_proxy_async_smem();
-        __syncwarp();
         tc16::mma_f16x3_rA_wait(d, ahi, alo);
 
         // ---- stage 3: φ = w3·SiLU(D/s + bc) per row; Δx·φ summed per destination row ------------------------------
@@ -374,7 +383,10 @@ __global__ void __launch_bounds__(CS_THREADS, 1) edge_layer_cs_kernel(const Edge
         }
 
         // ---- roll the next tile's edge into place -------------------------------------------------------------
+        // the wait covers this lane's copies; the warp barrier publishes every lane's Q rows of the next tile and
+        // orders every lane's reads of this tile's buffer before the copies that refill it at the start of the next
         cp_async_wait_all();
+        __syncwarp();
         row_c = n_row;
         float4 xi_n = make_float4(0.f, 0.f, 0.f, 0.f), xj_n = xi_n;
         if (n_row >= 0) {
@@ -410,6 +422,10 @@ static int edge_layer_fwd(int64_t n_nodes, int64_t n_edges, int A, int C, int Na
     if (int rc = check_dims(A, C, Na)) return rc;
     if (n_edges == 0) return DISTEGNN_OK;
     DEGNN_CHECK_ARG(n_nodes > 0 && n_edges > 0, "negative size");
+    // The kernel's tile numbers and edge ids are int32.  An edge id tile·64 + 16w + lane of a tile (tile < ⌈E/64⌉) is
+    // below E + 63, and tile + 2·stride (stride = 4·grid, grid <= the SM count) below 2^25 + 8·SMs: both fit when
+    // E + 63 <= INT32_MAX.  With n_edges_dev, E is the capacity and bounds the device count.
+    DEGNN_CHECK_ARG(n_edges <= INT32_MAX - (CS_TILE - 1), "n_edges (the capacity with n_edges_dev) above 2^31 - 64");
     DEGNN_CHECK_ARG(row && col && x4 && P && Q && layer_params && agg_x, "null pointer");
     DEGNN_CHECK_ARG(A == 0 || edge_attr_sorted, "null edge_attr with edge_attr_nf > 0");
     DEGNN_CHECK_ARG((flags & DISTEGNN_FLAG_LAST) || agg_m, "null agg_m");
@@ -421,7 +437,7 @@ static int edge_layer_fwd(int64_t n_nodes, int64_t n_edges, int A, int C, int Na
     }
     Layout L = make_layout(A, C, Na);
     EdgeCsArgs a;
-    a.N = n_nodes; a.E = n_edges; a.E_dev = n_edges_dev; a.A = A; a.flags = flags & 0xffffu;
+    a.N = n_nodes; a.E = (int)n_edges; a.E_dev = n_edges_dev; a.A = A; a.flags = flags & 0xffffu;
     a.row = row; a.col = col; a.ea = edge_attr_sorted; a.x4 = x4; a.P = P; a.Q = Q;
     a.w1r = layer_params + L.off[DISTEGNN_P_E_W1R];
     a.w1e = layer_params + L.off[DISTEGNN_P_E_W1E];

@@ -188,9 +188,10 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 // ---- per-thread async copies global -> shared (LDGSTS: per-lane addresses, no registers, generic proxy) ------------
 // Completion is per issuing thread (commit_group / wait_group); a thread that only reads what it copied itself needs
 // no barrier.  16-byte form bypasses L1 (.cg); the 4/8-byte forms allocate in L1 (.ca is the only variant).
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+__device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gsrc) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr), "l"(gsrc) : "memory");
 }
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) { cp_async16(smem_u32(smem_dst), gsrc); }
 __device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }

@@ -5,8 +5,9 @@ edge_attr_nf = 2, C = 8, the same seeded graph.
 
 Each launch is timed with CUDA events after a 256 MiB L2 flush, for both values of FLAG_LAST.  With two libraries the
 launches alternate between them (A, B, A, B, ...), so that clock and neighbour changes hit both alike, and the outputs of
-the two are compared.  GB/s uses bench.py's byte count for the kernel, E·284 + N·536, against the H100 SXM data-sheet
-HBM bandwidth of 3.35 TB/s.
+the two are compared: the default mode's as a relative difference (float atomics add in arrival order), the
+deterministic mode's (distegnn_edge_layer_fwd_det, then distegnn_edge_combine_det) bit for bit.  GB/s uses bench.py's
+byte count for the kernel, E·284 + N·536, against the H100 SXM data-sheet HBM bandwidth of 3.35 TB/s.
 """
 from __future__ import annotations
 
@@ -34,10 +35,13 @@ _i64, _i32, _u32, _vp = C.c_int64, C.c_int, C.c_uint, C.c_void_p
 
 def load(path):
     lib = C.CDLL(path)
-    fn = lib.distegnn_edge_layer_fwd
-    fn.argtypes = [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 11
-    fn.restype = C.c_int
-    return fn
+    for name, argtypes in (("distegnn_edge_layer_fwd", [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 11),
+                           ("distegnn_edge_layer_fwd_det", [_i64, _i64, _i32, _i32, _i32, _u32] + [_vp] * 11 + [_i64, _vp]),
+                           ("distegnn_edge_combine_det", [_i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+                           ("distegnn_deterministic_workspace_bytes", [_i64, _i64, _i32, _vp])):
+        getattr(lib, name).argtypes = argtypes
+        getattr(lib, name).restype = C.c_int
+    return lib
 
 
 def gpu_info():
@@ -55,7 +59,8 @@ def main():
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     libs = args.lib or [_lib.LIB_PATH]
-    fns = [load(p) for p in libs]
+    dets = [load(p) for p in libs]
+    fns = [lib.distegnn_edge_layer_fwd for lib in dets]
     assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda:0")
 
@@ -86,6 +91,25 @@ def main():
                     ptr(Q), ptr(lp), ptr(agg_m[i]), ptr(agg_x[i]), None, stream)
         assert rc == 0, f"{libs[i]}: distegnn_edge_layer_fwd returned {rc}"
 
+    ws_bytes = C.c_int64(0)
+    assert dets[0].distegnn_deterministic_workspace_bytes(N, E, w.virtual_channels, C.byref(ws_bytes)) == 0
+    ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=dev)
+
+    def deterministic(i, flags):
+        """One deterministic-mode edge stage (kernel, then combine) of library i: (agg_m or None, agg_x)."""
+        m = None if flags & _lib.FLAG_LAST else torch.zeros(N, 64, device=dev)
+        x = torch.zeros(N, 4, device=dev)
+        lib = dets[i]
+        rc = lib.distegnn_edge_layer_fwd_det(N, E, A, w.virtual_channels, w.node_attr_nf, flags, ptr(row), ptr(col),
+                                             ptr(ea), ptr(x4), ptr(P), ptr(Q), ptr(lp), ptr(m), ptr(x), None, ptr(ws),
+                                             ws.numel(), stream)
+        assert rc == 0, f"{libs[i]}: distegnn_edge_layer_fwd_det returned {rc}"
+        rc = lib.distegnn_edge_combine_det(N, E, w.virtual_channels, ptr(row), None, ptr(m), ptr(x), ptr(ws), ws.numel(),
+                                           stream)
+        assert rc == 0, f"{libs[i]}: distegnn_edge_combine_det returned {rc}"
+        torch.cuda.synchronize()
+        return m, x
+
     nbytes = E * 284 + N * 536
     result = {"gpu": gpu_info(), "N": N, "E": E, "A": A, "bytes_per_launch": nbytes, "peak_GBps": PEAK_GBS,
               "launches": args.launches, "libs": libs, "flags": {}}
@@ -113,6 +137,7 @@ def main():
             ms = [s.elapsed_time(e) for s, e in times[i]]
             mean = statistics.fmean(ms)
             entry[p] = {"mean_ms": mean, "median_ms": statistics.median(ms), "min_ms": min(ms), "max_ms": max(ms),
+                        "stdev_ms": statistics.stdev(ms),
                         "GBps": nbytes / (mean * 1e-3) / 1e9, "frac_of_peak": nbytes / (mean * 1e-3) / 1e9 / PEAK_GBS}
         if len(fns) == 2:
             ref_m, ref_x = outs[0]
@@ -120,6 +145,9 @@ def main():
                 "agg_x": float((outs[1][1] - ref_x).abs().max() / ref_x.abs().max()),
                 "agg_m": None if flags else float((outs[1][0] - ref_m).abs().max() / ref_m.abs().max())}
             entry["speedup"] = entry[libs[0]]["mean_ms"] / entry[libs[1]]["mean_ms"]
+            (m0, x0), (m1, x1) = deterministic(0, flags), deterministic(1, flags)
+            entry["deterministic_bitwise_equal"] = {"agg_x": bool(torch.equal(x0, x1)),
+                                                    "agg_m": None if flags else bool(torch.equal(m0, m1))}
         result["flags"][name] = entry
     print(json.dumps(result, indent=1))
     if args.out:
