@@ -19,6 +19,7 @@ Recipes (the reference's per-sample lines, restated exactly; `s` the scene's sta
                 attr = type
     largefluid  (:480-557)  x = pos[f], target = pos[f+Δ], v = vel[f], feat = [viscosity, mass, ‖vel[f]‖],
                 attr = [viscosity, mass]
+    protein     (:142-198)  Water-3D's columns with the charge q in place of the type: feat = [‖v‖, q / max q], attr = q
 
 `loc_mean` and the max are taken over the whole scene before any split (distribute_graphs.py:32; :346 then :348).  The
 graph: a radius graph per sample (of this rank's nodes) with `radius_graph_csr`, or for `radius` None / < 0 the fully
@@ -28,6 +29,8 @@ every graph (:103, `cutoff_edges_csr`).  `edge_attr` is the length in every colu
 Input layout.  N-body: the reference's own `loc_*.npy`, `vel_*.npy` [S,T,n,3] and `charges_*.npy` [S,n,1].  Water-3D and
 Fluid113K: one `.npz` per scene holding `position` [T,n,3], optionally `velocity` [T,n,3], and the static fields
 (`particle_type` [n], or `viscosity` and `mass` [n]).  Uncompressed `.npz` members (np.savez) are memory-mapped.
+Protein: one trajectory, a CHARMM PSF and DCD (or one `.npz` with `position` and `charges`), read by
+`distegnn_b200.protein.load_protein` (DESIGN §27).
 
 Training noise (DESIGN §22).  `FrameLoader(..., noise=(σ_x, σ_v))` trains on a perturbed input state, so that the model
 sees inputs like the slightly wrong ones it feeds itself in a rollout (GNS's input noise):
@@ -86,7 +89,11 @@ RECIPES = {
     "nbody": Recipe("nbody", _lib.FRAMES_NBODY, ("charges",), True, 2, 1, None, None),
     "water3d": Recipe("water3d", _lib.FRAMES_WATER3D, ("particle_type",), False, 2, 1, 250, 15),          # :245
     "largefluid": Recipe("largefluid", _lib.FRAMES_LARGEFLUID, ("viscosity", "mass"), True, 3, 2, 50, 16),  # :499
+    "protein": Recipe("protein", _lib.FRAMES_WATER3D, ("charges",), False, 2, 1, None, None),
 }
+
+# the protein recipe's samples: every frame of a fixed range of its one trajectory, per split (:205-209)
+PROTEIN_SPLITS = {"train": (0, 2481), "valid": (2481, 2481 + 827), "test": (2481 + 827, 2481 + 827 + 863)}
 
 
 def recipe_of(name: str) -> Recipe:
@@ -178,6 +185,9 @@ def load_scenes(paths: Sequence[str], recipe: str) -> Trajectories:
     """One .npz per scene (Water-3D: `position`, `particle_type`; Fluid113K: `position`, `velocity`, `viscosity`,
     `mass`)."""
     rc = recipe_of(recipe)
+    if rc.name == "protein":
+        raise ValueError("unknown recipe 'protein' for a list of .npz scenes: the protein recipe is one trajectory, "
+                         "read by distegnn_b200.protein.load_protein")
     scenes = []
     for p in paths:
         z = _npz_members(p)
@@ -209,14 +219,22 @@ def load_nbody(directory: str, partition: str = "train", tag: str = "charged100_
 
 def sample_list(traj: Trajectories, seed: int = 0, max_samples: Optional[int] = None, delta_t: int = 1,
                 frame_0: int = 0, frames_per_scene: Optional[int] = None,
-                max_frame: Optional[int] = None) -> List[Tuple[int, int]]:
+                max_frame: Optional[int] = None, split: Optional[str] = None) -> List[Tuple[int, int]]:
     """The reference's samples as (scene, frame) pairs.  N-body: every system at `frame_0`, the first `max_samples`
     (:81).  Water-3D / Fluid113K: scene by scene, min(frames_per_scene, max_samples − drawn) frames `randint(0,
     max_frame)` (:245, :499: 15 of [0, 250], 16 of [0, 50]) from `random.Random(seed)` — the reference's distribution
-    (its thread pool makes its exact set irreproducible).  Raises if a sample's frames fall outside its scene."""
+    (its thread pool makes its exact set irreproducible).  Protein: every frame of `PROTEIN_SPLITS[split]` of its one
+    scene, in order (:205-211; `max_samples` does not apply, as in the reference).  Raises if a sample's frames fall
+    outside its scene."""
     rc = traj.recipe
     cap = len(traj) * 10 ** 9 if max_samples is None else int(max_samples)
-    if rc.max_frame is None:
+    if rc.name == "protein":
+        if split not in PROTEIN_SPLITS:
+            raise ValueError(f"the protein recipe's samples need split= one of {', '.join(PROTEIN_SPLITS)} (got {split!r})")
+        if len(traj) != 1:
+            raise ValueError(f"the protein recipe reads one trajectory (got {len(traj)} scenes)")
+        out = [(0, t) for t in range(*PROTEIN_SPLITS[split])]
+    elif rc.max_frame is None:
         out = [(s, int(frame_0)) for s in range(min(len(traj), cap))]
     else:
         per = rc.per_scene if frames_per_scene is None else int(frames_per_scene)

@@ -23,8 +23,8 @@ fused forward AND backward kernels under DDP.  The synthetic path has no splits,
 (below); wandb logging stays with the reference (out of scope).
 
 `--trajectory PATH` trains and evaluates on real frames instead (distegnn_b200.frames.FrameLoader, DESIGN §18): the
-config's recipe (N-body, Water-3D, Fluid113K), radius / inner_radius, delta_t (N-body: frame_0, frame_T), split_mode and
-cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  With `--rollout_steps K`
+config's recipe (N-body, Water-3D, Fluid113K, protein: DESIGN §27), radius / inner_radius, delta_t (N-body: frame_0,
+frame_T), split_mode and cutoff_rate; every batch is assembled on the device from the raw trajectories as it is needed.  With `--rollout_steps K`
 it then rolls the trained model out K steps from every validation batch and prints the per-step MSE against the recorded
 frames f + Δ .. f + KΔ (DESIGN §19; `--rollout_tau` sets the velocity's time step, Water-3D defaults to Δ);
 `--rollout_chamfer` adds both directions of the normalised Chamfer distance to every step's line (DESIGN §20).
@@ -117,7 +117,8 @@ def parse():
     p.add_argument("--train_steps", type=int, default=0, help="(new) optimisation steps of the reference's training "
                    "step (utils/train.py:98-158) on the synthetic target")
     p.add_argument("--trajectory", type=str, default=None, help="(new) train and evaluate on raw frames under this "
-                   "directory (distegnn_b200.frames): N-body .npy files, or train/ and valid/ folders of .npz scenes; "
+                   "directory (distegnn_b200.frames): N-body .npy files, the protein's PSF and DCD, or train/ and valid/ "
+                   "folders of .npz scenes; "
                    "with --rollout_steps K also a K-step rollout from every validation batch against the recorded frames")
     p.add_argument("--rollout_chamfer", action="store_true", help="(new) with --trajectory and --rollout_steps: also "
                    "print each step's Chamfer distance to the recorded frame (prediction -> record, record -> "
@@ -150,8 +151,13 @@ def nbody_tag(cfg):
 
 
 def split_files(path, recipe, part, tag="charged100_0_0_1"):
-    """The files of split `part` under `path`: N-body's loc_`part`_`tag`.npy, or `path`/`part`/*.npz; [] if missing."""
+    """The files of split `part` under `path`: N-body's loc_`part`_`tag`.npy, the protein trajectory in `path` (one PSF
+    and one DCD, or one .npz: `protein.find_files`; the same files for every split), or `path`/`part`/*.npz; [] if
+    missing."""
     import glob
+    if recipe == "protein":
+        from distegnn_b200.protein import find_files
+        return find_files(path)
     if recipe == "nbody":
         f = os.path.join(path, f"loc_{part}_{tag}.npy")
         return [f] if os.path.exists(f) else []
@@ -239,6 +245,10 @@ def split_samples(path, cfg, part, horizon=1):
     files = split_files(path, recipe, part, nbody_tag(cfg))
     if not files:
         return None
+    if recipe == "protein":                                    # every frame of the split's fixed range
+        from distegnn_b200.protein import load_protein
+        traj = load_protein(files, backbone=bool(d.get("backbone", True)))
+        return traj, sample_list(traj, delta_t=delta, split=part)
     traj = load_nbody(path, part, nbody_tag(cfg)) if recipe == "nbody" else load_scenes(files, recipe)
     kw = {}
     if recipe != "nbody":
@@ -249,6 +259,53 @@ def split_samples(path, cfg, part, horizon=1):
                              f"{horizon} step(s) of delta_t={delta} frames after any frame")
     return traj, sample_list(traj, seed=int(cfg.get("seed", 0)), max_samples=d.get("max_samples"), delta_t=delta,
                              frame_0=frame_0, **kw)
+
+
+def protein_test_transform(path, cfg):
+    """FrameLoader's rotate / translate keywords for the protein recipe's test split: `data.test_rot` a Haar-uniform
+    rotation per sample, `data.test_trans` a translation S·N(0, I) with S half the edge of the DCD's cubic unit cell
+    (the reference's randn(3)·box/2, process_dataset.py:162-174).  ValueError when test_trans is set and the trajectory
+    has no single cubic cell over the test frames."""
+    from distegnn_b200.frames import PROTEIN_SPLITS
+    from distegnn_b200.protein import cubic_edge, read_dcd
+    d = cfg["data"]
+    rot, trans = bool(d.get("test_rot", False)), bool(d.get("test_trans", False))
+    out = dict(rotate=True) if rot else {}
+    if trans:
+        dcd = [f for f in split_files(path, "protein", "test") if f.endswith(".dcd")]
+        if not dcd:
+            raise ValueError(f"data.test_trans needs a DCD with a cubic unit cell (the translation is box/2·N(0, I)); "
+                             f"{path} has none")
+        try:                                                   # the cell of every sample's frame t
+            out["translate"] = cubic_edge(read_dcd(dcd[0]), range(*PROTEIN_SPLITS["test"])) / 2
+        except ValueError as e:
+            raise ValueError(f"data.test_trans needs a cubic unit cell (the translation is box/2·N(0, I)): {e}") from None
+    return out
+
+
+def protein_check(args, cfg):
+    """The protein recipe with --trajectory: exits with code 2 and a message, before any CUDA work, when the trajectory
+    is missing, cannot hold every sample of the three splits (delta_t frames after the last), or cannot give the test
+    split's translation (`protein_test_transform`)."""
+    if not args.trajectory or recipe_of_config(cfg)[0] != "protein":
+        return
+    from distegnn_b200.frames import check_samples
+    msg = None
+    try:
+        if not split_files(args.trajectory, "protein", "train"):
+            msg = (f"--trajectory {args.trajectory}: no protein trajectory (one .psf and one .dcd, or one .npz with "
+                   "position and charges)")
+        else:
+            for part in ("train", "valid", "test"):
+                traj, samples = split_samples(args.trajectory, cfg, part)
+                check_samples(traj, samples, recipe_of_config(cfg)[2])
+            protein_test_transform(args.trajectory, cfg)
+    except (OSError, ValueError) as e:
+        msg = f"--trajectory {args.trajectory}: {e}"
+    if msg is not None:
+        if int(os.environ.get("LOCAL_RANK", "0")) == 0:
+            print(msg, flush=True)
+        sys.exit(2)
 
 
 def train_rollout_of(args, cfg):
@@ -300,6 +357,7 @@ def main():
         cfg["data"]["inner_radius"] = args.inner_radius
     if args.virtual_channels is not None:
         cfg["model"]["virtual_channels"] = args.virtual_channels
+    protein_check(args, cfg)
     epochs = epochs_of(args, cfg)
     train_rollout = train_rollout_of(args, cfg)
 
@@ -427,7 +485,8 @@ def recipe_of_config(cfg):
     """(recipe name, frame_0, Δ) of the config's dataset (N-body: frame_T − frame_0; else data.delta_t)."""
     d = cfg["data"]
     ds = str(d.get("dataset_name", "")).lower()
-    recipe = "nbody" if ds.startswith("nbody") else "water3d" if ds.startswith("water") else "largefluid"
+    recipe = "nbody" if ds.startswith("nbody") else "water3d" if ds.startswith("water") else \
+        "protein" if ds.startswith("protein") else "largefluid"
     if recipe == "nbody":
         frame_0, frame_T = int(d.get("frame_0", 30)), int(d.get("frame_T", 40))
         return recipe, frame_0, frame_T - frame_0
@@ -445,7 +504,8 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
     N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only;
     `transform` (rotate, translate) to every loader built (the same samples as without it: a rotated and translated
-    copy of the split).  Returns (recipe name, {part: loader or None})."""
+    copy of the split); without it the protein recipe's test loader takes data.test_rot / data.test_trans
+    (`protein_test_transform`).  Returns (recipe name, {part: loader or None})."""
     from distegnn_b200.frames import FrameLoader
     d = cfg["data"]
     recipe, _, delta = recipe_of_config(cfg)
@@ -469,6 +529,8 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
             out[part] = None
             continue
         traj, samples = found
+        if recipe == "protein" and part == "test" and transform is None:
+            xf = protein_test_transform(path, cfg)
         out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
                                 seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
                                 cutoff_rate=rate or 0.0, horizon=horizon, noise=noise if part == "train" else None,
@@ -483,7 +545,8 @@ def rollout_args(args, cfg, local_rank, K=None, flag="--rollout_steps"):
     any training when the rollout could not run (no `--rollout_tau` for a recipe with physical velocities)."""
     recipe, _, delta = recipe_of_config(cfg)
     K = args.rollout_steps if K is None else K
-    tau = args.rollout_tau if args.rollout_tau is not None else (float(delta) if recipe == "water3d" else None)
+    tau = args.rollout_tau if args.rollout_tau is not None else \
+        (float(delta) if recipe in ("water3d", "protein") else None)
     if tau is None and recipe == "nbody" and args.trajectory:   # files written by distegnn_b200.nbody record their dt
         from distegnn_b200.nbody import meta_rollout_tau
         tau = meta_rollout_tau(args.trajectory, delta, "_" + nbody_tag(cfg))
@@ -858,8 +921,9 @@ def transform_label(transform):
         or "untransformed"
 
 
-# the |v| column of each recipe's node features (distegnn_b200/frames.py): N-body, Water-3D [‖v‖, ·], Fluid113K [·, ·, ‖v‖]
-SPEED_COL = {"nbody": 0, "water3d": 0, "largefluid": 2}
+# the |v| column of each recipe's node features (distegnn_b200/frames.py): N-body, Water-3D, protein [‖v‖, ·],
+# Fluid113K [·, ·, ‖v‖]
+SPEED_COL = {"nbody": 0, "water3d": 0, "largefluid": 2, "protein": 0}
 
 
 def rollout_eval(args, cfg, model, world_size, local_rank, rate, recipe, tau, transform=None):
