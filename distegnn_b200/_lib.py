@@ -47,6 +47,8 @@ SIGNATURES = {
     "distegnn_rollout_advance_bwd": [_i64, _i32, _i32, C.c_float] + [_vp] * 9,
     "distegnn_cutoff_csr_workspace_bytes": [_i64, _i32, _i64, C.POINTER(_i64)],
     "distegnn_cutoff_csr": [_i64, _i32, _vp, _vp, C.c_double, _i32, _vp, _vp, _vp, _vp, _i64] + [_vp] * 7 + [_i64, _vp],
+    "distegnn_csr_sorted_i64": [_i64, _i64] + [_vp] * 6,
+    "distegnn_metis_recursive": [_i64, _vp, _vp, _i64, _vp, _vp],
     "distegnn_kmeans_lloyd": [_i64, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp],
     "distegnn_kmeans_lloyd_d": [_i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp, C.c_float, _i32, _vp, _vp],
     "distegnn_spectral_workspace_bytes": [_i64, _i32, _i32, C.POINTER(_i64)],

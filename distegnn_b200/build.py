@@ -2,7 +2,9 @@
 
     python -m distegnn_b200.build [--force] [--verbose]
 
-  libdistegnn_b200.so          the product: every entry point of include/distegnn_b200.h (csrc/*.cu)
+  libdistegnn_b200.so          the product: every entry point of include/distegnn_b200.h (csrc/*.cu), with the CUDA
+                               toolkit's METIS 5 (libmetis_static.a, Apache-2.0, shipped for cuSOLVER) linked in and its
+                               symbols not exported (DESIGN §10)
   libdistegnn_b200_testing.so  cross-check twins of include/distegnn_b200_testing.h (csrc/testing/*.cu), the
                                deterministic mode's entry points with a grid cap, and W ranks of the virtual-node
                                exchange in one launch; loaded only by tests, never by the package
@@ -67,9 +69,19 @@ def _compile(src, verbose):
     return obj
 
 
-def _link(lib, objs):
+def metis_archive() -> str:
+    """The toolkit's METIS 5 (64-bit idx_t; cuSOLVER's dependency) next to the `NVCC` in use; raises if it is missing."""
+    path = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(NVCC))), "targets", "x86_64-linux", "lib",
+                        "libmetis_static.a")
+    if not os.path.exists(path):
+        raise RuntimeError(f"{path} not found: split_mode='metis' links the CUDA toolkit's METIS archive (shipped with "
+                           "cuSOLVER)")
+    return path
+
+
+def _link(lib, objs, extra=()):
     tmp = lib + ".tmp"                      # link aside, then rename: a snapshot of the tree never sees a half-written .so
-    p = subprocess.run([NVCC, *ARCH, "-shared", "-o", tmp, *objs, "-cudart", "shared",
+    p = subprocess.run([NVCC, *ARCH, "-shared", "-o", tmp, *objs, *extra, "-cudart", "shared",
                         "-Xlinker", "-rpath,/usr/local/cuda/lib64"], capture_output=True, text=True)
     if p.returncode != 0:
         raise RuntimeError(f"link failed:\n{p.stdout}\n{p.stderr}")
@@ -86,7 +98,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OBJ, exist_ok=True)
     with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs) + len(tsrcs))) as ex:
         objs = dict(zip(srcs + tsrcs, ex.map(lambda s: _compile(s, verbose), srcs + tsrcs)))
-    _link(LIB, [objs[s] for s in srcs])
+    # METIS (csrc/metis.cu) linked in statically, its and GKlib's symbols kept out of the dynamic symbol table
+    _link(LIB, [objs[s] for s in srcs], [metis_archive(), "-Xlinker", "--exclude-libs,libmetis_static.a"])
     _link(LIB_TESTING, [objs[s] for s in COMMON + DET_SHARED + COMM_SHARED] + [objs[s] for s in tsrcs])
     return LIB
 

@@ -314,8 +314,11 @@ class FrameLoader:
     delta_t         target frame offset (N-body: frame_T − frame_0)
     radius          radius of the graph (per partition: the reference's inner_radius); None or < 0 = fully connected
     world_size, rank, split_mode   this rank's share of every sample: "random" (a randperm chunk from a generator seeded
-                    per sample, `sample_generator(i)`, identical on every rank), "kmeans" or "spectral" (labels computed
-                    on first use and cached; spectral: world_size <= 16); every rank needs nodes of every sample, else ValueError
+                    per sample, `sample_generator(i)`, identical on every rank), "kmeans", "spectral" or "metis" (labels
+                    computed from the sample's frame on first use and cached; spectral: world_size <= 16; metis: on the
+                    graph of radius `outer_radius`); every rank needs nodes of every sample, else ValueError
+    outer_radius    the radius of the graph the metis split partitions (the reference's outer_radius; split_mode="metis"
+                    with world_size > 1 needs it)
     cutoff_rate     > 0: keep the int(E_b·(1 − rate)) shortest edges of every graph
     capacity        None: exact graph allocation (the edge counts are read back every batch).  K: edge buffers of K
                     entries and no host synchronisation at all; `check()` raises if a batch overflowed them
@@ -338,16 +341,20 @@ class FrameLoader:
                  split_mode: str = "random", split_seed: Optional[int] = None, cutoff_rate: float = 0.0,
                  capacity: Optional[int] = None, edge_attr_nf: int = 2, loop: bool = False, horizon: int = 1,
                  noise: Optional[Tuple[float, float]] = None, noise_seed: Optional[int] = None,
-                 rotate: bool = False, translate: float = 0.0, transform_seed: Optional[int] = None):
+                 rotate: bool = False, translate: float = 0.0, transform_seed: Optional[int] = None,
+                 outer_radius: Optional[float] = None):
         self.traj, self.samples, self.delta_t = traj, [(int(s), int(f)) for s, f in samples], int(delta_t)
         check_samples(traj, self.samples, self.delta_t, horizon)
         self.horizon = horizon
         if world_size < 1 or not 0 <= rank < world_size:
             raise ValueError(f"rank {rank} outside world_size {world_size}")
-        if world_size > 1 and split_mode not in ("random", "kmeans", "spectral"):
-            raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral)")
+        if world_size > 1 and split_mode not in ("random", "kmeans", "spectral", "metis"):
+            raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral|metis)")
         if world_size > 1 and split_mode == "spectral" and world_size > 16:
             raise ValueError(f"split_mode='spectral' splits into at most 16 parts (world_size {world_size})")
+        if world_size > 1 and split_mode == "metis" and outer_radius is None:
+            raise ValueError("split_mode='metis' needs outer_radius (the radius of the graph METIS partitions)")
+        self.outer_radius = None if outer_radius is None else float(outer_radius)
         self.radius = None if radius is None or radius < 0 else float(radius)
         self.batch_size, self.shuffle, self.drop_last = int(batch_size), shuffle, drop_last
         self.device = torch.device(device) if device is not None else None
@@ -402,12 +409,13 @@ class FrameLoader:
         n = self.traj.scenes[s].n_nodes
         if self.world_size == 1:
             return None, [n]
-        if self.split_mode in ("kmeans", "spectral"):
+        if self.split_mode in ("kmeans", "spectral", "metis"):
             if i not in self._kmeans:
                 if self.device is None or self.device.type != "cuda":
                     raise _lib.DistEGNNError(f"split_mode={self.split_mode!r} runs on a CUDA device")
                 pos = torch.from_numpy(np.array(self.traj.scenes[s].position[f], dtype=np.float32))
-                chunks = node_chunks(n, self.world_size, self.split_mode, pos=pos.to(self.device))
+                chunks = node_chunks(n, self.world_size, self.split_mode, pos=pos.to(self.device),
+                                     outer_radius=self.outer_radius)
                 counts = [int(c.numel()) for c in chunks]
                 self._check_counts(i, counts)
                 self._kmeans[i] = (chunks[self.rank].to("cpu", torch.int32), counts)

@@ -5,7 +5,8 @@
     graph, edge_attr = cutoff_edges_csr(graph, pos, 0.5, batch)      # FastEGNN's cutoff: the shortest half of each graph
     labels = kmeans_labels(pos, world_size)                          # == sklearn KMeans(random_state=0).fit_predict
     labels = spectral_labels(pos, world_size)                        # the reference's SpectralClustering (spectral.py)
-    parts = split_large_graph(pos, x, target, vel, attr, r, P, split_mode="random" | "kmeans" | "spectral")
+    labels = metis_labels(pos, world_size, outer_radius)             # the reference's METIS on the outer-radius graph
+    parts = split_large_graph(pos, x, target, vel, attr, r, P, split_mode="random" | "kmeans" | "spectral" | "metis")
 
 `radius_graph_csr` is one C-ABI call (csrc/radius_csr.cu): bounding box, grid sizing, cell keys, sort, counts, prefix sums
 and the fill all run on the device, so it never synchronises when the caller passes a `capacity` (rollouts: reuse the
@@ -15,6 +16,9 @@ a `CSRGraph` that `FastEGNN.forward` takes as is — no COO->CSR sort, no edge_a
 `kmeans_labels` keeps sklearn's own k-means++ seeding (`sklearn.cluster.kmeans_plusplus`, host — it reproduces the
 reference's `random_state=0`) and runs the Lloyd iterations with sklearn's stopping rules on the device (csrc/kmeans.cu).
 CUDA only; there is no CPU path.
+
+`metis_labels` builds the outer-radius graph and sorts its rows on the device (csrc/metis.cu), then runs the CUDA
+toolkit's METIS (`METIS_PartGraphRecursive`, linked into the library) on the host, as the reference does.
 """
 from __future__ import annotations
 
@@ -308,36 +312,117 @@ def kmeans_labels(pos: Tensor, n_clusters: int, random_state: int = 0, max_iter:
     return labels.to(torch.int64)
 
 
+def csr_sorted_i64(graph: CSRGraph) -> Tuple[Tensor, Tensor]:
+    """(xadj int64 [N+1], adjncy int64 [capacity]) of a device-built id-order CSR graph with every row's neighbours
+    ascending: `index2ptr(sort_edge_index(edge_index))` as the reference hands it to METIS (distribute_graphs.py:155-157).
+    One launch (csrc/metis.cu), no host synchronisation; the edge count on the device is honoured (`graph.n_edges_dev`),
+    entries of adjncy at and past it are left unwritten."""
+    if graph.rowptr.device.type != "cuda":
+        raise _lib.DistEGNNError("distegnn_b200.csr_sorted_i64 runs only on CUDA tensors (no CPU path)")
+    dev = graph.rowptr.device
+    N, cap = graph.num_nodes, int(graph.col.numel())
+    xadj = torch.empty(N + 1, dtype=torch.int64, device=dev)
+    adjncy = torch.empty(cap, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().distegnn_csr_sorted_i64(
+            N, cap, ptr(graph.rowptr.contiguous()), ptr(graph.col.contiguous() if cap else None),
+            ptr(graph.n_edges_dev), ptr(xadj), ptr(adjncy if cap else None), _lib.stream_ptr(dev)), "csr_sorted_i64")
+    return xadj, adjncy
+
+
+def metis_recursive(xadj, adjncy, n_parts: int) -> Tuple["np.ndarray", int]:
+    """(labels int64 [N], edge cut) of `METIS_PartGraphRecursive` on the host CSR (numpy int64 xadj [N+1], adjncy), with
+    the reference's arguments (distribute_graphs.py:151-185: no weights, default options) and its `num_parts <= 1` rule
+    (zeros, no METIS call).  Malformed input or n_parts outside [1, N] raises ValueError before METIS runs."""
+    import numpy as np
+    xadj = np.ascontiguousarray(xadj, dtype=np.int64)
+    adjncy = np.ascontiguousarray(adjncy, dtype=np.int64)
+    n = int(xadj.shape[0]) - 1
+    if n < 1:
+        raise ValueError("metis_recursive: the graph needs at least one node")
+    if int(xadj[-1]) > adjncy.shape[0]:
+        raise ValueError(f"metis_recursive: xadj[-1] = {int(xadj[-1])} past adjncy's {adjncy.shape[0]} entries")
+    part = np.empty(n, dtype=np.int64)
+    cut = C.c_int64(0)
+    check(_lib.load().distegnn_metis_recursive(n, xadj.ctypes.data, adjncy.ctypes.data if adjncy.size else None,
+                                                int(n_parts), part.ctypes.data, C.byref(cut)), "metis_recursive")
+    return part, int(cut.value)
+
+
+def metis_labels(pos: Tensor, n_parts: int, outer_radius: float) -> Tensor:
+    """The reference's METIS split (distribute_graphs.py:54-87, 151-185) as int64 labels [N] on `pos.device`: the
+    outer-radius graph `radius_graph(pos, outer_radius)` (symmetric, no self loops, no neighbour cap) built on the device,
+    its CSR sorted by (row, col) on the device (`csr_sorted_i64`), one copy to pinned host buffers,
+    `METIS_PartGraphRecursive` of the CUDA toolkit's METIS 5 on the host (`metis_recursive`), and one copy back.  The same
+    graph and the same call as the reference's, so the same labels wherever its METIS is the same version.  ValueError for
+    non-finite positions, outer_radius <= 0 or n_parts outside [1, N]."""
+    if pos.device.type != "cuda":
+        raise _lib.DistEGNNError("distegnn_b200.metis_labels runs only on CUDA tensors (no CPU path)")
+    import math
+    N = int(pos.shape[0])
+    if isinstance(n_parts, bool) or not isinstance(n_parts, numbers.Integral) or not 1 <= int(n_parts) <= N:
+        raise ValueError(f"metis_labels: n_parts must be an int in [1, N = {N}] (got {n_parts!r})")
+    if isinstance(outer_radius, bool) or not isinstance(outer_radius, numbers.Real) or \
+            not (math.isfinite(float(outer_radius)) and float(outer_radius) > 0):
+        raise ValueError(f"metis_labels: outer_radius must be finite and > 0 (got {outer_radius!r})")
+    dev = pos.device
+    p = pos.detach().to(torch.float32).contiguous()
+    if not bool(torch.isfinite(p).all()):
+        raise ValueError("metis_labels: positions must be finite (the radius graph gives a node with an inf or NaN "
+                         "coordinate no edges)")
+    if int(n_parts) == 1:                                        # the reference's metis(): zeros, no METIS call
+        return torch.zeros(N, dtype=torch.int64, device=dev)
+    g, _ = radius_graph_csr(p, float(outer_radius), edge_attr_nf=0)
+    xadj, adjncy = csr_sorted_i64(g)
+    xadj_h = torch.empty(N + 1, dtype=torch.int64, pin_memory=True)
+    adj_h = torch.empty(adjncy.numel(), dtype=torch.int64, pin_memory=True)
+    with torch.cuda.device(dev):
+        xadj_h.copy_(xadj, non_blocking=True)
+        adj_h.copy_(adjncy, non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()
+    part, _ = metis_recursive(xadj_h.numpy(), adj_h.numpy(), int(n_parts))
+    part_h = torch.from_numpy(part).pin_memory()
+    return part_h.to(dev, non_blocking=True)
+
+
 def node_chunks(n_nodes: int, world_size: int, split_mode: str = "random", pos: Optional[Tensor] = None,
-                generator=None) -> List[Tensor]:
+                generator=None, outer_radius: Optional[float] = None) -> List[Tensor]:
     """The node sets of the reference's partitioners, one int64 index tensor per rank: "random" = a host `randperm(n)` cut
     into P−1 chunks of ⌊n/P⌋ plus the remainder, in permutation order (distribute_graphs.py:26-30; host tensors);
     "kmeans" = `nonzero(kmeans_labels(pos) == i)`, nodes in index order (:188-198; on `pos.device`, needs `pos`);
-    "spectral" = the same with `spectral_labels(pos)` (:201-223; world_size <= 16)."""
+    "spectral" = the same with `spectral_labels(pos)` (:201-223; world_size <= 16); "metis" = the same with
+    `metis_labels(pos, world_size, outer_radius)` (:54-87; needs `outer_radius`)."""
     n = int(n_nodes)
     if split_mode == "random":
         idx = torch.randperm(n, generator=generator)             # on the host, as the reference (device == 'cpu')
         sizes = [n // world_size] * (world_size - 1)
         sizes.append(n - sum(sizes))
         return list(torch.split(idx, sizes))
-    if split_mode in ("kmeans", "spectral"):
+    if split_mode in ("kmeans", "spectral", "metis"):
         if pos is None:
             raise ValueError(f"split_mode={split_mode!r} needs the positions")
-        labels = kmeans_labels(pos, world_size) if split_mode == "kmeans" else spectral_labels(pos, world_size)
+        if split_mode == "metis":
+            if outer_radius is None:
+                raise ValueError("split_mode='metis' needs outer_radius (the radius of the graph METIS partitions)")
+            labels = metis_labels(pos, world_size, outer_radius)
+        else:
+            labels = kmeans_labels(pos, world_size) if split_mode == "kmeans" else spectral_labels(pos, world_size)
         return [torch.nonzero(labels == i, as_tuple=False).flatten() for i in range(world_size)]
-    raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral)")
+    raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral|metis)")
 
 
 def split_large_graph(pos: Tensor, x: Tensor, target: Tensor, vel: Tensor, attr: Optional[Tensor], radius: float,
                       world_size: int, split_mode: str = "random", special_nodes: Optional[Tensor] = None, generator=None,
-                      edge_attr_nf: int = 2) -> List[Dict[str, Tensor]]:
-    """Device-side form of the reference's partitioners (datasets/distribute_graphs.py:17-51 random, :118-143 k-means,
-    :90-115 spectral): node chunks by a host `randperm` (P−1 chunks of ⌊N/P⌋ + remainder) or by k-means or spectral
-    cluster (`pos[cluster == i]`, nodes in index order), every chunk with its own radius graph built on the device as CSR, `edge_attr` = the edge length in
-    `edge_attr_nf` columns (:44) and the GLOBAL `loc_mean` (:32).  Returns dicts with the reference's `Data` field names,
-    `edge_index` being a `CSRGraph` (what `FastEGNN.forward` consumes directly)."""
+                      edge_attr_nf: int = 2, outer_radius: Optional[float] = None) -> List[Dict[str, Tensor]]:
+    """Device-side form of the reference's partitioners (datasets/distribute_graphs.py:17-51 random, :54-87 METIS,
+    :118-143 k-means, :90-115 spectral): node chunks by a host `randperm` (P−1 chunks of ⌊N/P⌋ + remainder) or by METIS
+    part (of the `outer_radius` graph), k-means or spectral cluster (`pos[cluster == i]`, nodes in index order), every
+    chunk with its own radius graph (`radius`, the reference's inner_radius) built on the device as CSR, `edge_attr` =
+    the edge length in `edge_attr_nf` columns (:44) and the GLOBAL `loc_mean` (:32).  Returns dicts with the reference's
+    `Data` field names, `edge_index` being a `CSRGraph` (what `FastEGNN.forward` consumes directly)."""
     n = int(pos.shape[0])
-    chunks = [c.to(pos.device) for c in node_chunks(n, world_size, split_mode, pos=pos, generator=generator)]
+    chunks = [c.to(pos.device) for c in node_chunks(n, world_size, split_mode, pos=pos, generator=generator,
+                                                    outer_radius=outer_radius)]
     loc_mean = pos.mean(dim=0, keepdim=True)
     if special_nodes is None:
         special_nodes = torch.ones(n, dtype=torch.bool, device=pos.device)

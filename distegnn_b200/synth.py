@@ -9,8 +9,8 @@ synthetic restatement of what the reference's data pipeline hands to ``FastEGNN.
 * ``edge_attr`` = the edge length duplicated into two columns (``distribute_graphs.py:44``),
 * ``loc_mean`` = centroid of the *whole* graph, shared by all partitions (``distribute_graphs.py:32``),
 * ``split_mode=random`` (``distribute_graphs.py:26-30``), ``split_mode=kmeans``
-  (``distribute_graphs.py:118-143,188-198``) and ``split_mode=spectral`` (``:90-115,201-223``)
-  node partitioning with per-partition radius graphs
+  (``distribute_graphs.py:118-143,188-198``), ``split_mode=spectral`` (``:90-115,201-223``) and
+  ``split_mode=metis`` (``:54-87,151-185``) node partitioning with per-partition radius graphs
   (cross-partition edges are dropped, as in the reference).
 
 CPU/numpy only — this is input preparation, not part of the measured path.
@@ -149,16 +149,39 @@ def spectral_partition(pos: np.ndarray, world_size: int) -> List[np.ndarray]:
     return [np.nonzero(labels == i)[0] for i in range(world_size)]
 
 
+def metis_csr_np(pos: np.ndarray, outer_radius: float):
+    """(xadj, adjncy) int64 of the reference's METIS input (distribute_graphs.py:66-67, 155-157): the pairs of
+    ``radius_graph_np(pos, outer_radius)`` lexsorted by (row, col), the row counts as a pointer array."""
+    n = pos.shape[0]
+    ei = radius_graph_np(pos, outer_radius)
+    order = np.lexsort((ei[1], ei[0]))
+    xadj = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(np.bincount(ei[0], minlength=n), out=xadj[1:])
+    return xadj, np.ascontiguousarray(ei[1][order], dtype=np.int64)
+
+
+def metis_partition(pos: np.ndarray, world_size: int, outer_radius: float) -> List[np.ndarray]:
+    """distribute_graphs.py:54-87, 151-185 — ``METIS_PartGraphRecursive`` (the library's
+    ``distegnn_metis_recursive``, the toolkit's METIS) on the cKDTree outer-radius graph ``metis_csr_np``;
+    partition i = nodes with label i, in index order (``pos[cluster == i]``).  The host restatement of
+    ``distegnn_b200.metis_labels``: the same C call on a graph built without the device."""
+    from .partition import metis_recursive
+    xadj, adjncy = metis_csr_np(pos, outer_radius)
+    labels, _ = metis_recursive(xadj, adjncy, world_size)
+    return [np.nonzero(labels == i)[0] for i in range(world_size)]
+
+
 def make_partitions(w: Workload, world_size: int = 1, split_mode: str = "random", seed: int = 0,
-                    n_nodes: Optional[int] = None, only_rank: Optional[int] = None, device=None
-                    ) -> List[Optional[Dict[str, torch.Tensor]]]:
+                    n_nodes: Optional[int] = None, only_rank: Optional[int] = None, device=None,
+                    outer_radius: Optional[float] = None) -> List[Optional[Dict[str, torch.Tensor]]]:
     """One input dict per partition (= per rank), each with the forward() argument names.
 
     ``only_rank`` builds the (expensive) radius graph for that rank only and leaves ``None``
     elsewhere — every rank of a torchrun job calls this with its own rank and the same seed.
     ``device`` (a CUDA device) takes the spectral split's labels from the device partitioner
     (``distegnn_b200.spectral_labels``, O(N) memory) instead of the dense host restatement,
-    which only suits small clouds; the other modes ignore it.
+    which only suits small clouds; the other modes ignore it.  ``outer_radius`` is the radius of the
+    graph the metis split partitions (default: the workload's radius).
     """
     pts = make_points(w, seed, n_nodes)
     n = pts["pos"].shape[0]
@@ -175,8 +198,10 @@ def make_partitions(w: Workload, world_size: int = 1, split_mode: str = "random"
         chunks = [c.cpu().numpy() for c in node_chunks(n, world_size, "spectral", pos=pos)]
     elif split_mode == "spectral":
         chunks = spectral_partition(pts["pos"], world_size)
+    elif split_mode == "metis":
+        chunks = metis_partition(pts["pos"], world_size, w.radius if outer_radius is None else outer_radius)
     else:
-        raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral)")
+        raise ValueError(f"unsupported split_mode {split_mode!r} (random|kmeans|spectral|metis)")
     out: List[Optional[Dict[str, torch.Tensor]]] = []
     for r, idx in enumerate(chunks):
         if only_rank is not None and r != only_rank:

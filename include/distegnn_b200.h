@@ -310,6 +310,23 @@ DISTEGNN_API int distegnn_cutoff_csr(int64_t n_nodes, int n_graphs, const float 
                                      float *edge_attr_out, int32_t *info, void *workspace, int64_t workspace_bytes,
                                      void *stream);
 
+/* ---- METIS partitioner (csrc/metis.cu; distribute_graphs.py:54-87, 151-185) --------------------------------------------
+ * distegnn_csr_sorted_i64: the CSR METIS takes, from an id-order CSR (distegnn_radius_graph_csr: rowptr int32 [N+1], col
+ * int32 [n_edges], each row in cell-scan order): xadj int64 [N+1] = rowptr clamped to the valid edges, adjncy int64
+ * [n_edges] = every row's neighbours ascending, i.e. index2ptr(sort_edge_index(edge_index)).  n_edges is the capacity of
+ * col / adjncy; n_edges_dev (NULL: rowptr[N]) the valid count on the device; nothing at or past min(that, n_edges) is read.
+ * One launch, no host synchronisation, capturable; rows of any degree (longer rows cost O(degree²) each).
+ * distegnn_metis_recursive (host pointers, synchronous): part_host int64 [n_nodes] = METIS_PartGraphRecursive(n_nodes,
+ * ncon = 1, xadj, adjncy, no weights, n_parts, default options) of the CUDA toolkit's METIS 5, edge cut to *objval_host
+ * (may be NULL).  The input is checked first — xadj[0] = 0 and non-decreasing, every neighbour in [0, n_nodes) and not
+ * the row itself, 1 <= n_parts <= n_nodes — and rejected with DISTEGNN_EINVAL, so METIS never reaches its own error
+ * path.  n_parts = 1 gives zeros without calling METIS (the reference's `metis()`).  Calls are serialised (METIS keeps
+ * global state), and a given input gives the same labels on every call. */
+DISTEGNN_API int distegnn_csr_sorted_i64(int64_t n_nodes, int64_t n_edges, const int32_t *rowptr, const int32_t *col,
+                                         const int32_t *n_edges_dev, int64_t *xadj, int64_t *adjncy, void *stream);
+DISTEGNN_API int distegnn_metis_recursive(int64_t n_nodes, const int64_t *xadj_host, const int64_t *adjncy_host,
+                                          int64_t n_parts, int64_t *part_host, int64_t *objval_host);
+
 /* ---- k-means partitioner (csrc/kmeans.cu; distribute_graphs.py:188-198 and the label step of :201-223) ----------------
  * `iters` Lloyd iterations from `centers` with sklearn's stopping rules evaluated on the device (state [4], zero on the
  * first call: [0] 0 running / 1 final assignment pending / 2 done, [1] iterations done, [2] labels changed in the last

@@ -355,6 +355,8 @@ def main():
         cfg["model"]["checkpoint"] = args.checkpoint
     if args.inner_radius is not None:
         cfg["data"]["inner_radius"] = args.inner_radius
+    if args.outer_radius is not None:                          # the METIS split's graph radius (reference main.py)
+        cfg["data"]["outer_radius"] = args.outer_radius
     if args.virtual_channels is not None:
         cfg["model"]["virtual_channels"] = args.virtual_channels
     protein_check(args, cfg)
@@ -374,7 +376,8 @@ def main():
     # options of the reference CLI that belong to its data pipeline / epoch loop (out of scope here): say so, loudly
     ignored = [n for n, v in (("--wandb", args.wandb), ("--early_stop", None if epochs else args.early_stop),
                               ("--cutoff_rate", None if cutoff_mode else args.cutoff_rate),
-                              ("--outer_radius", args.outer_radius)) if v]
+                              ("--outer_radius", None if cfg["data"].get("split_mode") == "metis" else args.outer_radius))
+               if v]
     if ignored and int(os.environ.get("LOCAL_RANK", "0")) == 0:
         print(f"WARNING: {', '.join(ignored)} accepted for CLI compatibility but NOT used: logging, early stopping and "
               "the cutoff / outer-radius edge pruning live in the reference's data pipeline and epoch loop "
@@ -426,18 +429,18 @@ def main():
                        base.degree, m["node_feat_nf"], m["node_attr_nf"], m["edge_attr_nf"], m["virtual_channels"],
                        m["normalize"])
     split = d.get("split_mode", "random")
-    if world_size > 1 and split not in ("random", "kmeans", "spectral"):
+    if world_size > 1 and split == "metis":
+        outer = metis_outer_radius(d, local_rank)
         if local_rank == 0:
-            print(f"split_mode={split!r} needs the METIS partitioner of the reference's data pipeline; "
-                  "using 'random' for the synthetic graph")
-        split = "random"
+            print(f"split_mode='metis': METIS (recursive bisection) on the graph of outer_radius={outer}")
     cut = None
     if cutoff_mode:
         inp, cut = cutoff_inputs(w, int(d.get("batch_size", 1)), cfg.get("seed", 0), rate, local_rank)
         n_r, e_r = inp["node_loc"].shape[0], cut["kept"]
     else:
         part = synth.make_partitions(w, world_size=world_size, split_mode=split, seed=cfg.get("seed", 0),
-                                     only_rank=local_rank, device=torch.device("cuda", local_rank))[local_rank]
+                                     only_rank=local_rank, device=torch.device("cuda", local_rank),
+                                     outer_radius=d.get("outer_radius"))[local_rank]
         inp = {k: (v.to(local_rank) if v is not None else None) for k, v in part.items()}
         n_r, e_r = inp["node_loc"].shape[0], inp["edge_index"].shape[1]
 
@@ -500,8 +503,8 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     Fluid113K (`path`/train/*.npz, `path`/valid/*.npz, `path`/test/*.npz).  Only the train loader shuffles (the
     reference's same-seed sampler); a split without files gives None.  cutoff_edges mode: one graph per sample, radius = data.radius
     (−1 fully connected; Water-3D: the reference's hard-coded 0.035, :264), then the cutoff.  distribute mode: the
-    sample split over the ranks by split_mode (metis falls back to random, with a message), a radius graph per partition with
-    inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
+    sample split over the ranks by split_mode (metis on the graph of data.outer_radius), a radius graph per partition
+    with inner_radius.  `horizon` K: every sample holds frames f + Δ .. f + KΔ (the frame draw is capped for that; a fixed
     N-body frame_0 that cannot hold them exits with a message).  `noise` (σ_x, σ_v) goes to the train loader only;
     `transform` (rotate, translate) to every loader built (the same samples as without it: a rotated and translated
     copy of the split); without it the protein recipe's test loader takes data.test_rot / data.test_trans
@@ -515,11 +518,7 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
     else:
         radius = d.get("inner_radius")
     split = str(d.get("split_mode", "random"))
-    if split not in ("random", "kmeans", "spectral"):
-        if world_size > 1 and rank == 0:
-            print(f"split_mode={split!r} needs the METIS partitioner of the reference's data pipeline; "
-                  "using 'random' for the trajectories")
-        split = "random"
+    outer = metis_outer_radius(d, rank) if split == "metis" and world_size > 1 else None
     seed, bs = int(cfg.get("seed", 0)), int(d.get("batch_size", 1))
     xf = {} if transform is None else dict(rotate=transform[0], translate=transform[1])
     out = {}
@@ -534,10 +533,22 @@ def frame_loaders(path, cfg, world_size, rank, device, rate, horizon=1, parts=("
         out[part] = FrameLoader(traj, samples, delta_t=delta, radius=radius, batch_size=bs, shuffle=part == "train",
                                 seed=seed, device=device, world_size=world_size, rank=rank, split_mode=split,
                                 cutoff_rate=rate or 0.0, horizon=horizon, noise=noise if part == "train" else None,
-                                **xf)
+                                outer_radius=outer, **xf)
     if "train" in parts and out["train"] is None:
         raise SystemExit(f"--trajectory {path}: no training data for recipe {recipe!r}")
     return recipe, out
+
+
+def metis_outer_radius(d, rank):
+    """data.outer_radius (or --outer_radius), the radius of the graph the metis split partitions; exits with code 2 and
+    a message when it is missing or not > 0."""
+    r = d.get("outer_radius")
+    if r is None or not float(r) > 0:
+        if rank == 0:
+            print(f"split_mode='metis' needs data.outer_radius > 0 (or --outer_radius), the radius of the graph METIS "
+                  f"partitions (got {r!r})", flush=True)
+        sys.exit(2)
+    return float(r)
 
 
 def rollout_args(args, cfg, local_rank, K=None, flag="--rollout_steps"):
